@@ -5,7 +5,7 @@
   python bench.py --impl reference ...                    (the CPU path on the host cores; rank 0 only)
 
 A step = one pass of the hot path over the resident synthetic stream (BASELINE config 2: 10 GiB of random object bytes per
-GPU -> 10240 erasure blocks; inputs are far larger than the 126 MB L2, so no explicit flush is needed).
+GPU -> 10240 erasure blocks; inputs are far larger than the H100's 50 MB L2, so no explicit flush is needed).
   value     device-resident (inputs already in HBM), CUDA events, max over ranks
   e2e       the PutObject shape through the C ABI with HOST buffers: mec_encode_sg — H2D of the object bytes, fused kernel,
             parity frames + digests back by DMA — NUMA-local pinned buffers, rank bound to its GPU's node
@@ -14,6 +14,9 @@ GPU -> 10240 erasure blocks; inputs are far larger than the 126 MB L2, so no exp
   configs   BASELINE configs 3, 4 and 5 (device-resident kernels + config 4 through mec_heal_batch), each with its own
             roofline fraction and a check against the encode outputs
   cpu_baseline / --impl reference   the C oracle's SIMD path on a persistent, pinned pthread pool over all host cores
+  --dump-outputs DIR   after the timed steps, what the last step computed (rank 0) as float32 .npy files, for comparing builds:
+            digests.npy (blocks x 16 shards x 32 bytes), parity_sample.npy (a fixed seeded sample of blocks x 4 parity shards x S
+            bytes) and parity_sample_blocks.npy (which blocks); inputs depend on the arguments only
 """
 import argparse
 import ctypes as C
@@ -36,9 +39,6 @@ S = -(-BS // K)                      # 87382
 ALGO_BYTES_PER_BLOCK = BS + M * S + (K + M) * 32   # 1 398 616 (SURVEY.md §8d)
 GiB = float(1 << 30)
 METRIC = "fused RS(12,4) encode + HighwayHash256 bitrot, 1 MiB blocks"
-# ALU-pipe warp instructions of the steady-state loop per 256-byte tile of one erasure block (LOP3 + PRMT + IADD3 + IADD3.X in the
-# SASS of fused_rs_hh_kernel<GfStatic<12,4>,1,6,4,0,1>; profiles/r2_sass_loop.md says how to recount): 172 GF + 224 HighwayHash + 9 loop
-ALU_WARP_INSTR_PER_TILE_BLOCK = 405
 CPU_BLOCKS = int(os.environ.get("MEC_CPU_BLOCKS", "4096"))   # CPU arm: 4 GiB source per pass — larger than any last-level cache
 
 
@@ -46,17 +46,14 @@ def workload_config(nblocks, world):
     """The same dict for both arms (the driver compares them)."""
     return {"workload": f"BASELINE config 2: RS(12,4) encode+HighwayHash256S bitrot, 1 MiB blocks, {nblocks} blocks "
                         f"({nblocks * BS / GiB:.2f} GiB stream) per GPU",
-            "l2": "inputs (>=10 GiB per step) exceed the 126 MB L2; no explicit flush", "parallelism": f"sets-per-gpu x{world}"}
+            "l2": "inputs (>=10 GiB per step) exceed the 50 MB L2; no explicit flush", "parallelism": f"sets-per-gpu x{world}"}
 
 
-def read_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+# H100 SXM data-sheet HBM3 bandwidth (GB/s): the roofline fractions below are of this nominal figure, not of a measured one
+HBM_PEAK_GBS = 3350.0
+HBM_PEAK_SOURCE = "H100 SXM data sheet (3.35 TB/s HBM3)"
+# erasure blocks whose parity --dump-outputs writes, and most blocks whose digests it writes (float32: <= 64 MB in all)
+DUMP_PARITY_BLOCKS, DUMP_DIGEST_BLOCKS = 16, 16384
 
 
 class ClockSampler:
@@ -149,6 +146,31 @@ def reference_arm(args, threads):
 
 
 # ---------------------------------------------------------------------------------------------- helpers
+def gpu_name(index):
+    """The card and its power limit: absolute numbers are only meaningful next to both."""
+    try:
+        return subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip() or None
+    except Exception:
+        return None
+
+
+def dump_outputs(out_dir, par, dig, nblocks):
+    """The encode's outputs as float32 .npy: every block's 16 digests (a seeded sample of blocks beyond DUMP_DIGEST_BLOCKS) and the
+    parity shards of a seeded sample of DUMP_PARITY_BLOCKS blocks.  The sample depends on nblocks only."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0x4D494E494F)
+    pblocks = np.sort(rng.choice(nblocks, size=min(DUMP_PARITY_BLOCKS, nblocks), replace=False))
+    dblocks = np.sort(rng.choice(nblocks, size=DUMP_DIGEST_BLOCKS, replace=False)) if nblocks > DUMP_DIGEST_BLOCKS else None
+    idx = torch.from_numpy(pblocks).to(par.device)
+    parity = par.view(nblocks, M, -1)[idx, :, :S]
+    digests = dig if dblocks is None else dig[torch.from_numpy(dblocks).to(dig.device)]
+    np.save(os.path.join(out_dir, "parity_sample.npy"), parity.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "parity_sample_blocks.npy"), pblocks.astype(np.float64))
+    np.save(os.path.join(out_dir, "digests.npy"), digests.cpu().numpy().astype(np.float32))
+
+
 def pinned(nbytes, device):
     import minio_b200 as mb
     return mb.capi.pinned_array(nbytes, device=device)
@@ -170,6 +192,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-configs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (rank 0) to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -242,6 +265,8 @@ def main():
     barrier()
     mark1 = sampler.mark()
     launches = codec.launches - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, par, dig, nblocks)
     total_ms = max_over_ranks(t_all0.elapsed_time(t_all1))
     kern_ms = [a.elapsed_time(b) for a, b in evs]
     ms_per_step = total_ms / args.steps
@@ -396,7 +421,7 @@ def main():
             ms = max_over_ranks(res["ms"])
             return {"value": world * res["blocks"] * res["block_size"] / GiB / (ms / 1e3), "unit": "GiB/s", "ms": ms,
                     "roofline": {"bound": "hbm", "achieved": res["algorithmic_bytes_per_block"] * res["blocks"] / (ms / 1e3) / 1e9,
-                                 "frac": res["algorithmic_bytes_per_block"] * res["blocks"] / (ms / 1e3) / 1e9 / read_peaks()[0], "unit": "GB/s",
+                                 "frac": res["algorithmic_bytes_per_block"] * res["blocks"] / (ms / 1e3) / 1e9 / HBM_PEAK_GBS, "unit": "GB/s",
                                  "algorithmic_bytes_per_block": res["algorithmic_bytes_per_block"]},
                     "bit_exact_vs_encode": bool(res["bit_exact_vs_encode"]), "blocks_per_gpu": res["blocks"]}
         configs = {}
@@ -425,31 +450,17 @@ def main():
             dist.destroy_process_group()
         return
 
-    peak, peak_src = read_peaks()
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    traffic_src = None
-    if os.path.exists(tp):  # dram__bytes_read + dram__bytes_write of this kernel from the committed ncu capture, scaled per launch
-        tj = json.load(open(tp))
-        traffic = (tj["dram_bytes_read_per_block"] + tj["dram_bytes_write_per_block"]) * nblocks
-        traffic_src = f"profiles/r2_traffic.json: ncu --set full capture of {tj.get('blocks')} blocks, scaled per block (not measured in this run)"
     kavg_ms = sum(kern_ms) / len(kern_ms)
     achieved = ALGO_BYTES_PER_BLOCK * nblocks / (kavg_ms / 1e3) / 1e9
-    sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-    alu_ops = ALU_WARP_INSTR_PER_TILE_BLOCK * 32 * (S / 256.0) * nblocks        # lane-ops of the steady-state loop per launch
-    alu_rate = alu_ops / (kavg_ms / 1e3)
-    alu_peak = 64 * 148 * sm_mhz * 1e6
     cfg = workload_config(nblocks, world)
     out = {
         "metric": METRIC, "value": value, "unit": "GiB/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
         "data": "synthetic", "config": cfg,
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_block": ALGO_BYTES_PER_BLOCK,
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": HBM_PEAK_GBS, "unit": "GB/s", "frac": achieved / HBM_PEAK_GBS,
+                     "peak_source": HBM_PEAK_SOURCE, "algorithmic_bytes_per_block": ALGO_BYTES_PER_BLOCK,
                      "kernel_ms": kavg_ms, "blocks_per_launch": nblocks},
-        "alu_roofline": {"achieved_lane_ops_per_s": alu_rate, "peak_lane_ops_per_s": alu_peak, "frac": alu_rate / alu_peak,
-                         "alu_warp_instr_per_tile_block": ALU_WARP_INSTR_PER_TILE_BLOCK,
-                         "note": "the kernel is bound by the integer ALU pipe (64 lanes/clk/SM), not by HBM: this is the pipe's busy fraction from instruction counts"},
+        "gpu": gpu_name(local),
         "e2e": e2e, "e2e_frames": e2e_frames, "e2e_decode": e2e_decode, "e2e_verify": e2e_verify, "host_link": host_link,
         "gpu_launches": int(launches), "clocks": clocks, "verified_vs_oracle": verified,
     }
@@ -484,13 +495,13 @@ def main():
 
 
 def small_request_leg(mb, local):
-    """Launches that cannot fill the GPU: kernel time of a 1-block and a 148-block encode in the latency form (ec_small.cuh) and in the
-    throughput form, and the wall clock of one 1 MiB mec_encode_sg / mec_decode (four data drives offline) call from pinned buffers."""
+    """Launches that cannot fill the GPU: kernel time of a 1-block and a one-block-per-SM encode in the latency form (ec_small.cuh) and in
+    the throughput form, and the wall clock of one 1 MiB mec_encode_sg / mec_decode (four data drives offline) call from pinned buffers."""
     import torch
     k, m, bs = 12, 4, BS
     L = mb.lib()
     out = {"unit": "us"}
-    for nb in (1, 148):
+    for nb in (1, torch.cuda.get_device_properties(local).multi_processor_count):
         src = torch.randint(0, 256, (nb * bs,), dtype=torch.uint8, device=f"cuda:{local}")
         for name, small in (("latency_form", -1), ("throughput_form", 0)):
             c = mb.Codec(k, m, bs, device=local)

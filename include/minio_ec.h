@@ -1,5 +1,5 @@
 /*
- * minio_ec.h — C ABI of the B200 erasure-code + bitrot library (libminio_ec.so).
+ * minio_ec.h — C ABI of the H100 erasure-code + bitrot library (libminio_ec.so).
  *
  * Drop-in boundary for MinIO's erasure hot path.  The reference has no FFI here — the path sits
  * behind Go interfaces (reedsolomon.Encoder held by `Erasure.encoder`, hash.Hash from
@@ -174,7 +174,7 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
 
 /* ---- cross-request coalescer: many concurrent PutObject calls, one launch ---------------------------------------------------
  * MinIO encodes one block per loop iteration on every request goroutine (cmd/erasure-encode.go:76-108, one Erasure per request,
- * cmd/erasure-object.go:1371); a launch that small leaves 147 of 148 SMs idle.  A batcher owns one codec (k, m, block_size,
+ * cmd/erasure-object.go:1371); a launch that small leaves 131 of 132 SMs idle.  A batcher owns one codec (k, m, block_size,
  * HighwayHash256S) and a worker thread: callers block in mec_batcher_encode / mec_batcher_encode_sg (same arguments and results
  * as mec_encode / mec_encode_sg), the worker merges everything that is queued — up to max_batch_blocks erasure blocks, waiting
  * at most max_wait_us for company when the GPU is idle — into one staged buffer (one batched copy call) and ONE fused launch over
@@ -272,7 +272,7 @@ int mec_selftest(int device);
  * Compiled kernels are also kept on disk (MEC_JIT_CACHE_DIR, default $HOME/.cache/minio_b200, "off" disables), keyed by the kernel
  * sources, options and matrix: a restarted process loads the kernel of a pattern it has met before instead of recompiling.
  * "small_blocks": launches of at most this many erasure blocks run the latency form of the kernel (one CTA per block, hash warps
- *   decoupled from the GF warps: ~0.17 ms for a 1 MiB block instead of ~0.54 ms); -1 (default) = five per SM, 0 = never. */
+ *   decoupled from the GF warps: ~0.16 ms for a 1 MiB block instead of ~0.45 ms on an H100); -1 (default) = five per SM, 0 = never. */
 int mec_set_option(mec_codec* c, const char* name, int64_t value);
 /* Boundary counters (SURVEY §5 metrics row): name is one of "launches", "blocks_encoded", "blocks_read",
  * "shards_rebuilt", "corrupt_shards", "bytes_h2d", "bytes_d2h", "jit_compiles", "jit_ms", "jit_disk_hits" (process-wide), "jit_launches",

@@ -1,4 +1,4 @@
-"""minio_b200 — B200-native erasure-code + bitrot hot path of MinIO (RS GF(2^8) + HighwayHash-256).
+"""minio_b200 — H100-native (sm_90a) erasure-code + bitrot hot path of MinIO (RS GF(2^8) + HighwayHash-256).
 
 The product is the C-ABI shared library ``libminio_ec.so`` (include/minio_ec.h) built from
 ``minio_b200/csrc``; this package is only the thin ctypes binding tests and bench.py use.

@@ -94,7 +94,7 @@ extern "C" int mec_device_count(void) {
   return c;
 }
 extern "C" const char* mec_last_error(void) { return get_last_error(); }
-extern "C" const char* mec_version(void) { return "minio_b200 0.1 (sm_100a; fused RS+HighwayHash256)"; }
+extern "C" const char* mec_version(void) { return "minio_b200 0.1 (sm_90a; fused RS+HighwayHash256)"; }
 
 extern "C" int64_t mec_ceil_frac(int64_t a, int64_t b) { return ceil_frac(a, b); }
 extern "C" int64_t mec_shard_size(const mec_codec* c) { return c->S(); }
@@ -450,7 +450,7 @@ static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueu
   const int64_t nall = ceil_frac(len, bs);
   int64_t chunk = pick_chunk_blocks(c);
   // an object of a few chunks' worth or less is cut into ~four pieces so that its staging, kernel and copy-back overlap (a launch of
-  // a handful of blocks costs the same 0.17 ms as one of a hundred: for 8-64 MiB objects the copies are what is worth overlapping)
+  // a handful of blocks costs the same ~0.16 ms as one of a hundred: for 8-64 MiB objects the copies are what is worth overlapping)
   if (c->opt.chunk_blocks <= 0 && nall < 2 * chunk) chunk = std::max<int64_t>(4, ceil_frac(nall, 4));
   struct Drain {
     mec_codec* c;
@@ -932,7 +932,7 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
   } drain{c};
   const int64_t fstride = 32 + g.S, P = g.dpitch(), pitch = round_up(g.S, 16);
   // chunk: ~32 MiB of object per chunk keeps short ranges pipelined over several slots; long ranges take larger chunks (up to four
-  // times that) because every chunk costs a host round trip when it retires (measured: 34.3 -> 38.4 GiB/s on a 2 GiB GetObject)
+  // times that) because every chunk costs a host round trip when it retires
   int64_t chunk = std::max<int64_t>(1, (32ll << 20) / std::max<int64_t>(1, g.S * k));
   chunk = std::max(chunk, std::min(4 * chunk, g.nblocks / 12));
   if (g.nblocks < 2 * chunk) chunk = std::max<int64_t>(4, ceil_frac(g.nblocks, 4));  // short ranges: ~four pieces, copies overlap (see encode_pipeline)
@@ -973,8 +973,8 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     FrameGeom sub = g;  // geometry of the chunk: its last block is short only if it is the range's last block
     sub.nblocks = ch.nb;
     sub.last_len = (b0 + ch.nb == g.nblocks) ? g.last_len : g.S;
-    // (measured: one contiguous copy per survivor file + a device-side move to the aligned pitch is slower than these 2-D copies,
-    //  36.4 vs 38.3 GiB/s on the 2 GiB GetObject, although a bare copy-engine probe favours contiguous transfers — tools/copy_probe.cu)
+    // (one contiguous copy per survivor file + a device-side move to the aligned pitch was slower than these 2-D copies on a 2 GiB
+    //  GetObject, although a bare copy-engine probe favours contiguous transfers — tools/copy_probe.cu)
     const bool batched = ch.nb <= kBatchedCopyBlocks;
     CopyList list;
     if (batched) {
@@ -1955,7 +1955,7 @@ extern "C" int mec_selftest(int device) {
 // ------------------------------------------------------------------------------------------------
 // Cross-request coalescer.  MinIO builds one Erasure per request (cmd/erasure-object.go:1371) and encodes ONE block per loop
 // iteration (cmd/erasure-encode.go:76-108) on thousands of concurrent request goroutines (cmd/handler-api.go:139-143).  A GPU
-// launch that carries one 1 MiB block keeps one CTA busy on one of 148 SMs for as long as a launch of a thousand blocks takes.
+// launch that carries one 1 MiB block keeps one CTA busy on one of 132 SMs (H100) for as long as a launch of a thousand blocks takes.
 // The batcher turns concurrency into batch size: callers block in mec_batcher_encode*, a worker thread merges whatever is
 // queued (same k, m, block size by construction) into ONE staged buffer, ONE launch over all full blocks (plus one small
 // launch per short tail block), and one pass of DMA back into every caller's own frames; up to three merged batches are in
@@ -2130,7 +2130,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     cp.nreq = static_cast<int>(reqs.size()); cp.k = k; cp.m = m; cp.bs = bs; cp.S = S; cp.pitch = pitch;
     cp.staged = dsrc; cp.parity = dout; cp.digests = ddig;
     // staging: the copy engines are the faster reader of host memory (one call per request); the gather kernel (SM loads over
-    // PCIe, no per-request call at all) is kept for hosts where the worker thread is the bottleneck — measured in profiles/r2_concurrency.md
+    // PCIe, no per-request call at all) is kept for hosts where the worker thread is the bottleneck
     static const bool use_gather = getenv("MEC_BATCHER_GATHER") != nullptr;
     // requests [0, ndma) go through the copy engine, [ndma, nreq) through the gather kernel on the aux stream, concurrently
     size_t ndma = use_gather ? 0 : reqs.size();
@@ -2156,8 +2156,8 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
       if (ndma > 0) MEC_CUDA_OK(cudaEventRecord(b->ev_gather[si], gs));
     }
     {
-      // ONE cudaMemcpyBatchAsync for the whole batch: the copy engine runs a train of 1 MiB pieces at the link rate (55 GB/s) where
-      // the same pieces as separate cudaMemcpyAsync calls reach 40-46 GB/s (tools/copy_probe.cu, profiles/r2_concurrency.md)
+      // ONE cudaMemcpyBatchAsync for the whole batch: the copy engine runs a train of 1 MiB pieces at the link rate, faster than the
+      // same pieces as separate cudaMemcpyAsync calls (tools/copy_probe.cu compares the two)
       std::vector<void*> dsts, srcs;
       std::vector<size_t> sizes;
       for (size_t q = 0; q < ndma; q++) {
@@ -2313,7 +2313,7 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   if ((rc = s.hflags.ensure(static_cast<size_t>(nslots * k)))) return rc;
   // writeDataBlocks: 0 = the scatter kernel assembles every object in device memory and ONE copy per request takes it to the caller
   // (fewest driver-side copy descriptors), 1 = the scatter kernel stores straight into the callers' buffers over PCIe, 2 = the copy
-  // engine moves every (request, shard, block) piece itself — measured in profiles/r2_concurrency.md
+  // engine moves every (request, shard, block) piece itself
   static const int out_mode = getenv("MEC_BATCHER_GET_OUT") ? atoi(getenv("MEC_BATCHER_GET_OUT")) : 0;
   std::vector<int64_t> asm_off(reqs.size(), 0);
   if (out_mode == 0) {
@@ -2477,11 +2477,11 @@ static void batcher_main(mec_batcher* b) {
           return nb;
         };
         // an idle GPU gives the first caller up to max_wait_us of company before its batch is cut
-        // (measured, profiles/r2_concurrency.md: waiting while batches are in flight only adds latency to a closed loop of callers)
+        // (waiting while batches are in flight only adds latency to a closed loop of callers)
         if (nbusy == 0 && b->max_wait_us > 0 && blocks_queued() < b->max_blocks)
           b->cv_work.wait_for(lk, std::chrono::microseconds(b->max_wait_us), [&] { return b->stop || blocks_queued() >= b->max_blocks; });
         // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs, the same reader set)
-        // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.6 ms however few
+        // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.45 ms however few
         // blocks it is given (one warp walks one erasure block), so the copy of one batch has to overlap the kernel of another —
         // otherwise a closed loop of callers falls into a convoy (all of them in one batch, the GPU idle while they wake up)
         static const int depth = getenv("MEC_BATCHER_DEPTH") ? atoi(getenv("MEC_BATCHER_DEPTH")) : 4;
@@ -2578,7 +2578,7 @@ extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int
   if (max_wait_us >= 0) b->max_wait_us = max_wait_us;
   {
     // size every slot for a full batch up front: growing a buffer later means cudaFree + cudaMalloc, which stall the whole device
-    // (all six batches in flight) for tens of milliseconds — seen as p99 spikes of 150-450 ms before
+    // (all six batches in flight) for tens of milliseconds — seen as p99 spikes of hundreds of ms before
     std::lock_guard<std::mutex> lk(c->mu);
     int cur = 0;
     cudaGetDevice(&cur);

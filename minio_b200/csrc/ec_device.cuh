@@ -1,4 +1,4 @@
-// ec_device.cuh — device building blocks of the fused erasure-code + bitrot kernel (sm_100a).
+// ec_device.cuh — device building blocks of the fused erasure-code + bitrot kernel (sm_90a).
 //
 //   * packed GF(2^8) arithmetic on 4 bytes per 32-bit register (poly 0x11D — the field of
 //     klauspost/reedsolomon, used by cmd/erasure-coding.go:63,85,106,112)
@@ -48,7 +48,7 @@ __host__ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32
 // ---------------------------------------------------------------- packed GF(2^8)
 // multiply each of the 4 packed field elements by x (i.e. by 2) modulo x^8+x^4+x^3+x^2+1: PRMT sign-replicate gives
 // 0xff per byte whose msb is set, two ANDs and a shift finish it — 3 ALU-pipe ops, FMA pipe almost idle.  (Variants that
-// move work to the FMA pipe through IMAD.HI were measured in round 1 and lose: profiles/r1_pipe_microbench.md.)
+// move work to the FMA pipe through IMAD.HI lose to it; tools/ubench.cu measures the two pipes.)
 __host__ __device__ __forceinline__ uint32_t gf_xtime4(uint32_t a) {
   const uint32_t m = prmt(a, 0u, 0xba98u);
   return ((a & 0x7f7f7f7fu) << 1) ^ (m & 0x1d1d1d1du);

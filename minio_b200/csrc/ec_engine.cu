@@ -134,7 +134,7 @@ static NvrtcApi& nvrtc_api() {
 // The cache is process-wide (per device): MinIO builds one Erasure per request (cmd/erasure-object.go:1371), so a
 // per-codec cache would recompile the same erasure pattern for every object of a heal sweep.
 //
-// Policy.  A compile costs ≈0.4 s of one host core; the specialised kernel saves ≈1 ms per GiB over the generic one, so
+// Policy.  A compile costs ≈0.4 s of one host core; the specialised kernel saves ≈0.6 ms per GiB over the generic one, so
 // stalling a request for it never pays inside that request.  In automatic mode (option jit = -1) a pattern is therefore
 // compiled on a background thread once it has been seen with kJitHeatBytes of input, the requests that arrive meanwhile
 // run the generic runtime-matrix kernel, and later requests pick the specialised kernel up from the cache.  jit = 1
@@ -261,7 +261,7 @@ void* compile_specialised(const JitSpec& sp, bool load = true) {
   const char* expr = expr_s.c_str();
   if (api.create(&prog, src.c_str(), "mec_jit.cu", 4, bodies, names) != NVRTC_SUCCESS) return nullptr;
   api.add_name(prog, expr);
-  const char* opts[] = {"--gpu-architecture=sm_100a", "-std=c++17", "-default-device",
+  const char* opts[] = {"--gpu-architecture=sm_90a", "-std=c++17", "-default-device",
                         "-DMEC_HH_MUL=" MEC_STR(MEC_HH_MUL), "-DMEC_HH_VARIANT=" MEC_STR(MEC_HH_VARIANT),
                         "-DMEC_MIN_BLOCKS=" MEC_STR(MEC_MIN_BLOCKS),
                         "-DMEC_GF_LEVEL=" MEC_STR(MEC_GF_LEVEL), "-DMEC_GF_GROUP=" MEC_STR(MEC_GF_GROUP)};
@@ -461,8 +461,8 @@ int Engine::init() {
   cudaDeviceProp prop;
   MEC_CUDA_OK(cudaGetDeviceProperties(&prop, device_));
   num_sms_ = prop.multiProcessorCount;
-  if (prop.major < 10) {
-    set_last_error("device is not sm_100-class (kernels are built for sm_100a only)");
+  if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 only
+    set_last_error("device is not sm_90 (kernels are built for sm_90a only)");
     return MEC_ERR_UNSUPPORTED;
   }
   cudaDriverEntryPointQueryResult qres;
@@ -571,9 +571,9 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
   }
 
   // ---- launches that cannot fill the GPU take the latency kernel: one erasure block per CTA, hash warps decoupled from the GF
-  // warps (ec_small.cuh).  The throughput kernel needs ~0.6 ms for a 1 MiB block however few there are (one warp walks it);
-  // this one ~0.17 ms up to one block per SM and still less at five per SM (0.45 vs 0.6 ms); beyond ~six per SM both are bound by the
-  // same instruction count and the throughput kernel's occupancy wins (profiles/r2_small_latency.md).
+  // warps (ec_small.cuh).  The throughput kernel needs ~0.45 ms for a 1 MiB block however few there are (one warp walks it);
+  // this one ~0.16 ms up to one block per SM (RS(12,4), H100 80GB HBM3 at a 400 W power limit); a few blocks per SM later both are
+  // bound by the same instruction count and the throughput kernel's occupancy wins.
   {
     if (small_ok(opt, d.nblocks) && d.S > 0 && (d.contiguous || d.in_ptr[0] != nullptr)) {
       for (int t = 0; t < d.k; t++) p.in_ptr[t] = d.contiguous ? d.in_base + static_cast<int64_t>(t) * d.S : d.in_ptr[t];

@@ -64,7 +64,7 @@ struct EngineOptions {
   int64_t chunk_blocks = 0; // host pipeline chunk (0 = auto)
   int64_t small_blocks = -1; // launches of at most this many erasure blocks take the latency kernel (ec_small.cuh); -1: 5 per SM, 0: never
   int static_groups = 1;   // 1 (default): erasure-block groups are dealt to CTAs statically (g += gridDim.x); 0: through a claim counter —
-                           // measured equal on a dedicated GPU (profiles/r2_kernel_ab.md), useful when SMs are shared or uneven
+                           // useful when SMs are shared or uneven
 };
 
 class Engine {

@@ -1,4 +1,4 @@
-// ec_kernel.cuh — the fused Reed-Solomon + HighwayHash-256 kernel (sm_100a).
+// ec_kernel.cuh — the fused Reed-Solomon + HighwayHash-256 kernel (sm_90a).
 //
 // One launch consumes `nblocks` erasure blocks.  For each block it reads k input shards ONCE
 // (cmd/erasure-coding.go:81 Split layout for encode; surviving shards for reconstruct/heal),

@@ -1,8 +1,8 @@
-// ec_small.cuh — the latency form of the fused Reed-Solomon + HighwayHash-256 kernel (sm_100a).
+// ec_small.cuh — the latency form of the fused Reed-Solomon + HighwayHash-256 kernel (sm_90a).
 //
 // The throughput kernel (ec_kernel.cuh) gives every erasure block to ONE warp: its lanes multiply a 256-byte tile, then the same
-// lanes hash it, 341 times per 1 MiB block — ~0.6 ms however few blocks the launch brings (a PutObject of one small object, the
-// 1 MiB-per-iteration loop of cmd/erasure-encode.go:76-108, a merged batch of a few dozen requests), with 147 SMs idle.
+// lanes hash it, 341 times per 1 MiB block — ~0.45 ms however few blocks the launch brings (a PutObject of one small object, the
+// 1 MiB-per-iteration loop of cmd/erasure-encode.go:76-108, a merged batch of a few dozen requests), with most SMs idle.
 // HighwayHash is a serial chain per shard, so a block cannot be finished faster than 2731 dependent packet updates; what CAN be
 // removed is everything else on that critical path.  Here a CTA owns one block and is warp-specialised:
 //   * GF warps (three or four, one 8-byte column per thread of a 768- or 1024-byte super-tile): fetch with cp.async (16-byte chunks
@@ -18,8 +18,7 @@
 namespace mec {
 
 // GW = GF warps per CTA: three beside one hash warp (up to 16 streams; 55 KB of shared memory for RS(12,4): four CTAs per SM),
-// four beside two or three (wider stripes have more GF and fetch work per column: RS(16,4) takes 154 us per block with four GF
-// warps, 238 us with two).  A pipeline stage ("super-tile") is 256 bytes of every shard per GF warp.
+// four beside two or three (wider stripes have more GF and fetch work per column than two GF warps keep up with).  A pipeline stage ("super-tile") is 256 bytes of every shard per GF warp.
 __host__ __device__ constexpr int small_super(int gw) { return 256 * gw; }
 __host__ __device__ constexpr int small_chunks(int gw) { return small_super(gw) / 16 + 1; }  // 16-byte chunks per row and stage (lead <= 15 bytes + funnel slack)
 __host__ __device__ constexpr int small_raw_pitch(int gw) { return small_chunks(gw) * 16 + 16; }

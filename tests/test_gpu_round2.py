@@ -186,7 +186,7 @@ def test_parity_only_tail_block(mb, oracle):
 def test_group_claiming_modes_agree(mb, oracle, static_groups):
     """Dynamic group claiming (several passes per CTA) and the static deal produce the same bytes."""
     import torch
-    k, m, bs, nblocks = 12, 4, MiB, 9000   # > 7 CTAs x 148 SMs x 4 blocks: every CTA claims at least one more group
+    k, m, bs, nblocks = 12, 4, MiB, 9000   # > 7 CTAs x 132 SMs x 4 blocks: every CTA claims at least one more group
     dev = torch.device("cuda:0")
     g = torch.Generator(device=dev); g.manual_seed(1234)
     src = torch.randint(0, 256, (nblocks * bs,), dtype=torch.uint8, device=dev, generator=g)

@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 import minio_b200 as mb  # noqa: E402
 
 GiB = float(1 << 30)
-PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+PEAK = 3350.0  # GB/s: H100 SXM data-sheet HBM3 bandwidth; frac_of_hbm_peak is of this nominal figure
 dev = torch.device("cuda:0")
 
 

@@ -17,7 +17,7 @@ def main():
     k, m, bs = (int(sys.argv[1]), int(sys.argv[2]), 1 << 20) if len(sys.argv) > 2 else (12, 4, 1 << 20)
     torch.cuda.set_device(0)
     out = []
-    for nb in (1, 2, 4, 8, 16, 32, 64, 148, 296, 444, 592, 888, 1184, 2072, 4144):
+    for nb in (1, 2, 4, 8, 16, 32, 64, 132, 264, 396, 528, 792, 1056, 1848, 3696):
         row = {"blocks": nb}
         src = torch.randint(0, 256, (nb * bs,), dtype=torch.uint8, device="cuda")
         for name, small in (("latency_kernel", 1 << 30), ("throughput_kernel", 0)):

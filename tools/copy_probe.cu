@@ -1,5 +1,5 @@
 // copy_probe: what the copy engine sustains for a train of small pinned H2D copies (the coalescer's staging pattern), alone and
-// with a D2H train on another stream.  nvcc -O2 -arch=sm_100a -o copy_probe copy_probe.cu
+// with a D2H train on another stream.  nvcc -O2 -arch=sm_90a -o copy_probe copy_probe.cu
 #include <cuda_runtime.h>
 #include <chrono>
 #include <cstdio>

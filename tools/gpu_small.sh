@@ -1,6 +1,8 @@
 #!/bin/bash
-cd "${GRAFT_REPO_ROOT:-/root/repo}"
-mkdir -p gpurun_out
-python tools/bench_small.py 12 4 2>&1 | grep -E "\"blocks\": (1|148|592|888)," | tee gpurun_out/small_12_4_b.jsonl
-python tools/bench_small.py 16 4 2>&1 | grep -E "\"blocks\": (1|148|592)," | tee gpurun_out/small_16_4_b.jsonl
-timeout 1500 python -m pytest tests -q -m gpu --timeout 900 -x > gpurun_out/pytest_gpu.txt 2>&1; echo "rc=$?"; tail -3 gpurun_out/pytest_gpu.txt
+# latency-form sweep (one block, one block per SM and a few per SM) and the GPU tests; results go to $OUT (default bench_out/)
+cd "$(dirname "$0")/.."
+O=${OUT:-bench_out}
+mkdir -p "$O"
+python tools/bench_small.py 12 4 2>&1 | grep -E "\"blocks\": (1|132|528|792)," | tee "$O/small_12_4_b.jsonl"
+python tools/bench_small.py 16 4 2>&1 | grep -E "\"blocks\": (1|132|528)," | tee "$O/small_16_4_b.jsonl"
+timeout 1500 python -m pytest tests -q -m gpu --timeout 900 -x > "$O/pytest_gpu.txt" 2>&1; echo "rc=$?"; tail -3 "$O/pytest_gpu.txt"

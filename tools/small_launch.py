@@ -4,7 +4,7 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import minio_b200 as mb
-nb = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+nb = int(sys.argv[1]) if len(sys.argv) > 1 else 132
 k, m, bs = 12, 4, 1 << 20
 c = mb.Codec(k, m, bs)
 S = c.shard_size(); pitch = (S + 15) // 16 * 16

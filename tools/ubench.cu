@@ -1,7 +1,7 @@
-// tools/ubench.cu — integer-pipe throughput microbenchmarks for sm_100a (B200).
+// tools/ubench.cu — integer-pipe throughput microbenchmarks for sm_90a (H100).
 // Reports warp-instructions issued per clock per SM for the op classes the fused kernel is made of,
 // to decide how to balance GF(2^8)/HighwayHash work between the ALU pipe (LOP3/PRMT/IADD3/SHF) and
-// the FMA pipe (IMAD*).  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o ubench ubench.cu
+// the FMA pipe (IMAD*).  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o ubench ubench.cu
 #include <cstdio>
 #include <cstdint>
 #include <vector>

@@ -1,6 +1,6 @@
 // tools/ubench2.cu — compute-only ceilings of the two halves of the fused kernel (no memory traffic):
 //   HH: HighwayHash half-state updates per clock,  GF: (12 -> 4) packed GF(2^8) products per clock.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I minio_b200/csrc [-DMEC_XTIME=n] -o ubench2 tools/ubench2.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I minio_b200/csrc [-DMEC_XTIME=n] -o ubench2 tools/ubench2.cu
 #include <cstdio>
 #include <vector>
 #include <cuda_runtime.h>
