@@ -49,6 +49,8 @@ void DevBuf::release() {
 using KernelFn = void (*)(const FusedParams, const TmaMaps);
 using SmallFn = void (*)(const FusedParams);  // latency kernel (ec_small.cuh): one erasure block per CTA
 constexpr int kStaticEb = 4;  // erasure blocks per CTA of the compile-time specialised kernels
+// raw-tile bytes in flight per SM that the 3-D-fetch encode of misaligned rows is sized to (launch_fused): five RS(12,4) CTAs
+constexpr int64_t kRawBytesInFlightPerSm = 5 * 12 * 1152;
 
 struct StaticEntry {
   int k, m, sm16;
@@ -828,7 +830,16 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
     }
   }
   if (per_sm < 1) per_sm = 1;
-  if (opt.grid_mult > 0 && opt.grid_mult < per_sm) per_sm = opt.grid_mult;
+  // The encode of misaligned rows with the 3-D fetch is bound by the TMA loads in flight, not by occupancy: every CTA has one raw
+  // tile (k rows x eb blocks) outstanding, and on H100 the bytes move fastest with about kRawBytesInFlightPerSm of them per SM
+  // (DESIGN §4): fewer CTAs than fit, and more of them for narrow stripes than for wide ones
+  int cap = opt.grid_mult;
+  if (cap <= 0 && rows3d && any_misaligned) {
+    const int64_t raw_tile = static_cast<int64_t>(d.k) * raw_group_bytes(eb, p.raw_pitch);
+    cap = static_cast<int>(kRawBytesInFlightPerSm / raw_tile);
+    if (cap < 1) cap = 1;
+  }
+  if (cap > 0 && cap < per_sm) per_sm = cap;
   const int64_t ngroups = (d.nblocks + eb - 1) / eb;
   int64_t grid = static_cast<int64_t>(per_sm) * num_sms_;
   if (grid > ngroups) grid = ngroups;

@@ -57,7 +57,7 @@ struct EngineOptions {
   int force_bytewise = 0;  // 1: never use TMA
   int force_dynamic = 0;   // 1: never use the compile-time specialised GF kernels
   int balance_grid = 0;  // shrink the persistent grid so that every CTA makes the same number of passes
-  int grid_mult = 0;       // CTAs per SM (0 = occupancy)
+  int grid_mult = 0;       // CTAs per SM (0 = occupancy; the 3-D-fetch encode of misaligned rows is capped at a budget of load bytes in flight)
   int jit = -1;            // decode-matrix kernels specialised at run time with NVRTC: -1 auto (large launches), 0 never, 1 always
   int no_rows3d = 0;       // 1: never use the one-request-per-tile 3-D TMA fetch
   int use_auto = 0;        // 1: warp-autonomous pipeline (no CTA barriers) when k + r == 16; measured slower, off by default

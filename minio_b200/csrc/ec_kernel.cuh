@@ -9,7 +9,8 @@
 //
 // Work decomposition (all integer/byte work, ALU-issue- and HBM-bound; no tensor cores):
 //   CTA      = `eb` erasure blocks (4 in the specialised kernels: one warp per block), blockDim = 2*(k+r)*eb rounded
-//              up to a warp multiple; persistent grid of as many CTAs as fit (7 per SM for RS(12,4))
+//              up to a warp multiple; persistent grid of as many CTAs as fit (7 per SM for RS(12,4); the misaligned 3-D encode launches
+//              as many as a budget of load bytes in flight allows, 5 per SM for RS(12,4))
 //   tile     = 256 bytes of every shard.  Shards start at arbitrary byte offsets of the object
 //              (S = ceil(blockSize/k) is 87382 for RS(12,4)@1MiB) but TMA boxes must start on 16-byte boundaries
 //              (tools/tma_probe.cu), so each row is fetched as a 16B-aligned superset ("raw" tile, cp.async.bulk.tensor
