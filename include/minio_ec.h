@@ -277,6 +277,13 @@ int mec_set_option(mec_codec* c, const char* name, int64_t value);
 /* Boundary counters (SURVEY §5 metrics row): name is one of "launches", "blocks_encoded", "blocks_read",
  * "shards_rebuilt", "corrupt_shards", "bytes_h2d", "bytes_d2h", "jit_compiles", "jit_ms", "jit_disk_hits" (process-wide), "jit_launches",
  * "small_launches" (launches that took the latency form).  -1 for unknown names.
+ * Kernel dispatch (which form of the fused kernel ran, for tests and diagnosis): "form_<f>" counts the launches of form f, one of
+ *   small (latency kernel), fast3d, fast3d_auto, fast3d_semi, fast, fast_auto, aligned, aligned_auto, runtime, bytewise (the
+ *   compile-time (k, m) kernels), dyn_aligned, dyn_runtime, dyn_bytewise (runtime matrix), jit (NVRTC-specialised);
+ *   the last fused launch: "last_eb" (erasure blocks per CTA), "last_grid" (CTAs), "last_tma_mode" (0 byte-wise, 1 2-D boxes per
+ *   row, 2 one tensor map per input, 3 runs of uniformly spaced inputs; -1 latency kernel), "last_rows3d" (one 3-D request per
+ *   tile), "last_direct" (rows fetched straight into the hashed tile), "last_tiles3d" (tiles of a shard fetched in 3-D),
+ *   "last_row_chunk" (runtime-matrix rows per pass: 0, 1, 2 for 1, 2, 4; -1 for a compile-time matrix); "num_sms".
  * Every ABI call is also wrapped in an NVTX range (visible in Nsight Systems) — the tracing hook of SURVEY §5. */
 int64_t mec_get_stat(const mec_codec* c, const char* name);
 /* Stops background kernel specialisation and waits for a compile in flight.  Call before the process exits (exit()

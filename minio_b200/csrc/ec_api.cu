@@ -205,6 +205,9 @@ extern "C" int64_t mec_get_stat(const mec_codec* c, const char* name) {
   if (!strcmp(name, "small_launches")) return c->eng ? c->eng->small_launches() : 0;
   if (!strcmp(name, "jit_ms")) return c->eng ? static_cast<int64_t>(c->eng->jit_seconds() * 1e3) : 0;
   if (!strcmp(name, "jit_disk_hits")) return c->eng ? c->eng->jit_disk_hits() : 0;
+  static const Engine kNoLaunches(0);  // dispatch record of a handle that has not launched yet
+  int64_t v = 0;
+  if ((c->eng ? *c->eng : kNoLaunches).dispatch_stat(name, &v)) return v;
   return -1;
 }
 extern "C" void mec_shutdown(void) { mec::jit_shutdown(); }

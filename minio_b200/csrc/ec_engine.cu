@@ -638,6 +638,12 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
         MEC_CUDA_OK(cudaGetLastError());
         launches_++;
         small_launches_++;
+        LaunchRecord rec;
+        rec.form = kFormSmall;
+        rec.eb = 1;
+        rec.grid = d.nblocks;
+        rec.row_chunk = se ? -1 : (d.r <= 1 ? 0 : (d.r == 2 ? 1 : 2));
+        record_launch(rec);
         return MEC_OK;
       }
     }
@@ -651,6 +657,7 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
   const int64_t ntiles = (static_cast<int64_t>(d.S) + kTile - 1) / kTile;
   bool use_tma = !opt.force_bytewise && d.S > 0;
   bool any_misaligned = false, rows3d = false, direct = false;
+  int raw_rows = 0;           // rows of the raw tile with the 3-D fetch (raw_rows_3d)
   void* jit3d = nullptr;      // NVRTC-specialised encode kernel with the one-request-per-tile fetch, when it is ready
   bool jit3d_tried = false;
   p.in_block_stride = d.in_block_stride;
@@ -697,6 +704,7 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
                        static_cast<uint32_t>(raw3 / 4), static_cast<uint32_t>(eb), static_cast<uint64_t>(d.k),
                        static_cast<uint64_t>(row_stride), static_cast<uint32_t>(rg)) == MEC_OK) {
             rows3d = true;
+            raw_rows = raw_rows_3d(d.k, rg);
             maps.m[1] = m3;
             p.tiles_3d = static_cast<int>((row_stride - raw3 - shift_max) / kTile) + 1;
             p.raw_pitch = raw3;
@@ -784,17 +792,34 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
   else if (direct) p.raw_pitch = kRowPitch;
 
   KernelFn fn;
+  LaunchRecord rec;
   if (se) {
     const int sm16 = static_cast<int>(d.S & 15);
-    if (!use_tma) fn = se->bytewise;
-    else if (rows3d) fn = (opt.use_auto == 1 && se->fast3d_auto && !direct) ? se->fast3d_auto
-                          : ((opt.use_auto == 2 && se->fast3d_semi && !direct) ? se->fast3d_semi : se->fast3d);
-    else if (eb == kStaticEb && sm16 == se->sm16) fn = (opt.use_auto == 1 && se->fast_auto) ? se->fast_auto : se->fast;
-    else if (eb == kStaticEb && sm16 == 0) fn = (opt.use_auto == 1 && se->aligned_auto) ? se->aligned_auto : se->aligned;
-    else fn = se->runtime;
+    if (!use_tma) {
+      fn = se->bytewise;
+      rec.form = kFormBytewise;
+    } else if (rows3d) {
+      const bool autop = opt.use_auto == 1 && se->fast3d_auto && !direct;
+      const bool semi = !autop && opt.use_auto == 2 && se->fast3d_semi && !direct;
+      fn = autop ? se->fast3d_auto : (semi ? se->fast3d_semi : se->fast3d);
+      rec.form = autop ? kFormFast3dAuto : (semi ? kFormFast3dSemi : kFormFast3d);
+    } else if (eb == kStaticEb && sm16 == se->sm16) {
+      const bool autop = opt.use_auto == 1 && se->fast_auto;
+      fn = autop ? se->fast_auto : se->fast;
+      rec.form = autop ? kFormFastAuto : kFormFast;
+    } else if (eb == kStaticEb && sm16 == 0) {
+      const bool autop = opt.use_auto == 1 && se->aligned_auto;
+      fn = autop ? se->aligned_auto : se->aligned;
+      rec.form = autop ? kFormAlignedAuto : kFormAligned;
+    } else {
+      fn = se->runtime;
+      rec.form = kFormRuntime;
+    }
   } else {
     const int rc = d.r <= 1 ? 0 : (d.r == 2 ? 1 : 2);
     fn = !use_tma ? kDynBytewise[rc] : (any_misaligned ? kDynRuntime[rc] : kDynAligned[rc]);
+    rec.form = !use_tma ? kFormDynBytewise : (any_misaligned ? kFormDynRuntime : kFormDynAligned);
+    rec.row_chunk = rc;
   }
   const void* kfn = reinterpret_cast<const void*>(fn);
   bool jitted = false;
@@ -809,10 +834,15 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
         if (jit3d_tried) jk = rows3d ? jit3d : nullptr;  // the 3-D variant is the one being compiled for this geometry
         else jk = jit_kernel(d.k, d.r, d.coef, static_cast<int>(d.S & 15), kStaticEb, false, true, mode, in_bytes);
       }
-      if (jk) { kfn = jk; jitted = true; }
+      if (jk) {
+        kfn = jk;
+        jitted = true;
+        rec.form = kFormJit;
+        rec.row_chunk = -1;
+      }
     }
   }
-  const size_t smem = fused_smem_bytes(d.k, d.r, eb, p.raw_pitch, se == nullptr && !jitted, direct);
+  const size_t smem = fused_smem_bytes(d.k, d.r, eb, p.raw_pitch, se == nullptr && !jitted, direct, raw_rows);
   if (smem > 227 * 1024) return MEC_ERR_UNSUPPORTED;
   // the attribute and the occupancy query cost ~10 us of driver time per launch — a third of a small object's latency: remembered
   // per (kernel, CTA shape, shared memory)
@@ -863,7 +893,38 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
   MEC_CUDA_OK(cudaGetLastError());
   launches_++;
   if (jitted) jit_launches_++;
+  rec.eb = eb;
+  rec.grid = grid;
+  rec.tma_mode = p.tma_mode;
+  rec.rows3d = rows3d;
+  rec.direct = direct;
+  rec.tiles3d = p.tiles_3d;
+  record_launch(rec);
   return MEC_OK;
+}
+
+// KernelForm order
+static const char* const kFormNames[kNumForms] = {"small", "fast3d", "fast3d_auto", "fast3d_semi", "fast", "fast_auto", "aligned",
+                                                  "aligned_auto", "runtime", "bytewise", "dyn_aligned", "dyn_runtime", "dyn_bytewise", "jit"};
+
+bool Engine::dispatch_stat(const char* name, int64_t* value) const {
+  if (!strncmp(name, "form_", 5)) {
+    for (int f = 0; f < kNumForms; f++)
+      if (!strcmp(name + 5, kFormNames[f])) {
+        *value = form_launches_[f];
+        return true;
+      }
+    return false;
+  }
+  const struct { const char* name; int64_t v; } fields[] = {
+      {"last_eb", last_.eb},         {"last_grid", last_.grid},     {"last_tma_mode", last_.tma_mode}, {"last_rows3d", last_.rows3d},
+      {"last_direct", last_.direct}, {"last_tiles3d", last_.tiles3d}, {"last_row_chunk", last_.row_chunk}, {"num_sms", num_sms_}};
+  for (const auto& f : fields)
+    if (!strcmp(name, f.name)) {
+      *value = f.v;
+      return true;
+    }
+  return false;
 }
 
 }  // namespace mec

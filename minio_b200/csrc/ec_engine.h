@@ -67,6 +67,24 @@ struct EngineOptions {
                            // useful when SMs are shared or uneven
 };
 
+// Which kernel form a launch_fused call ran (Engine::dispatch_stat, mec_get_stat keys "form_<name>"): the StaticEntry field, the
+// runtime-matrix table, the NVRTC specialisation or the latency kernel
+enum KernelForm : int {
+  kFormSmall = 0, kFormFast3d, kFormFast3dAuto, kFormFast3dSemi, kFormFast, kFormFastAuto, kFormAligned, kFormAlignedAuto,
+  kFormRuntime, kFormBytewise, kFormDynAligned, kFormDynRuntime, kFormDynBytewise, kFormJit, kNumForms
+};
+
+// What the last launch_fused call that launched a kernel chose (mec_get_stat keys "last_<name>")
+struct LaunchRecord {
+  int form = -1;
+  int eb = 0;            // erasure blocks per CTA (1 for the latency kernel)
+  int64_t grid = 0;      // CTAs launched
+  int tma_mode = -1;     // LoaderMode; -1 for the latency kernel
+  int rows3d = 0, direct = 0;
+  int tiles3d = 0;       // FusedParams::tiles_3d (0 without the 3-D fetch)
+  int row_chunk = -1;    // index {0, 1, 2} = rows {1, 2, 4} of the runtime-matrix kernel picked; -1 for a compile-time matrix
+};
+
 class Engine {
  public:
   explicit Engine(int device);
@@ -86,6 +104,9 @@ class Engine {
   double jit_seconds() const;
   int64_t jit_disk_hits() const;  // specialised kernels loaded from the on-disk cache instead of compiled (process-wide)
   int num_sms() const { return num_sms_; }
+  // dispatch record: launches per kernel form ("form_<name>"), the last launch's shape ("last_<name>") and "num_sms";
+  // false for any other name
+  bool dispatch_stat(const char* name, int64_t* value) const;
   // queue the specialisation of a reconstruct matrix (r x k rows) on the background compiler, as if the pattern were already warm
   void jit_prewarm(int k, int r, const uint8_t* coef, int eb_t, bool hash_out) {
     jit_kernel(k, r, coef, 0, eb_t, false, hash_out, -1, int64_t{1} << 40);
@@ -98,6 +119,9 @@ class Engine {
   int64_t launches_ = 0;
   int64_t jit_launches_ = 0;
   int64_t small_launches_ = 0;
+  int64_t form_launches_[kNumForms] = {};
+  LaunchRecord last_;
+  void record_launch(const LaunchRecord& rec) { form_launches_[rec.form]++; last_ = rec; }
   struct LaunchMemo { const void* fn; int threads; size_t smem; int per_sm; };
   std::vector<LaunchMemo> launch_memo_;
   int raise_smem_limit(const void* kfn, size_t smem);

@@ -161,13 +161,15 @@ __host__ __device__ constexpr uint32_t raw_group_bytes(int eb, int raw_pitch) { 
 
 // `direct`: every input row is 16-byte aligned, TMA writes straight into the 288-byte-pitch rows the hash threads read —
 // two such buffers (tile i is hashed while tile i+1 lands), no re-aligned copy.  Otherwise: one raw tile + one aligned tile.
-__host__ __device__ constexpr uint32_t fused_smem_bytes(int k, int r, int eb, int raw_pitch, bool dynamic_gf, bool direct = false) {
+// raw_rows: rows of the raw tile when the 3-D fetch needs more than k of them (raw_rows_3d); 0 = k
+__host__ __device__ constexpr uint32_t fused_smem_bytes(int k, int r, int eb, int raw_pitch, bool dynamic_gf, bool direct = false,
+                                                        int raw_rows = 0) {
   uint32_t b = 0;  // the mbarriers live in row padding; the dynamic segment is declared 128-byte aligned
   if (direct) {
     b += static_cast<uint32_t>(2 * k + (r > 0 ? r : 0)) * raw_group_bytes(eb, kRowPitch);
     if (r <= 0) b += 128;  // no output rows to hide the barriers in
   } else {
-    b += static_cast<uint32_t>(k) * raw_group_bytes(eb, raw_pitch);
+    b += static_cast<uint32_t>(raw_rows > k ? raw_rows : k) * raw_group_bytes(eb, raw_pitch);
     b += static_cast<uint32_t>(k + (r > 0 ? r : 0)) * eb * kRowPitch;
   }
   if (dynamic_gf) b += static_cast<uint32_t>(k) * ((r + kRChunk - 1) / kRChunk) * kRChunk * 8 * 4;
@@ -196,6 +198,12 @@ __host__ __device__ constexpr int rows_per_request_3d(int k, int sm16, int eb) {
   return 1;
 }
 __host__ __device__ constexpr int raw_row_3d(int k, int sm16, int eb) { return raw_row_3d(k, sm16, eb, rows_per_request_3d(k, sm16, eb)); }
+// Rows of the raw tile with the 3-D fetch.  The last request of a tile lands RG whole rows even when fewer than RG shard rows are
+// left (those past k are out of bounds of the tensor map and arrive zero-filled), so the raw tile holds k rounded up to a multiple
+// of RG rows — RS(10,4) with S mod 16 = 5 takes two requests of seven rows.  Every compiled geometry has k % RG == 0.
+__host__ __device__ constexpr int raw_rows_3d(int k, int rg) { return (k + rg - 1) / rg * rg; }
+static_assert(raw_rows_3d(12, rows_per_request_3d(12, 6, 4)) == 12 && raw_rows_3d(6, rows_per_request_3d(6, 11, 4)) == 6 &&
+                  raw_rows_3d(10, rows_per_request_3d(10, 5, 4)) == 14, "raw tile rows of the 3-D fetch");
 
 // RS(12,4) at 1 MiB blocks (S mod 16 = 6): three requests of four rows at a 288-byte pitch, 32 256 bytes per CTA — seven
 // CTAs (7 x (32 256 + 1 024 reserved) <= 233 472) and 28 warps x 32 lanes x 72 registers = the whole register file.
@@ -257,7 +265,8 @@ __host__ __device__ constexpr int fused_min_blocks() {
   constexpr int t = fused_max_threads<GF, EB_T>();
   const int by_regs = 65536 / (72 * t);
   const int raw = ROWS3D ? raw_row_3d(GF::K > 0 ? GF::K : 1, ALIGN > 0 ? ALIGN : 0, EB_T > 0 ? EB_T : 1) : kRawRow;
-  const int by_smem = 233472 / (static_cast<int>(fused_smem_bytes(GF::K, GF::R, EB_T, raw, false, DIRECT)) + 1024);
+  const int rows = ROWS3D ? raw_rows_3d(GF::K, rows_per_request_3d(GF::K > 0 ? GF::K : 1, ALIGN > 0 ? ALIGN : 0, EB_T > 0 ? EB_T : 1)) : 0;
+  const int by_smem = 233472 / (static_cast<int>(fused_smem_bytes(GF::K, GF::R, EB_T, raw, false, DIRECT, rows)) + 1024);
   const int b = by_regs < by_smem ? by_regs : by_smem;
   return b > 0 ? b : 1;
 }
@@ -283,7 +292,7 @@ __global__ void __launch_bounds__((fused_max_threads<GF, EB_T>()), (fused_min_bl
   const uint32_t rawp = DIRECT ? static_cast<uint32_t>(kRowPitch)
                                : (ROWS3D ? static_cast<uint32_t>(kRaw3) : (EB_T > 0 ? static_cast<uint32_t>(kRawRow) : static_cast<uint32_t>(p.raw_pitch)));
   const uint32_t group_bytes = raw_group_bytes(eb, static_cast<int>(rawp));
-  const uint32_t buf_bytes = static_cast<uint32_t>(k) * group_bytes;
+  const uint32_t buf_bytes = static_cast<uint32_t>(ROWS3D ? raw_rows_3d(kK3, kRG) : k) * group_bytes;
   uint8_t* s_raw = smem;                                                     // [k][group]  (DIRECT: two of them)
   uint8_t* s_clean = DIRECT ? s_raw : s_raw + buf_bytes;                     // [eb][k][kRowPitch]  (not DIRECT)
   uint8_t* s_par = DIRECT ? s_raw + 2 * buf_bytes : s_clean + static_cast<uint32_t>(k) * eb * kRowPitch;
@@ -376,7 +385,8 @@ __global__ void __launch_bounds__((fused_max_threads<GF, EB_T>()), (fused_min_bl
         const uint32_t dst0 = smem_u32(s_raw) + sel * buf_bytes;
         if constexpr (ROWS3D) {
           constexpr int kGroups = (kK3 + kRG - 1) / kRG;
-          if (i < p.tiles_3d) {  // kGroups requests for the whole tile (rows past k are out of bounds: zero fill, still counted)
+          if (i < p.tiles_3d) {  // kGroups requests for the whole tile (rows past k are out of bounds: zero-filled into the raw tile's
+                                 // spare rows, raw_rows_3d, and still counted)
             if (part == 0) {
               mbar_expect_tx(bar, static_cast<uint32_t>(kGroups * kRG) * eb * kRaw3);
 #pragma unroll
