@@ -180,8 +180,11 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
  * at most max_wait_us for company when the GPU is idle — into one staged buffer (one batched copy call) and ONE fused launch over
  * all full blocks, then writes every caller's frames straight into that caller's buffers.  Up to six merged batches are in flight;
  * device staging for all six is allocated here (about 2.4 x max_batch_blocks x block_size each).
- * mec_batcher_stat: "batches", "requests", "blocks", "launches"; with MEC_BATCHER_TRACE=1 in the environment also the worker's and the
- * streams' accumulated phase times "us_submit", "us_sync", "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter". */
+ * mec_batcher_stat: "batches", "requests", "blocks", "kernel_batches" (batches moved by the gather / scatter kernels), "redone"
+ * (merged GETs that met a frame failing its digest check and were redone on their own), "launches";
+ * with MEC_BATCHER_TRACE=1 in the environment also the worker's and the streams' accumulated phase times "us_submit", "us_sync",
+ * "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter".  Any other name is answered by mec_get_stat on the batcher's own
+ * codec, so "form_*", "last_*", "small_launches", "num_sms" and the rest describe the merged launches. */
 typedef struct mec_batcher mec_batcher;
 int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out);
 void mec_batcher_free(mec_batcher* b);

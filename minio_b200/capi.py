@@ -436,6 +436,23 @@ class Batcher:
             raise MecError(rc, "mec_batcher_encode")
         return files
 
+    def encode_sg(self, src, online=None, write_quorum=0, pinned=False):
+        """mec_batcher_encode_sg: -> (files, data_digests) shaped like Codec.encode_sg.  pinned=True: the parity images and the
+        [block][k][32] digest array are page-locked (and `src` must be), so the scatter kernel writes both; the caller owns them."""
+        src = _u8(src)
+        fsz = self._sizes.bitrot_file_size(src.size)
+        nb = -(-src.size // self.block_size)
+        online = [True] * self.n if online is None else online
+        mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
+        marker = np.zeros(1, dtype=np.uint8)  # data drives: only NULL / non-NULL is looked at
+        files = [(mk(fsz) if i >= self.k else marker) if online[i] else None for i in range(self.n)]
+        dd = mk(max(nb, 1) * self.k * 32).reshape(max(nb, 1), self.k, 32)
+        rc = lib().mec_batcher_encode_sg(self.h, src.ctypes.data if src.size else None, src.size, _ptrs(files), dd.ctypes.data,
+                                         write_quorum)
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_encode_sg")
+        return [f if i >= self.k else None for i, f in enumerate(files)], dd[:nb]
+
     def decode(self, files, offset, length, total, dst=None):
         """mec_batcher_decode: files = part-file arrays (None = offline); pass page-locked arrays (and a page-locked dst) to ride in
         merged launches.  -> (bytes, heal_hint)"""

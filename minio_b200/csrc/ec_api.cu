@@ -555,16 +555,28 @@ extern "C" int mec_encode_blocks(mec_codec* c, const uint8_t* src, int64_t len, 
   return MEC_OK;
 }
 
-// a train of independent copies as one driver call (CUDA 12.8 cudaMemcpyBatchAsync); MEC_NO_BATCH_COPY=1: one call per copy
+// a train of independent copies as few driver calls (CUDA 12.8 cudaMemcpyBatchAsync, at most kMaxBatchCopies copies each);
+// MEC_NO_BATCH_COPY=1: one call per copy.  A merged GET stages k frames per block; merged GETs of a few hundred blocks whose
+// frames all went through ONE call of thousands of copies ended in an unspecified launch failure on an H100, while the same
+// batches staged by the gather kernel or by one call per copy did not (tests/test_gpu_batcher.py, get-dma-depth0).
+constexpr size_t kMaxBatchCopies = 256;
 static int copy_batch(std::vector<void*>& dsts, std::vector<void*>& srcs, std::vector<size_t>& sizes, cudaStream_t st) {
   if (dsts.empty()) return MEC_OK;
   static const bool no_batch = getenv("MEC_NO_BATCH_COPY") != nullptr;
   if (!no_batch && dsts.size() > 1) {
     cudaMemcpyAttributes at = {};
     at.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
-    size_t idx0 = 0, fail = 0;
-    const cudaError_t e = cudaMemcpyBatchAsync(dsts.data(), srcs.data(), sizes.data(), dsts.size(), &at, &idx0, 1, &fail, st);
+    size_t idx0 = 0, fail = 0, done = 0;
+    cudaError_t e = cudaSuccess;
+    for (; done < dsts.size() && e == cudaSuccess; done += kMaxBatchCopies) {
+      const size_t cnt = std::min(kMaxBatchCopies, dsts.size() - done);
+      e = cudaMemcpyBatchAsync(dsts.data() + done, srcs.data() + done, sizes.data() + done, cnt, &at, &idx0, 1, &fail, st);
+    }
     if (e == cudaSuccess) return MEC_OK;
+    if (done > kMaxBatchCopies) {  // part of the train is already queued
+      set_last_error(std::string("cudaMemcpyBatchAsync: ") + cudaGetErrorString(e));
+      return MEC_ERR_CUDA;
+    }
     cudaGetLastError();  // older driver: fall through to separate calls
   }
   for (size_t i = 0; i < dsts.size(); i++) MEC_CUDA_OK(cudaMemcpyAsync(dsts[i], srcs[i], sizes[i], cudaMemcpyDefault, st));
@@ -2001,6 +2013,7 @@ struct mec_batcher {
   bool stop = false;
   std::thread worker;
   std::atomic<int64_t> st_batches{0}, st_requests{0}, st_blocks{0}, st_kernel_batches{0};
+  std::atomic<int64_t> st_redone{0};  // merged GETs that met a frame failing its digest and were redone on their own
   // hybrid staging: part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
   cudaStream_t aux = nullptr;
   cudaEvent_t ev_table[kSlots] = {}, ev_gather[kSlots] = {};
@@ -2047,6 +2060,7 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
           for (int t = 0; t < k; t++) bad |= fl[slot * k + t] != 0;
         }
         if (bad) {
+          b->st_redone++;
           mec_codec* sc = batcher_serial(b);
           res = sc ? mec_decode_prefer(sc, r->gfiles, nullptr, r->offset, r->length, r->total, r->dst, r->heal_hint) : MEC_ERR_UNEXPECTED;
         } else if (r->heal_hint) {
@@ -2722,6 +2736,7 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "requests")) return b->st_requests.load();
   if (!strcmp(name, "blocks")) return b->st_blocks.load();
   if (!strcmp(name, "kernel_batches")) return b->st_kernel_batches.load();
+  if (!strcmp(name, "redone")) return b->st_redone.load();
   if (!strcmp(name, "launches")) return b->codec->eng ? b->codec->eng->launches() : 0;
   if (!strcmp(name, "us_submit")) return b->us_submit.load();
   if (!strcmp(name, "us_sync")) return b->us_sync.load();
@@ -2730,5 +2745,5 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "us_stage")) return b->us_stage.load();
   if (!strcmp(name, "us_kernel")) return b->us_kernel.load();
   if (!strcmp(name, "us_scatter")) return b->us_scatter.load();
-  return -1;
+  return mec_get_stat(b->codec, name);  // the batcher's codec: which kernel forms its merged launches ran ("form_*", "last_*", ...)
 }
