@@ -206,7 +206,8 @@ int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
  *   mec_checksums        : host buffer, staged through the codec's slots
  *   mec_checksum_combine : Checksum.AddPart (crc.go:32-73): checksum of A || B from those of A and B and |B|, on the host
  * mec_set_option(c, "checksums", mask) makes mec_encode / mec_encode_sg / mec_encode_blocks compute them on the bytes they stage
- * anyway (the object crosses PCIe once); mec_last_checksums returns the values of the codec's last such call and its length. */
+ * anyway (the object crosses PCIe once); mec_last_checksums returns the values of the codec's last such call and its length
+ * (an empty object included: (0, 0, 0) and 0). */
 #define MEC_CRC32 1
 #define MEC_CRC32C 2
 #define MEC_CRC64NVME 4
@@ -228,7 +229,9 @@ int64_t mec_encode_whole(mec_codec* c, const uint8_t* src, int64_t len, uint8_t*
 int mec_whole_hash(mec_codec* c, int algo, const uint8_t* msgs, int64_t msg_len, int64_t count, uint8_t* digests);
 int mec_bitrot_verify_whole(mec_codec* c, int algo, const uint8_t* file, int64_t file_len, const uint8_t* want);
 /* Device-resident mec_whole_hash: message i at d_msgs + i*pitch (pitch a multiple of 16, >= msg_len, with 128 readable
- * bytes after the last message), digest i at d_digests + i*64.  Asynchronous on `cuda_stream`. */
+ * bytes after the last message), digest i at d_digests + i*64 (bytes digest_size..63 of each slot are left as they were).
+ * d_msgs must be 16-byte aligned (NULL only when msg_len or count is 0) and d_digests non-NULL and 8-byte aligned; other
+ * pointers return MEC_ERR_INVALID_ARGUMENT before any device work.  Asynchronous on `cuda_stream`. */
 int mec_whole_hash_device(mec_codec* c, int algo, const uint8_t* d_msgs, int64_t pitch, int64_t msg_len, int64_t count,
                           uint8_t* d_digests, void* cuda_stream);
 /* Erasure.Decode / Erasure.Heal over whole-file bitrot readers (wholeBitrotReader.ReadAt, cmd/bitrot-whole.go:66-81): files[i] is

@@ -365,6 +365,15 @@ extern "C" int64_t mec_last_checksums(const mec_codec* c, uint64_t* out3) {
   return c->last_crc_len;
 }
 
+// An empty object never reaches encode_pipeline, which resets the carried checksums for every other object: its checksums are
+// those of the empty stream, (0, 0, 0) over 0 bytes, not what the previous object left behind.
+static void reset_last_checksums(mec_codec* c) {
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (!c->checksums) return;
+  for (auto& v : c->last_crc) v = 0;
+  c->last_crc_len = 0;
+}
+
 // ------------------------------------------------------------------------------------------------
 // encode
 static int encode_device_locked(mec_codec* c, const uint8_t* d_src, int64_t len, uint8_t* d_parity, int64_t pitch,
@@ -527,7 +536,10 @@ extern "C" int mec_encode_blocks(mec_codec* c, const uint8_t* src, int64_t len, 
   if (!c || len < 0) return MEC_ERR_INVALID_ARGUMENT;
   int rc = require_streaming(c);
   if (rc) return rc;
-  if (len == 0) return MEC_OK;  // cmd/erasure-coding.go:78-80
+  if (len == 0) {  // cmd/erasure-coding.go:78-80
+    reset_last_checksums(c);
+    return MEC_OK;
+  }
   if (c->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> lk(c->mu);
   MEC_CUDA_OK(cudaSetDevice(c->device));
@@ -686,7 +698,10 @@ static int64_t encode_frames(mec_codec* c, const uint8_t* src, int64_t len, uint
   int online = 0;
   for (int i = 0; i < c->n; i++) online += files[i] != nullptr;
   if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
-  if (len == 0) return 0;
+  if (len == 0) {
+    reset_last_checksums(c);
+    return 0;
+  }
   int rc = require_streaming(c);
   if (rc) return rc;
   if (c->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
@@ -1422,6 +1437,10 @@ extern "C" int mec_whole_hash(mec_codec* c, int algo, const uint8_t* msgs, int64
 extern "C" int mec_whole_hash_device(mec_codec* c, int algo, const uint8_t* d_msgs, int64_t pitch, int64_t msg_len, int64_t count,
                                      uint8_t* d_digests, void* stream) {
   if (!c || msg_len < 0 || count < 0 || mec_digest_size(algo) < 0 || (pitch & 15) || pitch < msg_len) return MEC_ERR_INVALID_ARGUMENT;
+  // the kernel reads every message with 16-byte vector loads and HighwayHash stores its digests as 64-bit words
+  if ((msg_len > 0 && count > 0 && !d_msgs) || (reinterpret_cast<uintptr_t>(d_msgs) & 15) || !d_digests ||
+      (reinterpret_cast<uintptr_t>(d_digests) & 7))
+    return MEC_ERR_INVALID_ARGUMENT;
   if (count == 0) return MEC_OK;
   if (count >= (1ll << 30)) return MEC_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> lk(c->mu);

@@ -191,9 +191,12 @@ def sha256_sweep(k, m, sizes, total_bytes, quiet=False):
             c.whole_hash_device(mb.SHA256, src.data_ptr(), S, S, nblocks * k, dig.data_ptr(), st)               # data shard (b, t) = stream b*k+t
             c.whole_hash_device(mb.SHA256, par.data_ptr(), pitch, S, nblocks * m, dig.data_ptr() + nblocks * k * 64, st)
         ms = timeit(fn, steps=5, warm=2)
-        h_src = src[:bs].cpu().numpy().tobytes(); h_par = par[:m, :S].cpu().numpy(); h_dig = dig.cpu().numpy()
-        ok = all(hashlib.sha256(h_src[t * S:(t + 1) * S]).digest() == h_dig[t, :32].tobytes() for t in range(k))
-        ok &= all(hashlib.sha256(h_par[j].tobytes()).digest() == h_dig[nblocks * k + j, :32].tobytes() for j in range(m))
+        h_dig = dig.cpu().numpy()
+        ok = True
+        for b in sorted({0, nblocks // 2, nblocks - 1}):   # the first, a middle and the last block: k + m digests each
+            h_src = src[b * bs:(b + 1) * bs].cpu().numpy().tobytes(); h_par = par[b * m:(b + 1) * m, :S].cpu().numpy()
+            ok &= all(hashlib.sha256(h_src[t * S:(t + 1) * S]).digest() == h_dig[b * k + t, :32].tobytes() for t in range(k))
+            ok &= all(hashlib.sha256(h_par[j].tobytes()).digest() == h_dig[nblocks * k + b * m + j, :32].tobytes() for j in range(m))
         algo = bs + m * S + (k + m) * 32   # what a single fused pass would move (the implementation makes two passes)
         res = {"config": "5: RS(%d,%d) + SHA256 whole-file bitrot, one-block objects" % (k, m), "k": k, "m": m, "block_size": bs,
                "blocks": nblocks, "ms": ms, "GiB_per_s_object": nblocks * bs / GiB / (ms / 1e3), "algorithmic_bytes_per_block": algo,
