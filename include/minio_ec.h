@@ -181,7 +181,7 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
  * all full blocks, then writes every caller's frames straight into that caller's buffers.  Up to six merged batches are in flight;
  * device staging for all six is allocated here (about 2.4 x max_batch_blocks x block_size each).
  * mec_batcher_stat: "batches", "requests", "blocks", "kernel_batches" (batches moved by the gather / scatter kernels), "redone"
- * (merged GETs that met a frame failing its digest check and were redone on their own), "launches";
+ * (merged GETs and heals that met a frame failing its digest check and were redone on their own), "launches";
  * with MEC_BATCHER_TRACE=1 in the environment also the worker's and the streams' accumulated phase times "us_submit", "us_sync",
  * "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter".  Any other name is answered by mec_get_stat on the batcher's own
  * codec, so "form_*", "last_*", "small_launches", "num_sms" and the rest describe the merged launches. */
@@ -196,6 +196,14 @@ int64_t mec_batcher_encode_sg(mec_batcher* b, const uint8_t* src, int64_t len, u
  * that meets a corrupt frame is redone on its own with parallelReader's exact fail-over; pageable buffers take the same private path. */
 int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* files, int64_t offset, int64_t length, int64_t total_length,
                            uint8_t* dst, int* heal_hint);
+/* Erasure.Heal (cmd/erasure-decode.go:317) through the coalescer (arguments and results of mec_heal_prefer): heals queued together
+ * that read the same k drives (the ones parallelReader picks for `files` and `prefer`) and rebuild the same stale drives (out_files[i]
+ * != NULL) are merged into one fused launch, and one scatter kernel writes every healed frame into every caller's out files.  A
+ * request whose chosen readers fail a digest check is redone on its own through mec_heal_prefer (MEC_ERR_FILE_CORRUPT, corrupt[]
+ * filled, counted in "redone"); pageable buffers, a drive that is both a reader and stale, and sets of more than 32 drives take that
+ * private path directly. */
+int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total_length,
+                     uint8_t* const* out_files, uint8_t* corrupt);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------

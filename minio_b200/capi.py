@@ -68,6 +68,7 @@ def lib():
     L.mec_batcher_encode_sg.argtypes = [vp, vp, i64, vp, vp, i32]
     L.mec_batcher_decode.restype = i64
     L.mec_batcher_decode.argtypes = [vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
+    L.mec_batcher_heal.argtypes = [vp, vp, vp, i64, vp, vp]
     L.mec_batcher_stat.restype = i64
     L.mec_batcher_stat.argtypes = [vp, C.c_char_p]
     L.mec_checksums.argtypes = [vp, vp, i64, i32, vp]
@@ -464,6 +465,20 @@ class Batcher:
         if rc < 0:
             raise MecError(rc, "mec_batcher_decode")
         return dst[:length], hint.value
+
+    def heal(self, files, stale, total, prefer=None, pinned=False):
+        """mec_batcher_heal: -> (outs, rc, corrupt[n]) like Codec.heal(report=True).  Page-locked part files and pinned=True (the out
+        files are allocated page-locked; the caller owns and should free them) let the heal ride in merged launches."""
+        files = [None if f is None else _u8(f) for f in files]
+        fsz = self._sizes.bitrot_file_size(total)
+        mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
+        outs = [mk(fsz) if stale[i] else None for i in range(self.n)]
+        corrupt = np.zeros(self.n, dtype=np.uint8)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        rc = lib().mec_batcher_heal(self.h, _ptrs(files), None if pf is None else pf.ctypes.data, total, _ptrs(outs), corrupt.ctypes.data)
+        if rc and rc != -7:
+            raise MecError(rc, "mec_batcher_heal")
+        return outs, rc, corrupt
 
     def stat(self, name):
         return lib().mec_batcher_stat(self.h, name.encode())

@@ -148,7 +148,7 @@ struct BatchGetParams {
   const BatchGetDesc* reqs;
   int nreq, k, r;
   int32_t chosen[32];                    // reader set (ascending shard indices), position t -> shard
-  int32_t targets[16];                   // rebuilt data shards, output row q -> shard
+  int32_t targets[16];                   // rebuilt shards (GET: data only; heal: the stale drives), output row q -> shard
   int64_t bs, S, P;                      // block size, full shard size, device frame pitch
   uint8_t* arena;                        // survivors: reader position t at arena + t*arena_stride, slot s at + s*P
   int64_t arena_stride;
@@ -194,6 +194,24 @@ __global__ void __launch_bounds__(128) batch_get_scatter_kernel(const BatchGetPa
     if (e <= a) continue;
     const uint8_t* src = t >= 0 ? p.arena + t * p.arena_stride + slot * p.P + 32 : p.rebuilt + (slot * p.r + q) * p.pitch;
     cta_copy(r.dst + (a - r.offset), src + (a - slo), e - a, false);
+  }
+}
+
+// grid (block stride, r rebuilt shards, nreq): healed frames of every stale drive of every request — multiWriter{writeQuorum: 1} +
+// streamingBitrotWriter.Write (cmd/erasure-decode.go:317-366, cmd/bitrot-streaming.go:57-69): [digest of the rebuilt shard][shard]
+// at frame b of outs[req * r + q], the part's short last frame 32 + last_len bytes.  Digests [slot][k + r][32] (outputs behind
+// the k inputs), rebuilt rows (slot * r + q) * pitch.  Nothing outside a frame is written.
+__global__ void __launch_bounds__(128) batch_heal_scatter_kernel(const BatchGetParams p, const uint8_t* digests, uint8_t* const* outs) {
+  const BatchGetDesc& r = p.reqs[blockIdx.z];
+  const int q = blockIdx.y;
+  uint8_t* f = outs[static_cast<int64_t>(blockIdx.z) * p.r + q];
+  const int64_t fstride = 32 + p.S;
+  for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
+    const bool is_tail = r.tail_slot >= 0 && b == r.nblocks - 1;
+    const int64_t slot = get_slot(r, b);
+    uint8_t* fr = f + (r.start_block + b) * fstride;
+    cta_copy(fr, digests + (slot * (p.k + p.r) + p.k + q) * 32, 32, false);  // hash first, then the shard
+    cta_copy(fr + 32, p.rebuilt + (slot * p.r + q) * p.pitch, is_tail ? r.last_len : p.S, false);
   }
 }
 

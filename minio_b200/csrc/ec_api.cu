@@ -1999,14 +1999,19 @@ extern "C" int mec_selftest(int device) {
 #include <deque>
 
 struct BatchReq {
-  int kind = 0;                      // 0 = PutObject (encode), 1 = GetObject (decode)
-  // GET
+  int kind = 0;                      // 0 = PutObject (encode), 1 = GetObject (decode), 2 = Heal
+  // GET and heal (a heal reads the whole part: offset 0, length = total)
   const uint8_t* const* gfiles = nullptr;
   int64_t offset = 0, length = 0, total = 0;
   uint8_t* dst = nullptr;
   int* heal_hint = nullptr;
-  uint64_t alive_mask = 0;           // bit i = reader i is online: requests with equal masks share a reader set and a launch
+  uint64_t alive_mask = 0;           // bit i = reader i is online (heal: one of the k chosen readers): equal masks share a launch
   int64_t get_slot0 = 0, get_tail_slot = -1, get_nblocks = 0;  // placement of the request's blocks in the merged batch
+  // heal
+  const uint8_t* prefer = nullptr;
+  uint8_t* const* outs = nullptr;
+  uint8_t* corrupt = nullptr;
+  uint64_t stale_mask = 0;           // bit i = out_files[i] != NULL: heals share a launch only with the same stale drives
   // PUT
   const uint8_t* src = nullptr;
   int64_t len = 0;
@@ -2032,7 +2037,7 @@ struct mec_batcher {
   bool stop = false;
   std::thread worker;
   std::atomic<int64_t> st_batches{0}, st_requests{0}, st_blocks{0}, st_kernel_batches{0};
-  std::atomic<int64_t> st_redone{0};  // merged GETs that met a frame failing its digest and were redone on their own
+  std::atomic<int64_t> st_redone{0};  // merged GETs and heals that met a frame failing its digest and were redone on their own
   // hybrid staging: part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
   cudaStream_t aux = nullptr;
   cudaEvent_t ev_table[kSlots] = {}, ev_gather[kSlots] = {};
@@ -2048,7 +2053,7 @@ struct InflightBatch {
   std::vector<BatchReq*> reqs;
   bool busy = false;
   bool needs_retire = true;  // false: the scatter kernel already assembled the frames
-  bool is_get = false;
+  bool is_get = false;       // a GET or heal batch: per-frame digest verdicts decide which requests are done
   bool traced = false;
   int get_k = 0;
 };
@@ -2066,12 +2071,14 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
   mec_codec* c = b->codec;
   if (fb.is_get) {
     // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own through the serial
-    // handle, which applies parallelReader's block-sequential fail-over exactly; the others are done (their bytes are in place)
+    // handle, which applies parallelReader's block-sequential fail-over exactly (a heal rewrites every out file in full and reports
+    // the failing readers); the others are done (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
     Slot& s = *fb.reqs.front()->ch.s;
     const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
     const int k = fb.get_k;
     for (BatchReq* r : fb.reqs) {
-      int64_t res = rc == MEC_OK ? r->length : rc;
+      const bool heal = r->kind == 2;
+      int64_t res = rc != MEC_OK ? rc : heal ? MEC_OK : r->length;
       if (rc == MEC_OK) {
         bool bad = false;
         for (int64_t bb = 0; bb < r->get_nblocks && !bad; bb++) {
@@ -2081,7 +2088,9 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
         if (bad) {
           b->st_redone++;
           mec_codec* sc = batcher_serial(b);
-          res = sc ? mec_decode_prefer(sc, r->gfiles, nullptr, r->offset, r->length, r->total, r->dst, r->heal_hint) : MEC_ERR_UNEXPECTED;
+          if (!sc) res = MEC_ERR_UNEXPECTED;
+          else if (heal) res = mec_heal_prefer(sc, r->gfiles, r->prefer, r->total, r->outs, r->corrupt);
+          else res = mec_decode_prefer(sc, r->gfiles, nullptr, r->offset, r->length, r->total, r->dst, r->heal_hint);
         } else if (r->heal_hint) {
           *r->heal_hint = 0;
         }
@@ -2282,6 +2291,139 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   return MEC_OK;
 }
 
+// Merged GET and heal batches share their layout and their staging.  Layout: every request's full blocks first, the short last
+// blocks behind them; fills the request table and each request's placement in the batch.
+struct ReadLayout {
+  int64_t nfull_slots = 0, ntails = 0, max_nb = 0;
+  int64_t nslots() const { return nfull_slots + ntails; }
+};
+static ReadLayout batch_read_layout(mec_codec* c, Slot& s, std::vector<BatchReq*>& reqs, BatchGetDesc* tab) {
+  const int n = c->n;
+  const int64_t bs = c->block_size, S = c->S();
+  ReadLayout lay;
+  for (size_t q = 0; q < reqs.size(); q++) {
+    BatchReq* rq = reqs[q];
+    BatchGetDesc& d = tab[q];
+    memset(&d, 0, sizeof(d));
+    const int64_t sfs = mec_shard_file_size(c, rq->total), nblocks_total = ceil_frac(sfs, S);
+    const int64_t start_block = rq->offset / bs;
+    int64_t last_block = (rq->offset + rq->length) / bs;
+    if ((rq->offset + rq->length) % bs == 0) last_block--;
+    if (last_block >= nblocks_total) last_block = nblocks_total - 1;
+    const int64_t last_len = std::min(S, sfs - last_block * S);
+    d.offset = rq->offset; d.length = rq->length; d.total = rq->total; d.dst = rq->dst;
+    for (int i = 0; i < n; i++) d.files[i] = rq->gfiles[i];
+    d.start_block = start_block; d.nblocks = last_block - start_block + 1;
+    d.last_len = last_len;
+    const bool tail = last_len != S;
+    d.slot0 = lay.nfull_slots;
+    lay.nfull_slots += d.nblocks - (tail ? 1 : 0);
+    d.tail_slot = tail ? lay.ntails : -1;  // provisional: offset by the number of full slots below
+    if (tail) lay.ntails++;
+    lay.max_nb = std::max(lay.max_nb, d.nblocks);
+    rq->get_nblocks = d.nblocks;
+  }
+  static const int64_t dma_blocks = getenv("MEC_BATCHER_DMA_BLOCKS") ? atoll(getenv("MEC_BATCHER_DMA_BLOCKS")) : 1;
+  for (size_t q = 0; q < reqs.size(); q++) {
+    tab[q].dma = tab[q].nblocks >= dma_blocks ? 1 : 0;
+    if (tab[q].tail_slot >= 0) tab[q].tail_slot += lay.nfull_slots;
+    reqs[q]->get_slot0 = tab[q].slot0;
+    reqs[q]->get_tail_slot = tab[q].tail_slot;
+    reqs[q]->ch = EncChunk();
+    reqs[q]->ch.s = &s;
+  }
+  return lay;
+}
+
+// Survivor frames of every block of every request -> the slot's arena, the fused reconstruct of gp.targets over all of them, and the
+// per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table gp.reqs points at; gp holds the geometry, reader
+// set and targets, and gets the arena and rebuilt rows here.
+static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* tab, BatchGetParams& gp, const uint8_t* rows,
+                                  const ReadLayout& lay, bool hash_outputs) {
+  mec_codec* c = b->codec;
+  const int k = gp.k, r = gp.r;
+  const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
+  const int64_t stride = round_up(nslots * P + 512, 256);
+  int rc;
+  if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
+  if ((rc = s.out.ensure(static_cast<size_t>(nslots * std::max(r, 1) * pitch)))) return rc;
+  if ((rc = s.dig.ensure(static_cast<size_t>(nslots * (k + r) * 32)))) return rc;
+  if ((rc = s.flags.ensure(static_cast<size_t>(nslots * k)))) return rc;
+  if ((rc = s.hflags.ensure(static_cast<size_t>(nslots * k)))) return rc;
+  gp.arena = static_cast<uint8_t*>(s.aux.p); gp.arena_stride = stride;
+  gp.rebuilt = static_cast<const uint8_t*>(s.out.p);
+  const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
+  // long ranges are staged by the copy engines (k strided copies per request are cheap next to megabytes of frames); short ones by
+  // the gather kernel (no per-request driver call at all)
+  const int64_t fstride = 32 + S;
+  {
+    // one 1-D copy per (request, survivor, block) frame — the arena pads frames to a 16-byte pitch — all of them in ONE batched call
+    std::vector<void*> dsts, srcs;
+    std::vector<size_t> sizes;
+    for (int q = 0; q < gp.nreq; q++) {
+      const BatchGetDesc& d = tab[q];
+      if (!d.dma) continue;
+      const int64_t nf = d.nblocks - (d.tail_slot >= 0 ? 1 : 0);
+      for (int t = 0; t < k; t++) {
+        const uint8_t* f = d.files[gp.chosen[t]] + d.start_block * fstride;
+        uint8_t* a = gp.arena + t * stride;
+        for (int64_t j = 0; j < nf; j++) {
+          dsts.push_back(a + (d.slot0 + j) * P); srcs.push_back(const_cast<uint8_t*>(f) + j * fstride); sizes.push_back(static_cast<size_t>(fstride));
+        }
+        if (d.tail_slot >= 0) {
+          dsts.push_back(a + d.tail_slot * P); srcs.push_back(const_cast<uint8_t*>(f) + nf * fstride); sizes.push_back(static_cast<size_t>(32 + d.last_len));
+        }
+      }
+    }
+    if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
+  }
+  bool any_gather = false;
+  for (int q = 0; q < gp.nreq; q++) any_gather |= !tab[q].dma;
+  if (any_gather) {
+    batch_get_gather_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp);
+    MEC_CUDA_OK(cudaGetLastError());
+    c->eng->count_launch();
+  }
+  const int phase_slot = static_cast<int>(&s - c->slots);
+  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
+  MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
+  const int32_t* block_len = nullptr;
+  auto launch = [&](int64_t slot0, int64_t cnt, int64_t shard_len) -> int {
+    FusedDesc d;
+    d.block_len = block_len;
+    d.k = k; d.r = r; d.coef = rows; d.static_encode = false; d.contiguous = false; d.hash_outputs = hash_outputs;
+    d.key = kMagicKey; d.out_pitch = pitch; d.expect_block_stride = P; d.in_block_stride = P;
+    d.nblocks = cnt; d.S = static_cast<int32_t>(shard_len);
+    for (int t = 0; t < k; t++) {
+      const uint8_t* base = gp.arena + t * stride + slot0 * P;
+      d.map_base[t] = base; d.map_len[t] = stride - slot0 * P; d.expect_ptr[t] = base; d.in_ptr[t] = base + 32;
+    }
+    d.out = static_cast<uint8_t*>(s.out.p) + slot0 * r * pitch;
+    d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * (k + r) * 32;
+    d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0 * k;
+    return c->eng->launch_fused(d, c->opt, s.st);
+  };
+  if (lay.ntails > 0 && c->eng->small_ok(c->opt, nslots)) {
+    // ONE launch for every block of every caller, the short last ones included (per-block shard lengths in the latency kernel)
+    if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
+    if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
+    int32_t* lens = static_cast<int32_t*>(s.hblk.p);
+    for (int64_t q = 0; q < lay.nfull_slots; q++) lens[q] = static_cast<int32_t>(S);
+    for (int q = 0; q < gp.nreq; q++)
+      if (tab[q].tail_slot >= 0) lens[tab[q].tail_slot] = static_cast<int32_t>(tab[q].last_len);
+    MEC_CUDA_OK(cudaMemcpyAsync(s.blk.p, lens, static_cast<size_t>(nslots) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
+    block_len = static_cast<const int32_t*>(s.blk.p);
+    if ((rc = launch(0, nslots, S))) return rc;
+  } else {
+    if (lay.nfull_slots > 0 && (rc = launch(0, lay.nfull_slots, S))) return rc;  // ONE launch for every caller's full blocks
+    for (int q = 0; q < gp.nreq; q++)
+      if (tab[q].tail_slot >= 0 && (rc = launch(tab[q].tail_slot, 1, tab[q].last_len))) return rc;
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
+  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][2], s.st);
+  return MEC_OK;
+}
+
 // one merged launch for the GETs of a batch that share a reader set (alive mask): gather kernel -> fused reconstruct over all full
 // blocks (+ one launch per short last block) -> scatter kernel into every caller's destination
 static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs) {
@@ -2303,50 +2445,12 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   std::vector<uint8_t> rows(static_cast<size_t>(std::max(r, 1)) * k);
   int valid[kMaxShards];
   if (r > 0 && !rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
-  // layout: every request's full blocks first, the short last blocks behind them
   int rc;
   if ((rc = s.hreq.ensure(reqs.size() * sizeof(BatchGetDesc)))) return rc;
   if ((rc = s.dreq.ensure(reqs.size() * sizeof(BatchGetDesc)))) return rc;
   BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
-  int64_t nfull_slots = 0, ntails = 0, max_nb = 0;
-  for (size_t q = 0; q < reqs.size(); q++) {
-    BatchReq* rq = reqs[q];
-    BatchGetDesc& d = tab[q];
-    memset(&d, 0, sizeof(d));
-    const int64_t sfs = mec_shard_file_size(c, rq->total), nblocks_total = ceil_frac(sfs, S);
-    const int64_t start_block = rq->offset / bs;
-    int64_t last_block = (rq->offset + rq->length) / bs;
-    if ((rq->offset + rq->length) % bs == 0) last_block--;
-    if (last_block >= nblocks_total) last_block = nblocks_total - 1;
-    const int64_t last_len = std::min(S, sfs - last_block * S);
-    d.offset = rq->offset; d.length = rq->length; d.total = rq->total; d.dst = rq->dst;
-    for (int i = 0; i < n; i++) d.files[i] = rq->gfiles[i];
-    d.start_block = start_block; d.nblocks = last_block - start_block + 1;
-    d.last_len = last_len;
-    const bool tail = last_len != S;
-    d.slot0 = nfull_slots;
-    nfull_slots += d.nblocks - (tail ? 1 : 0);
-    d.tail_slot = tail ? ntails : -1;  // provisional: offset by the number of full slots below
-    if (tail) ntails++;
-    max_nb = std::max(max_nb, d.nblocks);
-    rq->get_nblocks = d.nblocks;
-  }
-  static const int64_t dma_blocks = getenv("MEC_BATCHER_DMA_BLOCKS") ? atoll(getenv("MEC_BATCHER_DMA_BLOCKS")) : 1;
-  for (size_t q = 0; q < reqs.size(); q++) {
-    tab[q].dma = tab[q].nblocks >= dma_blocks ? 1 : 0;
-    if (tab[q].tail_slot >= 0) tab[q].tail_slot += nfull_slots;
-    reqs[q]->get_slot0 = tab[q].slot0;
-    reqs[q]->get_tail_slot = tab[q].tail_slot;
-    reqs[q]->ch = EncChunk();
-    reqs[q]->ch.s = &s;
-  }
-  const int64_t nslots = nfull_slots + ntails;
-  const int64_t stride = round_up(nslots * P + 512, 256);
-  if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
-  if ((rc = s.out.ensure(static_cast<size_t>(nslots * std::max(r, 1) * pitch)))) return rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(nslots * (k + r) * 32)))) return rc;
-  if ((rc = s.flags.ensure(static_cast<size_t>(nslots * k)))) return rc;
-  if ((rc = s.hflags.ensure(static_cast<size_t>(nslots * k)))) return rc;
+  const ReadLayout lay = batch_read_layout(c, s, reqs, tab);
+  const int64_t nslots = lay.nslots();
   // writeDataBlocks: 0 = the scatter kernel assembles every object in device memory and ONE copy per request takes it to the caller
   // (fewest driver-side copy descriptors), 1 = the scatter kernel stores straight into the callers' buffers over PCIe, 2 = the copy
   // engine moves every (request, shard, block) piece itself
@@ -2367,77 +2471,10 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   gp.nreq = static_cast<int>(reqs.size()); gp.k = k; gp.r = r;
   for (int t = 0; t < k; t++) gp.chosen[t] = chosen[t];
   for (int q = 0; q < r; q++) gp.targets[q] = targets[q];
-  gp.bs = bs; gp.S = S; gp.P = P;
-  gp.arena = static_cast<uint8_t*>(s.aux.p); gp.arena_stride = stride;
-  gp.rebuilt = static_cast<const uint8_t*>(s.out.p); gp.pitch = pitch;
-  const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(max_nb, 1), 16));
-  // long ranges are staged by the copy engines (k strided copies per request are cheap next to megabytes of frames); short ones by
-  // the gather kernel (no per-request driver call at all)
-  const int64_t fstride = 32 + S;
-  {
-    // one 1-D copy per (request, survivor, block) frame — the arena pads frames to a 16-byte pitch — all of them in ONE batched call
-    std::vector<void*> dsts, srcs;
-    std::vector<size_t> sizes;
-    for (size_t q = 0; q < reqs.size(); q++) {
-      const BatchGetDesc& d = tab[q];
-      if (!d.dma) continue;
-      const int64_t nf = d.nblocks - (d.tail_slot >= 0 ? 1 : 0);
-      for (int t = 0; t < k; t++) {
-        const uint8_t* f = d.files[chosen[t]] + d.start_block * fstride;
-        uint8_t* a = gp.arena + t * stride;
-        for (int64_t j = 0; j < nf; j++) {
-          dsts.push_back(a + (d.slot0 + j) * P); srcs.push_back(const_cast<uint8_t*>(f) + j * fstride); sizes.push_back(static_cast<size_t>(fstride));
-        }
-        if (d.tail_slot >= 0) {
-          dsts.push_back(a + d.tail_slot * P); srcs.push_back(const_cast<uint8_t*>(f) + nf * fstride); sizes.push_back(static_cast<size_t>(32 + d.last_len));
-        }
-      }
-    }
-    if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
-  }
-  bool any_gather = false;
-  for (size_t q = 0; q < reqs.size(); q++) any_gather |= !tab[q].dma;
-  if (any_gather) {
-    batch_get_gather_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(gp);
-    MEC_CUDA_OK(cudaGetLastError());
-    c->eng->count_launch();
-  }
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
-  MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
-  const int32_t* block_len = nullptr;
-  auto launch = [&](int64_t slot0, int64_t cnt, int64_t shard_len) -> int {
-    FusedDesc d;
-    d.block_len = block_len;
-    d.k = k; d.r = r; d.coef = rows.data(); d.static_encode = false; d.contiguous = false; d.hash_outputs = false;
-    d.key = kMagicKey; d.out_pitch = pitch; d.expect_block_stride = P; d.in_block_stride = P;
-    d.nblocks = cnt; d.S = static_cast<int32_t>(shard_len);
-    for (int t = 0; t < k; t++) {
-      const uint8_t* base = gp.arena + t * stride + slot0 * P;
-      d.map_base[t] = base; d.map_len[t] = stride - slot0 * P; d.expect_ptr[t] = base; d.in_ptr[t] = base + 32;
-    }
-    d.out = static_cast<uint8_t*>(s.out.p) + slot0 * r * pitch;
-    d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * (k + r) * 32;
-    d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0 * k;
-    return c->eng->launch_fused(d, c->opt, s.st);
-  };
-  if (ntails > 0 && c->eng->small_ok(c->opt, nslots)) {
-    // ONE launch for every block of every caller, the short last ones included (per-block shard lengths in the latency kernel)
-    if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
-    if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
-    int32_t* lens = static_cast<int32_t*>(s.hblk.p);
-    for (int64_t q = 0; q < nfull_slots; q++) lens[q] = static_cast<int32_t>(S);
-    for (size_t q = 0; q < reqs.size(); q++)
-      if (tab[q].tail_slot >= 0) lens[tab[q].tail_slot] = static_cast<int32_t>(tab[q].last_len);
-    MEC_CUDA_OK(cudaMemcpyAsync(s.blk.p, lens, static_cast<size_t>(nslots) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
-    block_len = static_cast<const int32_t*>(s.blk.p);
-    if ((rc = launch(0, nslots, S))) return rc;
-  } else {
-    if (nfull_slots > 0 && (rc = launch(0, nfull_slots, S))) return rc;  // ONE launch for every caller's full blocks
-    for (size_t q = 0; q < reqs.size(); q++)
-      if (tab[q].tail_slot >= 0 && (rc = launch(tab[q].tail_slot, 1, tab[q].last_len))) return rc;
-  }
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][2], s.st);
+  gp.bs = bs; gp.S = S; gp.P = P; gp.pitch = pitch;
+  if ((rc = batch_read_reconstruct(b, s, tab, gp, rows.data(), lay, false))) return rc;  // GetObject reads no digest of rebuilt data
+  const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
+  const int64_t stride = gp.arena_stride;
   if (out_mode == 2) {
     // writeDataBlocks by the copy engine: one 1-D copy per (request, data shard, block) piece, all in one batched call
     std::vector<void*> dsts, srcs;
@@ -2487,6 +2524,66 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   return MEC_OK;
 }
 
+// one merged launch for the heals of a batch that share a reader set and a stale set: survivor frames staged as for GETs -> fused
+// reconstruct of every stale shard, data and parity, with its digest (ONE latency launch when the batch is small enough, otherwise
+// one over all full blocks plus one per short last block) -> the heal scatter kernel writes the healed frames into every caller's
+// part-file images
+static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs) {
+  mec_codec* c = b->codec;
+  const int k = c->k, n = c->n;
+  const int64_t S = c->S(), P = round_up(32 + S, 16), pitch = round_up(S, 16);
+  // the k chosen readers and the stale drives of the batch's key (disjoint: mec_batcher_heal sends the rest to the serial handle)
+  int chosen[kMaxShards], nch = 0, targets[kMaxShards], r = 0;
+  const uint64_t rmask = reqs.front()->alive_mask, smask = reqs.front()->stale_mask;
+  std::vector<uint8_t> present(n, 0);
+  for (int i = 0; i < n; i++) {
+    if (rmask & (1ull << i)) { chosen[nch++] = i; present[i] = 1; }
+    if (smask & (1ull << i)) targets[r++] = i;
+  }
+  if (nch != k) return MEC_ERR_READ_QUORUM;
+  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
+  std::vector<uint8_t> rows(static_cast<size_t>(std::max(r, 1)) * k);
+  int valid[kMaxShards];
+  if (r > 0 && !rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
+  // device table: the requests' BatchGetDesc rows, then out_files[targets[q]] of request z at [z * r + q]
+  const size_t tab_bytes = reqs.size() * sizeof(BatchGetDesc), all_bytes = tab_bytes + reqs.size() * std::max(r, 1) * sizeof(uint8_t*);
+  int rc;
+  if ((rc = s.hreq.ensure(all_bytes))) return rc;
+  if ((rc = s.dreq.ensure(all_bytes))) return rc;
+  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
+  const ReadLayout lay = batch_read_layout(c, s, reqs, tab);
+  const int64_t nslots = lay.nslots();
+  uint8_t** outs = reinterpret_cast<uint8_t**>(static_cast<uint8_t*>(s.hreq.p) + tab_bytes);
+  for (size_t z = 0; z < reqs.size(); z++)
+    for (int q = 0; q < r; q++) outs[z * r + q] = reqs[z]->outs[targets[q]];
+  const int phase_slot = static_cast<int>(&s - c->slots);
+  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
+  MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, s.hreq.p, all_bytes, cudaMemcpyHostToDevice, s.st));
+  BatchGetParams gp;
+  memset(&gp, 0, sizeof(gp));
+  gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.p);
+  gp.nreq = static_cast<int>(reqs.size()); gp.k = k; gp.r = r;
+  for (int t = 0; t < k; t++) gp.chosen[t] = chosen[t];
+  for (int q = 0; q < r; q++) gp.targets[q] = targets[q];
+  gp.bs = c->block_size; gp.S = S; gp.P = P; gp.pitch = pitch;
+  if ((rc = batch_read_reconstruct(b, s, tab, gp, rows.data(), lay, true))) return rc;
+  if (r > 0) {
+    const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
+    batch_heal_scatter_kernel<<<dim3(gx, static_cast<unsigned>(r), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(
+        gp, static_cast<const uint8_t*>(s.dig.p), reinterpret_cast<uint8_t* const*>(static_cast<uint8_t*>(s.dreq.p) + tab_bytes));
+    MEC_CUDA_OK(cudaGetLastError());
+    c->eng->count_launch();
+  }
+  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][3], s.st);
+  c->st_blocks_read += nslots;
+  c->st_shards_rebuilt += nslots * r;
+  b->st_batches++;
+  b->st_kernel_batches++;
+  b->st_requests += static_cast<int64_t>(reqs.size());
+  b->st_blocks += nslots;
+  return MEC_OK;
+}
+
 static void batcher_main(mec_batcher* b) {
   mec_codec* c = b->codec;
   cudaSetDevice(c->device);
@@ -2505,7 +2602,9 @@ static void batcher_main(mec_batcher* b) {
       if (!b->queue.empty() && nbusy < kSlots) {
         // gather: whatever is queued now; when nothing is in flight, give concurrent callers max_wait_us to join
         auto req_blocks = [&](const BatchReq* r) -> int64_t {
-          return r->kind == 0 ? ceil_frac(r->len, c->block_size) : (r->length / c->block_size + 2);
+          return r->kind == 0 ? ceil_frac(r->len, c->block_size)
+                 : r->kind == 2 ? ceil_frac(r->total, c->block_size)
+                                : (r->length / c->block_size + 2);
         };
         auto blocks_queued = [&] {
           int64_t nb = 0;
@@ -2516,7 +2615,8 @@ static void batcher_main(mec_batcher* b) {
         // (waiting while batches are in flight only adds latency to a closed loop of callers)
         if (nbusy == 0 && b->max_wait_us > 0 && blocks_queued() < b->max_blocks)
           b->cv_work.wait_for(lk, std::chrono::microseconds(b->max_wait_us), [&] { return b->stop || blocks_queued() >= b->max_blocks; });
-        // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs, the same reader set)
+        // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs and heals, the same reader
+        // set; for heals also the same stale drives)
         // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.45 ms however few
         // blocks it is given (one warp walks one erasure block), so the copy of one batch has to overlap the kernel of another —
         // otherwise a closed loop of callers falls into a convoy (all of them in one batch, the GPU idle while they wake up)
@@ -2530,7 +2630,7 @@ static void batcher_main(mec_batcher* b) {
         const BatchReq* lead = b->queue.front();
         for (auto it = b->queue.begin(); it != b->queue.end();) {
           BatchReq* r = *it;
-          if (r->kind != lead->kind || (r->kind == 1 && r->alive_mask != lead->alive_mask)) { ++it; continue; }
+          if (r->kind != lead->kind || r->alive_mask != lead->alive_mask || r->stale_mask != lead->stale_mask) { ++it; continue; }
           const int64_t rb = req_blocks(r);
           if (!reqs.empty() && nb + rb > cap) break;
           reqs.push_back(r);
@@ -2545,10 +2645,10 @@ static void batcher_main(mec_batcher* b) {
       const auto t_submit = clk::now();
       {
         std::lock_guard<std::mutex> lk(c->mu);
-        inflight[head].is_get = reqs.front()->kind == 1;
+        inflight[head].is_get = reqs.front()->kind != 0;
         inflight[head].get_k = c->k;
         if (inflight[head].is_get) {
-          rc = batcher_submit_get(b, s, reqs);
+          rc = reqs.front()->kind == 2 ? batcher_submit_heal(b, s, reqs) : batcher_submit_get(b, s, reqs);
           if (rc != MEC_OK)
             for (BatchReq* r : reqs) r->ch.s = &s;  // batcher_finish looks the slot up through the first request
         } else {
@@ -2628,8 +2728,10 @@ extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int
       if (rc == MEC_OK) rc = s.aux.ensure(static_cast<size_t>(k * round_up(slots * P + 512, 256)));
       if (rc == MEC_OK) rc = s.flags.ensure(static_cast<size_t>(slots * k));
       if (rc == MEC_OK) rc = s.hflags.ensure(static_cast<size_t>(slots * k));
-      if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc)));
-      if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc)));
+      // request tables: PUT rows, or GET rows, or GET rows plus one out-file pointer per rebuilt shard (heal)
+      const size_t row = std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc) + kMaxR * sizeof(uint8_t*));
+      if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * row);
+      if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * row);
     }
     cudaSetDevice(cur);
   }
@@ -2747,6 +2849,52 @@ extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* file
   b->cv_work.notify_one();
   r.cv.wait(lk, [&] { return r.done; });
   return r.result;
+}
+
+// Erasure.Heal (cmd/erasure-decode.go:317) through the coalescer: heals queued together that read the same k drives and rebuild the
+// same stale drives are merged into one fused launch.  Calls the merged path cannot take (pageable buffers, a drive that is both a
+// reader and stale, more drives than the kernels' tables hold) and calls that meet bitrot run on their own through mec_heal_prefer
+// on a private handle.
+extern "C" int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
+                                uint8_t* const* out_files, uint8_t* corrupt) {
+  if (!b || !files || !out_files) return MEC_ERR_INVALID_ARGUMENT;
+  mec_codec* c = b->codec;
+  const int n = c->n, k = c->k;
+  auto serial = [&]() -> int {
+    mec_codec* sc = batcher_serial(b);
+    return sc ? mec_heal_prefer(sc, files, prefer, total, out_files, corrupt) : MEC_ERR_UNEXPECTED;
+  };
+  if (n > kBatchMaxFiles || n > 64) return serial();
+  if (corrupt) memset(corrupt, 0, static_cast<size_t>(n));
+  if (total <= 0) return MEC_OK;
+  // the readers parallelReader would pick, chosen here on the caller's thread: equal reader sets share a launch
+  uint8_t alive[kBatchMaxFiles];
+  int chosen[kBatchMaxFiles];
+  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
+  if (choose_readers(c, files, alive, prefer, chosen) < k) return MEC_ERR_READ_QUORUM;
+  BatchReq r;
+  r.kind = 2; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
+  r.prefer = prefer; r.outs = out_files; r.corrupt = corrupt;
+  bool mapped = getenv("MEC_BATCHER_MEMCPY") == nullptr;
+  for (int t = 0; t < k; t++) {
+    r.alive_mask |= 1ull << chosen[t];
+    mapped = mapped && mec_is_pinned(files[chosen[t]]) != 0;
+  }
+  int nstale = 0;
+  for (int i = 0; i < n; i++)
+    if (out_files[i]) {
+      r.stale_mask |= 1ull << i;
+      nstale++;
+      mapped = mapped && mec_is_pinned(out_files[i]) != 0;
+    }
+  // a drive that is read and also rewritten is passed through unchanged by reconstruct_range: the serial path does that
+  if (!mapped || (r.alive_mask & r.stale_mask) != 0 || nstale > kMaxR) return serial();
+  std::unique_lock<std::mutex> lk(b->mu);
+  if (b->stop) return MEC_ERR_INVALID_ARGUMENT;
+  b->queue.push_back(&r);
+  b->cv_work.notify_one();
+  r.cv.wait(lk, [&] { return r.done; });
+  return static_cast<int>(r.result);
 }
 
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {

@@ -3,6 +3,8 @@
 //   mode batcher : every PUT goes through ONE mec_batcher (cross-request coalescing into merged launches)
 //   mode pool    : every thread picks a codec handle from a pool of P (no coalescing: one launch per call)
 //   mode get     : degraded GETs (4 data drives offline) through the pool
+//   mode bheal   : heals of one stale data drive (Erasure.Heal, the MRF / new-disk traffic) through ONE mec_batcher
+//   mode heal    : the same heals, each a mec_heal_prefer call on a handle from the pool
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
 // Prints one JSON line: aggregate GiB/s, calls/s, p50/p99 latency.  Buffers are pinned (mec_alloc_pinned_on) for the GPU modes.
 // Build: g++ -O2 -std=c++17 tools/conc_bench.cc -o tools/conc_bench -Iinclude -Lminio_b200 -lminio_ec -Loracle -loracle -lpthread
@@ -49,10 +51,10 @@ int main(int argc, char** argv) {
   const int64_t nb = (osize + bs - 1) / bs;
   if (gpu) mec_bind_thread_to_device(device);
   auto alloc = [&](size_t b) -> uint8_t* { return gpu ? static_cast<uint8_t*>(mec_alloc_pinned_on(device, b)) : static_cast<uint8_t*>(malloc(b)); };
-  // per-thread buffers: object, 16 part files, digests, destination
-  struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; };
+  // per-thread buffers: object, 16 part files, digests, destination, the healed part file
+  struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; };
   std::vector<TB> tb(T);
-  uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + n * fsz + nb * n * 32 + nb * m * S + 4096 * 24));
+  uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
   if (!arena) { fprintf(stderr, "allocation failed\n"); return 1; }
   uint8_t* p = arena;
   auto take = [&](size_t b) { uint8_t* r = p; p += (b + 4095) / 4096 * 4096; return r; };
@@ -64,16 +66,17 @@ int main(int argc, char** argv) {
     tb[t].dd = take(nb * n * 32);
     tb[t].dst = take(osize);
     tb[t].parity = take(nb * m * S);
+    tb[t].healed = take(fsz);
   }
   mec_batcher* bat = nullptr;
   std::vector<mec_codec*> pool;
   if (mode == "batcher") {
     int rc = mec_batcher_new(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
-  } else if (gpu && mode != "bget") {
+  } else if (gpu && mode != "bget" && mode != "bheal") {
     for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
   }
-  if (mode == "bget") {  // coalesced GETs: part files through a temporary handle, then everything goes through the batcher
+  if (mode == "bget" || mode == "bheal") {  // coalesced GETs / heals: part files through a temporary handle, then everything goes through the batcher
     mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c0);
     for (int t = 0; t < T; t++) {
       std::vector<uint8_t*> f(tb[t].files);
@@ -83,7 +86,7 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, &bat);
     if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
   }
-  if (mode == "get") {  // every thread's part files must exist first
+  if (mode == "get" || mode == "heal") {  // every thread's part files must exist first
     for (int t = 0; t < T; t++) {
       std::vector<uint8_t*> f(tb[t].files);
       if (mec_encode(pool[t % P], tb[t].obj, osize, f.data(), k) != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
@@ -108,6 +111,15 @@ int main(int argc, char** argv) {
       int hint = 0;
       return mec_decode(pool[t % P], f, 0, osize, osize, b.dst, &hint);
     }
+    if (mode == "bheal" || mode == "heal") {  // drive 0 is stale: its part file is rebuilt from the first k of the others
+      const uint8_t* f[64];
+      uint8_t* o[64] = {};
+      uint8_t bad[64];
+      for (int i = 0; i < n; i++) f[i] = i == 0 ? nullptr : b.files[i];
+      o[0] = b.healed;
+      const int rc = mode == "bheal" ? mec_batcher_heal(bat, f, nullptr, osize, o, bad) : mec_heal_prefer(pool[t % P], f, nullptr, osize, o, bad);
+      return rc == MEC_OK ? osize : rc;
+    }
     orc_encode_hash_blocks_st(k, m, bs, b.obj, nb, b.parity, b.dd);
     return osize;
   };
@@ -129,6 +141,9 @@ int main(int argc, char** argv) {
   go = 1;
   for (auto& t : th) t.join();
   const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  if (mode == "bheal" || mode == "heal")  // every healed part file equals the drive's original one
+    for (int t = 0; t < T; t++)
+      if (memcmp(tb[t].healed, tb[t].files[0], static_cast<size_t>(fsz)) != 0) errors++;
   std::vector<double> all;
   for (auto& v : lat) all.insert(all.end(), v.begin(), v.end());
   std::sort(all.begin(), all.end());
@@ -145,7 +160,7 @@ int main(int argc, char** argv) {
            (long long)mec_batcher_stat(bat, "us_submit"), (long long)mec_batcher_stat(bat, "us_sync"), (long long)mec_batcher_stat(bat, "us_finish"),
            (long long)mec_batcher_stat(bat, "us_idle"), (long long)mec_batcher_stat(bat, "us_stage"), (long long)mec_batcher_stat(bat, "us_kernel"),
            (long long)mec_batcher_stat(bat, "us_scatter"));
-  if (mode == "pool" || mode == "get") printf(", \"pool\": %d", P);
+  if (mode == "pool" || mode == "get" || mode == "heal") printf(", \"pool\": %d", P);
   printf("}\n");
   if (bat) mec_batcher_free(bat);
   for (auto c : pool) mec_codec_free(c);

@@ -54,6 +54,19 @@ th = [threading.Thread(target=work, args=(t,)) for t in range(8)]
 [x.start() for x in th]; [x.join() for x in th]
 assert not errs, errs
 bat.close()
+# one merged heal round: four heals of stale drive 1 in one batch (staging, fused reconstruct with digests, heal scatter kernel)
+bat = mb.Batcher(k, m, bs, max_batch_blocks=sum(-(-a.size // bs) for a in pin), max_wait_us=500000)
+rd = [[None if i == 1 else mb.pinned_array(w[i].size) for i in range(k + m)] for w in want]
+for r, w in zip(rd, want):
+    for i, f in enumerate(r):
+        if f is not None: f[:] = w[i]
+res = [None] * 4
+def heal(t): res[t] = bat.heal(rd[t], [i == 1 for i in range(k + m)], pin[t].size, pinned=True)
+th = [threading.Thread(target=heal, args=(t,)) for t in range(4)]
+[x.start() for x in th]; [x.join() for x in th]
+assert all(r[1] == 0 and np.array_equal(r[0][1], want[t][1]) for t, r in enumerate(res)), [r[1] for r in res]
+assert bat.stat("kernel_batches") == 1 and bat.stat("requests") == 4
+bat.close()
 print("sanitizer case ok")
 PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
