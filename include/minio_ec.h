@@ -181,7 +181,8 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
  * all full blocks, then writes every caller's frames straight into that caller's buffers.  Up to six merged batches are in flight;
  * device staging for all six is allocated here (about 2.4 x max_batch_blocks x block_size each).
  * mec_batcher_stat: "batches", "requests", "blocks", "kernel_batches" (batches moved by the gather / scatter kernels), "redone"
- * (merged GETs and heals that met a frame failing its digest check and were redone on their own), "launches";
+ * (merged GETs and heals that met a frame failing its digest check and were redone on their own), "crc_requests" (PUTs through
+ * mec_batcher_encode_crc with a non-empty mask that got their checksums), "launches";
  * with MEC_BATCHER_TRACE=1 in the environment also the worker's and the streams' accumulated phase times "us_submit", "us_sync",
  * "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter".  Any other name is answered by mec_get_stat on the batcher's own
  * codec, so "form_*", "last_*", "small_launches", "num_sms" and the rest describe the merged launches. */
@@ -191,6 +192,16 @@ void mec_batcher_free(mec_batcher* b);
 int64_t mec_batcher_encode(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, int write_quorum);
 int64_t mec_batcher_encode_sg(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
                               int write_quorum);
+/* A PutObject through the coalescer together with the object checksums hash.Reader computes over the same bytes
+ * (internal/hash/reader.go:267-310).  data_digests == NULL: the outputs of mec_batcher_encode (complete part files); non-NULL: those
+ * of mec_batcher_encode_sg.  Returns what that call returns.  `which & 7` is a mask of MEC_CRC* (below); out3 receives CRC32,
+ * CRC32C and CRC64NVME as in mec_checksums (0 where not asked for), computed on the bytes the merged batch staged in device memory:
+ * two more launches per batch that holds such requests, however many, and one small copy back.  out3 is written only when the call
+ * returns >= 0 (len == 0: the checksums of the empty stream, all 0); an empty mask is mec_batcher_encode / _sg and out3 may then be
+ * NULL; a non-empty mask with out3 == NULL returns MEC_ERR_INVALID_ARGUMENT before anything is queued.  Requests with and without a
+ * mask share batches. */
+int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
+                               int write_quorum, int which, uint64_t* out3);
 /* Erasure.Decode through the coalescer (arguments and results of mec_decode): GETs queued together that see the same drives online
  * share one reader set and are merged into one fused launch (gather kernel, reconstruct, scatter into every caller's dst).  A request
  * that meets a corrupt frame is redone on its own with parallelReader's exact fail-over; pageable buffers take the same private path. */

@@ -66,6 +66,8 @@ def lib():
     L.mec_batcher_encode.argtypes = [vp, vp, i64, vp, i32]
     L.mec_batcher_encode_sg.restype = i64
     L.mec_batcher_encode_sg.argtypes = [vp, vp, i64, vp, vp, i32]
+    L.mec_batcher_encode_crc.restype = i64
+    L.mec_batcher_encode_crc.argtypes = [vp, vp, i64, vp, vp, i32, i32, vp]
     L.mec_batcher_decode.restype = i64
     L.mec_batcher_decode.argtypes = [vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_batcher_heal.argtypes = [vp, vp, vp, i64, vp, vp]
@@ -424,22 +426,36 @@ class Batcher:
         self.h, self.k, self.m, self.n, self.block_size = h, k, m, k + m, block_size
         self._sizes = Codec(k, m, block_size, device=device)
 
-    def encode(self, src, online=None, write_quorum=0, pinned=False):
+    def _encode_crc(self, src, files, dd, write_quorum, checksums):
+        """mec_batcher_encode_crc -> (CRC32, CRC32C, CRC64NVME), 0 where not asked for"""
+        out = (C.c_uint64 * 3)()
+        rc = lib().mec_batcher_encode_crc(self.h, src.ctypes.data if src.size else None, src.size, _ptrs(files),
+                                          None if dd is None else dd.ctypes.data, write_quorum, checksums, out)
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_encode_crc")
+        return tuple(int(v) for v in out)
+
+    def encode(self, src, online=None, write_quorum=0, pinned=False, checksums=0):
         """pinned=True: the part files are allocated page-locked (and `src` must be, e.g. a pinned_array) — the batch then moves
-        through the gather / scatter kernels instead of per-request copies.  The caller owns (and should free) those arrays."""
+        through the gather / scatter kernels instead of per-request copies.  The caller owns (and should free) those arrays.
+        checksums: a mask of CRC32 / CRC32C / CRC64NVME; non-zero returns (files, (crc32, crc32c, crc64nvme)) computed on the
+        bytes the batch staged (mec_batcher_encode_crc)."""
         src = _u8(src)
         fsz = self._sizes.bitrot_file_size(src.size)
         online = [True] * self.n if online is None else online
         mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
         files = [mk(fsz) if online[i] else None for i in range(self.n)]
+        if checksums:
+            return files, self._encode_crc(src, files, None, write_quorum, checksums)
         rc = lib().mec_batcher_encode(self.h, src.ctypes.data if src.size else None, src.size, _ptrs(files), write_quorum)
         if rc < 0:
             raise MecError(rc, "mec_batcher_encode")
         return files
 
-    def encode_sg(self, src, online=None, write_quorum=0, pinned=False):
+    def encode_sg(self, src, online=None, write_quorum=0, pinned=False, checksums=0):
         """mec_batcher_encode_sg: -> (files, data_digests) shaped like Codec.encode_sg.  pinned=True: the parity images and the
-        [block][k][32] digest array are page-locked (and `src` must be), so the scatter kernel writes both; the caller owns them."""
+        [block][k][32] digest array are page-locked (and `src` must be), so the scatter kernel writes both; the caller owns them.
+        checksums: as for encode(); non-zero returns (files, data_digests, (crc32, crc32c, crc64nvme))."""
         src = _u8(src)
         fsz = self._sizes.bitrot_file_size(src.size)
         nb = -(-src.size // self.block_size)
@@ -448,6 +464,9 @@ class Batcher:
         marker = np.zeros(1, dtype=np.uint8)  # data drives: only NULL / non-NULL is looked at
         files = [(mk(fsz) if i >= self.k else marker) if online[i] else None for i in range(self.n)]
         dd = mk(max(nb, 1) * self.k * 32).reshape(max(nb, 1), self.k, 32)
+        if checksums:
+            crcs = self._encode_crc(src, files, dd, write_quorum, checksums)
+            return [f if i >= self.k else None for i, f in enumerate(files)], dd[:nb], crcs
         rc = lib().mec_batcher_encode_sg(self.h, src.ctypes.data if src.size else None, src.size, _ptrs(files), dd.ctypes.data,
                                          write_quorum)
         if rc < 0:

@@ -83,8 +83,85 @@ struct CrcParams {
   uint64_t* out;             // [kCrcTypes]
 };
 
+// Object checksums of the PUTs of a merged coalescer batch (mec_batcher_encode_crc).  A request's bytes are two segments of the
+// staged buffer (its full blocks, then its short last block elsewhere), each cut into regions of at most kCrcRegion bytes that
+// never cross a segment edge: one work item per region, the items of a request consecutive and in stream order.
+struct CrcWork {
+  int64_t off;    // first byte of the region, from CrcSegParams::base (any alignment)
+  int32_t len;    // 1 .. kCrcRegion; kCrcRegion for every region of a segment but its last
+  int32_t which;  // types its request asked for
+};
+struct CrcReq {
+  int32_t w0, w1;  // the request's work items [w0, w1)
+  int32_t which;   // 0: no checksums for this request (no items)
+  int32_t pad;
+};
+struct CrcSegParams {
+  const uint8_t* base;
+  const CrcWork* work;
+  const CrcReq* reqs;
+  int64_t nwork;
+  int nreq;
+  int which;                 // union of the requests' masks: the byte tables to load
+  const CrcTables* tables;   // device copy
+  uint64_t* partial;         // [nwork][kCrcTypes]
+  uint64_t* out;             // [nreq][kCrcTypes], 0 where the request did not ask
+};
+constexpr int kCrcFoldThreads = 128;  // four requests per CTA of the fold kernel, one warp each
+static_assert(kCrcRegion == (1 << 18), "xp8[ty][18] is the factor of a whole region");
+
 #ifdef __CUDACC__
-// one CTA pass = one 256 KiB region: per-thread chunk CRCs, then a tree merge in shared memory
+// CRCs (types in `which`) of the region src[0, rlen), rlen <= kCrcRegion, by all kCrcThreads threads of the CTA: per-thread chunk
+// CRCs, then a tree merge in shared memory; thread 0 writes part[ty].  Every thread of the CTA must call it with the same arguments.
+__device__ inline void crc_region(const uint8_t* src, int64_t rlen, int which, const uint64_t (*s_tab)[256], uint64_t* s_part,
+                                  const CrcTables* tables, uint64_t* part) {
+  const int tid = threadIdx.x;
+  int64_t n = rlen - static_cast<int64_t>(tid) * kCrcChunk;
+  n = n < 0 ? 0 : (n > kCrcChunk ? kCrcChunk : n);
+  uint64_t crc[kCrcTypes];
+#pragma unroll
+  for (int ty = 0; ty < kCrcTypes; ty++) crc[ty] = crc_mask(crc_spec(ty).bits);  // init: all ones
+  const uint8_t* q = src + static_cast<int64_t>(tid) * kCrcChunk;
+  auto step = [&](uint32_t b) {
+#pragma unroll
+    for (int ty = 0; ty < kCrcTypes; ty++)
+      if (which & (1 << ty)) crc[ty] = s_tab[ty][(crc[ty] ^ b) & 0xffu] ^ (crc[ty] >> 8);
+  };
+  // bytes up to the first 16-byte boundary one at a time, then 16-byte loads (a chunk of a misaligned segment is misaligned too)
+  const int64_t head = (16 - static_cast<int64_t>(reinterpret_cast<uintptr_t>(q) & 15)) & 15;
+  int64_t i = 0;
+  for (; i < n && i < head; i++) step(q[i]);
+  for (; i + 16 <= n; i += 16) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(q + i));
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int k = 0; k < 16; k++) step((w[k >> 2] >> (8 * (k & 3))) & 0xffu);
+  }
+  for (; i < n; i++) step(q[i]);
+  // tree merge: at level `lv` thread t (t % 2^(lv+1) == 0) absorbs thread t + 2^lv; lengths follow from the region length
+#pragma unroll
+  for (int ty = 0; ty < kCrcTypes; ty++) {
+    if (!(which & (1 << ty))) continue;
+    const CrcSpec sp = crc_spec(ty);
+    uint64_t mine = crc[ty] ^ crc_mask(sp.bits);  // xorout
+    __syncthreads();
+    for (int lv = 0; (1 << lv) < kCrcThreads; lv++) {
+      s_part[tid] = mine;
+      __syncthreads();
+      const int span = 1 << lv;
+      if ((tid & (2 * span - 1)) == 0) {
+        // bytes covered by the right-hand subtree [tid + span, tid + 2 span) inside this region
+        int64_t rb = rlen - static_cast<int64_t>(tid + span) * kCrcChunk;
+        rb = rb < 0 ? 0 : (rb > static_cast<int64_t>(span) * kCrcChunk ? static_cast<int64_t>(span) * kCrcChunk : rb);
+        if (rb > 0) mine = crc_combine(tables->xp8[ty], mine, s_part[tid + span], rb, sp.poly, sp.bits);
+      }
+      __syncthreads();
+    }
+    if (tid == 0) part[ty] = mine;
+  }
+}
+
+// one CTA pass = one 256 KiB region of p.src
 __global__ void __launch_bounds__(kCrcThreads) crc_regions_kernel(const CrcParams p) {
   __shared__ uint64_t s_tab[kCrcTypes][256];
   __shared__ uint64_t s_part[kCrcThreads];
@@ -93,55 +170,57 @@ __global__ void __launch_bounds__(kCrcThreads) crc_regions_kernel(const CrcParam
     if (p.which & (1 << ty)) s_tab[ty][tid] = p.tables->byte_tab[ty][tid];
   __syncthreads();
   for (int64_t rg = blockIdx.x; rg < p.nregions; rg += gridDim.x) {
-    const int64_t base = rg * kCrcRegion + static_cast<int64_t>(tid) * kCrcChunk;
-    int64_t n = p.len - base;
-    n = n < 0 ? 0 : (n > kCrcChunk ? kCrcChunk : n);
-    uint64_t crc[kCrcTypes];
-#pragma unroll
-    for (int ty = 0; ty < kCrcTypes; ty++) crc[ty] = crc_mask(crc_spec(ty).bits);  // init: all ones
-    const uint8_t* q = p.src + base;
-    int64_t i = 0;
-    if ((reinterpret_cast<uintptr_t>(q) & 15) == 0) {
-      for (; i + 16 <= n; i += 16) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(q + i));
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int k = 0; k < 16; k++) {
-          const uint32_t b = (w[k >> 2] >> (8 * (k & 3))) & 0xffu;
-#pragma unroll
-          for (int ty = 0; ty < kCrcTypes; ty++)
-            if (p.which & (1 << ty)) crc[ty] = s_tab[ty][(crc[ty] ^ b) & 0xffu] ^ (crc[ty] >> 8);
-        }
-      }
-    }
-    for (; i < n; i++) {
-      const uint32_t b = q[i];
-#pragma unroll
-      for (int ty = 0; ty < kCrcTypes; ty++)
-        if (p.which & (1 << ty)) crc[ty] = s_tab[ty][(crc[ty] ^ b) & 0xffu] ^ (crc[ty] >> 8);
-    }
-    // tree merge: at level `lv` thread t (t % 2^(lv+1) == 0) absorbs thread t + 2^lv; lengths follow from the region length
     const int64_t rlen = (p.len - rg * kCrcRegion) > kCrcRegion ? kCrcRegion : (p.len - rg * kCrcRegion);
-#pragma unroll
-    for (int ty = 0; ty < kCrcTypes; ty++) {
-      if (!(p.which & (1 << ty))) continue;
-      const CrcSpec sp = crc_spec(ty);
-      uint64_t mine = crc[ty] ^ crc_mask(sp.bits);  // xorout
-      __syncthreads();
-      for (int lv = 0; (1 << lv) < kCrcThreads; lv++) {
-        s_part[tid] = mine;
-        __syncthreads();
-        const int span = 1 << lv;
-        if ((tid & (2 * span - 1)) == 0) {
-          // bytes covered by the right-hand subtree [tid + span, tid + 2 span) inside this region
-          int64_t rb = rlen - static_cast<int64_t>(tid + span) * kCrcChunk;
-          rb = rb < 0 ? 0 : (rb > static_cast<int64_t>(span) * kCrcChunk ? static_cast<int64_t>(span) * kCrcChunk : rb);
-          if (rb > 0) mine = crc_combine(p.tables->xp8[ty], mine, s_part[tid + span], rb, sp.poly, sp.bits);
-        }
-        __syncthreads();
-      }
-      if (tid == 0) p.partial[rg * kCrcTypes + ty] = mine;
+    crc_region(p.src + rg * kCrcRegion, rlen, p.which, s_tab, s_part, p.tables, p.partial + rg * kCrcTypes);
+  }
+}
+
+// one CTA pass = one work item of a merged batch
+__global__ void __launch_bounds__(kCrcThreads) crc_seg_regions_kernel(const CrcSegParams p) {
+  __shared__ uint64_t s_tab[kCrcTypes][256];
+  __shared__ uint64_t s_part[kCrcThreads];
+  const int tid = threadIdx.x;
+  for (int ty = 0; ty < kCrcTypes; ty++)
+    if (p.which & (1 << ty)) s_tab[ty][tid] = p.tables->byte_tab[ty][tid];
+  __syncthreads();
+  for (int64_t w = blockIdx.x; w < p.nwork; w += gridDim.x) {
+    const CrcWork wk = p.work[w];
+    crc_region(p.base + wk.off, wk.len, wk.which, s_tab, s_part, p.tables, p.partial + w * kCrcTypes);
+  }
+}
+
+// one warp per request: each lane folds a contiguous run of the request's items in order (a whole region appended = one product with
+// the constant x^(8 * kCrcRegion)), then the 32 runs are merged by a shuffle tree
+__global__ void __launch_bounds__(kCrcFoldThreads) crc_seg_fold_kernel(const CrcSegParams p) {
+  const int q = (blockIdx.x * kCrcFoldThreads + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (q >= p.nreq) return;  // whole warps
+  const CrcReq rq = p.reqs[q];
+  const int nw = rq.w1 - rq.w0, per = (nw + 31) / 32;
+  const int a = rq.w0 + min(nw, lane * per), e = rq.w0 + min(nw, (lane + 1) * per);
+  for (int ty = 0; ty < kCrcTypes; ty++) {
+    if (!(rq.which & (1 << ty))) {
+      if (lane == 0) p.out[q * kCrcTypes + ty] = 0;
+      continue;
     }
+    const CrcSpec sp = crc_spec(ty);
+    const uint64_t* xp8 = p.tables->xp8[ty];
+    uint64_t acc = 0;
+    int64_t alen = 0;
+    for (int w = a; w < e; w++) {
+      const int64_t len = p.work[w].len;
+      const uint64_t c = p.partial[static_cast<int64_t>(w) * kCrcTypes + ty];
+      acc = alen == 0 ? c : crc_mulmod(len == kCrcRegion ? xp8[18] : crc_xpow8(xp8, len, sp.poly, sp.bits), acc, sp.poly, sp.bits) ^ c;
+      alen += len;
+    }
+    for (int span = 1; span < 32; span <<= 1) {
+      const uint64_t rc = __shfl_down_sync(0xffffffffu, acc, span);
+      const int64_t rl = __shfl_down_sync(0xffffffffu, alen, span);
+      if ((lane & (2 * span - 1)) == 0 && rl > 0) {
+        acc = alen == 0 ? rc : crc_combine(xp8, acc, rc, rl, sp.poly, sp.bits);
+        alen += rl;
+      }
+    }
+    if (lane == 0) p.out[q * kCrcTypes + ty] = acc;
   }
 }
 

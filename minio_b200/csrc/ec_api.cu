@@ -61,10 +61,11 @@ struct PinBuf {
 
 struct Slot {
   DevBuf src, out, dig, aux, flags;  // aux: survivor arena of a reconstruct chunk / shard files of the whole-file path
-  DevBuf crc_part, crc_out;          // object checksums of an encode chunk (crc.cuh)
+  DevBuf crc_part, crc_out;          // object checksums of an encode chunk (crc.cuh); of a merged batch: per-item partials, per-request results
+  DevBuf crc_tab;                    // checksum work table of a merged batch ([CrcReq nreq][CrcWork nwork], crc.cuh)
   DevBuf dreq;                       // request table of a merged batch (batch_copy.cuh)
   DevBuf blk;                        // per-block geometry of a merged launch (SmallBlock / per-frame lengths)
-  PinBuf hdig, hflags, hcrc, hreq, hblk;
+  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab;
   cudaStream_t st = nullptr;
 };
 
@@ -167,6 +168,7 @@ extern "C" void mec_codec_free(mec_codec* c) {
     if (s.st) { cudaStreamSynchronize(s.st); cudaStreamDestroy(s.st); }
     s.src.release(); s.out.release(); s.dig.release(); s.aux.release(); s.flags.release();
     s.hdig.release(); s.hflags.release(); s.hcrc.release(); s.crc_part.release(); s.crc_out.release(); s.dreq.release(); s.hreq.release(); s.blk.release(); s.hblk.release();
+    s.crc_tab.release(); s.hcrc_tab.release();
   }
   c->flags.release();
   c->crc_tables.release();
@@ -2019,6 +2021,8 @@ struct BatchReq {
   uint8_t* data_digests = nullptr;
   bool with_data = false;
   bool mapped = false;   // every buffer of the call is page-locked (device-addressable): eligible for the gather / scatter kernels
+  int crc_which = 0;          // MEC_CRC* mask of mec_batcher_encode_crc; the results go to crc_out[0..3)
+  uint64_t* crc_out = nullptr;
   int64_t result = 0;
   bool done = false;
   std::condition_variable cv;  // one per request: a finished batch wakes its own callers, not every thread parked in the batcher
@@ -2038,6 +2042,7 @@ struct mec_batcher {
   std::thread worker;
   std::atomic<int64_t> st_batches{0}, st_requests{0}, st_blocks{0}, st_kernel_batches{0};
   std::atomic<int64_t> st_redone{0};  // merged GETs and heals that met a frame failing its digest and were redone on their own
+  std::atomic<int64_t> st_crc_requests{0};  // PUTs that got their object checksums (mec_batcher_encode_crc)
   // hybrid staging: part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
   cudaStream_t aux = nullptr;
   cudaEvent_t ev_table[kSlots] = {}, ev_gather[kSlots] = {};
@@ -2106,8 +2111,14 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
     fb.is_get = false;
     return;
   }
-  for (BatchReq* r : fb.reqs) {
+  for (size_t q = 0; q < fb.reqs.size(); q++) {
+    BatchReq* r = fb.reqs[q];
     if (rc == MEC_OK && fb.needs_retire) frames_retire(c, r->ch, r->files, r->with_data, r->data_digests);
+    if (rc == MEC_OK && r->crc_which) {  // batcher_crc_enqueue's results, row q of the slot's pinned mirror
+      const uint64_t* h = static_cast<const uint64_t*>(r->ch.s->hcrc.p) + q * kCrcTypes;
+      for (int ty = 0; ty < kCrcTypes; ty++) r->crc_out[ty] = h[ty];
+      b->st_crc_requests++;
+    }
     r->result = rc == MEC_OK ? r->len : rc;
   }
   {
@@ -2116,6 +2127,73 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
   }
   fb.reqs.clear();
   fb.busy = false;
+}
+
+// Object checksums of the PUTs of a batch that asked for them (mec_batcher_encode_crc).  Request q's bytes are two segments of s.src,
+// its full blocks at ch.d_src and its short last block at ch.d_src_tail; each is cut into kCrcRegion work items.  batcher_crc_table
+// writes the work table and enqueues its copy ahead of the staging (behind other slots' staging on the copy engine it would hold up
+// this batch's kernels); batcher_crc_launch, enqueued once the batch is staged, runs the region kernel over every item and the fold
+// kernel that merges each request's items into row q of s.crc_out, and copies the rows to s.hcrc, where batcher_finish reads them.
+// Two launches and one small copy each way per batch, whatever the number of requests; a batch without such requests (p->nreq == 0)
+// enqueues nothing.  The buffers were sized by mec_batcher_new; they only grow here for a batch led by a request larger than
+// max_batch_blocks.
+static int batcher_crc_table(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, CrcSegParams* p) {
+  *p = CrcSegParams();
+  int which = 0;
+  for (BatchReq* r : reqs) which |= r->crc_which;
+  if (!which) return MEC_OK;
+  mec_codec* c = b->codec;
+  const int64_t bs = c->block_size;
+  const uint8_t* base = static_cast<const uint8_t*>(s.src.p);
+  auto regions = [](int64_t n) { return (n + kCrcRegion - 1) / kCrcRegion; };
+  int64_t nwork = 0;
+  for (BatchReq* r : reqs)
+    if (r->crc_which) nwork += regions(r->ch.nfull * bs) + regions(r->ch.tail);
+  const size_t nreq = reqs.size(), tab_bytes = nreq * sizeof(CrcReq) + static_cast<size_t>(nwork) * sizeof(CrcWork);
+  int rc;
+  if ((rc = s.hcrc_tab.ensure(tab_bytes))) return rc;
+  if ((rc = s.crc_tab.ensure(tab_bytes))) return rc;
+  if ((rc = s.crc_part.ensure(static_cast<size_t>(nwork) * kCrcTypes * sizeof(uint64_t)))) return rc;
+  if ((rc = s.crc_out.ensure(nreq * kCrcTypes * sizeof(uint64_t)))) return rc;
+  if ((rc = s.hcrc.ensure(nreq * kCrcTypes * sizeof(uint64_t)))) return rc;
+  CrcReq* rt = static_cast<CrcReq*>(s.hcrc_tab.p);
+  CrcWork* wt = reinterpret_cast<CrcWork*>(rt + nreq);
+  int64_t w = 0;
+  for (size_t q = 0; q < nreq; q++) {
+    const BatchReq* r = reqs[q];
+    rt[q] = CrcReq{static_cast<int32_t>(w), 0, r->crc_which, 0};
+    if (r->crc_which) {
+      auto segment = [&](const uint8_t* p, int64_t n) {
+        for (int64_t off = 0; off < n; off += kCrcRegion)
+          wt[w++] = CrcWork{(p - base) + off, static_cast<int32_t>(std::min(kCrcRegion, n - off)), r->crc_which};
+      };
+      segment(r->ch.d_src, r->ch.nfull * bs);
+      segment(r->ch.d_src_tail, r->ch.tail);
+    }
+    rt[q].w1 = static_cast<int32_t>(w);
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(s.crc_tab.p, rt, tab_bytes, cudaMemcpyHostToDevice, s.st));
+  p->base = base;
+  p->reqs = static_cast<const CrcReq*>(s.crc_tab.p);
+  p->work = reinterpret_cast<const CrcWork*>(p->reqs + nreq);
+  p->nwork = nwork; p->nreq = static_cast<int>(nreq); p->which = which;
+  p->tables = static_cast<const CrcTables*>(c->crc_tables.p);
+  p->partial = static_cast<uint64_t*>(s.crc_part.p);
+  p->out = static_cast<uint64_t*>(s.crc_out.p);
+  return MEC_OK;
+}
+static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
+  if (p.nreq == 0) return MEC_OK;
+  mec_codec* c = b->codec;
+  const unsigned grid = static_cast<unsigned>(std::min<int64_t>(p.nwork, static_cast<int64_t>(c->eng->num_sms()) * 8));
+  crc_seg_regions_kernel<<<grid, kCrcThreads, 0, s.st>>>(p);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  crc_seg_fold_kernel<<<static_cast<unsigned>(ceil_frac(static_cast<int64_t>(p.nreq) * 32, kCrcFoldThreads)), kCrcFoldThreads, 0, s.st>>>(p);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, static_cast<size_t>(p.nreq) * kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
+  return MEC_OK;
 }
 
 // stage, launch and enqueue the copy-back of one merged batch on slot `s`
@@ -2158,8 +2236,8 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
       for (int i = 0; i < n; i++) d.files[i] = r->files[i];
       d.full0 = fb; d.tail_slot = tl ? tb : -1; d.tail_src_off = tl ? toff : 0;
       r->ch = EncChunk();
-      r->ch.nfull = nf; r->ch.tail = tl;
-      r->ch.d_src_tail = dsrc + toff; r->ch.d_out_tail = dout + tb * m * pitch; r->ch.h_dig_tail = hdig + tb * n * 32;
+      r->ch.nfull = nf; r->ch.tail = tl; r->ch.s = &s;
+      r->ch.d_src = dsrc + fb * bs; r->ch.d_src_tail = dsrc + toff; r->ch.d_out_tail = dout + tb * m * pitch; r->ch.h_dig_tail = hdig + tb * n * 32;
       fb += nf;
       if (tl) { tb++; toff += round_up(tl, 256); }
       max_len = std::max(max_len, r->len);
@@ -2170,6 +2248,8 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     const int phase_slot = static_cast<int>(&s - c->slots);
     if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
     MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, reqs.size() * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
+    CrcSegParams crc;
+    if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
     BatchCopyParams cp;
     cp.reqs = static_cast<const BatchReqDesc*>(s.dreq.p);
     cp.nreq = static_cast<int>(reqs.size()); cp.k = k; cp.m = m; cp.bs = bs; cp.S = S; cp.pitch = pitch;
@@ -2215,6 +2295,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     }
     if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[static_cast<int>(&s - c->slots)], 0));
     if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
+    if ((rc = batcher_crc_launch(b, s, crc))) return rc;
     if (c->eng->small_ok(c->opt, nslots)) {
       // ONE launch for every block of the batch, full or short (objects smaller than a block are nothing but a short block): the
       // latency kernel takes the geometry of each block from a table
@@ -2262,17 +2343,24 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     ch.b0 = 0; ch.nfull = r->len / bs; ch.tail = r->len % bs; ch.nb = ch.nfull + (ch.tail ? 1 : 0);
     ch.s = &s; ch.st = s.st; ch.pitch = pitch;
     ch.d_src = dsrc + fb * bs; ch.d_out = dout + fb * m * pitch; ch.h_dig = hdig + fb * n * 32;
-    if (ch.nfull > 0)
-      MEC_CUDA_OK(cudaMemcpyAsync(dsrc + fb * bs, r->src, static_cast<size_t>(ch.nfull * bs), cudaMemcpyHostToDevice, s.st));
     if (ch.tail > 0) {
       ch.d_src_tail = dsrc + toff; ch.d_out_tail = dout + tb * m * pitch; ch.h_dig_tail = hdig + tb * n * 32;
-      MEC_CUDA_OK(cudaMemcpyAsync(dsrc + toff, r->src + ch.nfull * bs, static_cast<size_t>(ch.tail), cudaMemcpyHostToDevice, s.st));
       toff += round_up(ch.tail, 256);
       tb++;
     }
     fb += ch.nfull;
+  }
+  CrcSegParams crc;
+  if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
+  for (BatchReq* r : reqs) {
+    const EncChunk& ch = r->ch;
+    if (ch.nfull > 0)
+      MEC_CUDA_OK(cudaMemcpyAsync(const_cast<uint8_t*>(ch.d_src), r->src, static_cast<size_t>(ch.nfull * bs), cudaMemcpyHostToDevice, s.st));
+    if (ch.tail > 0)
+      MEC_CUDA_OK(cudaMemcpyAsync(const_cast<uint8_t*>(ch.d_src_tail), r->src + ch.nfull * bs, static_cast<size_t>(ch.tail), cudaMemcpyHostToDevice, s.st));
     c->st_h2d += r->len;
   }
+  if ((rc = batcher_crc_launch(b, s, crc))) return rc;
   if (total_full > 0 && (rc = encode_device_locked(c, dsrc, total_full * bs, dout, pitch, ddig, s.st))) return rc;  // ONE launch for every caller's full blocks
   for (BatchReq* r : reqs) {
     const EncChunk& ch = r->ch;
@@ -2732,7 +2820,17 @@ extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int
       const size_t row = std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc) + kMaxR * sizeof(uint8_t*));
       if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * row);
       if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * row);
+      // object checksums (batcher_crc_enqueue): a batch of at most `slots` requests and slots x block_size bytes has at most
+      // slots x block_size / kCrcRegion whole regions plus two partial ones (full-block segment, short block) per request
+      const int64_t nwork = ceil_frac(slots * block_size, kCrcRegion) + 2 * slots;
+      const size_t tab = static_cast<size_t>(slots) * sizeof(CrcReq) + static_cast<size_t>(nwork) * sizeof(CrcWork);
+      if (rc == MEC_OK) rc = s.crc_tab.ensure(tab);
+      if (rc == MEC_OK) rc = s.hcrc_tab.ensure(tab);
+      if (rc == MEC_OK) rc = s.crc_part.ensure(static_cast<size_t>(nwork) * kCrcTypes * sizeof(uint64_t));
+      if (rc == MEC_OK) rc = s.crc_out.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
+      if (rc == MEC_OK) rc = s.hcrc.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
     }
+    if (rc == MEC_OK) rc = ensure_crc(c);
     cudaSetDevice(cur);
   }
   if (rc) { mec_codec_free(c); delete b; return rc; }
@@ -2784,14 +2882,21 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
 }
 
 static int64_t batcher_call(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests, bool with_data,
-                            int write_quorum) {
+                            int write_quorum, int crc_which = 0, uint64_t* crc_out = nullptr) {
   if (!b || len < 0 || !files || (len > 0 && !src)) return MEC_ERR_INVALID_ARGUMENT;
   int online = 0;
   for (int i = 0; i < b->codec->n; i++) online += files[i] != nullptr;
   if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
-  if (len == 0) return 0;
+  if (len == 0) {  // cmd/erasure-coding.go:78-80; the checksums of the empty stream
+    if (crc_which) {
+      for (int ty = 0; ty < kCrcTypes; ty++) crc_out[ty] = 0;
+      b->st_crc_requests++;
+    }
+    return 0;
+  }
   BatchReq r;
   r.src = src; r.len = len; r.files = files; r.data_digests = data_digests; r.with_data = with_data;
+  r.crc_which = crc_which; r.crc_out = crc_out;
   // page-locked buffers (mec_alloc_pinned*, or anything cudaHostRegister'ed) are moved by the gather / scatter kernels; checked here,
   // on the caller's thread, so the worker does not pay for it
   r.mapped = mec_is_pinned(src) && (!data_digests || mec_is_pinned(data_digests));
@@ -2812,6 +2917,12 @@ extern "C" int64_t mec_batcher_encode_sg(mec_batcher* b, const uint8_t* src, int
                                          int write_quorum) {
   if (!data_digests) return MEC_ERR_INVALID_ARGUMENT;
   return batcher_call(b, src, len, files, data_digests, false, write_quorum);
+}
+extern "C" int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
+                                          int write_quorum, int which, uint64_t* out3) {
+  which &= 7;
+  if (which && !out3) return MEC_ERR_INVALID_ARGUMENT;
+  return batcher_call(b, src, len, files, data_digests, data_digests == nullptr, write_quorum, which, out3);
 }
 // Erasure.Decode through the coalescer: GETs that are queued together and see the same drives online are merged into one launch.
 // Calls whose buffers are not page-locked, and calls that meet bitrot, run on their own through a private handle.
@@ -2904,6 +3015,7 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "blocks")) return b->st_blocks.load();
   if (!strcmp(name, "kernel_batches")) return b->st_kernel_batches.load();
   if (!strcmp(name, "redone")) return b->st_redone.load();
+  if (!strcmp(name, "crc_requests")) return b->st_crc_requests.load();
   if (!strcmp(name, "launches")) return b->codec->eng ? b->codec->eng->launches() : 0;
   if (!strcmp(name, "us_submit")) return b->us_submit.load();
   if (!strcmp(name, "us_sync")) return b->us_sync.load();

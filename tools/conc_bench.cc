@@ -1,6 +1,8 @@
 // conc_bench.cc — the many-small-concurrent-requests regime (cmd/erasure-object.go:1371-1441: one Erasure per request, one block
 // per loop iteration, thousands of request goroutines): T host threads each PUT (or degraded-GET) objects of a fixed size.
 //   mode batcher : every PUT goes through ONE mec_batcher (cross-request coalescing into merged launches)
+//   mode batcher_crc : the same PUTs, each also asking for its CRC32, CRC32C and CRC64NVME (mec_batcher_encode_crc); after the timed
+//                  window every thread's last checksums are checked against a table CRC computed here on the host
 //   mode pool    : every thread picks a codec handle from a pool of P (no coalescing: one launch per call)
 //   mode get     : degraded GETs (4 data drives offline) through the pool
 //   mode bheal   : heals of one stale data drive (Erasure.Heal, the MRF / new-disk traffic) through ONE mec_batcher
@@ -22,6 +24,20 @@
 #include <vector>
 #include "minio_ec.h"
 extern "C" void orc_encode_hash_blocks_st(int k, int m, int64_t bs, const uint8_t* src, int64_t nblocks, uint8_t* parity, uint8_t* digests);
+
+// byte-at-a-time table CRC (reflected, init and xorout all ones): CRC32, CRC32C, CRC64NVME as Go's hash/crc32 and hash/crc64 give them
+static uint64_t host_crc(const uint8_t* p, int64_t n, uint64_t poly, int bits) {
+  uint64_t tab[256];
+  for (int v = 0; v < 256; v++) {
+    uint64_t c = static_cast<uint64_t>(v);
+    for (int k = 0; k < 8; k++) c = (c & 1) ? (c >> 1) ^ poly : c >> 1;
+    tab[v] = c;
+  }
+  const uint64_t mask = bits == 64 ? ~0ull : (1ull << bits) - 1;
+  uint64_t c = mask;
+  for (int64_t i = 0; i < n; i++) c = tab[(c ^ p[i]) & 0xff] ^ (c >> 8);
+  return c ^ mask;
+}
 
 static void on_segv(int sig) {
   void* bt[48];
@@ -52,7 +68,7 @@ int main(int argc, char** argv) {
   if (gpu) mec_bind_thread_to_device(device);
   auto alloc = [&](size_t b) -> uint8_t* { return gpu ? static_cast<uint8_t*>(mec_alloc_pinned_on(device, b)) : static_cast<uint8_t*>(malloc(b)); };
   // per-thread buffers: object, 16 part files, digests, destination, the healed part file
-  struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; };
+  struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; uint64_t crc[3]; };
   std::vector<TB> tb(T);
   uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
   if (!arena) { fprintf(stderr, "allocation failed\n"); return 1; }
@@ -70,7 +86,7 @@ int main(int argc, char** argv) {
   }
   mec_batcher* bat = nullptr;
   std::vector<mec_codec*> pool;
-  if (mode == "batcher") {
+  if (mode == "batcher" || mode == "batcher_crc") {
     int rc = mec_batcher_new(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
   } else if (gpu && mode != "bget" && mode != "bheal") {
@@ -98,6 +114,7 @@ int main(int argc, char** argv) {
   auto one_call = [&](int t) -> int64_t {
     TB& b = tb[t];
     if (mode == "batcher") return mec_batcher_encode_sg(bat, b.obj, osize, b.files.data(), b.dd, k + 1);
+    if (mode == "batcher_crc") return mec_batcher_encode_crc(bat, b.obj, osize, b.files.data(), b.dd, k + 1, MEC_CRC32 | MEC_CRC32C | MEC_CRC64NVME, b.crc);
     if (mode == "pool") return mec_encode_sg(pool[t % P], b.obj, osize, b.files.data(), b.dd, k + 1);
     if (mode == "bget") {
       const uint8_t* f[64];
@@ -144,6 +161,11 @@ int main(int argc, char** argv) {
   if (mode == "bheal" || mode == "heal")  // every healed part file equals the drive's original one
     for (int t = 0; t < T; t++)
       if (memcmp(tb[t].healed, tb[t].files[0], static_cast<size_t>(fsz)) != 0) errors++;
+  if (mode == "batcher_crc")  // every thread's object checksums equal the host's
+    for (int t = 0; t < T; t++)
+      if (tb[t].crc[0] != host_crc(tb[t].obj, osize, 0xEDB88320ull, 32) || tb[t].crc[1] != host_crc(tb[t].obj, osize, 0x82F63B78ull, 32) ||
+          tb[t].crc[2] != host_crc(tb[t].obj, osize, 0x9A6C9329AC4BC9B5ull, 64))
+        errors++;
   std::vector<double> all;
   for (auto& v : lat) all.insert(all.end(), v.begin(), v.end());
   std::sort(all.begin(), all.end());
@@ -152,6 +174,7 @@ int main(int argc, char** argv) {
          "\"p50_us\": %.0f, \"p99_us\": %.0f, \"errors\": %lld",
          mode.c_str(), T, static_cast<long long>(osize >> 20), static_cast<long long>(osize), all.size(), sec, total / sec / (1 << 30), all.size() / sec, all[all.size() / 2],
          all[static_cast<size_t>(all.size() * 0.99)], static_cast<long long>(errors.load()));
+  if (mode == "batcher_crc") printf(", \"crc_requests\": %lld", static_cast<long long>(mec_batcher_stat(bat, "crc_requests")));
   if (bat) printf(", \"batches\": %lld, \"blocks_per_batch\": %.1f, \"launches\": %lld", static_cast<long long>(mec_batcher_stat(bat, "batches")),
                   static_cast<double>(mec_batcher_stat(bat, "blocks")) / std::max<int64_t>(1, mec_batcher_stat(bat, "batches")),
                   static_cast<long long>(mec_batcher_stat(bat, "launches")));

@@ -67,6 +67,23 @@ th = [threading.Thread(target=heal, args=(t,)) for t in range(4)]
 assert all(r[1] == 0 and np.array_equal(r[0][1], want[t][1]) for t, r in enumerate(res)), [r[1] for r in res]
 assert bat.stat("kernel_batches") == 1 and bat.stat("requests") == 4
 bat.close()
+# one merged batch of pinned PUTs with mixed checksum masks (mec_batcher_encode_crc): segmented CRC kernels over the staged batch;
+# the 2 MiB object spans eight 256 KiB regions
+objs = pin
+masks = [7, 1, 6, 0]
+bat = mb.Batcher(k, m, bs, max_batch_blocks=sum(-(-a.size // bs) for a in objs), max_wait_us=500000)
+res = [None] * len(objs)
+def put(t): res[t] = bat.encode(objs[t], pinned=True, checksums=masks[t]) if masks[t] else (bat.encode(objs[t], pinned=True), None)
+th = [threading.Thread(target=put, args=(t,)) for t in range(len(objs))]
+[x.start() for x in th]; [x.join() for x in th]
+for t, (fs, crc) in enumerate(res):
+    if masks[t]:
+        w = o.crcs(objs[t])
+        assert w[0] == zlib.crc32(objs[t].tobytes())
+        assert crc == tuple(v if masks[t] & (1 << i) else 0 for i, v in enumerate(w)), (t, crc, w)
+assert all(np.array_equal(x, y) for x, y in zip(res[0][0], want[0]))
+assert bat.stat("batches") == 1 and bat.stat("crc_requests") == 3
+bat.close()
 print("sanitizer case ok")
 PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
