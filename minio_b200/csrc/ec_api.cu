@@ -1,6 +1,6 @@
 // ec_api.cu — the C ABI of include/minio_ec.h on top of the fused kernel engine.
 //
-// Host-buffer entry points stage through device memory owned by the codec with a 3-slot
+// Host-buffer entry points stage through device memory owned by the codec with a kSlots-deep (six-slot)
 // H2D -> kernel -> D2H pipeline; *_device entry points run on caller-provided device memory.
 // There is NO CPU fallback anywhere in this file: without a usable GPU every call fails.
 #include <algorithm>
@@ -86,6 +86,42 @@ struct mec_codec {
   // boundary counters (mec_get_stat)
   int64_t st_blocks_encoded = 0, st_blocks_read = 0, st_shards_rebuilt = 0, st_corrupt = 0, st_h2d = 0, st_d2h = 0;
   int64_t S() const { return ceil_frac(block_size, k); }
+};
+
+// Drains slot streams on every return, errors included, so that no copy a failed call enqueued is still writing into caller
+// memory (or reading staging the next call reuses) when the caller sees the error code.  Every slot, or the one slot of a
+// whole-file path.
+struct SlotDrain {
+  Slot* s;
+  int n;
+  explicit SlotDrain(mec_codec* c) : s(c->slots), n(kSlots) {}
+  explicit SlotDrain(Slot& one) : s(&one), n(1) {}
+  ~SlotDrain() { for (int i = 0; i < n; i++) if (s[i].st) cudaStreamSynchronize(s[i].st); }
+};
+
+// The codec's slots as a round-robin ring for pipelines that retire their chunks in submission order.  acquire() syncs slot `si`
+// and retires the chunk it carried; submitted() marks it busy and moves on; finish() retires everything still in flight, oldest
+// first.  retire(si) runs on the host once slot si's stream has drained.
+template <class Retire>
+struct SlotRing {
+  mec_codec* c;
+  Retire retire;
+  bool busy[kSlots] = {};
+  int si = 0;
+  SlotRing(mec_codec* c_, Retire r) : c(c_), retire(r) {}
+  int acquire() {
+    MEC_CUDA_OK(cudaStreamSynchronize(c->slots[si].st));
+    if (busy[si]) { retire(si); busy[si] = false; }
+    return MEC_OK;
+  }
+  void submitted() { busy[si] = true; si = (si + 1) % kSlots; }
+  int finish() {
+    for (int q = 0; q < kSlots; q++, si = (si + 1) % kSlots) {
+      MEC_CUDA_OK(cudaStreamSynchronize(c->slots[si].st));
+      if (busy[si]) { retire(si); busy[si] = false; }
+    }
+    return MEC_OK;
+  }
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -219,6 +255,32 @@ extern "C" int64_t mec_jit_compile_check(int k, int r, const uint8_t* coef, int 
   return mec::jit_compile_check(k, r, coef, align, eb, rows3d != 0, hash_outputs != 0);
 }
 
+// What a read through k readers rebuilds, and how (parallelReader.Read + reedsolomon's Reconstruct, cmd/erasure-decode.go:145-221):
+// every wanted shard that is not read is a target; rows are the r x k decode rows that rebuild the targets from the read shards.
+struct DecodePlan {
+  uint8_t present[kMaxShards] = {};  // shard i is one of the k readers
+  int targets[kMaxShards];
+  int r = 0;
+  std::vector<uint8_t> rows;  // r x k (one zero row when r == 0)
+};
+
+// chosen[0..nch): the readers in ascending shard order, of which the first k are read.  want == NULL wants every shard;
+// data_only leaves the parity shards out.
+static int plan_decode(const mec_codec* c, const int* chosen, int nch, const uint8_t* want, int data_only, DecodePlan* p) {
+  const int k = c->k;
+  if (nch < k) return MEC_ERR_READ_QUORUM;
+  memset(p->present, 0, sizeof(p->present));
+  for (int t = 0; t < k; t++) p->present[chosen[t]] = 1;
+  p->r = 0;
+  for (int i = 0; i < c->n; i++)
+    if ((!want || want[i]) && !p->present[i] && !(data_only && i >= k)) p->targets[p->r++] = i;
+  if (p->r > kMaxR) return MEC_ERR_UNSUPPORTED;
+  p->rows.assign(static_cast<size_t>(std::max(p->r, 1)) * k, 0);
+  int valid[kMaxShards];
+  if (p->r > 0 && !rs_decode_rows(k, c->m, p->present, p->targets, p->r, p->rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
+  return MEC_OK;
+}
+
 // Pre-warm the kernel cache for the erasure patterns a drive failure will produce: every single missing data shard (the degraded
 // GET of cmd/erasure-decode.go:239 with one drive gone, and the heal of that drive), both CTA shapes.  Compiles run on the
 // background thread (and land in the on-disk cache), nothing waits for them.
@@ -231,15 +293,16 @@ extern "C" int mec_jit_prewarm(mec_codec* c) {
   if (k > kMaxK || n > kMaxShards || c->m < 1) return 0;
   int queued = 0;
   for (int miss = 0; miss < k; miss++) {
-    std::vector<uint8_t> present(n, 0), rows(k);
-    int cnt = 0;
+    int chosen[kMaxK], cnt = 0;
+    uint8_t want[kMaxShards] = {};
+    want[miss] = 1;
     for (int i = 0; i < n && cnt < k; i++)
-      if (i != miss) { present[i] = 1; cnt++; }
-    int valid[kMaxShards];
-    if (!rs_decode_rows(k, c->m, present.data(), &miss, 1, rows.data(), valid)) continue;
+      if (i != miss) chosen[cnt++] = i;
+    DecodePlan p;
+    if (plan_decode(c, chosen, cnt, want, 0, &p)) continue;
     for (int eb_t : {4, 0})
       for (bool hash_out : {false, true}) {
-        c->eng->jit_prewarm(k, 1, rows.data(), eb_t, hash_out);
+        c->eng->jit_prewarm(k, 1, p.rows.data(), eb_t, hash_out);
         queued++;
       }
   }
@@ -322,26 +385,23 @@ extern "C" int mec_checksums(mec_codec* c, const uint8_t* src, int64_t len, int 
   if (rc) return rc;
   if ((rc = ensure_crc(c))) return rc;
   MEC_CUDA_OK(cudaSetDevice(c->device));
-  struct Drain { mec_codec* c; ~Drain() { for (auto& s : c->slots) if (s.st) cudaStreamSynchronize(s.st); } } drain{c};
+  SlotDrain drain(c);
   const int64_t chunk = 64ll << 20;
   uint64_t acc[kCrcTypes] = {0, 0, 0};
   int64_t done = 0;
   int64_t clen[kSlots] = {};
-  bool busy[kSlots] = {};
-  auto retire = [&](int si) {
+  SlotRing ring(c, [&](int si) {
     const uint64_t* h = static_cast<const uint64_t*>(c->slots[si].hcrc.p);
     for (int ty = 0; ty < kCrcTypes; ty++) {
       const CrcSpec sp = crc_spec(ty);
       acc[ty] = done == 0 ? h[ty] : crc_combine(c->crc_host->xp8[ty], acc[ty], h[ty], clen[si], sp.poly, sp.bits);
     }
     done += clen[si];
-    busy[si] = false;
-  };
-  int si = 0;
-  for (int64_t off = 0; off < len; off += chunk, si = (si + 1) % kSlots) {
+  });
+  for (int64_t off = 0; off < len; off += chunk) {
+    if ((rc = ring.acquire())) return rc;
+    const int si = ring.si;
     Slot& s = c->slots[si];
-    MEC_CUDA_OK(cudaStreamSynchronize(s.st));
-    if (busy[si]) retire(si);
     const int64_t n = std::min(chunk, len - off);
     if ((rc = s.src.ensure(static_cast<size_t>(round_up(n, 16) + 256)))) return rc;
     if ((rc = s.crc_out.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
@@ -350,13 +410,10 @@ extern "C" int mec_checksums(mec_codec* c, const uint8_t* src, int64_t len, int 
     if ((rc = checksums_enqueue(c, static_cast<const uint8_t*>(s.src.p), n, which, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), s.st))) return rc;
     MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
     clen[si] = n;
-    busy[si] = true;
     c->st_h2d += n;
+    ring.submitted();
   }
-  for (int q = 0; q < kSlots; q++, si = (si + 1) % kSlots) {
-    MEC_CUDA_OK(cudaStreamSynchronize(c->slots[si].st));
-    if (busy[si]) retire(si);
-  }
+  if ((rc = ring.finish())) return rc;
   for (int ty = 0; ty < kCrcTypes; ty++) out3[ty] = (which & (1 << ty)) ? acc[ty] : 0;
   return MEC_OK;
 }
@@ -454,10 +511,9 @@ struct EncChunk {
   cudaStream_t st = nullptr;
 };
 
-// The 3-slot H2D -> fused kernel -> D2H pipeline behind every host-buffer encode entry point.  `enqueue(ch)` adds the
+// The six-slot H2D -> fused kernel -> D2H pipeline behind every host-buffer encode entry point.  `enqueue(ch)` adds the
 // chunk's device->host copies to ch.s->st right behind the kernel; `retire(ch)` runs on the host once that stream has
-// drained (digest scatter into frames).  On any error every slot stream is drained before returning, so no copy is
-// still writing into caller memory (or reading freed staging) when the caller sees the error code.
+// drained (digest scatter into frames).  On any error every slot stream is drained before returning (SlotDrain).
 template <class Enqueue, class Retire>
 static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueue&& enqueue, Retire&& retire) {
   const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
@@ -466,13 +522,9 @@ static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueu
   // an object of a few chunks' worth or less is cut into ~four pieces so that its staging, kernel and copy-back overlap (a launch of
   // a handful of blocks costs the same ~0.16 ms as one of a hundred: for 8-64 MiB objects the copies are what is worth overlapping)
   if (c->opt.chunk_blocks <= 0 && nall < 2 * chunk) chunk = std::max<int64_t>(4, ceil_frac(nall, 4));
-  struct Drain {
-    mec_codec* c;
-    ~Drain() { for (auto& s : c->slots) if (s.st) cudaStreamSynchronize(s.st); }
-  } drain{c};
+  SlotDrain drain(c);
   EncChunk inflight[kSlots];
-  bool busy[kSlots] = {};
-  int si = 0, rc;
+  int rc;
   // option "checksums": CRCs of the object bytes ride along — computed on the chunk that was just staged for the encode (the
   // bytes cross PCIe once), merged across chunks on the host the way Checksum.AddPart merges parts
   const int ck = c->checksums;
@@ -482,21 +534,23 @@ static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueu
     for (auto& v : c->last_crc) v = 0;
     c->last_crc_len = 0;
   }
-  auto ck_retire = [&](int q) {
-    if (!ck) return;
-    const uint64_t* h = static_cast<const uint64_t*>(c->slots[q].hcrc.p);
-    for (int ty = 0; ty < kCrcTypes; ty++) {
-      if (!(ck & (1 << ty))) continue;
-      const CrcSpec sp = crc_spec(ty);
-      c->last_crc[ty] = ck_done == 0 ? h[ty] : crc_combine(c->crc_host->xp8[ty], c->last_crc[ty], h[ty], ck_len[q], sp.poly, sp.bits);
+  SlotRing ring(c, [&](int q) {
+    if (ck) {
+      const uint64_t* h = static_cast<const uint64_t*>(c->slots[q].hcrc.p);
+      for (int ty = 0; ty < kCrcTypes; ty++) {
+        if (!(ck & (1 << ty))) continue;
+        const CrcSpec sp = crc_spec(ty);
+        c->last_crc[ty] = ck_done == 0 ? h[ty] : crc_combine(c->crc_host->xp8[ty], c->last_crc[ty], h[ty], ck_len[q], sp.poly, sp.bits);
+      }
+      ck_done += ck_len[q];
+      c->last_crc_len = ck_done;
     }
-    ck_done += ck_len[q];
-    c->last_crc_len = ck_done;
-  };
-  for (int64_t b0 = 0; b0 < nall; b0 += chunk, si = (si + 1) % kSlots) {
+    retire(inflight[q]);
+  });
+  for (int64_t b0 = 0; b0 < nall; b0 += chunk) {
+    if ((rc = ring.acquire())) return rc;
+    const int si = ring.si;
     Slot& s = c->slots[si];
-    MEC_CUDA_OK(cudaStreamSynchronize(s.st));
-    if (busy[si]) { ck_retire(si); retire(inflight[si]); busy[si] = false; }
     EncChunk ch;
     ch.b0 = b0; ch.nb = std::min(chunk, nall - b0); ch.s = &s; ch.pitch = pitch;
     const int64_t off = b0 * bs, bytes = std::min(len - off, ch.nb * bs);
@@ -522,12 +576,9 @@ static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueu
     }
     if ((rc = enqueue(ch))) return rc;
     inflight[si] = ch;
-    busy[si] = true;
+    ring.submitted();
   }
-  for (int q = 0; q < kSlots; q++, si = (si + 1) % kSlots) {  // oldest first
-    MEC_CUDA_OK(cudaStreamSynchronize(c->slots[si].st));
-    if (busy[si]) { ck_retire(si); retire(inflight[si]); busy[si] = false; }
-  }
+  if ((rc = ring.finish())) return rc;
   c->st_blocks_encoded += nall;
   c->st_h2d += len;
   return MEC_OK;
@@ -774,11 +825,9 @@ struct RangeSink {
 };
 
 // One chunk of the reconstruct pipeline: blocks [b0, b0 + nb) of the range, read through reader set `chosen`.
-struct RChunk {
+struct RChunk : DecodePlan {
   int64_t b0 = 0, nb = 0;
   int chosen[kMaxK];
-  int targets[kMaxR];
-  int r = 0;
   uint64_t epoch = 0;  // reader-set generation the chunk was submitted under
 };
 
@@ -854,6 +903,16 @@ static int choose_readers(const mec_codec* c, const uint8_t* const* frames, cons
   return nch;
 }
 
+// writeDataBlocks (cmd/erasure-utils.go:42) for data shard i of part block B, whose shards hold `cur` bytes each: the part bytes
+// [a, e) it contributes to the wanted bytes [lo, hi) (none when e <= a), found at `off` in the shard.
+struct DataSlice { int64_t a, e, off; };
+static inline DataSlice data_slice(int64_t B, int i, int64_t cur, int64_t bs, int64_t total, int64_t lo, int64_t hi) {
+  const int64_t blo = B * bs, bhi = std::min(blo + bs, total);
+  const int64_t slo = blo + static_cast<int64_t>(i) * cur, shi = std::min(slo + cur, bhi);
+  const int64_t a = std::max(slo, lo), e = std::min(shi, hi);
+  return DataSlice{a, e, a - slo};
+}
+
 // device->host copies of one verified-or-not chunk into the object sink (optimistic: a chunk that turns out to hold a corrupt
 // frame is redone from the bad block with other readers and its bytes are overwritten before the call returns)
 static int emit_object(mec_codec* c, const FrameGeom& g, const RangeSink& sk, const RChunk& ch, Slot& s, int64_t stride, int64_t pitch,
@@ -896,12 +955,11 @@ static int emit_object(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
       const bool whole = blo >= sk.lo && bhi <= sk.hi && bhi - blo == bs && cur == S;
       if (whole) { if (run0 < 0) run0 = b; continue; }
       if ((rc = flush(b))) return rc;
-      const int64_t slo = blo + static_cast<int64_t>(i) * cur, shi = std::min(slo + cur, bhi);
-      const int64_t a = std::max(slo, sk.lo), e = std::min(shi, sk.hi);
-      if (e > a) {
-        if (list) list->add(sk.dst + (a - sk.lo), base + b * spitch + (a - slo), e - a);
-        else MEC_CUDA_OK(cudaMemcpyAsync(sk.dst + (a - sk.lo), base + b * spitch + (a - slo), static_cast<size_t>(e - a), cudaMemcpyDeviceToHost, s.st));
-        c->st_d2h += e - a;
+      const DataSlice sl = data_slice(B, i, cur, bs, sk.total, sk.lo, sk.hi);
+      if (sl.e > sl.a) {
+        if (list) list->add(sk.dst + (sl.a - sk.lo), base + b * spitch + sl.off, sl.e - sl.a);
+        else MEC_CUDA_OK(cudaMemcpyAsync(sk.dst + (sl.a - sk.lo), base + b * spitch + sl.off, static_cast<size_t>(sl.e - sl.a), cudaMemcpyDeviceToHost, s.st));
+        c->st_d2h += sl.e - sl.a;
       }
     }
     if ((rc = flush(ch.nb))) return rc;
@@ -945,7 +1003,7 @@ static int emit_frames(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
 }
 
 // Core of Decode / Heal: frames[i] point at the first frame of the range (host).  The range is cut into chunks that run through
-// the codec's three slots — while chunk c is in the kernel, chunk c+1 is being staged and chunk c-1 is on its way back — each
+// the codec's six slots — while chunk c is in the kernel, chunk c+1 is being staged and chunk c-1 is on its way back — each
 // slot with its own stream, survivor arena, output and flag buffers.  Chunks retire in order: the per-frame digest verdicts
 // ([block][reader] flags written by the hash threads) are read, and on the first mismatch the failing readers are dropped
 // for the rest of the call (parallelReader.Read: p.readers[i] = nil, cmd/erasure-decode.go:196-199), everything submitted
@@ -958,10 +1016,7 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
   const int k = c->k, n = c->n;
   if (k > kMaxK) return MEC_ERR_UNSUPPORTED;
   MEC_CUDA_OK(cudaSetDevice(c->device));
-  struct Drain {
-    mec_codec* c;
-    ~Drain() { for (auto& s : c->slots) if (s.st) cudaStreamSynchronize(s.st); }
-  } drain{c};
+  SlotDrain drain(c);
   const int64_t fstride = 32 + g.S, P = g.dpitch(), pitch = round_up(g.S, 16);
   // chunk: ~32 MiB of object per chunk keeps short ranges pipelined over several slots; long ranges take larger chunks (up to four
   // times that) because every chunk costs a host round trip when it retires
@@ -973,7 +1028,6 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
   const int64_t stride = round_up(chunk * P + 512, 256);
 
   RChunk inflight[kSlots];
-  std::vector<uint8_t> rows_of[kSlots];
   bool busy[kSlots] = {};
   int head = 0, tail = 0, nbusy = 0;  // ring: tail = oldest in flight, head = next free slot
   int64_t next = 0, done = 0;         // next block to submit, blocks accepted so far
@@ -984,19 +1038,9 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     Slot& s = c->slots[si];
     RChunk& ch = inflight[si];
     ch.b0 = b0; ch.nb = std::min(chunk, g.nblocks - b0); ch.epoch = epoch;
-    if (choose_readers(c, frames, alive, prefer, ch.chosen) < k) return MEC_ERR_READ_QUORUM;
-    std::vector<uint8_t> present(n, 0);
-    for (int t = 0; t < k; t++) present[ch.chosen[t]] = 1;
-    ch.r = 0;
-    for (int i = 0; i < n; i++)
-      if (want[i] && !present[i] && !(data_only && i >= k)) {
-        if (ch.r >= kMaxR) return MEC_ERR_UNSUPPORTED;
-        ch.targets[ch.r++] = i;
-      }
-    rows_of[si].assign(static_cast<size_t>(std::max(ch.r, 1)) * k, 0);
-    int valid[kMaxShards];
-    if (ch.r > 0 && !rs_decode_rows(k, c->m, present.data(), ch.targets, ch.r, rows_of[si].data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
-    int e;
+    const int nch = choose_readers(c, frames, alive, prefer, ch.chosen);
+    int e = plan_decode(c, ch.chosen, nch, want, data_only, &ch);
+    if (e) return e;
     if ((e = s.aux.ensure(static_cast<size_t>(k * stride)))) return e;
     if ((e = s.out.ensure(static_cast<size_t>(ch.nb * std::max(ch.r, 1) * pitch)))) return e;
     if ((e = s.dig.ensure(static_cast<size_t>(ch.nb * (k + ch.r) * 32)))) return e;
@@ -1020,7 +1064,7 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     }
     c->st_h2d += sub.file_bytes() * k;
     MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(ch.nb * k), s.st));
-    if ((e = launch_reconstruct(c, g, ch, s, stride, rows_of[si].data(), pitch, hash_outputs))) return e;
+    if ((e = launch_reconstruct(c, g, ch, s, stride, ch.rows.data(), pitch, hash_outputs))) return e;
     MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(ch.nb * k), cudaMemcpyDeviceToHost, s.st));
     if (sk.dst) { if ((e = emit_object(c, g, sk, ch, s, stride, pitch, batched ? &list : nullptr))) return e; }
     else if (sk.out) { if ((e = emit_frames(c, g, sk, ch, s, pitch, batched ? &list : nullptr))) return e; }
@@ -1050,10 +1094,8 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
         if (fl[b * k + t]) { bad = b; break; }
     const int64_t good = bad;  // blocks [b0, b0 + good) are accepted
     if (good > 0 && sk.out) {  // wanted shards that were read are passed through unchanged
-      std::vector<uint8_t> present(n, 0);
-      for (int t = 0; t < k; t++) present[ch.chosen[t]] = 1;
       for (int i = 0; i < n; i++) {
-        if (!want[i] || !present[i] || !sk.out[i] || sk.out[i] == frames[i]) continue;
+        if (!want[i] || !ch.present[i] || !sk.out[i] || sk.out[i] == frames[i]) continue;
         const int64_t bytes = (ch.b0 + good == g.nblocks) ? (g.file_bytes() - ch.b0 * fstride) : good * fstride;
         memcpy(sk.out[i] + ch.b0 * fstride, frames[i] + ch.b0 * fstride, static_cast<size_t>(bytes));
       }
@@ -1092,21 +1134,14 @@ extern "C" int mec_reconstruct_device(mec_codec* c, const uint8_t* const* d_fram
   if ((frame_pitch & 15) || frame_pitch < 32 + S) return MEC_ERR_INVALID_ARGUMENT;
   if (d_corrupt && !d_digests) return MEC_ERR_INVALID_ARGUMENT;  // the digest check runs in the hash threads: no digests, no bitrot verdict
   int chosen[kMaxShards], nch = 0;
-  std::vector<uint8_t> present(n, 0);
   for (int i = 0; i < n && nch < k; i++)
-    if (d_frames[i]) { chosen[nch++] = i; present[i] = 1; }
-  if (nch < k) return MEC_ERR_READ_QUORUM;
-  int targets[kMaxShards], r = 0;
-  for (int i = 0; i < n; i++)
-    if (want[i] && !present[i] && !(data_only && i >= k)) targets[r++] = i;
-  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
-  std::vector<uint8_t> rows(static_cast<size_t>(std::max(r, 1)) * k);
-  int valid[kMaxShards];
-  if (r > 0 && !rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
+    if (d_frames[i]) chosen[nch++] = i;
+  DecodePlan p;
+  if ((rc = plan_decode(c, chosen, nch, want, data_only, &p))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   MEC_CUDA_OK(cudaSetDevice(c->device));
   FusedDesc d;
-  d.k = k; d.r = r; d.coef = rows.data(); d.static_encode = false; d.contiguous = false;
+  d.k = k; d.r = p.r; d.coef = p.rows.data(); d.static_encode = false; d.contiguous = false;
   d.key = kMagicKey; d.nblocks = nblocks; d.S = static_cast<int32_t>(S);
   d.in_block_stride = frame_pitch; d.expect_block_stride = frame_pitch;
   for (int t = 0; t < k; t++) {
@@ -1144,6 +1179,21 @@ extern "C" int64_t mec_decode(mec_codec* c, const uint8_t* const* files, int64_t
   return mec_decode_prefer(c, files, nullptr, offset, length, total, dst, heal_hint);
 }
 
+// The blocks Erasure.Decode reads for part bytes [offset, offset + length) of a part of `total` bytes (cmd/erasure-decode.go:
+// 251-281): [start_block, last_block], nblocks of them, the last with shards of last_len bytes.
+struct ReadRange { int64_t start_block, last_block, nblocks, last_len; };
+static ReadRange read_range(const mec_codec* c, int64_t offset, int64_t length, int64_t total) {
+  const int64_t bs = c->block_size, S = c->S(), sfs = mec_shard_file_size(c, total);
+  ReadRange rr;
+  rr.start_block = offset / bs;
+  rr.last_block = (offset + length) / bs;
+  if ((offset + length) % bs == 0) rr.last_block--;  // blockLength == 0 => loop breaks (:279-281)
+  rr.last_block = std::min(rr.last_block, ceil_frac(sfs, S) - 1);
+  rr.nblocks = rr.last_block - rr.start_block + 1;
+  rr.last_len = std::min(S, sfs - rr.last_block * S);
+  return rr;
+}
+
 extern "C" int64_t mec_decode_prefer(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset,
                                      int64_t length, int64_t total, uint8_t* dst, int* heal_hint) {
   NvtxRange nvtx("mec_decode");
@@ -1157,27 +1207,19 @@ extern "C" int64_t mec_decode_prefer(mec_codec* c, const uint8_t* const* files, 
   if (rc) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   const int k = c->k, n = c->n;
-  const int64_t bs = c->block_size, S = c->S(), sfs = mec_shard_file_size(c, total);
-  const int64_t start_block = offset / bs, end_block = (offset + length) / bs;
-  // blocks that are actually read: [start_block, last_block]
-  int64_t last_block = end_block;
-  if ((offset + length) % bs == 0) last_block = end_block - 1;  // blockLength == 0 => loop breaks (:279-281)
-  const int64_t nblocks_total = ceil_frac(sfs, S);
-  if (last_block >= nblocks_total) last_block = nblocks_total - 1;
-  FrameGeom g;
-  g.nblocks = last_block - start_block + 1;
-  g.S = S;
-  g.last_len = std::min(S, sfs - last_block * S);
+  const int64_t bs = c->block_size, S = c->S();
+  const ReadRange rr = read_range(c, offset, length, total);
+  const FrameGeom g{rr.nblocks, S, rr.last_len};
   // writeDataBlocks (cmd/erasure-utils.go:42): a block whose k shards hold fewer bytes than asked of it is ErrShortData
   // (every block but the part's last holds k*S >= block_size bytes, so only that one can fall short)
-  if (static_cast<int64_t>(k) * g.last_len < std::min(offset + length, total) - last_block * bs) return MEC_ERR_SHORT_DATA;
-  const int64_t fstride = 32 + S, foff = start_block * fstride;
+  if (static_cast<int64_t>(k) * g.last_len < std::min(offset + length, total) - rr.last_block * bs) return MEC_ERR_SHORT_DATA;
+  const int64_t fstride = 32 + S, foff = rr.start_block * fstride;
   std::vector<const uint8_t*> in(n);
   std::vector<uint8_t> alive(n), want(n, 0), corrupt(n, 0);
   for (int i = 0; i < n; i++) { in[i] = files[i] ? files[i] + foff : nullptr; alive[i] = files[i] != nullptr; }
   for (int i = 0; i < k; i++) want[i] = 1;
   RangeSink sk;
-  sk.dst = dst; sk.first_block = start_block; sk.lo = offset; sk.hi = offset + length; sk.bs = bs; sk.total = total;
+  sk.dst = dst; sk.first_block = rr.start_block; sk.lo = offset; sk.hi = offset + length; sk.bs = bs; sk.total = total;
   // GetObject only consumes the data bytes of the rebuilt shards: their digests are not computed
   rc = reconstruct_range(c, in.data(), g, want.data(), 1, sk, corrupt.data(), alive.data(), prefer, false);
   if (rc) return rc;
@@ -1259,12 +1301,12 @@ static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* cons
                                int* results) {
   const int64_t S = c->S(), fstride = 32 + S, P = round_up(32 + S, 16);
   MEC_CUDA_OK(cudaSetDevice(c->device));
-  struct Drain { mec_codec* c; ~Drain() { for (auto& s : c->slots) if (s.st) cudaStreamSynchronize(s.st); } } drain{c};
+  SlotDrain drain(c);
   struct Piece { int64_t file, nb; };
   std::vector<Piece> inflight[kSlots];
   const int64_t chunk = std::max<int64_t>(1, (32ll << 20) / fstride);  // frames per chunk (~32 MiB)
   int rc;
-  auto retire = [&](int si) {
+  SlotRing ring(c, [&](int si) {
     const uint8_t* fl = static_cast<const uint8_t*>(c->slots[si].hflags.p);
     int64_t o = 0;
     for (const Piece& pc : inflight[si]) {
@@ -1273,13 +1315,12 @@ static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* cons
       o += pc.nb;
     }
     inflight[si].clear();
-  };
-  int si = 0;
+  });
   int64_t f = 0, b0 = 0;  // next file / next frame of it
   while (f < nfiles) {
+    if ((rc = ring.acquire())) return rc;
+    const int si = ring.si;
     Slot& s = c->slots[si];
-    MEC_CUDA_OK(cudaStreamSynchronize(s.st));
-    retire(si);
     if ((rc = s.src.ensure(static_cast<size_t>(chunk * P + 512)))) return rc;
     if ((rc = s.dig.ensure(static_cast<size_t>(chunk * 32)))) return rc;
     if ((rc = s.flags.ensure(static_cast<size_t>(chunk)))) return rc;
@@ -1353,13 +1394,9 @@ static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* cons
     }
     MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(used), cudaMemcpyDeviceToHost, s.st));
     c->st_blocks_read += used;
-    si = (si + 1) % kSlots;
+    ring.submitted();
   }
-  for (int q = 0; q < kSlots; q++, si = (si + 1) % kSlots) {
-    MEC_CUDA_OK(cudaStreamSynchronize(c->slots[si].st));
-    retire(si);
-  }
-  return MEC_OK;
+  return ring.finish();
 }
 
 extern "C" int mec_bitrot_verify_batch(mec_codec* c, int64_t nfiles, const uint8_t* const* files, const int64_t* file_lens,
@@ -1533,9 +1570,9 @@ static int require_whole(mec_codec* c) {
   return ensure_engine(c);
 }
 
-// stage + verify: on return chosen[0..k) (ascending) name k verified files, file chosen[t] at s.aux + t*fpitch
+// stage + verify: on return chosen[0..k) (ascending) name k verified files, file chosen[t] at s.aux + pos[t]*fpitch
 static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const uint8_t* sums, int64_t sfs, uint8_t* alive,
-                                uint8_t* corrupt, int* chosen, int64_t fpitch, Slot& s) {
+                                uint8_t* corrupt, int* chosen, int* pos, int64_t fpitch, Slot& s) {
   const int k = c->k, n = c->n, ds = mec_digest_size(c->algo);
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * fpitch + 256)))) return rc;
@@ -1594,20 +1631,20 @@ static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const
   // compact into ascending order: position t must hold the t-th chosen file (decode rows are defined on ascending indices)
   int nch = 0;
   for (int i = 0; i < n && nch < k; i++)
-    if (alive[i] && verified[i]) chosen[nch++] = i;
+    if (alive[i] && verified[i]) { chosen[nch] = i; pos[nch++] = slot_of[i]; }
   if (nch < k) return MEC_ERR_READ_QUORUM;
-  for (int t = 0; t < k; t++) chosen[t] = chosen[t] | (slot_of[chosen[t]] << 16);  // low 16 bits: shard index, high: arena position
   return MEC_OK;
 }
 
-// launch the rebuild of `targets` over blocks [first, first + nb) of raw shard files (stride S between blocks, no frames)
-static int launch_whole_rebuild(mec_codec* c, Slot& s, const int* chosen, int64_t fpitch, int64_t S, int64_t last_len, int64_t first,
-                                int64_t nb, int64_t nblocks_file, const uint8_t* rows, int r, int64_t pitch) {
+// launch the rebuild of `targets` over blocks [first, first + nb) of raw shard files (stride S between blocks, no frames); the
+// last of those blocks has shards of last_len bytes
+static int launch_whole_rebuild(mec_codec* c, Slot& s, const int* pos, int64_t fpitch, int64_t S, int64_t last_len, int64_t first,
+                                int64_t nb, const uint8_t* rows, int r, int64_t pitch) {
   const int k = c->k;
   FusedDesc d;
   d.k = k; d.r = r; d.coef = rows; d.static_encode = false; d.contiguous = false; d.hash_outputs = false;
   d.key = kMagicKey; d.out_pitch = pitch; d.in_block_stride = S; d.digests = nullptr;
-  const bool has_short = (first + nb == nblocks_file) && last_len != S;
+  const bool has_short = last_len != S;
   const int64_t nfull = has_short ? nb - 1 : nb;
   for (int pass = 0; pass < 2; pass++) {
     const int64_t f0 = pass == 0 ? 0 : nfull, cnt = pass == 0 ? nfull : nb - nfull;
@@ -1615,7 +1652,7 @@ static int launch_whole_rebuild(mec_codec* c, Slot& s, const int* chosen, int64_
     d.nblocks = cnt;
     d.S = static_cast<int32_t>(pass == 0 ? S : last_len);
     for (int t = 0; t < k; t++) {
-      const uint8_t* base = static_cast<const uint8_t*>(s.aux.p) + (chosen[t] >> 16) * fpitch;
+      const uint8_t* base = static_cast<const uint8_t*>(s.aux.p) + pos[t] * fpitch;
       d.in_ptr[t] = base + (first + f0) * S;
       d.map_base[t] = base;
       d.map_len[t] = fpitch;
@@ -1643,49 +1680,36 @@ extern "C" int64_t mec_decode_whole(mec_codec* c, const uint8_t* const* files, c
   if (k > kMaxK || n > kMaxShards || c->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
   MEC_CUDA_OK(cudaSetDevice(c->device));
   const int64_t bs = c->block_size, S = c->S(), sfs = mec_shard_file_size(c, total);
-  const int64_t nblocks_file = ceil_frac(sfs, S), last_len_file = sfs - (nblocks_file - 1) * S;
-  const int64_t start_block = offset / bs;
-  int64_t last_block = (offset + length) / bs;
-  if ((offset + length) % bs == 0) last_block--;
-  if (last_block >= nblocks_file) last_block = nblocks_file - 1;
-  const int64_t nb = last_block - start_block + 1;
+  const ReadRange rr = read_range(c, offset, length, total);
+  const int64_t nb = rr.nblocks;
   Slot& s = c->slots[0];
-  struct Drain { Slot& s; ~Drain() { if (s.st) cudaStreamSynchronize(s.st); } } drain{s};
+  SlotDrain drain(s);
   const int64_t fpitch = round_up(sfs, 16) + 256, pitch = round_up(S, 16);
   std::vector<uint8_t> alive(n), corrupt(n, 0);
   for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
-  int chosen[kMaxShards];
-  if ((rc = stage_verified_whole(c, files, sums, sfs, alive.data(), corrupt.data(), chosen, fpitch, s))) return rc;
-  std::vector<uint8_t> present(n, 0);
-  for (int t = 0; t < k; t++) present[chosen[t] & 0xffff] = 1;
-  int targets[kMaxShards], r = 0;
-  for (int i = 0; i < k; i++)
-    if (!present[i]) targets[r++] = i;
-  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
-  std::vector<uint8_t> rows(static_cast<size_t>(std::max(r, 1)) * k);
-  int valid[kMaxShards];
-  if (r > 0 && !rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
+  int chosen[kMaxShards], pos[kMaxK];
+  if ((rc = stage_verified_whole(c, files, sums, sfs, alive.data(), corrupt.data(), chosen, pos, fpitch, s))) return rc;
+  DecodePlan p;
+  if ((rc = plan_decode(c, chosen, k, nullptr, 1, &p))) return rc;
+  const int r = p.r;
   if (r > 0) {
     if ((rc = s.out.ensure(static_cast<size_t>(nb * r * pitch)))) return rc;
-    if ((rc = launch_whole_rebuild(c, s, chosen, fpitch, S, last_len_file, start_block, nb, nblocks_file, rows.data(), r, pitch))) return rc;
+    if ((rc = launch_whole_rebuild(c, s, pos, fpitch, S, rr.last_len, rr.start_block, nb, p.rows.data(), r, pitch))) return rc;
   }
   // writeDataBlocks by DMA: data shard i of block B sits in a verified shard file (stride S) or in a rebuilt row
   for (int i = 0; i < k; i++) {
     const uint8_t* base = nullptr;
     int64_t spitch = 0;
     for (int t = 0; t < k && !base; t++)
-      if ((chosen[t] & 0xffff) == i) { base = static_cast<const uint8_t*>(s.aux.p) + (chosen[t] >> 16) * fpitch + start_block * S; spitch = S; }
+      if (chosen[t] == i) { base = static_cast<const uint8_t*>(s.aux.p) + pos[t] * fpitch + rr.start_block * S; spitch = S; }
     for (int q = 0; q < r && !base; q++)
-      if (targets[q] == i) { base = static_cast<const uint8_t*>(s.out.p) + q * pitch; spitch = r * pitch; }
+      if (p.targets[q] == i) { base = static_cast<const uint8_t*>(s.out.p) + q * pitch; spitch = r * pitch; }
     if (!base) return MEC_ERR_UNEXPECTED;
     for (int64_t b = 0; b < nb; b++) {
-      const int64_t B = start_block + b, blo = B * bs, bhi = std::min(blo + bs, total);
-      const int64_t cur = (B == nblocks_file - 1) ? last_len_file : S;
-      const int64_t slo = blo + static_cast<int64_t>(i) * cur, shi = std::min(slo + cur, bhi);
-      const int64_t a = std::max(slo, offset), e = std::min(shi, offset + length);
-      if (e > a) {
-        MEC_CUDA_OK(cudaMemcpyAsync(dst + (a - offset), base + b * spitch + (a - slo), static_cast<size_t>(e - a), cudaMemcpyDeviceToHost, s.st));
-        c->st_d2h += e - a;
+      const DataSlice sl = data_slice(rr.start_block + b, i, b == nb - 1 ? rr.last_len : S, bs, total, offset, offset + length);
+      if (sl.e > sl.a) {
+        MEC_CUDA_OK(cudaMemcpyAsync(dst + (sl.a - offset), base + b * spitch + sl.off, static_cast<size_t>(sl.e - sl.a), cudaMemcpyDeviceToHost, s.st));
+        c->st_d2h += sl.e - sl.a;
       }
     }
   }
@@ -1713,24 +1737,19 @@ extern "C" int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const u
   const int64_t S = c->S(), sfs = mec_shard_file_size(c, total);
   const int64_t nblocks = ceil_frac(sfs, S), last_len = sfs - (nblocks - 1) * S;
   Slot& s = c->slots[0];
-  struct Drain { Slot& s; ~Drain() { if (s.st) cudaStreamSynchronize(s.st); } } drain{s};
+  SlotDrain drain(s);
   const int64_t fpitch = round_up(sfs, 16) + 256, pitch = round_up(S, 16);
-  std::vector<uint8_t> alive(n), corrupt(n, 0);
-  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
-  int chosen[kMaxShards];
-  if ((rc = stage_verified_whole(c, files, sums, sfs, alive.data(), corrupt.data(), chosen, fpitch, s))) return rc;
-  std::vector<uint8_t> present(n, 0);
-  for (int t = 0; t < k; t++) present[chosen[t] & 0xffff] = 1;
-  int targets[kMaxShards], r = 0;
-  for (int i = 0; i < n; i++)
-    if (out_files[i] && !present[i]) targets[r++] = i;
-  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
+  std::vector<uint8_t> alive(n), corrupt(n, 0), want(n);
+  for (int i = 0; i < n; i++) { alive[i] = files[i] != nullptr; want[i] = out_files[i] != nullptr; }
+  int chosen[kMaxShards], pos[kMaxK];
+  if ((rc = stage_verified_whole(c, files, sums, sfs, alive.data(), corrupt.data(), chosen, pos, fpitch, s))) return rc;
+  DecodePlan p;
+  if ((rc = plan_decode(c, chosen, k, want.data(), 0, &p))) return rc;
+  const int r = p.r;
+  const int* targets = p.targets;
   if (r > 0) {
-    std::vector<uint8_t> rows(static_cast<size_t>(r) * k);
-    int valid[kMaxShards];
-    if (!rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
     if ((rc = s.out.ensure(static_cast<size_t>(nblocks * r * pitch)))) return rc;
-    if ((rc = launch_whole_rebuild(c, s, chosen, fpitch, S, last_len, 0, nblocks, nblocks, rows.data(), r, pitch))) return rc;
+    if ((rc = launch_whole_rebuild(c, s, pos, fpitch, S, last_len, 0, nblocks, p.rows.data(), r, pitch))) return rc;
     // rebuilt rows -> contiguous shard files on the device (for the whole-file hash), then files and sums go home
     if ((rc = s.src.ensure(static_cast<size_t>(r * fpitch + 256)))) return rc;
     if ((rc = s.dig.ensure(static_cast<size_t>((k + r) * 64)))) return rc;
@@ -1757,7 +1776,7 @@ extern "C" int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const u
   }
   // wanted shards that were read and verified are passed through
   for (int i = 0; i < n; i++)
-    if (out_files[i] && present[i] && out_files[i] != files[i]) {
+    if (out_files[i] && p.present[i] && out_files[i] != files[i]) {
       memcpy(out_files[i], files[i], static_cast<size_t>(sfs));
       if (out_sums) memcpy(out_sums + static_cast<size_t>(i) * 64, sums + static_cast<size_t>(i) * 64, 64);
     }
@@ -1820,21 +1839,24 @@ extern "C" int mec_rs_reconstruct_shards(mec_codec* c, uint8_t* const* shards, c
   if (np == n) return MEC_OK;
   if (np < k) return MEC_ERR_TOO_FEW_SHARDS;
   if (len >= (1ll << 31) || k > kMaxK) return MEC_ERR_UNSUPPORTED;
-  int targets[kMaxShards], r = 0;
-  for (int i = 0; i < n; i++)
-    if (!present[i] && !(data_only && i >= k)) targets[r++] = i;
+  // Reconstruct reads the first k present shards and rebuilds every missing one
+  int chosen[kMaxShards], nch = 0;
+  uint8_t want[kMaxShards];
+  for (int i = 0; i < n; i++) {
+    want[i] = !present[i];
+    if (present[i] && nch < k) chosen[nch++] = i;
+  }
+  DecodePlan p;
+  if (int rc = plan_decode(c, chosen, nch, want, data_only, &p)) return rc;
+  const int r = p.r;
   if (r == 0) return MEC_OK;
-  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
-  std::vector<uint8_t> rows(static_cast<size_t>(r) * k);
-  int valid[kMaxShards];
-  if (!rs_decode_rows(k, c->m, present, targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
   std::vector<const uint8_t*> in(k);
   std::vector<uint8_t*> outp(r);
-  for (int t = 0; t < k; t++) in[t] = shards[valid[t]];
-  for (int q = 0; q < r; q++) outp[q] = shards[targets[q]];
+  for (int t = 0; t < k; t++) in[t] = shards[chosen[t]];
+  for (int q = 0; q < r; q++) outp[q] = shards[p.targets[q]];
   std::lock_guard<std::mutex> lk(c->mu);
   if (int rc = ensure_engine(c)) return rc;
-  return apply_rows_host(c, rows.data(), r, in.data(), outp.data(), len, false);
+  return apply_rows_host(c, p.rows.data(), r, in.data(), outp.data(), len, false);
 }
 
 extern "C" int mec_hh256_batch(mec_codec* c, const uint8_t* msgs, int64_t msg_len, int64_t count, uint8_t* digests) {
@@ -1994,8 +2016,8 @@ extern "C" int mec_selftest(int device) {
 // launch that carries one 1 MiB block keeps one CTA busy on one of 132 SMs (H100) for as long as a launch of a thousand blocks takes.
 // The batcher turns concurrency into batch size: callers block in mec_batcher_encode*, a worker thread merges whatever is
 // queued (same k, m, block size by construction) into ONE staged buffer, ONE launch over all full blocks (plus one small
-// launch per short tail block), and one pass of DMA back into every caller's own frames; up to three merged batches are in
-// flight on the codec's three slots, so staging, kernel and copy-back of consecutive batches overlap.
+// launch per short tail block), and one pass of DMA back into every caller's own frames; up to six merged batches are in
+// flight on the codec's six slots, so staging, kernel and copy-back of consecutive batches overlap.
 #include <chrono>
 #include <condition_variable>
 #include <deque>
@@ -2196,8 +2218,8 @@ static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
   return MEC_OK;
 }
 
-// stage, launch and enqueue the copy-back of one merged batch on slot `s`
-static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, bool* needs_retire) {
+// stage, launch and enqueue the copy-back of one merged batch on slot `s`; *nblocks = the erasure blocks it encodes
+static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, bool* needs_retire, int64_t* nblocks) {
   mec_codec* c = b->codec;
   const int k = c->k, m = c->m, n = c->n;
   const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
@@ -2210,6 +2232,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     if (r->len % bs) { ntails++; tail_bytes += round_up(r->len % bs, 256); }
   }
   const int64_t nslots = total_full + ntails;
+  *nblocks = nslots;
   int rc;
   if ((rc = s.src.ensure(static_cast<size_t>(total_full * bs + tail_bytes + 512)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * std::max(m, 1) * pitch)))) return rc;
@@ -2331,10 +2354,6 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][3], s.st);
     *needs_retire = false;
     c->st_blocks_encoded += nslots;
-    b->st_batches++;
-    b->st_kernel_batches++;
-    b->st_requests += static_cast<int64_t>(reqs.size());
-    b->st_blocks += nslots;
     return MEC_OK;
   }
   for (BatchReq* r : reqs) {
@@ -2372,38 +2391,47 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   for (BatchReq* r : reqs)
     if ((rc = frames_enqueue(c, r->ch, r->files, r->with_data, r->data_digests))) return rc;
   c->st_blocks_encoded += nslots;
-  b->st_batches++;
-  b->st_requests += static_cast<int64_t>(reqs.size());
-  b->st_blocks += nslots;
-  (void)k;
   return MEC_OK;
 }
 
-// Merged GET and heal batches share their layout and their staging.  Layout: every request's full blocks first, the short last
-// blocks behind them; fills the request table and each request's placement in the batch.
+// Merged GET and heal batches share their plan, layout and staging.  Layout: every request's full blocks first, the short last
+// blocks behind them.
 struct ReadLayout {
   int64_t nfull_slots = 0, ntails = 0, max_nb = 0;
+  size_t table_bytes = 0;  // of the request table (s.hreq -> s.dreq)
   int64_t nslots() const { return nfull_slots + ntails; }
 };
-static ReadLayout batch_read_layout(mec_codec* c, Slot& s, std::vector<BatchReq*>& reqs, BatchGetDesc* tab) {
-  const int n = c->n;
+// The k readers of the batch's reader set and the decode plan of what it rebuilds: the data shards those readers miss for a GET,
+// the stale drives for a heal (disjoint from the readers: mec_batcher_heal sends the rest to the serial handle).  Fills the request
+// table in s.hreq — a heal's carries out_files[targets[q]] of request z at [z * r + q] behind the rows — each request's placement
+// in the batch, and gp.
+static int batch_read_plan(mec_codec* c, Slot& s, std::vector<BatchReq*>& reqs, DecodePlan& p, BatchGetParams& gp, ReadLayout& lay) {
+  const int k = c->k, n = c->n;
   const int64_t bs = c->block_size, S = c->S();
-  ReadLayout lay;
-  for (size_t q = 0; q < reqs.size(); q++) {
+  const BatchReq* lead = reqs.front();
+  const bool heal = lead->kind == 2;
+  int chosen[kMaxShards], nch = 0;
+  for (int i = 0; i < n && nch < k; i++)
+    if (lead->alive_mask & (1ull << i)) chosen[nch++] = i;
+  uint8_t stale[64] = {};
+  for (int i = 0; i < n && i < 64; i++) stale[i] = (lead->stale_mask >> i) & 1;
+  int rc = plan_decode(c, chosen, nch, heal ? stale : nullptr, !heal, &p);
+  if (rc) return rc;
+  const size_t nreq = reqs.size();
+  lay.table_bytes = nreq * sizeof(BatchGetDesc) + (heal ? nreq * std::max(p.r, 1) * sizeof(uint8_t*) : 0);
+  if ((rc = s.hreq.ensure(lay.table_bytes))) return rc;
+  if ((rc = s.dreq.ensure(lay.table_bytes))) return rc;
+  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
+  for (size_t q = 0; q < nreq; q++) {
     BatchReq* rq = reqs[q];
     BatchGetDesc& d = tab[q];
     memset(&d, 0, sizeof(d));
-    const int64_t sfs = mec_shard_file_size(c, rq->total), nblocks_total = ceil_frac(sfs, S);
-    const int64_t start_block = rq->offset / bs;
-    int64_t last_block = (rq->offset + rq->length) / bs;
-    if ((rq->offset + rq->length) % bs == 0) last_block--;
-    if (last_block >= nblocks_total) last_block = nblocks_total - 1;
-    const int64_t last_len = std::min(S, sfs - last_block * S);
+    const ReadRange rr = read_range(c, rq->offset, rq->length, rq->total);
     d.offset = rq->offset; d.length = rq->length; d.total = rq->total; d.dst = rq->dst;
     for (int i = 0; i < n; i++) d.files[i] = rq->gfiles[i];
-    d.start_block = start_block; d.nblocks = last_block - start_block + 1;
-    d.last_len = last_len;
-    const bool tail = last_len != S;
+    d.start_block = rr.start_block; d.nblocks = rr.nblocks;
+    d.last_len = rr.last_len;
+    const bool tail = rr.last_len != S;
     d.slot0 = lay.nfull_slots;
     lay.nfull_slots += d.nblocks - (tail ? 1 : 0);
     d.tail_slot = tail ? lay.ntails : -1;  // provisional: offset by the number of full slots below
@@ -2412,7 +2440,7 @@ static ReadLayout batch_read_layout(mec_codec* c, Slot& s, std::vector<BatchReq*
     rq->get_nblocks = d.nblocks;
   }
   static const int64_t dma_blocks = getenv("MEC_BATCHER_DMA_BLOCKS") ? atoll(getenv("MEC_BATCHER_DMA_BLOCKS")) : 1;
-  for (size_t q = 0; q < reqs.size(); q++) {
+  for (size_t q = 0; q < nreq; q++) {
     tab[q].dma = tab[q].nblocks >= dma_blocks ? 1 : 0;
     if (tab[q].tail_slot >= 0) tab[q].tail_slot += lay.nfull_slots;
     reqs[q]->get_slot0 = tab[q].slot0;
@@ -2420,18 +2448,32 @@ static ReadLayout batch_read_layout(mec_codec* c, Slot& s, std::vector<BatchReq*
     reqs[q]->ch = EncChunk();
     reqs[q]->ch.s = &s;
   }
-  return lay;
+  if (heal) {
+    uint8_t** outs = reinterpret_cast<uint8_t**>(tab + nreq);
+    for (size_t z = 0; z < nreq; z++)
+      for (int q = 0; q < p.r; q++) outs[z * p.r + q] = reqs[z]->outs[p.targets[q]];
+  }
+  memset(&gp, 0, sizeof(gp));
+  gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.p);
+  gp.nreq = static_cast<int>(nreq); gp.k = k; gp.r = p.r;
+  for (int t = 0; t < k; t++) gp.chosen[t] = chosen[t];
+  for (int q = 0; q < p.r; q++) gp.targets[q] = p.targets[q];
+  gp.bs = bs; gp.S = S; gp.P = round_up(32 + S, 16); gp.pitch = round_up(S, 16);
+  return MEC_OK;
 }
 
-// Survivor frames of every block of every request -> the slot's arena, the fused reconstruct of gp.targets over all of them, and the
-// per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table gp.reqs points at; gp holds the geometry, reader
-// set and targets, and gets the arena and rebuilt rows here.
+// The request table to the device, survivor frames of every block of every request -> the slot's arena, the fused reconstruct of
+// gp.targets over all of them, and the per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table gp.reqs
+// points at; gp holds the geometry, reader set and targets, and gets the arena and rebuilt rows here.
 static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* tab, BatchGetParams& gp, const uint8_t* rows,
                                   const ReadLayout& lay, bool hash_outputs) {
   mec_codec* c = b->codec;
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
   const int64_t stride = round_up(nslots * P + 512, 256);
+  const int phase_slot = static_cast<int>(&s - c->slots);
+  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
+  MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, lay.table_bytes, cudaMemcpyHostToDevice, s.st));
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(nslots * std::max(r, 1) * pitch)))) return rc;
@@ -2472,7 +2514,6 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
   }
-  const int phase_slot = static_cast<int>(&s - c->slots);
   if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
   MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
   const int32_t* block_len = nullptr;
@@ -2514,31 +2555,16 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
 
 // one merged launch for the GETs of a batch that share a reader set (alive mask): gather kernel -> fused reconstruct over all full
 // blocks (+ one launch per short last block) -> scatter kernel into every caller's destination
-static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs) {
+static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
-  const int k = c->k, n = c->n;
-  const int64_t bs = c->block_size, S = c->S(), P = round_up(32 + S, 16), pitch = round_up(S, 16);
-  // reader set and decode rows of the shared pattern
-  int chosen[kMaxShards], nch = 0;
-  const uint64_t mask = reqs.front()->alive_mask;
-  for (int i = 0; i < n && nch < k; i++)
-    if (mask & (1ull << i)) chosen[nch++] = i;
-  if (nch < k) return MEC_ERR_READ_QUORUM;
-  std::vector<uint8_t> present(n, 0);
-  for (int t = 0; t < k; t++) present[chosen[t]] = 1;
-  int targets[kMaxShards], r = 0;
-  for (int i = 0; i < k; i++)
-    if (!present[i]) targets[r++] = i;
-  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
-  std::vector<uint8_t> rows(static_cast<size_t>(std::max(r, 1)) * k);
-  int valid[kMaxShards];
-  if (r > 0 && !rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
-  int rc;
-  if ((rc = s.hreq.ensure(reqs.size() * sizeof(BatchGetDesc)))) return rc;
-  if ((rc = s.dreq.ensure(reqs.size() * sizeof(BatchGetDesc)))) return rc;
+  DecodePlan p;
+  BatchGetParams gp;
+  ReadLayout lay;
+  int rc = batch_read_plan(c, s, reqs, p, gp, lay);
+  if (rc) return rc;
+  const int k = gp.k, r = gp.r;
+  const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
   BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
-  const ReadLayout lay = batch_read_layout(c, s, reqs, tab);
-  const int64_t nslots = lay.nslots();
   // writeDataBlocks: 0 = the scatter kernel assembles every object in device memory and ONE copy per request takes it to the caller
   // (fewest driver-side copy descriptors), 1 = the scatter kernel stores straight into the callers' buffers over PCIe, 2 = the copy
   // engine moves every (request, shard, block) piece itself
@@ -2550,17 +2576,7 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
     if ((rc = s.src.ensure(static_cast<size_t>(total + 256)))) return rc;
     for (size_t q = 0; q < reqs.size(); q++) tab[q].dst = static_cast<uint8_t*>(s.src.p) + asm_off[q];
   }
-  const int phase_slot = static_cast<int>(&s - c->slots);
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
-  MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, reqs.size() * sizeof(BatchGetDesc), cudaMemcpyHostToDevice, s.st));
-  BatchGetParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.p);
-  gp.nreq = static_cast<int>(reqs.size()); gp.k = k; gp.r = r;
-  for (int t = 0; t < k; t++) gp.chosen[t] = chosen[t];
-  for (int q = 0; q < r; q++) gp.targets[q] = targets[q];
-  gp.bs = bs; gp.S = S; gp.P = P; gp.pitch = pitch;
-  if ((rc = batch_read_reconstruct(b, s, tab, gp, rows.data(), lay, false))) return rc;  // GetObject reads no digest of rebuilt data
+  if ((rc = batch_read_reconstruct(b, s, tab, gp, p.rows.data(), lay, false))) return rc;  // GetObject reads no digest of rebuilt data
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
   const int64_t stride = gp.arena_stride;
   if (out_mode == 2) {
@@ -2569,21 +2585,18 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
     std::vector<size_t> sizes;
     int tpos[kMaxShards], qpos[kMaxShards];
     for (int i = 0; i < k; i++) { tpos[i] = qpos[i] = -1; }
-    for (int t = 0; t < k; t++) if (chosen[t] < k) tpos[chosen[t]] = t;
-    for (int q = 0; q < r; q++) qpos[targets[q]] = q;
+    for (int t = 0; t < k; t++) if (gp.chosen[t] < k) tpos[gp.chosen[t]] = t;
+    for (int q = 0; q < r; q++) qpos[gp.targets[q]] = q;
     for (size_t rq = 0; rq < reqs.size(); rq++) {
       const BatchGetDesc& d = tab[rq];
-      const int64_t hi = d.offset + d.length;
       for (int64_t bb = 0; bb < d.nblocks; bb++) {
         const bool is_tail = d.tail_slot >= 0 && bb == d.nblocks - 1;
         const int64_t cur = is_tail ? d.last_len : S, slot = is_tail ? d.tail_slot : d.slot0 + bb;
-        const int64_t B = d.start_block + bb, blo = B * bs, bhi = std::min(blo + bs, d.total);
         for (int i = 0; i < k; i++) {
-          const int64_t slo = blo + static_cast<int64_t>(i) * cur, shi = std::min(slo + cur, bhi);
-          const int64_t a = std::max(slo, d.offset), e = std::min(shi, hi);
-          if (e <= a) continue;
+          const DataSlice sl = data_slice(d.start_block + bb, i, cur, gp.bs, d.total, d.offset, d.offset + d.length);
+          if (sl.e <= sl.a) continue;
           const uint8_t* src = tpos[i] >= 0 ? gp.arena + tpos[i] * stride + slot * P + 32 : gp.rebuilt + (slot * r + qpos[i]) * pitch;
-          dsts.push_back(d.dst + (a - d.offset)); srcs.push_back(const_cast<uint8_t*>(src) + (a - slo)); sizes.push_back(static_cast<size_t>(e - a));
+          dsts.push_back(d.dst + (sl.a - d.offset)); srcs.push_back(const_cast<uint8_t*>(src) + sl.off); sizes.push_back(static_cast<size_t>(sl.e - sl.a));
         }
       }
     }
@@ -2602,13 +2615,10 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
       if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
     }
   }
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][3], s.st);
+  if (b->trace) cudaEventRecord(b->ev_ph[&s - c->slots][3], s.st);
   c->st_blocks_read += nslots;
   c->st_shards_rebuilt += nslots * r;
-  b->st_batches++;
-  b->st_kernel_batches++;
-  b->st_requests += static_cast<int64_t>(reqs.size());
-  b->st_blocks += nslots;
+  *nblocks = nslots;
   return MEC_OK;
 }
 
@@ -2616,59 +2626,27 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
 // reconstruct of every stale shard, data and parity, with its digest (ONE latency launch when the batch is small enough, otherwise
 // one over all full blocks plus one per short last block) -> the heal scatter kernel writes the healed frames into every caller's
 // part-file images
-static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs) {
+static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
-  const int k = c->k, n = c->n;
-  const int64_t S = c->S(), P = round_up(32 + S, 16), pitch = round_up(S, 16);
-  // the k chosen readers and the stale drives of the batch's key (disjoint: mec_batcher_heal sends the rest to the serial handle)
-  int chosen[kMaxShards], nch = 0, targets[kMaxShards], r = 0;
-  const uint64_t rmask = reqs.front()->alive_mask, smask = reqs.front()->stale_mask;
-  std::vector<uint8_t> present(n, 0);
-  for (int i = 0; i < n; i++) {
-    if (rmask & (1ull << i)) { chosen[nch++] = i; present[i] = 1; }
-    if (smask & (1ull << i)) targets[r++] = i;
-  }
-  if (nch != k) return MEC_ERR_READ_QUORUM;
-  if (r > kMaxR) return MEC_ERR_UNSUPPORTED;
-  std::vector<uint8_t> rows(static_cast<size_t>(std::max(r, 1)) * k);
-  int valid[kMaxShards];
-  if (r > 0 && !rs_decode_rows(k, c->m, present.data(), targets, r, rows.data(), valid)) return MEC_ERR_TOO_FEW_SHARDS;
-  // device table: the requests' BatchGetDesc rows, then out_files[targets[q]] of request z at [z * r + q]
-  const size_t tab_bytes = reqs.size() * sizeof(BatchGetDesc), all_bytes = tab_bytes + reqs.size() * std::max(r, 1) * sizeof(uint8_t*);
-  int rc;
-  if ((rc = s.hreq.ensure(all_bytes))) return rc;
-  if ((rc = s.dreq.ensure(all_bytes))) return rc;
-  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
-  const ReadLayout lay = batch_read_layout(c, s, reqs, tab);
-  const int64_t nslots = lay.nslots();
-  uint8_t** outs = reinterpret_cast<uint8_t**>(static_cast<uint8_t*>(s.hreq.p) + tab_bytes);
-  for (size_t z = 0; z < reqs.size(); z++)
-    for (int q = 0; q < r; q++) outs[z * r + q] = reqs[z]->outs[targets[q]];
-  const int phase_slot = static_cast<int>(&s - c->slots);
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
-  MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, s.hreq.p, all_bytes, cudaMemcpyHostToDevice, s.st));
+  DecodePlan p;
   BatchGetParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.p);
-  gp.nreq = static_cast<int>(reqs.size()); gp.k = k; gp.r = r;
-  for (int t = 0; t < k; t++) gp.chosen[t] = chosen[t];
-  for (int q = 0; q < r; q++) gp.targets[q] = targets[q];
-  gp.bs = c->block_size; gp.S = S; gp.P = P; gp.pitch = pitch;
-  if ((rc = batch_read_reconstruct(b, s, tab, gp, rows.data(), lay, true))) return rc;
+  ReadLayout lay;
+  int rc = batch_read_plan(c, s, reqs, p, gp, lay);
+  if (rc) return rc;
+  const int r = gp.r;
+  const int64_t nslots = lay.nslots();
+  if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, p.rows.data(), lay, true))) return rc;
   if (r > 0) {
     const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
     batch_heal_scatter_kernel<<<dim3(gx, static_cast<unsigned>(r), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(
-        gp, static_cast<const uint8_t*>(s.dig.p), reinterpret_cast<uint8_t* const*>(static_cast<uint8_t*>(s.dreq.p) + tab_bytes));
+        gp, static_cast<const uint8_t*>(s.dig.p), reinterpret_cast<uint8_t* const*>(gp.reqs + gp.nreq));
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
   }
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][3], s.st);
+  if (b->trace) cudaEventRecord(b->ev_ph[&s - c->slots][3], s.st);
   c->st_blocks_read += nslots;
   c->st_shards_rebuilt += nslots * r;
-  b->st_batches++;
-  b->st_kernel_batches++;
-  b->st_requests += static_cast<int64_t>(reqs.size());
-  b->st_blocks += nslots;
+  *nblocks = nslots;
   return MEC_OK;
 }
 
@@ -2729,28 +2707,36 @@ static void batcher_main(mec_batcher* b) {
     }
     if (!reqs.empty()) {
       Slot& s = c->slots[head];
+      InflightBatch& fb = inflight[head];
       int rc;
+      int64_t nblocks = 0;
       const auto t_submit = clk::now();
       {
         std::lock_guard<std::mutex> lk(c->mu);
-        inflight[head].is_get = reqs.front()->kind != 0;
-        inflight[head].get_k = c->k;
-        if (inflight[head].is_get) {
-          rc = reqs.front()->kind == 2 ? batcher_submit_heal(b, s, reqs) : batcher_submit_get(b, s, reqs);
+        fb.is_get = reqs.front()->kind != 0;
+        fb.get_k = c->k;
+        if (fb.is_get) {
+          rc = reqs.front()->kind == 2 ? batcher_submit_heal(b, s, reqs, &nblocks) : batcher_submit_get(b, s, reqs, &nblocks);
           if (rc != MEC_OK)
             for (BatchReq* r : reqs) r->ch.s = &s;  // batcher_finish looks the slot up through the first request
         } else {
-          rc = batcher_submit(b, s, reqs, &inflight[head].needs_retire);
+          rc = batcher_submit(b, s, reqs, &fb.needs_retire, &nblocks);
         }
       }
       b->us_submit += us_since(t_submit);
-      inflight[head].reqs = reqs;
-      inflight[head].busy = true;
-      inflight[head].traced = b->trace && rc == MEC_OK && (inflight[head].is_get || !inflight[head].needs_retire);
+      fb.reqs = reqs;
+      fb.busy = true;
+      // a batch the kernels carry end to end: every GET or heal batch, a PUT batch unless it took the memcpy path
+      const bool kernel_batch = fb.is_get || !fb.needs_retire;
+      fb.traced = b->trace && rc == MEC_OK && kernel_batch;
       if (rc != MEC_OK) {  // drain what was enqueued before the failure, then fail the whole batch
         cudaStreamSynchronize(s.st);
-        batcher_finish(b, inflight[head], rc);
+        batcher_finish(b, fb, rc);
       } else {
+        b->st_batches++;
+        if (kernel_batch) b->st_kernel_batches++;
+        b->st_requests += static_cast<int64_t>(reqs.size());
+        b->st_blocks += nblocks;
         head = (head + 1) % kSlots;
         nbusy++;
       }
@@ -2881,6 +2867,19 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
   delete b;
 }
 
+// Queues `r` for the worker and waits until its batch is done.  A PUT wakes the worker only as the first arrival or as the one that
+// fills a batch, not as every caller; a GET or heal always wakes it.
+static int64_t batcher_enqueue_wait(mec_batcher* b, BatchReq& r) {
+  std::unique_lock<std::mutex> lk(b->mu);
+  if (b->stop) return MEC_ERR_INVALID_ARGUMENT;
+  b->queue.push_back(&r);
+  if (r.kind != 0 || b->queue.size() == 1 ||
+      static_cast<int64_t>(b->queue.size()) * std::max<int64_t>(1, r.len / b->codec->block_size) >= b->max_blocks)
+    b->cv_work.notify_one();
+  r.cv.wait(lk, [&] { return r.done; });
+  return r.result;
+}
+
 static int64_t batcher_call(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests, bool with_data,
                             int write_quorum, int crc_which = 0, uint64_t* crc_out = nullptr) {
   if (!b || len < 0 || !files || (len > 0 && !src)) return MEC_ERR_INVALID_ARGUMENT;
@@ -2902,13 +2901,7 @@ static int64_t batcher_call(mec_batcher* b, const uint8_t* src, int64_t len, uin
   r.mapped = mec_is_pinned(src) && (!data_digests || mec_is_pinned(data_digests));
   for (int i = 0; i < b->codec->n && r.mapped; i++)
     if (files[i] && (i >= b->codec->k || with_data)) r.mapped = mec_is_pinned(files[i]) != 0;
-  std::unique_lock<std::mutex> lk(b->mu);
-  if (b->stop) return MEC_ERR_INVALID_ARGUMENT;
-  b->queue.push_back(&r);
-  if (b->queue.size() == 1 || static_cast<int64_t>(b->queue.size()) * std::max<int64_t>(1, len / b->codec->block_size) >= b->max_blocks)
-    b->cv_work.notify_one();  // the worker is woken by the first arrival and by the one that fills the batch, not by every caller
-  r.cv.wait(lk, [&] { return r.done; });
-  return r.result;
+  return batcher_enqueue_wait(b, r);
 }
 extern "C" int64_t mec_batcher_encode(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, int write_quorum) {
   return batcher_call(b, src, len, files, nullptr, true, write_quorum);
@@ -2954,12 +2947,7 @@ extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* file
     mec_codec* sc = batcher_serial(b);
     return sc ? mec_decode_prefer(sc, files, nullptr, offset, length, total, dst, heal_hint) : MEC_ERR_UNEXPECTED;
   }
-  std::unique_lock<std::mutex> lk(b->mu);
-  if (b->stop) return MEC_ERR_INVALID_ARGUMENT;
-  b->queue.push_back(&r);
-  b->cv_work.notify_one();
-  r.cv.wait(lk, [&] { return r.done; });
-  return r.result;
+  return batcher_enqueue_wait(b, r);
 }
 
 // Erasure.Heal (cmd/erasure-decode.go:317) through the coalescer: heals queued together that read the same k drives and rebuild the
@@ -3000,12 +2988,7 @@ extern "C" int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, con
     }
   // a drive that is read and also rewritten is passed through unchanged by reconstruct_range: the serial path does that
   if (!mapped || (r.alive_mask & r.stale_mask) != 0 || nstale > kMaxR) return serial();
-  std::unique_lock<std::mutex> lk(b->mu);
-  if (b->stop) return MEC_ERR_INVALID_ARGUMENT;
-  b->queue.push_back(&r);
-  b->cv_work.notify_one();
-  r.cv.wait(lk, [&] { return r.done; });
-  return static_cast<int>(r.result);
+  return static_cast<int>(batcher_enqueue_wait(b, r));
 }
 
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
