@@ -182,12 +182,24 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
  * device staging for all six is allocated here (about 2.4 x max_batch_blocks x block_size each).
  * mec_batcher_stat: "batches", "requests", "blocks", "kernel_batches" (batches moved by the gather / scatter kernels), "redone"
  * (merged GETs and heals that met a frame failing its digest check and were redone on their own), "crc_requests" (PUTs through
- * mec_batcher_encode_crc with a non-empty mask that got their checksums), "launches";
+ * mec_batcher_encode_crc with a non-empty mask that got their checksums), "launches", "patterns" (distinct erasure patterns — reader
+ * set plus rebuilt shards — summed over GET and heal batches) and "mixed_batches" (GET and heal batches of more than one pattern);
  * with MEC_BATCHER_TRACE=1 in the environment also the worker's and the streams' accumulated phase times "us_submit", "us_sync",
  * "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter".  Any other name is answered by mec_get_stat on the batcher's own
  * codec, so "form_*", "last_*", "small_launches", "num_sms" and the rest describe the merged launches. */
 typedef struct mec_batcher mec_batcher;
 int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out);
+/* mec_batcher_new with creation flags (mec_batcher_new is flags = 0); unknown bits return MEC_ERR_INVALID_ARGUMENT.
+ * MEC_BATCHER_MIX_PATTERNS: GETs merge with GETs and heals with heals whatever drives they read and rebuild.  MinIO rotates every
+ * object's shard indices over the drives (hashOrder, cmd/erasure-metadata-utils.go:178, applied by getObjectWithFileInfo and
+ * healObject: cmd/erasure-object.go:313, cmd/erasure-healing.go:501,511), so with one drive offline or stale, concurrent reads of
+ * different objects rarely share a reader set or a stale set, and without the flag they split into one batch per pattern.  With
+ * it a batch of several patterns is ONE launch of the latency kernel, every erasure block with its own decode matrix; such a batch
+ * is cut at the blocks one latency launch takes (5 per SM), and a single request larger than that keeps a batch of its own.  A
+ * codec whose options rule out the latency kernel ignores the flag. */
+#define MEC_BATCHER_MIX_PATTERNS 1
+int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
+                       mec_batcher** out);
 void mec_batcher_free(mec_batcher* b);
 int64_t mec_batcher_encode(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, int write_quorum);
 int64_t mec_batcher_encode_sg(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
@@ -207,9 +219,16 @@ int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, int64_t len, 
  * that meets a corrupt frame is redone on its own with parallelReader's exact fail-over; pageable buffers take the same private path. */
 int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* files, int64_t offset, int64_t length, int64_t total_length,
                            uint8_t* dst, int* heal_hint);
+/* getObjectWithFileInfo's Erasure.Decode with `prefer` (local drives first, cmd/erasure-object.go:387) through the coalescer:
+ * arguments and results of mec_decode_prefer; prefer == NULL is mec_batcher_decode.  With `prefer` the readers are chosen on the
+ * caller's thread exactly as mec_decode_prefer chooses them, and GETs that read the same k drives share a launch (any GETs on a
+ * batcher created with MEC_BATCHER_MIX_PATTERNS).  A request that meets a corrupt frame is redone on its own through
+ * mec_decode_prefer with the same `prefer`. */
+int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
+                                  int64_t total_length, uint8_t* dst, int* heal_hint);
 /* Erasure.Heal (cmd/erasure-decode.go:317) through the coalescer (arguments and results of mec_heal_prefer): heals queued together
  * that read the same k drives (the ones parallelReader picks for `files` and `prefer`) and rebuild the same stale drives (out_files[i]
- * != NULL) are merged into one fused launch, and one scatter kernel writes every healed frame into every caller's out files.  A
+ * != NULL) are merged into one fused launch (any heals with MEC_BATCHER_MIX_PATTERNS), and one scatter kernel writes every healed frame into every caller's out files.  A
  * request whose chosen readers fail a digest check is redone on its own through mec_heal_prefer (MEC_ERR_FILE_CORRUPT, corrupt[]
  * filled, counted in "redone"); pageable buffers, a drive that is both a reader and stale, and sets of more than 32 drives take that
  * private path directly. */

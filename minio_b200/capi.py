@@ -10,6 +10,7 @@ ERRORS = {-1: "ErrInvShardNum", -2: "ErrMaxShardNum", -3: "ErrTooFewShards", -4:
           -6: "ErrShortData", -7: "errFileCorrupt", -8: "errLessData", -9: "errUnexpected", -10: "errErasureReadQuorum",
           -11: "errErasureWriteQuorum", -12: "errInvalidArgument", -100: "CUDA error", -101: "no CUDA device",
           -102: "unsupported on the GPU path"}
+MIX_PATTERNS = 1  # MEC_BATCHER_MIX_PATTERNS
 
 _LIB = None
 
@@ -60,6 +61,7 @@ def lib():
     L.mec_encode_sg.argtypes = [vp, vp, i64, vp, vp, i32]
     L.mec_heal_prefer.argtypes = [vp, vp, vp, i64, vp, vp]
     L.mec_batcher_new.argtypes = [i32, i32, i64, i32, i64, i32, C.POINTER(vp)]
+    L.mec_batcher_new_ex.argtypes = [i32, i32, i64, i32, i64, i32, i32, C.POINTER(vp)]
     L.mec_batcher_free.argtypes = [vp]
     L.mec_batcher_free.restype = None
     L.mec_batcher_encode.restype = i64
@@ -70,6 +72,8 @@ def lib():
     L.mec_batcher_encode_crc.argtypes = [vp, vp, i64, vp, vp, i32, i32, vp]
     L.mec_batcher_decode.restype = i64
     L.mec_batcher_decode.argtypes = [vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
+    L.mec_batcher_decode_prefer.restype = i64
+    L.mec_batcher_decode_prefer.argtypes = [vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_batcher_heal.argtypes = [vp, vp, vp, i64, vp, vp]
     L.mec_batcher_stat.restype = i64
     L.mec_batcher_stat.argtypes = [vp, C.c_char_p]
@@ -416,13 +420,15 @@ class Codec:
 
 class Batcher:
     """mec_batcher: concurrent PutObject calls of one geometry merged into shared launches.  encode() may be called from many
-    threads at once (ctypes releases the GIL for the duration of the call)."""
+    threads at once (ctypes releases the GIL for the duration of the call).  mix_patterns=True (MEC_BATCHER_MIX_PATTERNS): GETs
+    and heals of different erasure patterns (reader sets, stale sets) share batches."""
 
-    def __init__(self, k, m, block_size=1 << 20, device=0, max_batch_blocks=256, max_wait_us=200):
+    def __init__(self, k, m, block_size=1 << 20, device=0, max_batch_blocks=256, max_wait_us=200, mix_patterns=False):
         h = C.c_void_p()
-        rc = lib().mec_batcher_new(k, m, block_size, device, max_batch_blocks, max_wait_us, C.byref(h))
+        rc = lib().mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, MIX_PATTERNS if mix_patterns else 0,
+                                      C.byref(h))
         if rc:
-            raise MecError(rc, "mec_batcher_new")
+            raise MecError(rc, "mec_batcher_new_ex")
         self.h, self.k, self.m, self.n, self.block_size = h, k, m, k + m, block_size
         self._sizes = Codec(k, m, block_size, device=device)
 
@@ -473,16 +479,18 @@ class Batcher:
             raise MecError(rc, "mec_batcher_encode_sg")
         return [f if i >= self.k else None for i, f in enumerate(files)], dd[:nb]
 
-    def decode(self, files, offset, length, total, dst=None):
-        """mec_batcher_decode: files = part-file arrays (None = offline); pass page-locked arrays (and a page-locked dst) to ride in
-        merged launches.  -> (bytes, heal_hint)"""
+    def decode(self, files, offset, length, total, dst=None, prefer=None):
+        """mec_batcher_decode_prefer: files = part-file arrays (None = offline); pass page-locked arrays (and a page-locked dst) to
+        ride in merged launches.  prefer = n flags (preferReaders), None = mec_batcher_decode.  -> (bytes, heal_hint)"""
         files = [None if f is None else _u8(f) for f in files]
         if dst is None:
             dst = np.zeros(max(length, 1), dtype=np.uint8)
         hint = C.c_int(0)
-        rc = lib().mec_batcher_decode(self.h, _ptrs(files), offset, length, total, dst.ctypes.data, C.byref(hint))
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        rc = lib().mec_batcher_decode_prefer(self.h, _ptrs(files), None if pf is None else pf.ctypes.data, offset, length, total,
+                                             dst.ctypes.data, C.byref(hint))
         if rc < 0:
-            raise MecError(rc, "mec_batcher_decode")
+            raise MecError(rc, "mec_batcher_decode_prefer")
         return dst[:length], hint.value
 
     def heal(self, files, stale, total, prefer=None, pinned=False):

@@ -129,7 +129,7 @@ __global__ void __launch_bounds__(128) batch_scatter_kernel(const BatchCopyParam
 
 }  // namespace mec
 
-// ---- degraded / plain GETs of many requests that share one reader set ------------------------------------------------------
+// ---- degraded / plain GETs of many requests, each with its own reader set -----------------------------------------------------
 namespace mec {
 
 struct BatchGetDesc {
@@ -142,13 +142,16 @@ struct BatchGetDesc {
   int64_t last_len;                      // shard length of that block
   int32_t dma;                           // 1: the copy engines stage this request's frames (long ranges), the gather kernel skips it
   int32_t pad;
+  // the request's decode plan (a batch of one erasure pattern: the same for every request)
+  int8_t chosen[32];                     // reader set (ascending shard indices), arena position t -> shard
+  int8_t targets[16];                    // rebuilt shards (GET: the data shards not read; heal: the stale drives), output row q -> shard
+  int32_t r;                             // targets of this request (<= BatchGetParams::r)
+  int32_t pattern;                       // its plan in the launch's pattern table
 };
 
 struct BatchGetParams {
   const BatchGetDesc* reqs;
-  int nreq, k, r;
-  int32_t chosen[32];                    // reader set (ascending shard indices), position t -> shard
-  int32_t targets[16];                   // rebuilt shards (GET: data only; heal: the stale drives), output row q -> shard
+  int nreq, k, r;                        // r: the most targets of any request (rows per slot of `rebuilt`, digests per slot k + r)
   int64_t bs, S, P;                      // block size, full shard size, device frame pitch
   uint8_t* arena;                        // survivors: reader position t at arena + t*arena_stride, slot s at + s*P
   int64_t arena_stride;
@@ -156,7 +159,7 @@ struct BatchGetParams {
   int64_t pitch;
 };
 
-__device__ __forceinline__ int64_t get_slot(const BatchGetDesc& r, int64_t b) {
+__host__ __device__ __forceinline__ int64_t get_slot(const BatchGetDesc& r, int64_t b) {
   return (r.tail_slot >= 0 && b == r.nblocks - 1) ? r.tail_slot : r.slot0 + b;
 }
 
@@ -165,7 +168,7 @@ __global__ void __launch_bounds__(128) batch_get_gather_kernel(const BatchGetPar
   const BatchGetDesc& r = p.reqs[blockIdx.z];
   if (r.dma) return;
   const int t = blockIdx.y;
-  const uint8_t* f = r.files[p.chosen[t]];
+  const uint8_t* f = r.files[r.chosen[t]];
   const int64_t fstride = 32 + p.S;
   __shared__ __align__(16) uint8_t stage[kStageBytes + 32];
   for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
@@ -181,8 +184,8 @@ __global__ void __launch_bounds__(128) batch_get_scatter_kernel(const BatchGetPa
   const BatchGetDesc& r = p.reqs[blockIdx.z];
   const int i = blockIdx.y;
   int t = -1, q = -1;
-  for (int x = 0; x < p.k; x++) if (p.chosen[x] == i) t = x;
-  for (int x = 0; x < p.r; x++) if (p.targets[x] == i) q = x;
+  for (int x = 0; x < p.k; x++) if (r.chosen[x] == i) t = x;
+  for (int x = 0; x < r.r; x++) if (r.targets[x] == i) q = x;
   if (t < 0 && q < 0) return;
   const int64_t hi = r.offset + r.length;
   for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
@@ -199,11 +202,12 @@ __global__ void __launch_bounds__(128) batch_get_scatter_kernel(const BatchGetPa
 
 // grid (block stride, r rebuilt shards, nreq): healed frames of every stale drive of every request — multiWriter{writeQuorum: 1} +
 // streamingBitrotWriter.Write (cmd/erasure-decode.go:317-366, cmd/bitrot-streaming.go:57-69): [digest of the rebuilt shard][shard]
-// at frame b of outs[req * r + q], the part's short last frame 32 + last_len bytes.  Digests [slot][k + r][32] (outputs behind
+// at frame b of outs[req * r + q] (r = the batch's most stale drives, q < the request's own), the part's short last frame 32 + last_len bytes.  Digests [slot][k + r][32] (outputs behind
 // the k inputs), rebuilt rows (slot * r + q) * pitch.  Nothing outside a frame is written.
 __global__ void __launch_bounds__(128) batch_heal_scatter_kernel(const BatchGetParams p, const uint8_t* digests, uint8_t* const* outs) {
   const BatchGetDesc& r = p.reqs[blockIdx.z];
   const int q = blockIdx.y;
+  if (q >= r.r) return;
   uint8_t* f = outs[static_cast<int64_t>(blockIdx.z) * p.r + q];
   const int64_t fstride = 32 + p.S;
   for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {

@@ -2021,6 +2021,7 @@ extern "C" int mec_selftest(int device) {
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <unordered_map>
 
 struct BatchReq {
   int kind = 0;                      // 0 = PutObject (encode), 1 = GetObject (decode), 2 = Heal
@@ -2029,10 +2030,10 @@ struct BatchReq {
   int64_t offset = 0, length = 0, total = 0;
   uint8_t* dst = nullptr;
   int* heal_hint = nullptr;
-  uint64_t alive_mask = 0;           // bit i = reader i is online (heal: one of the k chosen readers): equal masks share a launch
+  uint64_t alive_mask = 0;           // bit i = reader i is online (heal, GET with `prefer`: one of the k chosen readers)
   int64_t get_slot0 = 0, get_tail_slot = -1, get_nblocks = 0;  // placement of the request's blocks in the merged batch
+  const uint8_t* prefer = nullptr;   // preferReaders (cmd/erasure-decode.go:92-123), for the redo of a request that met bitrot
   // heal
-  const uint8_t* prefer = nullptr;
   uint8_t* const* outs = nullptr;
   uint8_t* corrupt = nullptr;
   uint64_t stale_mask = 0;           // bit i = out_files[i] != NULL: heals share a launch only with the same stale drives
@@ -2051,6 +2052,13 @@ struct BatchReq {
   EncChunk ch;   // placement inside the merged batch
 };
 
+// The decode plan of one erasure pattern of merged reads: the host plan and the latency kernel's per-block table entry
+struct BatchPattern {
+  DecodePlan plan;
+  SmallPattern sp;
+};
+constexpr size_t kMaxCachedPatterns = 4096;
+
 struct mec_batcher {
   mec_codec* codec = nullptr;
   mec_codec* serial = nullptr;       // private handle for calls that cannot ride in a batch (pageable buffers, bitrot fail-over)
@@ -2065,6 +2073,12 @@ struct mec_batcher {
   std::atomic<int64_t> st_batches{0}, st_requests{0}, st_blocks{0}, st_kernel_batches{0};
   std::atomic<int64_t> st_redone{0};  // merged GETs and heals that met a frame failing its digest and were redone on their own
   std::atomic<int64_t> st_crc_requests{0};  // PUTs that got their object checksums (mec_batcher_encode_crc)
+  // MEC_BATCHER_MIX_PATTERNS (and a codec whose options allow the latency kernel): GETs merge with GETs and heals with heals
+  // whatever their reader and stale sets, as long as a batch of several erasure patterns fits one latency launch
+  bool mix = false;
+  std::atomic<int64_t> st_patterns{0}, st_mixed{0};  // distinct patterns summed over read batches; read batches of more than one
+  // decode plans by (reader mask, target mask), owned by the worker thread: a steady workload inverts no matrix
+  std::unordered_map<uint64_t, BatchPattern> patterns;
   // hybrid staging: part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
   cudaStream_t aux = nullptr;
   cudaEvent_t ev_table[kSlots] = {}, ev_gather[kSlots] = {};
@@ -2117,7 +2131,7 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
           mec_codec* sc = batcher_serial(b);
           if (!sc) res = MEC_ERR_UNEXPECTED;
           else if (heal) res = mec_heal_prefer(sc, r->gfiles, r->prefer, r->total, r->outs, r->corrupt);
-          else res = mec_decode_prefer(sc, r->gfiles, nullptr, r->offset, r->length, r->total, r->dst, r->heal_hint);
+          else res = mec_decode_prefer(sc, r->gfiles, r->prefer, r->offset, r->length, r->total, r->dst, r->heal_hint);
         } else if (r->heal_hint) {
           *r->heal_hint = 0;
         }
@@ -2399,26 +2413,73 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
 struct ReadLayout {
   int64_t nfull_slots = 0, ntails = 0, max_nb = 0;
   size_t table_bytes = 0;  // of the request table (s.hreq -> s.dreq)
+  int npat = 0;            // distinct erasure patterns of the batch
+  const uint8_t* rows = nullptr;  // npat == 1: the r x k decode rows of that pattern
+  size_t pat_off = 0, bp_off = 0; // npat > 1: SmallPattern[npat] and the uint16_t pattern of every slot, offsets in the table
   int64_t nslots() const { return nfull_slots + ntails; }
 };
-// The k readers of the batch's reader set and the decode plan of what it rebuilds: the data shards those readers miss for a GET,
-// the stale drives for a heal (disjoint from the readers: mec_batcher_heal sends the rest to the serial handle).  Fills the request
-// table in s.hreq — a heal's carries out_files[targets[q]] of request z at [z * r + q] behind the rows — each request's placement
-// in the batch, and gp.
-static int batch_read_plan(mec_codec* c, Slot& s, std::vector<BatchReq*>& reqs, DecodePlan& p, BatchGetParams& gp, ReadLayout& lay) {
+// Every request's reader set — the first k readers of its alive mask — and the decode plan of what it rebuilds: the data shards
+// those readers miss for a GET, the stale drives for a heal (disjoint from the readers: mec_batcher_heal sends the rest to the
+// serial handle).  Fills the request table in s.hreq — a heal's carries out_files[targets[q]] of request z at [z * gp.r + q] behind
+// the rows; a batch of several patterns then the pattern table and the per-slot pattern index — each request's placement in the
+// batch, and gp (gp.r = the most targets of any request).
+static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, BatchGetParams& gp, ReadLayout& lay) {
+  mec_codec* c = b->codec;
   const int k = c->k, n = c->n;
   const int64_t bs = c->block_size, S = c->S();
-  const BatchReq* lead = reqs.front();
-  const bool heal = lead->kind == 2;
-  int chosen[kMaxShards], nch = 0;
-  for (int i = 0; i < n && nch < k; i++)
-    if (lead->alive_mask & (1ull << i)) chosen[nch++] = i;
-  uint8_t stale[64] = {};
-  for (int i = 0; i < n && i < 64; i++) stale[i] = (lead->stale_mask >> i) & 1;
-  int rc = plan_decode(c, chosen, nch, heal ? stale : nullptr, !heal, &p);
-  if (rc) return rc;
+  const bool heal = reqs.front()->kind == 2;
   const size_t nreq = reqs.size();
-  lay.table_bytes = nreq * sizeof(BatchGetDesc) + (heal ? nreq * std::max(p.r, 1) * sizeof(uint8_t*) : 0);
+  if (b->patterns.size() + nreq > kMaxCachedPatterns) b->patterns.clear();  // pointers into the cache stay valid for this batch
+  std::vector<const BatchPattern*> pats;
+  std::vector<uint64_t> pat_keys;
+  std::vector<int> req_pat(nreq);
+  std::vector<ReadRange> rrs(nreq);
+  int rmax = 0;
+  int64_t nslots = 0;
+  for (size_t q = 0; q < nreq; q++) {
+    const BatchReq* rq = reqs[q];
+    uint64_t rmask = 0;
+    for (int i = 0, cnt = 0; i < n && cnt < k; i++)
+      if ((rq->alive_mask >> i) & 1) { rmask |= 1ull << i; cnt++; }
+    const uint64_t tmask = heal ? rq->stale_mask : (~rmask & ((1ull << k) - 1));
+    const uint64_t key = rmask | (tmask << 32);  // n <= kBatchMaxFiles = 32
+    int pi = 0;
+    while (pi < static_cast<int>(pats.size()) && pat_keys[pi] != key) pi++;
+    if (pi == static_cast<int>(pats.size())) {
+      auto it = b->patterns.find(key);
+      if (it == b->patterns.end()) {
+        BatchPattern bp;
+        int chosen[kMaxShards], nch = 0;
+        uint8_t want[kMaxShards] = {};
+        for (int i = 0; i < n; i++) {
+          if ((rmask >> i) & 1) chosen[nch++] = i;
+          want[i] = (tmask >> i) & 1;
+        }
+        int rc = plan_decode(c, chosen, nch, want, 0, &bp.plan);
+        if (rc) return rc;
+        memset(&bp.sp, 0, sizeof(bp.sp));
+        bp.sp.r = bp.plan.r;
+        for (int j = 0; j < bp.plan.r; j++)
+          for (int t = 0; t < k; t++) bp.sp.coef[j][t] = bp.plan.rows[static_cast<size_t>(j) * k + t];
+        it = b->patterns.emplace(key, std::move(bp)).first;
+      }
+      pats.push_back(&it->second);
+      pat_keys.push_back(key);
+      rmax = std::max(rmax, it->second.plan.r);
+    }
+    req_pat[q] = pi;
+    rrs[q] = read_range(c, rq->offset, rq->length, rq->total);
+    nslots += rrs[q].nblocks;
+  }
+  lay.npat = static_cast<int>(pats.size());
+  lay.rows = lay.npat == 1 ? pats[0]->plan.rows.data() : nullptr;
+  lay.table_bytes = nreq * sizeof(BatchGetDesc) + (heal ? nreq * std::max(rmax, 1) * sizeof(uint8_t*) : 0);
+  if (lay.npat > 1) {
+    lay.pat_off = round_up(static_cast<int64_t>(lay.table_bytes), 16);
+    lay.bp_off = lay.pat_off + pats.size() * sizeof(SmallPattern);
+    lay.table_bytes = lay.bp_off + static_cast<size_t>(nslots) * sizeof(uint16_t);
+  }
+  int rc;
   if ((rc = s.hreq.ensure(lay.table_bytes))) return rc;
   if ((rc = s.dreq.ensure(lay.table_bytes))) return rc;
   BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
@@ -2426,11 +2487,17 @@ static int batch_read_plan(mec_codec* c, Slot& s, std::vector<BatchReq*>& reqs, 
     BatchReq* rq = reqs[q];
     BatchGetDesc& d = tab[q];
     memset(&d, 0, sizeof(d));
-    const ReadRange rr = read_range(c, rq->offset, rq->length, rq->total);
+    const ReadRange& rr = rrs[q];
     d.offset = rq->offset; d.length = rq->length; d.total = rq->total; d.dst = rq->dst;
     for (int i = 0; i < n; i++) d.files[i] = rq->gfiles[i];
     d.start_block = rr.start_block; d.nblocks = rr.nblocks;
     d.last_len = rr.last_len;
+    const DecodePlan& pl = pats[req_pat[q]]->plan;
+    for (int i = 0, t = 0; i < n; i++)
+      if (pl.present[i]) d.chosen[t++] = static_cast<int8_t>(i);
+    for (int j = 0; j < pl.r; j++) d.targets[j] = static_cast<int8_t>(pl.targets[j]);
+    d.r = pl.r;
+    d.pattern = req_pat[q];
     const bool tail = rr.last_len != S;
     d.slot0 = lay.nfull_slots;
     lay.nfull_slots += d.nblocks - (tail ? 1 : 0);
@@ -2451,22 +2518,29 @@ static int batch_read_plan(mec_codec* c, Slot& s, std::vector<BatchReq*>& reqs, 
   if (heal) {
     uint8_t** outs = reinterpret_cast<uint8_t**>(tab + nreq);
     for (size_t z = 0; z < nreq; z++)
-      for (int q = 0; q < p.r; q++) outs[z * p.r + q] = reqs[z]->outs[p.targets[q]];
+      for (int q = 0; q < tab[z].r; q++) outs[z * rmax + q] = reqs[z]->outs[tab[z].targets[q]];
+  }
+  if (lay.npat > 1) {
+    uint8_t* base = static_cast<uint8_t*>(s.hreq.p);
+    SmallPattern* sp = reinterpret_cast<SmallPattern*>(base + lay.pat_off);
+    for (int pi = 0; pi < lay.npat; pi++) sp[pi] = pats[pi]->sp;
+    uint16_t* bp = reinterpret_cast<uint16_t*>(base + lay.bp_off);
+    for (size_t q = 0; q < nreq; q++)
+      for (int64_t bb = 0; bb < tab[q].nblocks; bb++) bp[get_slot(tab[q], bb)] = static_cast<uint16_t>(req_pat[q]);
   }
   memset(&gp, 0, sizeof(gp));
   gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.p);
-  gp.nreq = static_cast<int>(nreq); gp.k = k; gp.r = p.r;
-  for (int t = 0; t < k; t++) gp.chosen[t] = chosen[t];
-  for (int q = 0; q < p.r; q++) gp.targets[q] = p.targets[q];
+  gp.nreq = static_cast<int>(nreq); gp.k = k; gp.r = rmax;
   gp.bs = bs; gp.S = S; gp.P = round_up(32 + S, 16); gp.pitch = round_up(S, 16);
   return MEC_OK;
 }
 
 // The request table to the device, survivor frames of every block of every request -> the slot's arena, the fused reconstruct of
-// gp.targets over all of them, and the per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table gp.reqs
-// points at; gp holds the geometry, reader set and targets, and gets the arena and rebuilt rows here.
-static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* tab, BatchGetParams& gp, const uint8_t* rows,
-                                  const ReadLayout& lay, bool hash_outputs) {
+// every request's targets over all of them, and the per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table
+// gp.reqs points at; gp holds the geometry and gets the arena and rebuilt rows here.  A batch of several erasure patterns is ONE
+// latency launch with a decode plan per block (batcher_main only merges such a batch when its blocks fit one).
+static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* tab, BatchGetParams& gp, const ReadLayout& lay,
+                                  bool hash_outputs) {
   mec_codec* c = b->codec;
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
@@ -2495,7 +2569,7 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
       if (!d.dma) continue;
       const int64_t nf = d.nblocks - (d.tail_slot >= 0 ? 1 : 0);
       for (int t = 0; t < k; t++) {
-        const uint8_t* f = d.files[gp.chosen[t]] + d.start_block * fstride;
+        const uint8_t* f = d.files[d.chosen[t]] + d.start_block * fstride;
         uint8_t* a = gp.arena + t * stride;
         for (int64_t j = 0; j < nf; j++) {
           dsts.push_back(a + (d.slot0 + j) * P); srcs.push_back(const_cast<uint8_t*>(f) + j * fstride); sizes.push_back(static_cast<size_t>(fstride));
@@ -2517,10 +2591,16 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
   if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
   MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
   const int32_t* block_len = nullptr;
+  const bool mixed = lay.npat > 1;
+  const uint8_t* dtab = static_cast<const uint8_t*>(s.dreq.p);
   auto launch = [&](int64_t slot0, int64_t cnt, int64_t shard_len) -> int {
     FusedDesc d;
     d.block_len = block_len;
-    d.k = k; d.r = r; d.coef = rows; d.static_encode = false; d.contiguous = false; d.hash_outputs = hash_outputs;
+    if (mixed) {
+      d.patterns = reinterpret_cast<const SmallPattern*>(dtab + lay.pat_off);
+      d.block_pattern = reinterpret_cast<const uint16_t*>(dtab + lay.bp_off);
+    }
+    d.k = k; d.r = r; d.coef = lay.rows; d.static_encode = false; d.contiguous = false; d.hash_outputs = hash_outputs;
     d.key = kMagicKey; d.out_pitch = pitch; d.expect_block_stride = P; d.in_block_stride = P;
     d.nblocks = cnt; d.S = static_cast<int32_t>(shard_len);
     for (int t = 0; t < k; t++) {
@@ -2532,7 +2612,10 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0 * k;
     return c->eng->launch_fused(d, c->opt, s.st);
   };
-  if (lay.ntails > 0 && c->eng->small_ok(c->opt, nslots)) {
+  if (mixed && !c->eng->small_ok(c->opt, nslots)) return MEC_ERR_UNSUPPORTED;
+  if (mixed && lay.ntails == 0) {
+    if ((rc = launch(0, nslots, S))) return rc;
+  } else if (lay.ntails > 0 && c->eng->small_ok(c->opt, nslots)) {
     // ONE launch for every block of every caller, the short last ones included (per-block shard lengths in the latency kernel)
     if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
     if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
@@ -2550,6 +2633,12 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
   }
   MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
   if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][2], s.st);
+  b->st_patterns += lay.npat;
+  if (mixed) b->st_mixed++;
+  int64_t rebuilt = 0;
+  for (int q = 0; q < gp.nreq; q++) rebuilt += tab[q].nblocks * tab[q].r;
+  c->st_blocks_read += nslots;
+  c->st_shards_rebuilt += rebuilt;
   return MEC_OK;
 }
 
@@ -2557,10 +2646,9 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
 // blocks (+ one launch per short last block) -> scatter kernel into every caller's destination
 static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
-  DecodePlan p;
   BatchGetParams gp;
   ReadLayout lay;
-  int rc = batch_read_plan(c, s, reqs, p, gp, lay);
+  int rc = batch_read_plan(b, s, reqs, gp, lay);
   if (rc) return rc;
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
@@ -2576,7 +2664,7 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
     if ((rc = s.src.ensure(static_cast<size_t>(total + 256)))) return rc;
     for (size_t q = 0; q < reqs.size(); q++) tab[q].dst = static_cast<uint8_t*>(s.src.p) + asm_off[q];
   }
-  if ((rc = batch_read_reconstruct(b, s, tab, gp, p.rows.data(), lay, false))) return rc;  // GetObject reads no digest of rebuilt data
+  if ((rc = batch_read_reconstruct(b, s, tab, gp, lay, false))) return rc;  // GetObject reads no digest of rebuilt data
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
   const int64_t stride = gp.arena_stride;
   if (out_mode == 2) {
@@ -2584,11 +2672,11 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
     std::vector<void*> dsts, srcs;
     std::vector<size_t> sizes;
     int tpos[kMaxShards], qpos[kMaxShards];
-    for (int i = 0; i < k; i++) { tpos[i] = qpos[i] = -1; }
-    for (int t = 0; t < k; t++) if (gp.chosen[t] < k) tpos[gp.chosen[t]] = t;
-    for (int q = 0; q < r; q++) qpos[gp.targets[q]] = q;
     for (size_t rq = 0; rq < reqs.size(); rq++) {
       const BatchGetDesc& d = tab[rq];
+      for (int i = 0; i < k; i++) { tpos[i] = qpos[i] = -1; }
+      for (int t = 0; t < k; t++) if (d.chosen[t] < k) tpos[d.chosen[t]] = t;
+      for (int q = 0; q < d.r; q++) qpos[d.targets[q]] = q;
       for (int64_t bb = 0; bb < d.nblocks; bb++) {
         const bool is_tail = d.tail_slot >= 0 && bb == d.nblocks - 1;
         const int64_t cur = is_tail ? d.last_len : S, slot = is_tail ? d.tail_slot : d.slot0 + bb;
@@ -2616,8 +2704,6 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
     }
   }
   if (b->trace) cudaEventRecord(b->ev_ph[&s - c->slots][3], s.st);
-  c->st_blocks_read += nslots;
-  c->st_shards_rebuilt += nslots * r;
   *nblocks = nslots;
   return MEC_OK;
 }
@@ -2628,14 +2714,13 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
 // part-file images
 static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
-  DecodePlan p;
   BatchGetParams gp;
   ReadLayout lay;
-  int rc = batch_read_plan(c, s, reqs, p, gp, lay);
+  int rc = batch_read_plan(b, s, reqs, gp, lay);
   if (rc) return rc;
   const int r = gp.r;
   const int64_t nslots = lay.nslots();
-  if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, p.rows.data(), lay, true))) return rc;
+  if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, lay, true))) return rc;
   if (r > 0) {
     const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
     batch_heal_scatter_kernel<<<dim3(gx, static_cast<unsigned>(r), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(
@@ -2644,8 +2729,6 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
     c->eng->count_launch();
   }
   if (b->trace) cudaEventRecord(b->ev_ph[&s - c->slots][3], s.st);
-  c->st_blocks_read += nslots;
-  c->st_shards_rebuilt += nslots * r;
   *nblocks = nslots;
   return MEC_OK;
 }
@@ -2682,7 +2765,8 @@ static void batcher_main(mec_batcher* b) {
         if (nbusy == 0 && b->max_wait_us > 0 && blocks_queued() < b->max_blocks)
           b->cv_work.wait_for(lk, std::chrono::microseconds(b->max_wait_us), [&] { return b->stop || blocks_queued() >= b->max_blocks; });
         // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs and heals, the same reader
-        // set; for heals also the same stale drives)
+        // set; for heals also the same stale drives — unless b->mix: then reads of other patterns join while the batch's blocks fit
+        // one latency launch, and a batch of several patterns is cut at that limit)
         // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.45 ms however few
         // blocks it is given (one warp walks one erasure block), so the copy of one batch has to overlap the kernel of another —
         // otherwise a closed loop of callers falls into a convoy (all of them in one batch, the GPU idle while they wake up)
@@ -2692,13 +2776,23 @@ static void batcher_main(mec_batcher* b) {
           const int64_t q = blocks_queued();
           if (q > 8) cap = std::min(cap, std::max<int64_t>(4, ceil_frac(q, depth - nbusy)));
         }
-        int64_t nb = 0;
+        int64_t nb = 0, nread = 0;
+        bool mixed = false;
         const BatchReq* lead = b->queue.front();
+        const bool mix = b->mix && lead->kind != 0;
+        const int64_t limit = std::min<int64_t>(c->eng->small_limit(c->opt), 1 << 16);  // block_pattern holds uint16_t indices
         for (auto it = b->queue.begin(); it != b->queue.end();) {
           BatchReq* r = *it;
-          if (r->kind != lead->kind || r->alive_mask != lead->alive_mask || r->stale_mask != lead->stale_mask) { ++it; continue; }
+          const bool same = r->alive_mask == lead->alive_mask && r->stale_mask == lead->stale_mask;
+          if (r->kind != lead->kind || (!same && !mix)) { ++it; continue; }
           const int64_t rb = req_blocks(r);
           if (!reqs.empty() && nb + rb > cap) break;
+          if (mix) {  // the exact blocks of the read
+            const int64_t rs = read_range(c, r->offset, r->length, r->total).nblocks;
+            if ((mixed || !same) && nread + rs > limit) break;
+            mixed |= !same;
+            nread += rs;
+          }
           reqs.push_back(r);
           it = b->queue.erase(it);
           nb += rb;
@@ -2768,9 +2862,11 @@ static void batcher_main(mec_batcher* b) {
 }
 }  // namespace
 
-extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out) {
+extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
+                                  mec_batcher** out) {
   if (!out) return MEC_ERR_INVALID_ARGUMENT;
   *out = nullptr;
+  if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;
   mec_codec* c = nullptr;
   int rc = mec_codec_new(k, m, block_size, MEC_HIGHWAYHASH256S, device, &c);
   if (rc) return rc;
@@ -2782,6 +2878,7 @@ extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int
   if (c->S() >= (1ll << 31)) { mec_codec_free(c); return MEC_ERR_UNSUPPORTED; }
   mec_batcher* b = new mec_batcher;
   b->codec = c;
+  b->mix = (flags & MEC_BATCHER_MIX_PATTERNS) && c->eng->small_ok(c->opt, 1);  // per-block decode plans exist in the latency kernel only
   if (max_batch_blocks > 0) b->max_blocks = max_batch_blocks;
   // a merged batch stages at most 1 GiB of object bytes: six slots are sized for a full batch up front (below)
   b->max_blocks = std::max<int64_t>(1, std::min<int64_t>(b->max_blocks, (1ll << 30) / std::max<int64_t>(block_size, 1)));
@@ -2802,10 +2899,12 @@ extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int
       if (rc == MEC_OK) rc = s.aux.ensure(static_cast<size_t>(k * round_up(slots * P + 512, 256)));
       if (rc == MEC_OK) rc = s.flags.ensure(static_cast<size_t>(slots * k));
       if (rc == MEC_OK) rc = s.hflags.ensure(static_cast<size_t>(slots * k));
-      // request tables: PUT rows, or GET rows, or GET rows plus one out-file pointer per rebuilt shard (heal)
-      const size_t row = std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc) + kMaxR * sizeof(uint8_t*));
-      if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * row);
-      if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * row);
+      // request tables: PUT rows, or GET rows, or GET rows plus one out-file pointer per rebuilt shard (heal); reads of several
+      // erasure patterns add a pattern (at most one per request) and a pattern index per block
+      const size_t row = std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc) + kMaxR * sizeof(uint8_t*) +
+                                                            (b->mix ? sizeof(SmallPattern) + sizeof(uint16_t) : 0));
+      if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * row + 16);
+      if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * row + 16);
       // object checksums (batcher_crc_enqueue): a batch of at most `slots` requests and slots x block_size bytes has at most
       // slots x block_size / kCrcRegion whole regions plus two partial ones (full-block segment, short block) per request
       const int64_t nwork = ceil_frac(slots * block_size, kCrcRegion) + 2 * slots;
@@ -2845,6 +2944,9 @@ extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int
   b->worker = std::thread(batcher_main, b);
   *out = b;
   return MEC_OK;
+}
+extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out) {
+  return mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, 0, out);
 }
 
 extern "C" void mec_batcher_free(mec_batcher* b) {
@@ -2917,10 +3019,11 @@ extern "C" int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, in
   if (which && !out3) return MEC_ERR_INVALID_ARGUMENT;
   return batcher_call(b, src, len, files, data_digests, data_digests == nullptr, write_quorum, which, out3);
 }
-// Erasure.Decode through the coalescer: GETs that are queued together and see the same drives online are merged into one launch.
+// Erasure.Decode through the coalescer: GETs that are queued together and read the same drives are merged into one launch — without
+// `prefer` the same drives online, with it the same k readers parallelReader picks; with MEC_BATCHER_MIX_PATTERNS any reads.
 // Calls whose buffers are not page-locked, and calls that meet bitrot, run on their own through a private handle.
-extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* files, int64_t offset, int64_t length, int64_t total,
-                                      uint8_t* dst, int* heal_hint) {
+extern "C" int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset,
+                                             int64_t length, int64_t total, uint8_t* dst, int* heal_hint) {
   if (heal_hint) *heal_hint = 0;
   if (!b || !files) return MEC_ERR_INVALID_ARGUMENT;
   if (offset < 0 || length < 0 || offset + length > total) return MEC_ERR_INVALID_ARGUMENT;  // cmd/erasure-decode.go:240-245
@@ -2930,24 +3033,41 @@ extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* file
   const int n = c->n, k = c->k;
   BatchReq r;
   r.kind = 1; r.gfiles = files; r.offset = offset; r.length = length; r.total = total; r.dst = dst; r.heal_hint = heal_hint;
+  r.prefer = prefer;
   bool mapped = n <= kBatchMaxFiles && n <= 64 && k <= 32 && mec_is_pinned(dst) != 0;
-  int online = 0;
-  for (int i = 0; i < n; i++) {
-    if (!files[i]) continue;
-    online++;
-    if (i < 64) r.alive_mask |= 1ull << i;
-  }
-  if (online < k) return MEC_ERR_READ_QUORUM;
-  {  // only the k readers that will be used have to be mapped
-    int cnt = 0;
-    for (int i = 0; i < n && cnt < k && mapped; i++)
+  if (prefer && n <= kBatchMaxFiles) {
+    // the readers parallelReader picks (preferReaders, cmd/erasure-decode.go:92-123), chosen here on the caller's thread: the
+    // request's key is that reader set (a k-bit mask equals an alive mask only when exactly those k drives are online)
+    uint8_t alive[kBatchMaxFiles];
+    int chosen[kBatchMaxFiles];
+    for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
+    const int nch = choose_readers(c, files, alive, prefer, chosen);
+    if (nch < k) return MEC_ERR_READ_QUORUM;
+    for (int t = 0; t < k; t++) {
+      r.alive_mask |= 1ull << chosen[t];
+      mapped = mapped && mec_is_pinned(files[chosen[t]]) != 0;
+    }
+  } else {
+    int online = 0;
+    for (int i = 0; i < n; i++) {
+      if (!files[i]) continue;
+      online++;
+      if (i < 64) r.alive_mask |= 1ull << i;
+    }
+    if (online < k) return MEC_ERR_READ_QUORUM;
+    // only the k readers that will be used have to be mapped
+    for (int i = 0, cnt = 0; i < n && cnt < k && mapped; i++)
       if (files[i]) { mapped = mec_is_pinned(files[i]) != 0; cnt++; }
   }
   if (!mapped || getenv("MEC_BATCHER_MEMCPY") != nullptr) {
     mec_codec* sc = batcher_serial(b);
-    return sc ? mec_decode_prefer(sc, files, nullptr, offset, length, total, dst, heal_hint) : MEC_ERR_UNEXPECTED;
+    return sc ? mec_decode_prefer(sc, files, prefer, offset, length, total, dst, heal_hint) : MEC_ERR_UNEXPECTED;
   }
   return batcher_enqueue_wait(b, r);
+}
+extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* files, int64_t offset, int64_t length, int64_t total,
+                                      uint8_t* dst, int* heal_hint) {
+  return mec_batcher_decode_prefer(b, files, nullptr, offset, length, total, dst, heal_hint);
 }
 
 // Erasure.Heal (cmd/erasure-decode.go:317) through the coalescer: heals queued together that read the same k drives and rebuild the
@@ -2999,6 +3119,8 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "kernel_batches")) return b->st_kernel_batches.load();
   if (!strcmp(name, "redone")) return b->st_redone.load();
   if (!strcmp(name, "crc_requests")) return b->st_crc_requests.load();
+  if (!strcmp(name, "patterns")) return b->st_patterns.load();
+  if (!strcmp(name, "mixed_batches")) return b->st_mixed.load();
   if (!strcmp(name, "launches")) return b->codec->eng ? b->codec->eng->launches() : 0;
   if (!strcmp(name, "us_submit")) return b->us_submit.load();
   if (!strcmp(name, "us_sync")) return b->us_sync.load();

@@ -603,7 +603,8 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
   if (d.static_encode && d.contiguous && d.hash_outputs && !opt.force_dynamic)
     for (const auto& ent : kStaticTable)
       if (ent.k == d.k && ent.m == d.r) se = &ent;
-  if (!se) {
+  if (d.block_pattern != nullptr && (se || d.patterns == nullptr)) return MEC_ERR_INVALID_ARGUMENT;
+  if (!se && d.block_pattern == nullptr) {
     if (d.r > 0 && d.coef == nullptr) return MEC_ERR_INVALID_ARGUMENT;
     for (int j = 0; j < d.r; j++)
       for (int t = 0; t < d.k; t++) {
@@ -624,6 +625,8 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
       p.in_shard_step = d.contiguous ? d.S : 0;
       p.block_len = d.block_len;
       p.blocks = d.blocks;
+      p.patterns = d.patterns;
+      p.block_pattern = d.block_pattern;
       p.tail_block = d.tail_block; p.tail_in_off = d.tail_in_off; p.tail_S = d.tail_S; p.tail_bytes = d.tail_bytes;
       const int gw = small_gf_warps(n);
       const SmallFn sfn = se ? se->small : kDynSmall[gw - 3][d.r <= 1 ? 0 : (d.r == 2 ? 1 : 2)];
@@ -649,7 +652,8 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
     }
   }
 
-  if (d.block_len != nullptr || d.blocks != nullptr || d.tail_block >= 0) return MEC_ERR_UNSUPPORTED;  // per-block geometry exists in the latency kernel only
+  // per-block geometry and per-block decode plans exist in the latency kernel only
+  if (d.block_len != nullptr || d.blocks != nullptr || d.tail_block >= 0 || d.block_pattern != nullptr) return MEC_ERR_UNSUPPORTED;
   p.tail_block = -1;
 
   // ---- input addressing + loader choice.  TMA boxes must start on 16-byte boundaries, so each row is

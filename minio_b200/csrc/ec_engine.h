@@ -47,6 +47,9 @@ struct FusedDesc {
   const uint8_t* key = nullptr;    // 32-byte HighwayHash key (host)
   const int32_t* block_len = nullptr;  // device: per-block shard bytes (<= S); only launches that take the latency kernel (see small_ok)
   const SmallBlock* blocks = nullptr;  // device, contiguous encode: per-block geometry relative to in_base; S = the largest shard length
+  // device, latency kernel only: per-block decode plans (r = the largest plan's rows; coef may then be nullptr)
+  const SmallPattern* patterns = nullptr;
+  const uint16_t* block_pattern = nullptr;  // one entry per block: its plan in `patterns`
   // one block of the launch is an object's short last block (latency kernel only, see small_ok): no table needed
   int64_t tail_block = -1, tail_in_off = -1;  // index; contiguous encode: byte offset from in_base (rows tail_S apart)
   int32_t tail_S = 0, tail_bytes = 0;

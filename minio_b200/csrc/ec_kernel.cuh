@@ -58,6 +58,13 @@ struct SmallBlock {
   int32_t bytes;    // object bytes in the block (Split pads the rest of k * S with zeros)
 };
 
+// latency kernel, runtime matrix: the decode plan of one erasure pattern — reads of many objects whose shard indices are rotated
+// differently (hashOrder, cmd/erasure-metadata-utils.go:178) ride in ONE launch, each block with its own matrix
+struct SmallPattern {
+  int32_t r;                     // rows this pattern rebuilds (<= the launch's r); 0: hash and verify only
+  uint8_t coef[kMaxR][kMaxK];    // r x k decode rows
+};
+
 struct FusedParams {
   int k, r, eb, tma_mode;
   int tiles_3d;                    // ROWS3D: tiles [0, tiles_3d) of a shard are fetched with one 3-D request
@@ -84,6 +91,8 @@ struct FusedParams {
   uint32_t* work_counter;          // optional: groups beyond the first of every CTA are claimed from this counter (zeroed per launch)
   const int32_t* block_len;        // latency kernel only: shard bytes of every erasure block (nullptr: S for all) — frames of many files in one launch
   const SmallBlock* blocks;        // latency kernel only, contiguous encode: per-block offset / shard bytes / object bytes (nullptr: uniform)
+  const SmallPattern* patterns;    // latency kernel only, runtime matrix: decode plans of the launch (nullptr: coef / r for all blocks)
+  const uint16_t* block_pattern;   // ... and the index of every block's plan in `patterns`
   // latency kernel only: ONE block of the launch (an object's short last block) differs from the rest — no table needed
   int64_t tail_block;              // its index, -1 = none
   int64_t tail_in_off;             // contiguous encode: bytes from in_ptr[0] to its first byte (rows S_tail apart); -1: rows addressed like the others

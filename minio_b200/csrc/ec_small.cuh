@@ -71,6 +71,16 @@ __global__ void __launch_bounds__(256, 2) small_rs_hh_kernel(const __grid_consta
   const bool is_tail = p.tail_block == b;
   const int32_t S = p.blocks != nullptr ? p.blocks[b].S : (p.block_len != nullptr ? p.block_len[b] : (is_tail ? p.tail_S : p.S));
   const int nst = (S + kSmallSuper - 1) / kSmallSuper;
+  // a launch of mixed erasure patterns: this block's own decode plan.  The launch's r (the largest of its plans) sizes shared
+  // memory, the digest and output layouts; only rows j < br are computed, stored and hashed here
+  int br = r;
+  const SmallPattern* pat = nullptr;
+  if constexpr (!GF::kIsStatic) {
+    if (p.block_pattern != nullptr) {
+      pat = p.patterns + p.block_pattern[b];
+      br = pat->r;
+    }
+  }
 
   if (tid == 0) {
     mbar_init(smem_u32(&bars[0]), kSmallGfThreads);
@@ -99,7 +109,7 @@ __global__ void __launch_bounds__(256, 2) small_rs_hh_kernel(const __grid_consta
   if constexpr (!GF::kIsStatic) {
     for (int i = tid; i < k * rpad * 8; i += blockDim.x) {
       const int bit = i & 7, j = (i >> 3) % rpad, t = (i >> 3) / rpad;
-      const uint32_t c = j < r ? p.coef[j][t] : 0u;
+      const uint32_t c = j < br ? (pat != nullptr ? pat->coef[j][t] : p.coef[j][t]) : 0u;
       s_masks[i] = 0u - ((c >> bit) & 1u);
     }
   }
@@ -164,7 +174,7 @@ __global__ void __launch_bounds__(256, 2) small_rs_hh_kernel(const __grid_consta
         }
       } else {
         constexpr int RC = GF::RC;
-        for (int j0 = 0; j0 < (r > 0 ? r : 1); j0 += RC) {
+        for (int j0 = 0; j0 < (br > 0 ? br : 1); j0 += RC) {
           uint32_t pl[RC][8], ph[RC][8];
 #pragma unroll
           for (int j = 0; j < RC; j++)
@@ -174,7 +184,7 @@ __global__ void __launch_bounds__(256, 2) small_rs_hh_kernel(const __grid_consta
           for (int t = 0; t < k; t++) {
             const uint2 v = load_col_rt(rcol + t * kSmallRawPitch, static_cast<uint32_t>(rows[t].lead));
             if (j0 == 0) *reinterpret_cast<uint2*>(ccol + t * kSmallRowPitch) = v;
-            if (r == 0) continue;
+            if (br == 0) continue;
             const uint4* mk = reinterpret_cast<const uint4*>(s_masks + (t * rpad + j0) * 8);
 #pragma unroll
             for (int j = 0; j < RC; j++) {
@@ -191,7 +201,7 @@ __global__ void __launch_bounds__(256, 2) small_rs_hh_kernel(const __grid_consta
           }
 #pragma unroll
           for (int j = 0; j < RC; j++) {
-            if (j0 + j >= r) break;
+            if (j0 + j >= br) break;
             uint32_t al = pl[j][7], ah = ph[j][7];
 #pragma unroll
             for (int q = 6; q >= 0; q--) {
@@ -210,7 +220,9 @@ __global__ void __launch_bounds__(256, 2) small_rs_hh_kernel(const __grid_consta
 
   // -------------------------------------------------------------------- hash warps: two lanes per stream
   const int s = tid >> 1, h = tid & 1;
-  const int nhash = GF::kHashOut == 1 ? nstreams : (GF::kHashOut == 0 ? k : p.nhash);
+  int nhash = GF::kHashOut == 1 ? nstreams : (GF::kHashOut == 0 ? k : p.nhash);
+  if constexpr (!GF::kIsStatic)
+    if (pat != nullptr && nhash > k) nhash = k + br;
   const bool live = p.digests != nullptr && s < nhash;
   const bool is_out = s >= k;
   HHHalf hs;

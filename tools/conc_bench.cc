@@ -7,6 +7,10 @@
 //   mode get     : degraded GETs (4 data drives offline) through the pool
 //   mode bheal   : heals of one stale data drive (Erasure.Heal, the MRF / new-disk traffic) through ONE mec_batcher
 //   mode heal    : the same heals, each a mec_heal_prefer call on a handle from the pool
+//   mode bget_rot / bheal_rot : bget / bheal as MinIO lays objects out: thread t's object has its shard indices rotated by t % n over
+//                  the drives (hashOrder, cmd/erasure-metadata-utils.go:178), and ONE physical drive (drive 0) is offline (GET) or
+//                  stale (heal) — so the shard it held rotates from object to object: n erasure patterns in every round of requests
+//   MIX=1        : the batcher of the b* modes is created with MEC_BATCHER_MIX_PATTERNS (reads of different patterns share batches)
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
 // Prints one JSON line: aggregate GiB/s, calls/s, p50/p99 latency.  Buffers are pinned (mec_alloc_pinned_on) for the GPU modes.
 // Build: g++ -O2 -std=c++17 tools/conc_bench.cc -o tools/conc_bench -Iinclude -Lminio_b200 -lminio_ec -Loracle -loracle -lpthread
@@ -51,6 +55,10 @@ int main(int argc, char** argv) {
   signal(SIGSEGV, on_segv);
   signal(SIGABRT, on_segv);
   std::string mode = argc > 1 ? argv[1] : "batcher";
+  const bool rot = mode == "bget_rot" || mode == "bheal_rot";
+  if (rot) mode.resize(mode.size() - 4);
+  const std::string mode_name = rot ? mode + "_rot" : mode;
+  const int bflags = getenv("MIX") && atoi(getenv("MIX")) ? MEC_BATCHER_MIX_PATTERNS : 0;
   const int T = argc > 2 ? atoi(argv[2]) : 256;
   // object size: MiB, or KiB with a 'k' suffix (objects smaller than one erasure block: "256k")
   const std::string osz = argc > 3 ? argv[3] : "1";
@@ -87,7 +95,8 @@ int main(int argc, char** argv) {
   mec_batcher* bat = nullptr;
   std::vector<mec_codec*> pool;
   if (mode == "batcher" || mode == "batcher_crc") {
-    int rc = mec_batcher_new(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, &bat);
+    int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
+                                bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
   } else if (gpu && mode != "bget" && mode != "bheal") {
     for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
@@ -99,7 +108,8 @@ int main(int argc, char** argv) {
       if (mec_encode(c0, tb[t].obj, osize, f.data(), k) != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
     }
     mec_codec_free(c0);
-    int rc = mec_batcher_new(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, &bat);
+    int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
+                                bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
   }
   if (mode == "get" || mode == "heal") {  // every thread's part files must exist first
@@ -111,6 +121,8 @@ int main(int argc, char** argv) {
   std::atomic<int> ready{0}, go{0};
   std::atomic<int64_t> errors{0};
   std::vector<std::vector<double>> lat(T);
+  // the shard index physical drive 0 holds for thread t's object: its rotation is t % n (the _rot modes), none otherwise
+  auto drive0_shard = [&](int t) { return rot ? (n - t % n) % n : 0; };
   auto one_call = [&](int t) -> int64_t {
     TB& b = tb[t];
     if (mode == "batcher") return mec_batcher_encode_sg(bat, b.obj, osize, b.files.data(), b.dd, k + 1);
@@ -118,7 +130,7 @@ int main(int argc, char** argv) {
     if (mode == "pool") return mec_encode_sg(pool[t % P], b.obj, osize, b.files.data(), b.dd, k + 1);
     if (mode == "bget") {
       const uint8_t* f[64];
-      for (int i = 0; i < n; i++) f[i] = i < 4 ? nullptr : b.files[i];
+      for (int i = 0; i < n; i++) f[i] = (rot ? i == drive0_shard(t) : i < 4) ? nullptr : b.files[i];
       int hint = 0;
       return mec_batcher_decode(bat, f, 0, osize, osize, b.dst, &hint);
     }
@@ -132,8 +144,9 @@ int main(int argc, char** argv) {
       const uint8_t* f[64];
       uint8_t* o[64] = {};
       uint8_t bad[64];
-      for (int i = 0; i < n; i++) f[i] = i == 0 ? nullptr : b.files[i];
-      o[0] = b.healed;
+      const int st = drive0_shard(t);
+      for (int i = 0; i < n; i++) f[i] = i == st ? nullptr : b.files[i];
+      o[st] = b.healed;
       const int rc = mode == "bheal" ? mec_batcher_heal(bat, f, nullptr, osize, o, bad) : mec_heal_prefer(pool[t % P], f, nullptr, osize, o, bad);
       return rc == MEC_OK ? osize : rc;
     }
@@ -160,7 +173,7 @@ int main(int argc, char** argv) {
   const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   if (mode == "bheal" || mode == "heal")  // every healed part file equals the drive's original one
     for (int t = 0; t < T; t++)
-      if (memcmp(tb[t].healed, tb[t].files[0], static_cast<size_t>(fsz)) != 0) errors++;
+      if (memcmp(tb[t].healed, tb[t].files[drive0_shard(t)], static_cast<size_t>(fsz)) != 0) errors++;
   if (mode == "batcher_crc")  // every thread's object checksums equal the host's
     for (int t = 0; t < T; t++)
       if (tb[t].crc[0] != host_crc(tb[t].obj, osize, 0xEDB88320ull, 32) || tb[t].crc[1] != host_crc(tb[t].obj, osize, 0x82F63B78ull, 32) ||
@@ -172,12 +185,14 @@ int main(int argc, char** argv) {
   const double total = static_cast<double>(T) * calls_per_thread * osize;
   printf("{\"mode\": \"%s\", \"threads\": %d, \"object_MiB\": %lld, \"object_bytes\": %lld, \"calls\": %zu, \"seconds\": %.4f, \"GiB_per_s\": %.2f, \"calls_per_s\": %.0f, "
          "\"p50_us\": %.0f, \"p99_us\": %.0f, \"errors\": %lld",
-         mode.c_str(), T, static_cast<long long>(osize >> 20), static_cast<long long>(osize), all.size(), sec, total / sec / (1 << 30), all.size() / sec, all[all.size() / 2],
+         mode_name.c_str(), T, static_cast<long long>(osize >> 20), static_cast<long long>(osize), all.size(), sec, total / sec / (1 << 30), all.size() / sec, all[all.size() / 2],
          all[static_cast<size_t>(all.size() * 0.99)], static_cast<long long>(errors.load()));
   if (mode == "batcher_crc") printf(", \"crc_requests\": %lld", static_cast<long long>(mec_batcher_stat(bat, "crc_requests")));
-  if (bat) printf(", \"batches\": %lld, \"blocks_per_batch\": %.1f, \"launches\": %lld", static_cast<long long>(mec_batcher_stat(bat, "batches")),
+  if (bat) printf(", \"mix\": %d, \"batches\": %lld, \"blocks_per_batch\": %.1f, \"launches\": %lld, \"patterns\": %lld, \"mixed_batches\": %lld",
+                  bflags ? 1 : 0, static_cast<long long>(mec_batcher_stat(bat, "batches")),
                   static_cast<double>(mec_batcher_stat(bat, "blocks")) / std::max<int64_t>(1, mec_batcher_stat(bat, "batches")),
-                  static_cast<long long>(mec_batcher_stat(bat, "launches")));
+                  static_cast<long long>(mec_batcher_stat(bat, "launches")), static_cast<long long>(mec_batcher_stat(bat, "patterns")),
+                  static_cast<long long>(mec_batcher_stat(bat, "mixed_batches")));
   if (bat && getenv("MEC_BATCHER_TRACE"))
     printf(", \"worker_us\": {\"submit\": %lld, \"sync\": %lld, \"finish\": %lld, \"idle\": %lld}, \"stream_us\": {\"stage\": %lld, \"kernel\": %lld, \"scatter\": %lld}",
            (long long)mec_batcher_stat(bat, "us_submit"), (long long)mec_batcher_stat(bat, "us_sync"), (long long)mec_batcher_stat(bat, "us_finish"),

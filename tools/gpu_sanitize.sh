@@ -67,6 +67,34 @@ th = [threading.Thread(target=heal, args=(t,)) for t in range(4)]
 assert all(r[1] == 0 and np.array_equal(r[0][1], want[t][1]) for t, r in enumerate(res)), [r[1] for r in res]
 assert bat.stat("kernel_batches") == 1 and bat.stat("requests") == 4
 bat.close()
+# mixed erasure patterns (MEC_BATCHER_MIX_PATTERNS): four GETs of the one-block object with a different drive offline each (shard 0
+# and 5 rebuilt; 13 and 15: parity, nothing rebuilt), then four heals of different stale sets (one and two drives) — each ONE latency
+# launch with a decode plan per block
+bat = mb.Batcher(k, m, bs, max_batch_blocks=8, max_wait_us=500000, mix_patterns=True)
+offl = [0, 5, 13, 15]
+gd = [[None if i == offl[t] else mb.pinned_array(want[3][i].size) for i in range(k + m)] for t in range(4)]
+for t, r in enumerate(gd):
+    for i, f in enumerate(r):
+        if f is not None: f[:] = want[3][i]
+res = [None] * 4
+def get(t): res[t] = bat.decode(gd[t], 0, pin[3].size, pin[3].size, dst=mb.pinned_array(pin[3].size))
+th = [threading.Thread(target=get, args=(t,)) for t in range(4)]
+[x.start() for x in th]; [x.join() for x in th]
+assert all(np.array_equal(r[0], pin[3]) and r[1] == 0 for r in res)
+assert bat.stat("batches") == 1 and bat.stat("mixed_batches") == 1 and bat.stat("patterns") == 3
+bat.close()
+stale = [{0}, {3, 14}, {15}, {7, 8}]
+bat = mb.Batcher(k, m, bs, max_batch_blocks=sum(-(-a.size // bs) for a in pin), max_wait_us=500000, mix_patterns=True)
+hd = [[None if i in stale[t] else mb.pinned_array(want[t][i].size) for i in range(k + m)] for t in range(4)]
+for t, r in enumerate(hd):
+    for i, f in enumerate(r):
+        if f is not None: f[:] = want[t][i]
+def heal(t): res[t] = bat.heal(hd[t], [i in stale[t] for i in range(k + m)], pin[t].size, pinned=True)
+th = [threading.Thread(target=heal, args=(t,)) for t in range(4)]
+[x.start() for x in th]; [x.join() for x in th]
+assert all(r[1] == 0 and all(np.array_equal(r[0][i], want[t][i]) for i in stale[t]) for t, r in enumerate(res))
+assert bat.stat("batches") == 1 and bat.stat("mixed_batches") == 1 and bat.stat("patterns") == 4
+bat.close()
 # one merged batch of pinned PUTs with mixed checksum masks (mec_batcher_encode_crc): segmented CRC kernels over the staged batch;
 # the 2 MiB object spans eight 256 KiB regions
 objs = pin
