@@ -172,6 +172,21 @@ int mec_heal_prefer(mec_codec* c, const uint8_t* const* files, const uint8_t* pr
 int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const uint8_t* const* const* files,
                    const int64_t* total_lengths, uint8_t* const* const* out_files, int* rcs);
 
+/* Data movement between pools (decommissionObject / rebalanceObject, cmd/erasure-server-pool-decom.go:605,
+ * cmd/erasure-server-pool-rebalance.go:848): Erasure.Decode of a whole part on `src` followed by Erasure.Encode of the same
+ * bytes on `dst`, without the object leaving the device.  files / prefer / total_length as mec_decode_prefer (whole part,
+ * offset 0): the first k readable files are read, preferred ones first, and a reader whose frame fails its digest is dropped for
+ * the rest of the call, the part resuming at that block with the next reader.  out_files / write_quorum as mec_encode (complete
+ * part.N images of dst's geometry, NULL = offline writer).  Returns total_length, or a negative MEC_ERR_*; *heal_hint =
+ * MEC_ERR_FILE_CORRUPT when a source frame failed its digest but the part was still moved.
+ * Refused before any device work: src == dst or a NULL src / dst / files / out_files (MEC_ERR_INVALID_ARGUMENT; for the same
+ * geometry use a second handle), different block sizes or devices or an algorithm other than HighwayHash256S on either side
+ * (MEC_ERR_UNSUPPORTED), fewer than write_quorum non-NULL out_files (MEC_ERR_WRITE_QUORUM).  total_length == 0 returns 0 and
+ * writes nothing.  Fewer than k readable source files is MEC_ERR_READ_QUORUM.  Both codecs are held for the call.  Counters:
+ * "blocks_read" and "bytes_h2d" grow on src, "blocks_encoded" and "bytes_d2h" on dst. */
+int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, const uint8_t* prefer, int64_t total_length,
+                      mec_codec* dst, uint8_t* const* out_files, int write_quorum, int* heal_hint);
+
 /* ---- cross-request coalescer: many concurrent PutObject calls, one launch ---------------------------------------------------
  * MinIO encodes one block per loop iteration on every request goroutine (cmd/erasure-encode.go:76-108, one Erasure per request,
  * cmd/erasure-object.go:1371); a launch that small leaves 131 of 132 SMs idle.  A batcher owns one codec (k, m, block_size,

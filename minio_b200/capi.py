@@ -98,6 +98,8 @@ def lib():
     L.mec_heal_batch.argtypes = [vp, i32, i64, vp, vp, vp, vp]
     L.mec_decode_prefer.restype = i64
     L.mec_decode_prefer.argtypes = [vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
+    L.mec_transcode.restype = i64
+    L.mec_transcode.argtypes = [vp, vp, vp, i64, vp, vp, i32, C.POINTER(i32)]
     L.mec_jit_compile_check.restype = i64
     L.mec_jit_compile_check.argtypes = [i32, i32, vp, i32, i32, i32, i32]
     L.mec_jit_prewarm.argtypes = [vp]
@@ -272,6 +274,25 @@ class Codec:
         if rc < 0:
             raise MecError(rc, "mec_decode")
         return dst[:length], hint.value
+
+    def transcode(self, files, total, dst, prefer=None, online=None, write_quorum=0):
+        """mec_transcode: move a whole part of `total` bytes from this codec's part files (None = offline) to the geometry of the
+        Codec `dst` without the object bytes leaving the device.  online = dst's writers (None = all).  -> (out_files, heal_hint):
+        dst's complete part files (None where offline) and -7 when a source frame failed its digest on the way."""
+        files = [None if f is None else _u8(f) for f in files]
+        fsz = dst.bitrot_file_size(total)
+        online = [True] * dst.n if online is None else online
+        outs = [np.zeros(fsz, dtype=np.uint8) if online[i] else None for i in range(dst.n)]
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        # an empty part has empty out files, yet an online writer must still count against the quorum
+        marker = np.zeros(1, dtype=np.uint8)
+        optrs = _ptrs([(o if o.size else marker) if o is not None else None for o in outs])
+        rc = lib().mec_transcode(self.h, _ptrs(files), None if pf is None else pf.ctypes.data, total, dst.h, optrs, write_quorum,
+                                 C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_transcode")
+        return outs, hint.value
 
     def heal(self, files, stale, total, prefer=None, report=False):
         """Erasure.Heal.  Like the reference, bitrot met in a source reader does not stop the rebuild but is reported:

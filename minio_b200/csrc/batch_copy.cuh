@@ -220,3 +220,40 @@ __global__ void __launch_bounds__(128) batch_heal_scatter_kernel(const BatchGetP
 }
 
 }  // namespace mec
+
+// ---- data movement between pools (mec_transcode): the data shards of a reconstructed chunk -> its contiguous object bytes -------
+namespace mec {
+
+struct ResplitParams {
+  uint8_t* obj;                 // device: object bytes of the chunk's blocks, block b at b*bs (the short last block right behind the full ones)
+  const uint8_t* arena;         // survivors: reader position t at arena + t*arena_stride, block b's frame at + b*P (shard at + 32)
+  int64_t arena_stride, P;
+  const uint8_t* rebuilt;       // rebuilt data shards: block b, row q at (b*r + q)*pitch
+  int64_t pitch;
+  int64_t bs, S;                // block size, full shard length
+  int64_t nfull;                // full blocks of the chunk
+  int64_t tail, tail_S;         // object bytes and shard length of the part's short last block behind them (tail 0: none)
+  int r;
+  int8_t src[kBatchMaxFiles];   // data shard i: read at arena position src[i] >= 0, or rebuilt row -1 - src[i]
+};
+
+// grid (blocks of the chunk, k source data shards), 128 threads: writeDataBlocks (cmd/erasure-utils.go:42) into device memory.
+// CTA (b, i) copies the object bytes of data shard i of block b, never Split's zero padding, to obj + b*bs + i*S_b.  Sources are
+// 16-byte aligned rows; destinations land at any offset (S = 87382 for RS(12,4)), so cta_copy stores destination-aligned 16-byte
+// vectors from a funnel-shifted source.  It reads up to one word past a row: inside the arena's 512-byte padding, and inside the
+// slack DevBuf keeps behind every rebuilt-row buffer (at least 256 bytes) for the chunk's last row, which ends at round_up(S, 16).
+// __grid_constant__: src[i] is read straight from the parameter bank (a by-value parameter indexed at run time is copied to the stack).
+__global__ void __launch_bounds__(128) transcode_resplit_kernel(const __grid_constant__ ResplitParams p) {
+  const int64_t b = blockIdx.x;
+  const int i = blockIdx.y;
+  const bool is_tail = b >= p.nfull;
+  const int64_t per = is_tail ? p.tail_S : p.S, blen = is_tail ? p.tail : p.bs;
+  int64_t have = blen - static_cast<int64_t>(i) * per;
+  have = have < 0 ? 0 : (have > per ? per : have);
+  if (have == 0) return;
+  const int t = p.src[i];
+  const uint8_t* src = t >= 0 ? p.arena + t * p.arena_stride + b * p.P + 32 : p.rebuilt + (b * p.r + (-1 - t)) * p.pitch;
+  cta_copy(p.obj + b * p.bs + static_cast<int64_t>(i) * per, src, have, false);
+}
+
+}  // namespace mec

@@ -744,6 +744,18 @@ static void frames_retire(mec_codec* c, const EncChunk& ch, uint8_t* const* file
   }
 }
 
+// a chunk's digests into its slot's pinned staging (scattered by frames_retire) and its frames into `files` (frames_enqueue)
+static int frames_enqueue_chunk(mec_codec* c, const EncChunk& ch, uint8_t* const* files, bool with_data, uint8_t* data_digests) {
+  if (ch.nb <= kBatchedCopyBlocks) {  // a small object: digests and every frame piece in ONE batched copy call
+    CopyList list;
+    list.add(ch.s->hdig.p, ch.s->dig.p, ch.nb * c->n * 32);
+    const int e = frames_enqueue(c, ch, files, with_data, data_digests, &list);
+    return e ? e : list.flush(ch.st);
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(ch.s->hdig.p, ch.s->dig.p, static_cast<size_t>(ch.nb * c->n * 32), cudaMemcpyDeviceToHost, ch.st));
+  return frames_enqueue(c, ch, files, with_data, data_digests);
+}
+
 static int64_t encode_frames(mec_codec* c, const uint8_t* src, int64_t len, uint8_t* const* files, bool with_data,
                              uint8_t* data_digests, int write_quorum, const char* what) {
   NvtxRange nvtx(what);
@@ -762,16 +774,7 @@ static int64_t encode_frames(mec_codec* c, const uint8_t* src, int64_t len, uint
   MEC_CUDA_OK(cudaSetDevice(c->device));
   rc = encode_pipeline(
       c, src, len,
-      [&](const EncChunk& ch) -> int {
-        if (ch.nb <= kBatchedCopyBlocks) {  // a small object: digests and every frame piece in ONE batched copy call
-          CopyList list;
-          list.add(ch.s->hdig.p, ch.s->dig.p, ch.nb * c->n * 32);
-          const int e = frames_enqueue(c, ch, files, with_data, data_digests, &list);
-          return e ? e : list.flush(ch.st);
-        }
-        MEC_CUDA_OK(cudaMemcpyAsync(ch.s->hdig.p, ch.s->dig.p, static_cast<size_t>(ch.nb * c->n * 32), cudaMemcpyDeviceToHost, ch.st));
-        return frames_enqueue(c, ch, files, with_data, data_digests);
-      },
+      [&](const EncChunk& ch) { return frames_enqueue_chunk(c, ch, files, with_data, data_digests); },
       [&](const EncChunk& ch) { frames_retire(c, ch, files, with_data, data_digests); });
   return rc ? rc : len;
 }
@@ -816,9 +819,13 @@ static int stage_frames(const uint8_t* host, void* dev, const FrameGeom& g, cuda
 //   frame sink  (Heal, mec_reconstruct_frames): out[i] = frame-layout image of shard i, same geometry as the inputs
 //   object sink (Decode): the data shards of every block, cut to the object bytes [lo, hi) and laid end to end in dst —
 //                writeDataBlocks (cmd/erasure-utils.go:42) done by the copy engines: one 2-D copy per data shard and chunk
+//   transcode sink (data movement between pools, mec_transcode): the data shards of every block re-split on the device into the
+//                object bytes of the whole part, encoded by the codec `enc` and written as complete frames of its geometry to enc_files
 struct RangeSink {
   uint8_t* const* out = nullptr;
   uint8_t* dst = nullptr;
+  mec_codec* enc = nullptr;
+  uint8_t* const* enc_files = nullptr;
   int64_t first_block = 0;   // index (within the part) of the range's first block
   int64_t lo = 0, hi = 0;    // wanted part bytes
   int64_t bs = 0, total = 0; // block size, part size
@@ -1002,6 +1009,46 @@ static int emit_frames(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
   return list ? list->flush(s.st) : MEC_OK;
 }
 
+// Transcode sink of one chunk (whole part, so chunk block b is part block ch.b0 + b): the chunk's data shards, read or rebuilt,
+// re-split by ONE launch into the object bytes of its blocks in the destination codec's slot `si` (the same index as the source
+// slot, whose stream carries everything), then encoded there and queued as destination frames like mec_encode's.  *out is what
+// frames_retire needs once the chunk is accepted.
+static_assert(kMaxK <= kBatchMaxFiles, "ResplitParams::src holds one entry per source data shard");
+static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk, const RChunk& ch, int si, int64_t stride,
+                          int64_t pitch, EncChunk* out) {
+  mec_codec* e = sk.enc;
+  Slot& s = c->slots[si];
+  Slot& d = e->slots[si];
+  const int k = c->k;
+  const int64_t bs = sk.bs, bytes = std::min(sk.total - ch.b0 * bs, ch.nb * bs);
+  const int64_t epitch = round_up(e->S(), 16);
+  int rc;
+  if ((rc = d.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
+  if ((rc = d.out.ensure(static_cast<size_t>(ch.nb * std::max(e->m, 1) * epitch)))) return rc;
+  if ((rc = d.dig.ensure(static_cast<size_t>(ch.nb * e->n * 32)))) return rc;
+  if ((rc = d.hdig.ensure(static_cast<size_t>(ch.nb * e->n * 32)))) return rc;
+  ResplitParams p;
+  p.obj = static_cast<uint8_t*>(d.src.p);
+  p.arena = static_cast<const uint8_t*>(s.aux.p); p.arena_stride = stride; p.P = g.dpitch();
+  p.rebuilt = static_cast<const uint8_t*>(s.out.p); p.pitch = pitch; p.r = ch.r;
+  p.bs = bs; p.S = g.S;
+  p.nfull = bytes / bs; p.tail = bytes % bs; p.tail_S = ceil_frac(p.tail, k);
+  for (int t = 0; t < k; t++)
+    if (ch.chosen[t] < k) p.src[ch.chosen[t]] = static_cast<int8_t>(t);
+  for (int q = 0; q < ch.r; q++) p.src[ch.targets[q]] = static_cast<int8_t>(-1 - q);
+  transcode_resplit_kernel<<<dim3(static_cast<unsigned>(ch.nb), static_cast<unsigned>(k)), 128, 0, s.st>>>(p);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  if ((rc = encode_device_locked(e, p.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.p), s.st))) return rc;
+  EncChunk& ec = *out;
+  ec = EncChunk{};
+  ec.b0 = ch.b0; ec.nb = ch.nb; ec.nfull = p.nfull; ec.tail = p.tail; ec.s = &d; ec.pitch = epitch; ec.st = s.st;
+  ec.d_src = p.obj; ec.d_src_tail = p.obj + p.nfull * bs;
+  ec.d_out = static_cast<uint8_t*>(d.out.p); ec.d_out_tail = ec.d_out + p.nfull * e->m * epitch;
+  ec.h_dig = static_cast<const uint8_t*>(d.hdig.p); ec.h_dig_tail = ec.h_dig + p.nfull * e->n * 32;
+  return frames_enqueue_chunk(e, ec, sk.enc_files, true, nullptr);
+}
+
 // Core of Decode / Heal: frames[i] point at the first frame of the range (host).  The range is cut into chunks that run through
 // the codec's six slots — while chunk c is in the kernel, chunk c+1 is being staged and chunk c-1 is on its way back — each
 // slot with its own stream, survivor arena, output and flag buffers.  Chunks retire in order: the per-frame digest verdicts
@@ -1028,6 +1075,7 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
   const int64_t stride = round_up(chunk * P + 512, 256);
 
   RChunk inflight[kSlots];
+  EncChunk enc_inflight[kSlots];  // transcode sink: the destination frames of each chunk
   bool busy[kSlots] = {};
   int head = 0, tail = 0, nbusy = 0;  // ring: tail = oldest in flight, head = next free slot
   int64_t next = 0, done = 0;         // next block to submit, blocks accepted so far
@@ -1066,7 +1114,8 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(ch.nb * k), s.st));
     if ((e = launch_reconstruct(c, g, ch, s, stride, ch.rows.data(), pitch, hash_outputs))) return e;
     MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(ch.nb * k), cudaMemcpyDeviceToHost, s.st));
-    if (sk.dst) { if ((e = emit_object(c, g, sk, ch, s, stride, pitch, batched ? &list : nullptr))) return e; }
+    if (sk.enc) { if ((e = emit_transcode(c, g, sk, ch, si, stride, pitch, &enc_inflight[si]))) return e; }
+    else if (sk.dst) { if ((e = emit_object(c, g, sk, ch, s, stride, pitch, batched ? &list : nullptr))) return e; }
     else if (sk.out) { if ((e = emit_frames(c, g, sk, ch, s, pitch, batched ? &list : nullptr))) return e; }
     return MEC_OK;
   };
@@ -1099,6 +1148,12 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
         const int64_t bytes = (ch.b0 + good == g.nblocks) ? (g.file_bytes() - ch.b0 * fstride) : good * fstride;
         memcpy(sk.out[i] + ch.b0 * fstride, frames[i] + ch.b0 * fstride, static_cast<size_t>(bytes));
       }
+    }
+    if (good > 0 && sk.enc) {  // destination digests of the accepted blocks only; a redo rewrites every frame from the bad block on
+      EncChunk acc = enc_inflight[si];
+      if (good < acc.nb) { acc.nb = acc.nfull = good; acc.tail = 0; }  // the short last block, if any, is the chunk's last: not accepted
+      frames_retire(sk.enc, acc, sk.enc_files, true, nullptr);
+      sk.enc->st_blocks_encoded += good;
     }
     c->st_blocks_read += good;
     c->st_shards_rebuilt += good * ch.r;
@@ -1259,6 +1314,47 @@ extern "C" int mec_heal_prefer(mec_codec* c, const uint8_t* const* files, const 
 }
 extern "C" int mec_heal(mec_codec* c, const uint8_t* const* files, int64_t total, uint8_t* const* out_files) {
   return mec_heal_prefer(c, files, nullptr, total, out_files, nullptr);
+}
+
+// Data movement between pools (decommissionObject / rebalanceObject, cmd/erasure-server-pool-decom.go:605,
+// cmd/erasure-server-pool-rebalance.go:848): Erasure.Decode of a whole part on `src` piped into Erasure.Encode on `dst`.  The
+// reconstruct pipeline of mec_decode_prefer runs with the transcode sink, so the object bytes never leave the device: each chunk
+// is read, verified (and rebuilt where readers are missing), re-split, encoded and written out as dst's frames on one stream.
+extern "C" int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
+                                 mec_codec* dst, uint8_t* const* out_files, int write_quorum, int* heal_hint) {
+  NvtxRange nvtx("mec_transcode");
+  if (heal_hint) *heal_hint = 0;
+  // one handle cannot be both ends: the source slots hold the survivors while the destination slots hold the re-split bytes
+  if (!src || !dst || src == dst || !files || !out_files || total < 0) return MEC_ERR_INVALID_ARGUMENT;
+  if (src->block_size != dst->block_size || src->device != dst->device || src->algo != MEC_HIGHWAYHASH256S ||
+      dst->algo != MEC_HIGHWAYHASH256S)
+    return MEC_ERR_UNSUPPORTED;
+  int online = 0;
+  for (int i = 0; i < dst->n; i++) online += out_files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  if (total == 0) return 0;
+  if (src->k > kMaxK || src->n > kMaxShards || dst->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
+  int rc;
+  if ((rc = require_streaming(src)) || (rc = require_streaming(dst))) return rc;
+  std::scoped_lock lk(src->mu, dst->mu);  // two threads moving parts in opposite directions lock in the same order
+  const int n = src->n;
+  const int64_t S = src->S(), sfs = mec_shard_file_size(src, total);
+  FrameGeom g;
+  g.nblocks = ceil_frac(total, src->block_size);
+  g.S = S;
+  g.last_len = sfs - (g.nblocks - 1) * S;
+  std::vector<uint8_t> alive(n), want(n, 0), corrupt(n, 0);
+  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
+  for (int i = 0; i < src->k; i++) want[i] = 1;
+  RangeSink sk;
+  sk.enc = dst; sk.enc_files = out_files; sk.hi = total; sk.bs = src->block_size; sk.total = total;
+  // as mec_decode_prefer: the rebuilt data shards are consumed, not stored, so they are not hashed
+  rc = reconstruct_range(src, files, g, want.data(), 1, sk, corrupt.data(), alive.data(), prefer, false);
+  if (rc) return rc;
+  if (heal_hint)
+    for (int i = 0; i < n; i++)
+      if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
+  return total;
 }
 
 // Batched heal (SURVEY §8f rank 2, BASELINE config 4): objects are independent, so a pool of codec handles — each with
