@@ -249,6 +249,33 @@ int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* const* files, c
  * private path directly. */
 int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total_length,
                      uint8_t* const* out_files, uint8_t* corrupt);
+/* A batcher that also moves parts from its own geometry (k, m) to a destination geometry (dst_k, dst_m) of the same block size on
+ * the same device.  mec_batcher_new_ex with a second, private destination codec; flags as there.  Geometry errors of either side
+ * are those of mec_codec_new; dst_k == k && dst_m == m is allowed (rebalance between equal pools).  The batcher still serves
+ * mec_batcher_encode*, mec_batcher_decode* and mec_batcher_heal for (k, m) exactly as a mec_batcher_new_ex batcher does.
+ * Extra device memory: the destination codec's six slots are sized up front like the source's, each for B = max_batch_blocks
+ * + min(64, max_batch_blocks / 8 + 4) blocks: B x (block_size + dst_m x round_up(S', 16) + (dst_k + dst_m) x 32) bytes plus small
+ * tables (S' = ceil(block_size / dst_k)) — about 6 x B x block_size x (1 + dst_m / dst_k) in all: 4.5 GiB for RS(6,2) at 1 MiB
+ * blocks and max_batch_blocks = 512. */
+int mec_batcher_new_transcode(int k, int m, int dst_k, int dst_m, int64_t block_size, int device, int64_t max_batch_blocks,
+                              int max_wait_us, int flags, mec_batcher** out);
+/* mec_transcode through the coalescer: arguments, results, heal_hint and refusals of mec_transcode (files / prefer / total_length
+ * of the source, out_files / write_quorum of the destination).  Checked on the caller's thread before anything is queued: a NULL
+ * batcher, files or out_files, total_length < 0 or a batcher not made by mec_batcher_new_transcode (MEC_ERR_INVALID_ARGUMENT), fewer
+ * than write_quorum non-NULL out_files (MEC_ERR_WRITE_QUORUM), total_length == 0 (returns 0, writes nothing), fewer than k readable
+ * source files (MEC_ERR_READ_QUORUM).  The readers are chosen there as parallelReader chooses them (`prefer` first, then index
+ * order); moves that read the same k drives share one merged batch (any moves with MEC_BATCHER_MIX_PATTERNS, cut at one latency
+ * launch as GET and heal batches are): staged and rebuilt as whole-part GETs, re-split on the device, encoded and scattered as
+ * merged PUTs of the destination geometry — the object bytes never leave the device.  A move whose readers fail a digest check is
+ * redone on its own with mec_transcode on a private pair of handles (every out file rewritten, heal_hint = MEC_ERR_FILE_CORRUPT,
+ * counted in "redone"); moves with a chosen reader or an out file that is not page-locked, geometries of more than 32 drives,
+ * MEC_BATCHER_MEMCPY in the environment, and parts of more than max_batch_blocks blocks take that private path directly.
+ * mec_batcher_stat: "transcodes" (moves completed by merged batches), "transcodes_serial" (moves of the private path, redos
+ * included); names prefixed "dst_" are answered by mec_get_stat on the destination codec ("dst_blocks_encoded", "dst_bytes_d2h",
+ * "dst_form_small", "dst_launches", ...).  As with mec_transcode, "blocks_read" and "bytes_h2d" grow on the source codec,
+ * "blocks_encoded" and "bytes_d2h" on the destination codec. */
+int64_t mec_batcher_transcode(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total_length,
+                              uint8_t* const* out_files, int write_quorum, int* heal_hint);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------

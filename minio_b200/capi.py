@@ -75,6 +75,9 @@ def lib():
     L.mec_batcher_decode_prefer.restype = i64
     L.mec_batcher_decode_prefer.argtypes = [vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_batcher_heal.argtypes = [vp, vp, vp, i64, vp, vp]
+    L.mec_batcher_new_transcode.argtypes = [i32, i32, i32, i32, i64, i32, i64, i32, i32, C.POINTER(vp)]
+    L.mec_batcher_transcode.restype = i64
+    L.mec_batcher_transcode.argtypes = [vp, vp, vp, i64, vp, i32, C.POINTER(i32)]
     L.mec_batcher_stat.restype = i64
     L.mec_batcher_stat.argtypes = [vp, C.c_char_p]
     L.mec_checksums.argtypes = [vp, vp, i64, i32, vp]
@@ -442,16 +445,22 @@ class Codec:
 class Batcher:
     """mec_batcher: concurrent PutObject calls of one geometry merged into shared launches.  encode() may be called from many
     threads at once (ctypes releases the GIL for the duration of the call).  mix_patterns=True (MEC_BATCHER_MIX_PATTERNS): GETs
-    and heals of different erasure patterns (reader sets, stale sets) share batches."""
+    and heals of different erasure patterns (reader sets, stale sets) share batches.  dst=(k2, m2) (mec_batcher_new_transcode): the
+    batcher also moves parts of its geometry to RS(k2, m2) of the same block size (transcode())."""
 
-    def __init__(self, k, m, block_size=1 << 20, device=0, max_batch_blocks=256, max_wait_us=200, mix_patterns=False):
+    def __init__(self, k, m, block_size=1 << 20, device=0, max_batch_blocks=256, max_wait_us=200, mix_patterns=False, dst=None):
         h = C.c_void_p()
-        rc = lib().mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, MIX_PATTERNS if mix_patterns else 0,
-                                      C.byref(h))
+        flags = MIX_PATTERNS if mix_patterns else 0
+        if dst is None:
+            rc = lib().mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, flags, C.byref(h))
+        else:
+            rc = lib().mec_batcher_new_transcode(k, m, dst[0], dst[1], block_size, device, max_batch_blocks, max_wait_us, flags,
+                                                 C.byref(h))
         if rc:
-            raise MecError(rc, "mec_batcher_new_ex")
+            raise MecError(rc, "mec_batcher_new_ex" if dst is None else "mec_batcher_new_transcode")
         self.h, self.k, self.m, self.n, self.block_size = h, k, m, k + m, block_size
         self._sizes = Codec(k, m, block_size, device=device)
+        self._dst_sizes = None if dst is None else Codec(dst[0], dst[1], block_size, device=device)
 
     def _encode_crc(self, src, files, dd, write_quorum, checksums):
         """mec_batcher_encode_crc -> (CRC32, CRC32C, CRC64NVME), 0 where not asked for"""
@@ -528,6 +537,30 @@ class Batcher:
             raise MecError(rc, "mec_batcher_heal")
         return outs, rc, corrupt
 
+    def transcode(self, files, total, prefer=None, online=None, write_quorum=0, pinned=False):
+        """mec_batcher_transcode (a batcher made with dst=): move a whole part of `total` bytes from this geometry's part files (None
+        = offline) to the destination geometry.  online = the destination's writers (None = all).  Page-locked part files and
+        pinned=True (the out files are allocated page-locked; the caller owns and should free them) let the move ride in merged
+        batches.  -> (out_files, heal_hint) as Codec.transcode."""
+        if self._dst_sizes is None:
+            raise MecError(-12, "mec_batcher_transcode")
+        files = [None if f is None else _u8(f) for f in files]
+        n2 = self._dst_sizes.n
+        fsz = self._dst_sizes.bitrot_file_size(total)
+        online = [True] * n2 if online is None else online
+        mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
+        outs = [mk(fsz) if online[i] else None for i in range(n2)]
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        # an empty part has empty out files, yet an online writer must still count against the quorum
+        marker = np.zeros(1, dtype=np.uint8)
+        optrs = _ptrs([(o if o.size else marker) if o is not None else None for o in outs])
+        rc = lib().mec_batcher_transcode(self.h, _ptrs(files), None if pf is None else pf.ctypes.data, total, optrs, write_quorum,
+                                         C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_transcode")
+        return outs, hint.value
+
     def stat(self, name):
         return lib().mec_batcher_stat(self.h, name.encode())
 
@@ -536,6 +569,8 @@ class Batcher:
             lib().mec_batcher_free(self.h)
             self.h = None
             self._sizes.close()
+            if self._dst_sizes is not None:
+                self._dst_sizes.close()
 
     __del__ = close
 

@@ -256,4 +256,34 @@ __global__ void __launch_bounds__(128) transcode_resplit_kernel(const __grid_con
   cta_copy(p.obj + b * p.bs + static_cast<int64_t>(i) * per, src, have, false);
 }
 
+// grid (block stride, k source data shards, nreq), 128 threads: the batched form of transcode_resplit_kernel for a merged batch of
+// moves (mec_batcher_transcode).  Request z's decode plan (chosen readers, rebuilt data shards) and its source slots come from the
+// read table p.reqs[z], which covers the whole part (start_block 0); where its object bytes go comes from the PUT table d.reqs[z]
+// (len = total): full blocks at d.staged + (full0 + b) * bs, the short last block at d.staged + tail_src_off.  CTA (x, i, z) copies
+// the object bytes of data shard i of every block of request z, never Split's zero padding.  Both geometries share the block size,
+// so source block b is destination block b; the source's short last slot (shard length last_len) may still hold a short object
+// block when ceil(tail / k) == S, so each block's byte count is taken from the part length.  Source rows are read up to one word
+// past their end, inside the arena's padding and the slack behind the rebuilt rows (see transcode_resplit_kernel).
+__global__ void __launch_bounds__(128) batch_transcode_resplit_kernel(const BatchGetParams p, const BatchCopyParams d) {
+  const BatchGetDesc& r = p.reqs[blockIdx.z];
+  const BatchReqDesc& w = d.reqs[blockIdx.z];
+  const int i = blockIdx.y;
+  int t = -1, q = -1;
+  for (int x = 0; x < p.k; x++) if (r.chosen[x] == i) t = x;
+  for (int x = 0; x < r.r; x++) if (r.targets[x] == i) q = x;
+  if (t < 0 && q < 0) return;
+  const int64_t nfull = w.len / p.bs;
+  for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
+    const bool is_tail = r.tail_slot >= 0 && b == r.nblocks - 1;
+    const int64_t cur = is_tail ? r.last_len : p.S, slot = get_slot(r, b);
+    const int64_t blen = w.len - b * p.bs < p.bs ? w.len - b * p.bs : p.bs;
+    int64_t have = blen - static_cast<int64_t>(i) * cur;
+    have = have > cur ? cur : have;
+    if (have <= 0) continue;
+    const uint8_t* src = t >= 0 ? p.arena + t * p.arena_stride + slot * p.P + 32 : p.rebuilt + (slot * p.r + q) * p.pitch;
+    uint8_t* dst = d.staged + (b < nfull ? (w.full0 + b) * p.bs : w.tail_src_off) + static_cast<int64_t>(i) * cur;
+    cta_copy(dst, src, have, false);
+  }
+}
+
 }  // namespace mec

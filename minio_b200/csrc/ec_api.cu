@@ -2120,8 +2120,8 @@ extern "C" int mec_selftest(int device) {
 #include <unordered_map>
 
 struct BatchReq {
-  int kind = 0;                      // 0 = PutObject (encode), 1 = GetObject (decode), 2 = Heal
-  // GET and heal (a heal reads the whole part: offset 0, length = total)
+  int kind = 0;                      // 0 = PutObject (encode), 1 = GetObject (decode), 2 = Heal, 3 = transcode (move between pools)
+  // GET, heal and transcode (a heal and a transcode read the whole part: offset 0, length = total; a transcode writes `outs`)
   const uint8_t* const* gfiles = nullptr;
   int64_t offset = 0, length = 0, total = 0;
   uint8_t* dst = nullptr;
@@ -2183,6 +2183,11 @@ struct mec_batcher {
   bool trace = false;
   cudaEvent_t ev_ph[kSlots][4] = {};
   std::atomic<int64_t> us_submit{0}, us_sync{0}, us_finish{0}, us_idle{0}, us_stage{0}, us_kernel{0}, us_scatter{0};
+  // mec_batcher_new_transcode: the destination codec of merged moves (private; its slot i carries the destination side of the batch
+  // on source slot i), and the destination half of the private pair for moves that cannot ride in a batch (with `serial`)
+  mec_codec* dst = nullptr;
+  mec_codec* serial_dst = nullptr;
+  std::atomic<int64_t> st_transcodes{0}, st_transcodes_serial{0};  // moves completed by merged batches / by the private pair
 };
 
 namespace {
@@ -2204,18 +2209,37 @@ static mec_codec* batcher_serial(mec_batcher* b) {
   return b->serial;
 }
 
+// mec_transcode on the private pair (serial, serial_dst), for moves that cannot ride in a merged batch and for the redo of one that
+// met bitrot in a merged batch
+static int64_t batcher_transcode_serial(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
+                                        uint8_t* const* out_files, int write_quorum, int* heal_hint) {
+  b->st_transcodes_serial++;
+  mec_codec* sc = batcher_serial(b);
+  mec_codec* sd = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(b->serial_mu);
+    if (!b->serial_dst) {
+      mec_codec* e = nullptr;
+      if (mec_codec_new(b->dst->k, b->dst->m, b->dst->block_size, MEC_HIGHWAYHASH256S, b->dst->device, &e) == MEC_OK) b->serial_dst = e;
+    }
+    sd = b->serial_dst;
+  }
+  return sc && sd ? mec_transcode(sc, files, prefer, total, sd, out_files, write_quorum, heal_hint) : MEC_ERR_UNEXPECTED;
+}
+
 static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
   mec_codec* c = b->codec;
   if (fb.is_get) {
     // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own through the serial
     // handle, which applies parallelReader's block-sequential fail-over exactly (a heal rewrites every out file in full and reports
-    // the failing readers); the others are done (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
+    // the failing readers, a transcode rewrites every out file in full through mec_transcode on the private pair); the others are
+    // done (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
     Slot& s = *fb.reqs.front()->ch.s;
     const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
     const int k = fb.get_k;
     for (BatchReq* r : fb.reqs) {
-      const bool heal = r->kind == 2;
-      int64_t res = rc != MEC_OK ? rc : heal ? MEC_OK : r->length;
+      const bool heal = r->kind == 2, move = r->kind == 3;
+      int64_t res = rc != MEC_OK ? rc : heal ? MEC_OK : move ? r->total : r->length;
       if (rc == MEC_OK) {
         bool bad = false;
         for (int64_t bb = 0; bb < r->get_nblocks && !bad; bb++) {
@@ -2224,12 +2248,17 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
         }
         if (bad) {
           b->st_redone++;
-          mec_codec* sc = batcher_serial(b);
-          if (!sc) res = MEC_ERR_UNEXPECTED;
-          else if (heal) res = mec_heal_prefer(sc, r->gfiles, r->prefer, r->total, r->outs, r->corrupt);
-          else res = mec_decode_prefer(sc, r->gfiles, r->prefer, r->offset, r->length, r->total, r->dst, r->heal_hint);
-        } else if (r->heal_hint) {
-          *r->heal_hint = 0;
+          if (move) {
+            res = batcher_transcode_serial(b, r->gfiles, r->prefer, r->total, r->outs, 0, r->heal_hint);
+          } else {
+            mec_codec* sc = batcher_serial(b);
+            if (!sc) res = MEC_ERR_UNEXPECTED;
+            else if (heal) res = mec_heal_prefer(sc, r->gfiles, r->prefer, r->total, r->outs, r->corrupt);
+            else res = mec_decode_prefer(sc, r->gfiles, r->prefer, r->offset, r->length, r->total, r->dst, r->heal_hint);
+          }
+        } else {
+          if (r->heal_hint) *r->heal_hint = 0;
+          if (move) b->st_transcodes++;
         }
       }
       r->result = res;
@@ -2325,6 +2354,57 @@ static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
   MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, static_cast<size_t>(p.nreq) * kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
+  return MEC_OK;
+}
+
+// Encode and frame scatter of a staged batch in the PUT layout (`tab`: every request's full blocks contiguous from s.src, its short
+// last block at tail_src_off; parity rows in s.out, digests in s.dig, `cp` describes them): ONE latency launch with a per-block
+// geometry table when the batch fits one, otherwise one launch over all full blocks plus one per short block; then the scatter
+// kernel writes every frame into every caller's part-file images.  Used by merged PUTs on the batcher's codec and by merged
+// transcodes on the destination codec (slot `s` of codec `c`, enqueued on stream `st`).  `ev_encoded` (may be null) is recorded
+// between the encode and the scatter.
+static int batch_encode_scatter(mec_codec* c, Slot& s, cudaStream_t st, const BatchReqDesc* tab, size_t nreq, int64_t total_full,
+                                int64_t nslots, int64_t max_nb, const BatchCopyParams& cp, cudaEvent_t ev_encoded) {
+  const int k = c->k, m = c->m, n = c->n;
+  const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
+  uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
+  uint8_t* dout = static_cast<uint8_t*>(s.out.p);
+  uint8_t* ddig = static_cast<uint8_t*>(s.dig.p);
+  int rc;
+  if (c->eng->small_ok(c->opt, nslots)) {
+    // ONE launch for every block of the batch, full or short (objects smaller than a block are nothing but a short block): the
+    // latency kernel takes the geometry of each block from a table
+    if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(SmallBlock)))) return rc;
+    if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(SmallBlock)))) return rc;
+    SmallBlock* bt = static_cast<SmallBlock*>(s.hblk.p);
+    for (int64_t q = 0; q < total_full; q++) bt[q] = SmallBlock{q * bs, static_cast<int32_t>(S), static_cast<int32_t>(bs)};
+    for (size_t q = 0; q < nreq; q++)
+      if (tab[q].tail_slot >= 0) {
+        const int64_t tl = tab[q].len % bs;
+        bt[tab[q].tail_slot] = SmallBlock{tab[q].tail_src_off, static_cast<int32_t>(ceil_frac(tl, k)), static_cast<int32_t>(tl)};
+      }
+    MEC_CUDA_OK(cudaMemcpyAsync(s.blk.p, bt, static_cast<size_t>(nslots) * sizeof(SmallBlock), cudaMemcpyHostToDevice, st));
+    FusedDesc d;
+    d.k = k; d.r = m;
+    d.coef = c->matrix.data() + static_cast<size_t>(k) * k;
+    d.static_encode = true; d.contiguous = true; d.key = kMagicKey; d.out_pitch = pitch;
+    d.nblocks = nslots; d.S = static_cast<int32_t>(S);
+    d.in_base = dsrc; d.in_block_stride = bs; d.in_block_len = bs;
+    d.out = dout; d.digests = ddig;
+    d.blocks = static_cast<const SmallBlock*>(s.blk.p);
+    if ((rc = c->eng->launch_fused(d, c->opt, st))) return rc;
+  } else {
+    if (total_full > 0 && (rc = encode_device_locked(c, dsrc, total_full * bs, dout, pitch, ddig, st))) return rc;
+    for (size_t q = 0; q < nreq; q++)
+      if (tab[q].tail_slot >= 0 &&
+          (rc = encode_device_locked(c, dsrc + tab[q].tail_src_off, tab[q].len % bs, dout + tab[q].tail_slot * m * pitch, pitch,
+                                     ddig + tab[q].tail_slot * n * 32, st)))
+        return rc;
+  }
+  if (ev_encoded) cudaEventRecord(ev_encoded, st);
+  batch_scatter_kernel<<<dim3(static_cast<unsigned>(std::min<int64_t>(max_nb, 16)), static_cast<unsigned>(n), static_cast<unsigned>(nreq)), 128, 0, st>>>(cp);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
   return MEC_OK;
 }
 
@@ -2429,38 +2509,8 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[static_cast<int>(&s - c->slots)], 0));
     if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
     if ((rc = batcher_crc_launch(b, s, crc))) return rc;
-    if (c->eng->small_ok(c->opt, nslots)) {
-      // ONE launch for every block of the batch, full or short (objects smaller than a block are nothing but a short block): the
-      // latency kernel takes the geometry of each block from a table
-      if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(SmallBlock)))) return rc;
-      if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(SmallBlock)))) return rc;
-      SmallBlock* bt = static_cast<SmallBlock*>(s.hblk.p);
-      for (int64_t q = 0; q < total_full; q++) bt[q] = SmallBlock{q * bs, static_cast<int32_t>(S), static_cast<int32_t>(bs)};
-      for (size_t q = 0; q < reqs.size(); q++)
-        if (tab[q].tail_slot >= 0) {
-          const int64_t tl = tab[q].len % bs;
-          bt[tab[q].tail_slot] = SmallBlock{tab[q].tail_src_off, static_cast<int32_t>(ceil_frac(tl, k)), static_cast<int32_t>(tl)};
-        }
-      MEC_CUDA_OK(cudaMemcpyAsync(s.blk.p, bt, static_cast<size_t>(nslots) * sizeof(SmallBlock), cudaMemcpyHostToDevice, s.st));
-      FusedDesc d;
-      d.k = k; d.r = m;
-      d.coef = c->matrix.data() + static_cast<size_t>(k) * k;
-      d.static_encode = true; d.contiguous = true; d.key = kMagicKey; d.out_pitch = pitch;
-      d.nblocks = nslots; d.S = static_cast<int32_t>(S);
-      d.in_base = dsrc; d.in_block_stride = bs; d.in_block_len = bs;
-      d.out = dout; d.digests = ddig;
-      d.blocks = static_cast<const SmallBlock*>(s.blk.p);
-      if ((rc = c->eng->launch_fused(d, c->opt, s.st))) return rc;
-    } else {
-      if (total_full > 0 && (rc = encode_device_locked(c, dsrc, total_full * bs, dout, pitch, ddig, s.st))) return rc;
-      for (BatchReq* r : reqs)
-        if (r->ch.tail > 0 && (rc = encode_device_locked(c, r->ch.d_src_tail, r->ch.tail, r->ch.d_out_tail, pitch, ddig + (r->ch.h_dig_tail - hdig), s.st)))
-          return rc;
-    }
-    if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][2], s.st);
-    batch_scatter_kernel<<<dim3(static_cast<unsigned>(std::min<int64_t>(max_nb, 16)), static_cast<unsigned>(n), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(cp);
-    MEC_CUDA_OK(cudaGetLastError());
-    c->eng->count_launch();
+    if ((rc = batch_encode_scatter(c, s, s.st, tab, reqs.size(), total_full, nslots, max_nb, cp, b->trace ? b->ev_ph[phase_slot][2] : nullptr)))
+      return rc;
     if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][3], s.st);
     *needs_retire = false;
     c->st_blocks_encoded += nslots;
@@ -2829,6 +2879,67 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
   return MEC_OK;
 }
 
+// one merged batch of moves between pools (mec_batcher_transcode), everything on the source slot's stream: survivor frames staged and
+// the missing data shards rebuilt as for whole-part GETs (not hashed: they are consumed here) -> batch_transcode_resplit_kernel
+// writes every request's object bytes into the destination slot's staging in the PUT layout -> the destination codec's encode and
+// frame scatter of a merged PUT batch into every caller's out files.  The destination codec's slot with the same index holds the
+// destination side (as emit_transcode uses it), so the six batches in flight never share staging.
+static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
+  mec_codec* c = b->codec;
+  mec_codec* e = b->dst;
+  const int si = static_cast<int>(&s - c->slots);
+  Slot& d = e->slots[si];
+  BatchGetParams gp;
+  ReadLayout lay;
+  int rc = batch_read_plan(b, s, reqs, gp, lay);
+  if (rc) return rc;
+  const size_t nreq = reqs.size();
+  const int ek = e->k, en = e->n;
+  const int64_t bs = e->block_size, eS = e->S(), epitch = round_up(eS, 16);
+  int64_t total_full = 0, ntails = 0, tail_bytes = 0;
+  for (BatchReq* r : reqs) {
+    total_full += r->total / bs;
+    if (r->total % bs) { ntails++; tail_bytes += round_up(r->total % bs, 256); }
+  }
+  const int64_t nslots = total_full + ntails;
+  if ((rc = d.src.ensure(static_cast<size_t>(total_full * bs + tail_bytes + 512)))) return rc;
+  if ((rc = d.out.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * std::max(e->m, 1) * epitch)))) return rc;
+  if ((rc = d.dig.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * en * 32)))) return rc;
+  if ((rc = d.hreq.ensure(nreq * sizeof(BatchReqDesc)))) return rc;
+  if ((rc = d.dreq.ensure(nreq * sizeof(BatchReqDesc)))) return rc;
+  BatchReqDesc* dt = static_cast<BatchReqDesc*>(d.hreq.p);
+  int64_t fb = 0, tb = total_full, toff = total_full * bs, max_nb = 0;
+  for (size_t q = 0; q < nreq; q++) {
+    const BatchReq* r = reqs[q];
+    BatchReqDesc& w = dt[q];
+    memset(&w, 0, sizeof(w));
+    const int64_t nf = r->total / bs, tl = r->total % bs;
+    w.len = r->total; w.with_data = 1;
+    for (int i = 0; i < en; i++) w.files[i] = r->outs[i];
+    w.full0 = fb; w.tail_slot = tl ? tb : -1; w.tail_src_off = tl ? toff : 0;
+    fb += nf;
+    if (tl) { tb++; toff += round_up(tl, 256); }
+    max_nb = std::max(max_nb, nf + (tl ? 1 : 0));
+    c->st_h2d += static_cast<int64_t>(c->k) * mec_bitrot_shard_file_size(mec_shard_file_size(c, r->total), c->S(), MEC_HIGHWAYHASH256S);
+    e->st_d2h += (nf * eS + (tl ? ceil_frac(tl, ek) : 0)) * en;
+  }
+  if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, lay, false))) return rc;
+  MEC_CUDA_OK(cudaMemcpyAsync(d.dreq.p, dt, nreq * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
+  BatchCopyParams cp;
+  cp.reqs = static_cast<const BatchReqDesc*>(d.dreq.p);
+  cp.nreq = static_cast<int>(nreq); cp.k = ek; cp.m = e->m; cp.bs = bs; cp.S = eS; cp.pitch = epitch;
+  cp.staged = static_cast<uint8_t*>(d.src.p); cp.parity = static_cast<const uint8_t*>(d.out.p); cp.digests = static_cast<const uint8_t*>(d.dig.p);
+  const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
+  batch_transcode_resplit_kernel<<<dim3(gx, static_cast<unsigned>(c->k), static_cast<unsigned>(nreq)), 128, 0, s.st>>>(gp, cp);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  if ((rc = batch_encode_scatter(e, d, s.st, dt, nreq, total_full, nslots, max_nb, cp, nullptr))) return rc;
+  if (b->trace) cudaEventRecord(b->ev_ph[si][3], s.st);
+  e->st_blocks_encoded += nslots;
+  *nblocks = lay.nslots();
+  return MEC_OK;
+}
+
 static void batcher_main(mec_batcher* b) {
   mec_codec* c = b->codec;
   cudaSetDevice(c->device);
@@ -2848,7 +2959,7 @@ static void batcher_main(mec_batcher* b) {
         // gather: whatever is queued now; when nothing is in flight, give concurrent callers max_wait_us to join
         auto req_blocks = [&](const BatchReq* r) -> int64_t {
           return r->kind == 0 ? ceil_frac(r->len, c->block_size)
-                 : r->kind == 2 ? ceil_frac(r->total, c->block_size)
+                 : r->kind >= 2 ? ceil_frac(r->total, c->block_size)
                                 : (r->length / c->block_size + 2);
         };
         auto blocks_queued = [&] {
@@ -2860,7 +2971,7 @@ static void batcher_main(mec_batcher* b) {
         // (waiting while batches are in flight only adds latency to a closed loop of callers)
         if (nbusy == 0 && b->max_wait_us > 0 && blocks_queued() < b->max_blocks)
           b->cv_work.wait_for(lk, std::chrono::microseconds(b->max_wait_us), [&] { return b->stop || blocks_queued() >= b->max_blocks; });
-        // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs and heals, the same reader
+        // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs, heals and transcodes, the same reader
         // set; for heals also the same stale drives — unless b->mix: then reads of other patterns join while the batch's blocks fit
         // one latency launch, and a batch of several patterns is cut at that limit)
         // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.45 ms however few
@@ -2905,7 +3016,12 @@ static void batcher_main(mec_batcher* b) {
         std::lock_guard<std::mutex> lk(c->mu);
         fb.is_get = reqs.front()->kind != 0;
         fb.get_k = c->k;
-        if (fb.is_get) {
+        if (reqs.front()->kind == 3) {
+          std::lock_guard<std::mutex> lk_dst(b->dst->mu);  // source, then destination: mec_transcode's order
+          rc = batcher_submit_transcode(b, s, reqs, &nblocks);
+          if (rc != MEC_OK)
+            for (BatchReq* r : reqs) r->ch.s = &s;
+        } else if (fb.is_get) {
           rc = reqs.front()->kind == 2 ? batcher_submit_heal(b, s, reqs, &nblocks) : batcher_submit_get(b, s, reqs, &nblocks);
           if (rc != MEC_OK)
             for (BatchReq* r : reqs) r->ch.s = &s;  // batcher_finish looks the slot up through the first request
@@ -2958,22 +3074,26 @@ static void batcher_main(mec_batcher* b) {
 }
 }  // namespace
 
-extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
-                                  mec_batcher** out) {
-  if (!out) return MEC_ERR_INVALID_ARGUMENT;
-  *out = nullptr;
-  if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;
+// mec_batcher_new_ex, and with `dst` (a codec of the destination geometry without an engine yet, owned from here on, freed on
+// failure) mec_batcher_new_transcode: the destination's engine and slots are set up before the worker starts
+static int batcher_create(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
+                          mec_codec* dst, mec_batcher** out) {
   mec_codec* c = nullptr;
   int rc = mec_codec_new(k, m, block_size, MEC_HIGHWAYHASH256S, device, &c);
-  if (rc) return rc;
+  if (rc) { mec_codec_free(dst); return rc; }
   {
     std::lock_guard<std::mutex> lk(c->mu);
     rc = ensure_engine(c);
   }
-  if (rc) { mec_codec_free(c); return rc; }
-  if (c->S() >= (1ll << 31)) { mec_codec_free(c); return MEC_ERR_UNSUPPORTED; }
+  if (rc == MEC_OK && dst) {
+    std::lock_guard<std::mutex> lk(dst->mu);
+    rc = ensure_engine(dst);
+  }
+  if (rc == MEC_OK && (c->S() >= (1ll << 31) || (dst && dst->S() >= (1ll << 31)))) rc = MEC_ERR_UNSUPPORTED;
+  if (rc) { mec_codec_free(c); mec_codec_free(dst); return rc; }
   mec_batcher* b = new mec_batcher;
   b->codec = c;
+  b->dst = dst;
   b->mix = (flags & MEC_BATCHER_MIX_PATTERNS) && c->eng->small_ok(c->opt, 1);  // per-block decode plans exist in the latency kernel only
   if (max_batch_blocks > 0) b->max_blocks = max_batch_blocks;
   // a merged batch stages at most 1 GiB of object bytes: six slots are sized for a full batch up front (below)
@@ -3012,9 +3132,24 @@ extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, 
       if (rc == MEC_OK) rc = s.hcrc.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
     }
     if (rc == MEC_OK) rc = ensure_crc(c);
+    if (dst) {
+      // the destination side of a merged transcode batch, laid out as a merged PUT batch of the destination geometry: object bytes,
+      // parity rows, digests, the PUT request table and the latency kernel's block table
+      std::lock_guard<std::mutex> lk_dst(dst->mu);
+      const int64_t epitch = round_up(dst->S(), 16);
+      for (Slot& s : dst->slots) {
+        if (rc == MEC_OK) rc = s.src.ensure(static_cast<size_t>(slots * block_size));
+        if (rc == MEC_OK) rc = s.out.ensure(static_cast<size_t>(slots * std::max(dst->m, 1) * epitch));
+        if (rc == MEC_OK) rc = s.dig.ensure(static_cast<size_t>(slots * dst->n * 32));
+        if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
+        if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
+        if (rc == MEC_OK) rc = s.blk.ensure(static_cast<size_t>(slots) * sizeof(SmallBlock));
+        if (rc == MEC_OK) rc = s.hblk.ensure(static_cast<size_t>(slots) * sizeof(SmallBlock));
+      }
+    }
     cudaSetDevice(cur);
   }
-  if (rc) { mec_codec_free(c); delete b; return rc; }
+  if (rc) { mec_codec_free(c); mec_codec_free(dst); delete b; return rc; }
   b->trace = getenv("MEC_BATCHER_TRACE") != nullptr;
   if (b->trace) {
     int cur = 0;
@@ -3041,6 +3176,26 @@ extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, 
   *out = b;
   return MEC_OK;
 }
+extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
+                                  mec_batcher** out) {
+  if (!out) return MEC_ERR_INVALID_ARGUMENT;
+  *out = nullptr;
+  if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;
+  return batcher_create(k, m, block_size, device, max_batch_blocks, max_wait_us, flags, nullptr, out);
+}
+extern "C" int mec_batcher_new_transcode(int k, int m, int dst_k, int dst_m, int64_t block_size, int device, int64_t max_batch_blocks,
+                                         int max_wait_us, int flags, mec_batcher** out) {
+  if (!out) return MEC_ERR_INVALID_ARGUMENT;
+  *out = nullptr;
+  if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;
+  mec_codec* probe = nullptr;
+  int rc = mec_codec_new(k, m, block_size, MEC_HIGHWAYHASH256S, device, &probe);  // the source geometry's errors come first
+  mec_codec_free(probe);
+  if (rc) return rc;
+  mec_codec* dst = nullptr;
+  if ((rc = mec_codec_new(dst_k, dst_m, block_size, MEC_HIGHWAYHASH256S, device, &dst))) return rc;
+  return batcher_create(k, m, block_size, device, max_batch_blocks, max_wait_us, flags, dst, out);
+}
 extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out) {
   return mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, 0, out);
 }
@@ -3061,6 +3216,8 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
   }
   if (b->aux) cudaStreamDestroy(b->aux);
   mec_codec_free(b->serial);
+  mec_codec_free(b->serial_dst);
+  mec_codec_free(b->dst);
   mec_codec_free(b->codec);
   delete b;
 }
@@ -3207,6 +3364,42 @@ extern "C" int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, con
   return static_cast<int>(batcher_enqueue_wait(b, r));
 }
 
+// mec_transcode through the coalescer: moves queued together that read the same k drives (any, with MEC_BATCHER_MIX_PATTERNS) are
+// merged into one batch.  Moves the merged path cannot take (pageable buffers, more drives than the kernels' tables hold, parts of
+// more than max_batch_blocks blocks, which mec_transcode pipelines over its slots anyway) and moves that meet bitrot run on their own
+// through mec_transcode on the private pair.
+extern "C" int64_t mec_batcher_transcode(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
+                                         uint8_t* const* out_files, int write_quorum, int* heal_hint) {
+  if (heal_hint) *heal_hint = 0;
+  if (!b || !b->dst || !files || !out_files || total < 0) return MEC_ERR_INVALID_ARGUMENT;
+  mec_codec* c = b->codec;
+  mec_codec* e = b->dst;
+  int online = 0;
+  for (int i = 0; i < e->n; i++) online += out_files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  if (total == 0) return 0;
+  const int n = c->n, k = c->k;
+  auto serial = [&]() -> int64_t { return batcher_transcode_serial(b, files, prefer, total, out_files, write_quorum, heal_hint); };
+  if (n > kBatchMaxFiles || e->n > kBatchMaxFiles) return serial();
+  // the readers parallelReader would pick, chosen here on the caller's thread: equal reader sets share a batch
+  uint8_t alive[kBatchMaxFiles];
+  int chosen[kBatchMaxFiles];
+  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
+  if (choose_readers(c, files, alive, prefer, chosen) < k) return MEC_ERR_READ_QUORUM;
+  BatchReq r;
+  r.kind = 3; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
+  r.prefer = prefer; r.outs = out_files; r.heal_hint = heal_hint;
+  bool mapped = getenv("MEC_BATCHER_MEMCPY") == nullptr;
+  for (int t = 0; t < k; t++) {
+    r.alive_mask |= 1ull << chosen[t];
+    mapped = mapped && mec_is_pinned(files[chosen[t]]) != 0;
+  }
+  for (int i = 0; i < e->n && mapped; i++)
+    if (out_files[i]) mapped = mec_is_pinned(out_files[i]) != 0;
+  if (!mapped || ceil_frac(total, c->block_size) > b->max_blocks) return serial();
+  return batcher_enqueue_wait(b, r);
+}
+
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!b || !name) return -1;
   if (!strcmp(name, "batches")) return b->st_batches.load();
@@ -3225,5 +3418,8 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "us_stage")) return b->us_stage.load();
   if (!strcmp(name, "us_kernel")) return b->us_kernel.load();
   if (!strcmp(name, "us_scatter")) return b->us_scatter.load();
+  if (!strcmp(name, "transcodes")) return b->st_transcodes.load();
+  if (!strcmp(name, "transcodes_serial")) return b->st_transcodes_serial.load();
+  if (!strncmp(name, "dst_", 4)) return b->dst ? mec_get_stat(b->dst, name + 4) : -1;  // the destination codec of merged moves
   return mec_get_stat(b->codec, name);  // the batcher's codec: which kernel forms its merged launches ran ("form_*", "last_*", ...)
 }

@@ -10,6 +10,11 @@
 //   mode bget_rot / bheal_rot : bget / bheal as MinIO lays objects out: thread t's object has its shard indices rotated by t % n over
 //                  the drives (hashOrder, cmd/erasure-metadata-utils.go:178), and ONE physical drive (drive 0) is offline (GET) or
 //                  stale (heal) — so the shard it held rotates from object to object: n erasure patterns in every round of requests
+//   mode btranscode : moves of whole parts from RS(12,4) to the destination geometry DST="k2,m2" (default 6,2; decommission and
+//                  rebalance, mec_batcher_transcode) through ONE transcode batcher (mec_batcher_new_transcode)
+//   mode transcode : the same moves, each a mec_transcode call on the handle pair t % P (source and destination codec)
+//   btranscode_rot / transcode_rot : as bget_rot, drive 0 offline and thread t's object rotated by t % n
+//                  (after the timed window every thread's out files are compared with a plain mec_encode on the destination geometry)
 //   MIX=1        : the batcher of the b* modes is created with MEC_BATCHER_MIX_PATTERNS (reads of different patterns share batches)
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
 // Prints one JSON line: aggregate GiB/s, calls/s, p50/p99 latency.  Buffers are pinned (mec_alloc_pinned_on) for the GPU modes.
@@ -55,7 +60,7 @@ int main(int argc, char** argv) {
   signal(SIGSEGV, on_segv);
   signal(SIGABRT, on_segv);
   std::string mode = argc > 1 ? argv[1] : "batcher";
-  const bool rot = mode == "bget_rot" || mode == "bheal_rot";
+  const bool rot = mode == "bget_rot" || mode == "bheal_rot" || mode == "btranscode_rot" || mode == "transcode_rot";
   if (rot) mode.resize(mode.size() - 4);
   const std::string mode_name = rot ? mode + "_rot" : mode;
   const int bflags = getenv("MIX") && atoi(getenv("MIX")) ? MEC_BATCHER_MIX_PATTERNS : 0;
@@ -73,10 +78,18 @@ int main(int argc, char** argv) {
   mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &probe);
   const int64_t S = mec_shard_size(probe), fsz = mec_bitrot_shard_file_size(mec_shard_file_size(probe, osize), S, MEC_HIGHWAYHASH256S);
   const int64_t nb = (osize + bs - 1) / bs;
+  const bool move = mode == "btranscode" || mode == "transcode";
+  int k2 = 6, m2 = 2;
+  if (const char* e = getenv("DST")) sscanf(e, "%d,%d", &k2, &m2);
+  const int n2 = k2 + m2;
+  mec_codec* probe2 = nullptr;
+  mec_codec_new(k2, m2, bs, MEC_HIGHWAYHASH256S, device, &probe2);
+  const int64_t fsz2 = mec_bitrot_shard_file_size(mec_shard_file_size(probe2, osize), mec_shard_size(probe2), MEC_HIGHWAYHASH256S);
   if (gpu) mec_bind_thread_to_device(device);
   auto alloc = [&](size_t b) -> uint8_t* { return gpu ? static_cast<uint8_t*>(mec_alloc_pinned_on(device, b)) : static_cast<uint8_t*>(malloc(b)); };
   // per-thread buffers: object, 16 part files, digests, destination, the healed part file
-  struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; uint64_t crc[3]; };
+  struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; uint64_t crc[3];
+              std::vector<uint8_t*> outs; };  // outs: the destination part files of the transcode modes
   std::vector<TB> tb(T);
   uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
   if (!arena) { fprintf(stderr, "allocation failed\n"); return 1; }
@@ -91,14 +104,19 @@ int main(int argc, char** argv) {
     tb[t].dst = take(osize);
     tb[t].parity = take(nb * m * S);
     tb[t].healed = take(fsz);
+    if (move)
+      for (int i = 0; i < n2; i++) {
+        tb[t].outs.push_back(alloc(static_cast<size_t>(fsz2)));
+        if (!tb[t].outs.back()) { fprintf(stderr, "allocation failed\n"); return 1; }
+      }
   }
   mec_batcher* bat = nullptr;
-  std::vector<mec_codec*> pool;
+  std::vector<mec_codec*> pool, pool2;
   if (mode == "batcher" || mode == "batcher_crc") {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
-  } else if (gpu && mode != "bget" && mode != "bheal") {
+  } else if (gpu && mode != "bget" && mode != "bheal" && mode != "btranscode") {
     for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
   }
   if (mode == "bget" || mode == "bheal") {  // coalesced GETs / heals: part files through a temporary handle, then everything goes through the batcher
@@ -111,6 +129,21 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
+  }
+  if (move) {  // source part files through a temporary handle; the transcode batcher, or the pool's destination handles
+    mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c0);
+    for (int t = 0; t < T; t++) {
+      std::vector<uint8_t*> f(tb[t].files);
+      if (mec_encode(c0, tb[t].obj, osize, f.data(), k) != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
+    }
+    mec_codec_free(c0);
+    if (mode == "btranscode") {
+      int rc = mec_batcher_new_transcode(k, m, k2, m2, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
+                                         getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
+      if (rc) { fprintf(stderr, "transcode batcher: %d %s\n", rc, mec_last_error()); return 1; }
+    } else {
+      for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k2, m2, bs, MEC_HIGHWAYHASH256S, device, &c); pool2.push_back(c); }
+    }
   }
   if (mode == "get" || mode == "heal") {  // every thread's part files must exist first
     for (int t = 0; t < T; t++) {
@@ -150,6 +183,13 @@ int main(int argc, char** argv) {
       const int rc = mode == "bheal" ? mec_batcher_heal(bat, f, nullptr, osize, o, bad) : mec_heal_prefer(pool[t % P], f, nullptr, osize, o, bad);
       return rc == MEC_OK ? osize : rc;
     }
+    if (move) {  // drive 0 offline in the _rot modes
+      const uint8_t* f[64];
+      for (int i = 0; i < n; i++) f[i] = rot && i == drive0_shard(t) ? nullptr : b.files[i];
+      int hint = 0;
+      return mode == "btranscode" ? mec_batcher_transcode(bat, f, nullptr, osize, b.outs.data(), k2, &hint)
+                                  : mec_transcode(pool[t % P], f, nullptr, osize, pool2[t % P], b.outs.data(), k2, &hint);
+    }
     orc_encode_hash_blocks_st(k, m, bs, b.obj, nb, b.parity, b.dd);
     return osize;
   };
@@ -174,6 +214,16 @@ int main(int argc, char** argv) {
   if (mode == "bheal" || mode == "heal")  // every healed part file equals the drive's original one
     for (int t = 0; t < T; t++)
       if (memcmp(tb[t].healed, tb[t].files[drive0_shard(t)], static_cast<size_t>(fsz)) != 0) errors++;
+  if (move) {  // every destination part file equals what a plain mec_encode of the destination geometry writes
+    std::vector<uint8_t*> want(n2);
+    for (int i = 0; i < n2; i++) want[i] = static_cast<uint8_t*>(malloc(static_cast<size_t>(fsz2)));
+    for (int t = 0; t < T; t++) {
+      if (mec_encode(probe2, tb[t].obj, osize, want.data(), k2) != osize) { errors++; continue; }
+      for (int i = 0; i < n2; i++)
+        if (memcmp(tb[t].outs[i], want[i], static_cast<size_t>(fsz2)) != 0) errors++;
+    }
+    for (auto w : want) free(w);
+  }
   if (mode == "batcher_crc")  // every thread's object checksums equal the host's
     for (int t = 0; t < T; t++)
       if (tb[t].crc[0] != host_crc(tb[t].obj, osize, 0xEDB88320ull, 32) || tb[t].crc[1] != host_crc(tb[t].obj, osize, 0x82F63B78ull, 32) ||
@@ -198,11 +248,17 @@ int main(int argc, char** argv) {
            (long long)mec_batcher_stat(bat, "us_submit"), (long long)mec_batcher_stat(bat, "us_sync"), (long long)mec_batcher_stat(bat, "us_finish"),
            (long long)mec_batcher_stat(bat, "us_idle"), (long long)mec_batcher_stat(bat, "us_stage"), (long long)mec_batcher_stat(bat, "us_kernel"),
            (long long)mec_batcher_stat(bat, "us_scatter"));
-  if (mode == "pool" || mode == "get" || mode == "heal") printf(", \"pool\": %d", P);
+  if (move) printf(", \"dst\": \"%d,%d\"", k2, m2);
+  if (mode == "btranscode")
+    printf(", \"transcodes\": %lld, \"transcodes_serial\": %lld, \"redone\": %lld", static_cast<long long>(mec_batcher_stat(bat, "transcodes")),
+           static_cast<long long>(mec_batcher_stat(bat, "transcodes_serial")), static_cast<long long>(mec_batcher_stat(bat, "redone")));
+  if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode") printf(", \"pool\": %d", P);
   printf("}\n");
   if (bat) mec_batcher_free(bat);
   for (auto c : pool) mec_codec_free(c);
+  for (auto c : pool2) mec_codec_free(c);
   mec_codec_free(probe);
+  mec_codec_free(probe2);
   mec_shutdown();  // no NVRTC compile may be in flight when the C runtime runs its exit handlers (a degraded-GET pattern warms up during the run)
   return errors.load() ? 2 : 0;
 }

@@ -112,6 +112,17 @@ for t, (fs, crc) in enumerate(res):
 assert all(np.array_equal(x, y) for x, y in zip(res[0][0], want[0]))
 assert bat.stat("batches") == 1 and bat.stat("crc_requests") == 3
 bat.close()
+# one merged transcode round: four moves RS(12,4) -> RS(6,2) with source drive 1 offline in one batch (staging, fused reconstruct,
+# batch_transcode_resplit_kernel, the destination's encode and frame scatter)
+bat = mb.Batcher(k, m, bs, max_batch_blocks=sum(-(-a.size // bs) for a in pin), max_wait_us=500000, dst=(6, 2))
+tw = [o.erasure_encode(6, 2, bs, 3, a)[0] for a in pin]
+res = [None] * 4
+def move(t): res[t] = bat.transcode(rd[t], pin[t].size, pinned=True)
+th = [threading.Thread(target=move, args=(t,)) for t in range(4)]
+[x.start() for x in th]; [x.join() for x in th]
+assert all(r[1] == 0 and all(np.array_equal(x, y) for x, y in zip(r[0], tw[t])) for t, r in enumerate(res))
+assert bat.stat("batches") == 1 and bat.stat("transcodes") == 4
+bat.close()
 print("sanitizer case ok")
 PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
