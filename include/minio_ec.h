@@ -201,7 +201,8 @@ int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, const uint8_t
  * set plus rebuilt shards — summed over GET and heal batches) and "mixed_batches" (GET and heal batches of more than one pattern);
  * with MEC_BATCHER_TRACE=1 in the environment also the worker's and the streams' accumulated phase times "us_submit", "us_sync",
  * "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter".  Any other name is answered by mec_get_stat on the batcher's own
- * codec, so "form_*", "last_*", "small_launches", "num_sms" and the rest describe the merged launches. */
+ * codec, so "form_*", "last_*", "small_launches", "num_sms" and the rest describe the merged launches.
+ * The MEC_BATCHER_* environment switches (MEC_BATCHER_TRACE, MEC_BATCHER_MEMCPY, ...) are read once, when the batcher is created. */
 typedef struct mec_batcher mec_batcher;
 int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out);
 /* mec_batcher_new with creation flags (mec_batcher_new is flags = 0); unknown bits return MEC_ERR_INVALID_ARGUMENT.

@@ -2119,9 +2119,13 @@ extern "C" int mec_selftest(int device) {
 #include <deque>
 #include <unordered_map>
 
+enum class ReqKind { Put, Get, Heal, Transcode };  // PutObject (encode), GetObject (decode), Heal, a move between pools
+// a GET, heal or transcode: stages survivor frames, and per-frame digest verdicts decide which of its requests are done
+static inline bool is_read(ReqKind k) { return k != ReqKind::Put; }
+
 struct BatchReq {
-  int kind = 0;                      // 0 = PutObject (encode), 1 = GetObject (decode), 2 = Heal, 3 = transcode (move between pools)
-  // GET, heal and transcode (a heal and a transcode read the whole part: offset 0, length = total; a transcode writes `outs`)
+  ReqKind kind = ReqKind::Put;
+  // GET, heal and transcode (a heal and a transcode read the whole part: offset 0, length = total)
   const uint8_t* const* gfiles = nullptr;
   int64_t offset = 0, length = 0, total = 0;
   uint8_t* dst = nullptr;
@@ -2133,7 +2137,7 @@ struct BatchReq {
   uint8_t* const* outs = nullptr;
   uint8_t* corrupt = nullptr;
   uint64_t stale_mask = 0;           // bit i = out_files[i] != NULL: heals share a launch only with the same stale drives
-  // PUT
+  // PUT, and the destination side of a transcode (len = total, files = out_files, with_data): both laid out by put_layout
   const uint8_t* src = nullptr;
   int64_t len = 0;
   uint8_t* const* files = nullptr;
@@ -2155,6 +2159,17 @@ struct BatchPattern {
 };
 constexpr size_t kMaxCachedPatterns = 4096;
 
+// The environment switches of the coalescer's staging and output paths, read once per batcher by batcher_create
+struct BatcherSwitches {
+  bool memcpy = false;     // MEC_BATCHER_MEMCPY: PUTs take the copy-engine path, reads and moves the private handles
+  bool gather = false;     // MEC_BATCHER_GATHER: the gather kernel stages every PUT
+  int gather_pct = 0;      // MEC_BATCHER_GATHER_PCT (0-100): that share of a PUT batch is staged by the gather kernel on `aux`
+  int64_t dma_blocks = 1;  // MEC_BATCHER_DMA_BLOCKS: reads of fewer blocks are staged by the gather kernel
+  int get_out = 0;         // MEC_BATCHER_GET_OUT: how merged GETs reach the callers' buffers (batcher_submit_get)
+  int depth = 4;           // MEC_BATCHER_DEPTH: batches the worker aims to keep in flight (0: cut batches at max_batch_blocks only)
+  bool trace = false;      // MEC_BATCHER_TRACE: device phase times of every kernel batch (mec_batcher_stat "us_stage", ...)
+};
+
 struct mec_batcher {
   mec_codec* codec = nullptr;
   mec_codec* serial = nullptr;       // private handle for calls that cannot ride in a batch (pageable buffers, bitrot fail-over)
@@ -2175,12 +2190,11 @@ struct mec_batcher {
   std::atomic<int64_t> st_patterns{0}, st_mixed{0};  // distinct patterns summed over read batches; read batches of more than one
   // decode plans by (reader mask, target mask), owned by the worker thread: a steady workload inverts no matrix
   std::unordered_map<uint64_t, BatchPattern> patterns;
-  // hybrid staging: part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
+  BatcherSwitches sw;
+  // hybrid staging (sw.gather_pct): part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
   cudaStream_t aux = nullptr;
   cudaEvent_t ev_table[kSlots] = {}, ev_gather[kSlots] = {};
-  int gather_pct = 0;
-  // where the worker's time and each batch's stream time go (mec_batcher_stat "us_*"); device phases need MEC_BATCHER_TRACE=1
-  bool trace = false;
+  // where the worker's time and each batch's stream time go (mec_batcher_stat "us_*"); device phases need sw.trace
   cudaEvent_t ev_ph[kSlots][4] = {};
   std::atomic<int64_t> us_submit{0}, us_sync{0}, us_finish{0}, us_idle{0}, us_stage{0}, us_kernel{0}, us_scatter{0};
   // mec_batcher_new_transcode: the destination codec of merged moves (private; its slot i carries the destination side of the batch
@@ -2193,53 +2207,47 @@ struct mec_batcher {
 namespace {
 struct InflightBatch {
   std::vector<BatchReq*> reqs;
-  bool busy = false;
+  ReqKind kind = ReqKind::Put;
   bool needs_retire = true;  // false: the scatter kernel already assembled the frames
-  bool is_get = false;       // a GET or heal batch: per-frame digest verdicts decide which requests are done
   bool traced = false;
-  int get_k = 0;
 };
 
-static mec_codec* batcher_serial(mec_batcher* b) {
+// The private handle `h` of `g`'s geometry, created on first use
+static mec_codec* batcher_private(mec_batcher* b, const mec_codec* g, mec_codec*& h) {
   std::lock_guard<std::mutex> lk(b->serial_mu);
-  if (!b->serial) {
-    mec_codec* c = nullptr;
-    if (mec_codec_new(b->codec->k, b->codec->m, b->codec->block_size, MEC_HIGHWAYHASH256S, b->codec->device, &c) == MEC_OK) b->serial = c;
+  if (!h) {
+    mec_codec* p = nullptr;
+    if (mec_codec_new(g->k, g->m, g->block_size, MEC_HIGHWAYHASH256S, g->device, &p) == MEC_OK) h = p;
   }
-  return b->serial;
+  return h;
 }
 
-// mec_transcode on the private pair (serial, serial_dst), for moves that cannot ride in a merged batch and for the redo of one that
-// met bitrot in a merged batch
-static int64_t batcher_transcode_serial(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
-                                        uint8_t* const* out_files, int write_quorum, int* heal_hint) {
-  b->st_transcodes_serial++;
-  mec_codec* sc = batcher_serial(b);
-  mec_codec* sd = nullptr;
-  {
-    std::lock_guard<std::mutex> lk(b->serial_mu);
-    if (!b->serial_dst) {
-      mec_codec* e = nullptr;
-      if (mec_codec_new(b->dst->k, b->dst->m, b->dst->block_size, MEC_HIGHWAYHASH256S, b->dst->device, &e) == MEC_OK) b->serial_dst = e;
-    }
-    sd = b->serial_dst;
+// A read or move on its own, through the private handles: a call the merged path cannot take, or the redo of a merged one that met
+// a frame failing its digest, which applies parallelReader's block-sequential fail-over exactly (a heal rewrites every out file in
+// full and reports the failing readers; a transcode rewrites every out file in full through mec_transcode on the private pair, its
+// write quorum already checked on the caller's thread)
+static int64_t batcher_run_alone(mec_batcher* b, const BatchReq& r) {
+  if (r.kind == ReqKind::Transcode) b->st_transcodes_serial++;
+  mec_codec* sc = batcher_private(b, b->codec, b->serial);
+  if (r.kind == ReqKind::Transcode) {
+    mec_codec* sd = batcher_private(b, b->dst, b->serial_dst);
+    return sc && sd ? mec_transcode(sc, r.gfiles, r.prefer, r.total, sd, r.files, 0, r.heal_hint) : MEC_ERR_UNEXPECTED;
   }
-  return sc && sd ? mec_transcode(sc, files, prefer, total, sd, out_files, write_quorum, heal_hint) : MEC_ERR_UNEXPECTED;
+  if (!sc) return MEC_ERR_UNEXPECTED;
+  if (r.kind == ReqKind::Heal) return mec_heal_prefer(sc, r.gfiles, r.prefer, r.total, r.outs, r.corrupt);
+  return mec_decode_prefer(sc, r.gfiles, r.prefer, r.offset, r.length, r.total, r.dst, r.heal_hint);
 }
 
-static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
+// Completes the batch that ran on slot `s` (rc: how its stream ended) and wakes its callers.
+static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int rc) {
   mec_codec* c = b->codec;
-  if (fb.is_get) {
-    // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own through the serial
-    // handle, which applies parallelReader's block-sequential fail-over exactly (a heal rewrites every out file in full and reports
-    // the failing readers, a transcode rewrites every out file in full through mec_transcode on the private pair); the others are
-    // done (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
-    Slot& s = *fb.reqs.front()->ch.s;
+  if (is_read(fb.kind)) {
+    // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own; the others are done
+    // (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
     const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
-    const int k = fb.get_k;
+    const int k = c->k;
     for (BatchReq* r : fb.reqs) {
-      const bool heal = r->kind == 2, move = r->kind == 3;
-      int64_t res = rc != MEC_OK ? rc : heal ? MEC_OK : move ? r->total : r->length;
+      int64_t res = rc != MEC_OK ? rc : r->kind == ReqKind::Heal ? MEC_OK : r->kind == ReqKind::Transcode ? r->total : r->length;
       if (rc == MEC_OK) {
         bool bad = false;
         for (int64_t bb = 0; bb < r->get_nblocks && !bad; bb++) {
@@ -2248,46 +2256,37 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, int rc) {
         }
         if (bad) {
           b->st_redone++;
-          if (move) {
-            res = batcher_transcode_serial(b, r->gfiles, r->prefer, r->total, r->outs, 0, r->heal_hint);
-          } else {
-            mec_codec* sc = batcher_serial(b);
-            if (!sc) res = MEC_ERR_UNEXPECTED;
-            else if (heal) res = mec_heal_prefer(sc, r->gfiles, r->prefer, r->total, r->outs, r->corrupt);
-            else res = mec_decode_prefer(sc, r->gfiles, r->prefer, r->offset, r->length, r->total, r->dst, r->heal_hint);
-          }
+          res = batcher_run_alone(b, *r);
         } else {
           if (r->heal_hint) *r->heal_hint = 0;
-          if (move) b->st_transcodes++;
+          if (r->kind == ReqKind::Transcode) b->st_transcodes++;
         }
       }
       r->result = res;
     }
-    {
-      std::lock_guard<std::mutex> lk(b->mu);
-      for (BatchReq* r : fb.reqs) { r->done = true; r->cv.notify_one(); }
+  } else {
+    for (size_t q = 0; q < fb.reqs.size(); q++) {
+      BatchReq* r = fb.reqs[q];
+      if (rc == MEC_OK && fb.needs_retire) frames_retire(c, r->ch, r->files, r->with_data, r->data_digests);
+      if (rc == MEC_OK && r->crc_which) {  // batcher_crc_enqueue's results, row q of the slot's pinned mirror
+        const uint64_t* h = static_cast<const uint64_t*>(s.hcrc.p) + q * kCrcTypes;
+        for (int ty = 0; ty < kCrcTypes; ty++) r->crc_out[ty] = h[ty];
+        b->st_crc_requests++;
+      }
+      r->result = rc == MEC_OK ? r->len : rc;
     }
-    fb.reqs.clear();
-    fb.busy = false;
-    fb.is_get = false;
-    return;
-  }
-  for (size_t q = 0; q < fb.reqs.size(); q++) {
-    BatchReq* r = fb.reqs[q];
-    if (rc == MEC_OK && fb.needs_retire) frames_retire(c, r->ch, r->files, r->with_data, r->data_digests);
-    if (rc == MEC_OK && r->crc_which) {  // batcher_crc_enqueue's results, row q of the slot's pinned mirror
-      const uint64_t* h = static_cast<const uint64_t*>(r->ch.s->hcrc.p) + q * kCrcTypes;
-      for (int ty = 0; ty < kCrcTypes; ty++) r->crc_out[ty] = h[ty];
-      b->st_crc_requests++;
-    }
-    r->result = rc == MEC_OK ? r->len : rc;
   }
   {
     std::lock_guard<std::mutex> lk(b->mu);
     for (BatchReq* r : fb.reqs) { r->done = true; r->cv.notify_one(); }  // under the lock: `r` lives on its caller's stack
   }
   fb.reqs.clear();
-  fb.busy = false;
+}
+
+// With sw.trace, records mark j of the batch on the batcher's slot `s`: 0 before staging, 1 staged, 2 encoded or rebuilt, 3 done
+// (mec_batcher_stat "us_stage", "us_kernel" and "us_scatter" sum the gaps)
+static void mark_phase(mec_batcher* b, Slot& s, int j) {
+  if (b->sw.trace) cudaEventRecord(b->ev_ph[&s - b->codec->slots][j], s.st);
 }
 
 // Object checksums of the PUTs of a batch that asked for them (mec_batcher_encode_crc).  Request q's bytes are two segments of s.src,
@@ -2357,16 +2356,71 @@ static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
   return MEC_OK;
 }
 
-// Encode and frame scatter of a staged batch in the PUT layout (`tab`: every request's full blocks contiguous from s.src, its short
-// last block at tail_src_off; parity rows in s.out, digests in s.dig, `cp` describes them): ONE latency launch with a per-block
-// geometry table when the batch fits one, otherwise one launch over all full blocks plus one per short block; then the scatter
-// kernel writes every frame into every caller's part-file images.  Used by merged PUTs on the batcher's codec and by merged
-// transcodes on the destination codec (slot `s` of codec `c`, enqueued on stream `st`).  `ev_encoded` (may be null) is recorded
-// between the encode and the scatter.
-static int batch_encode_scatter(mec_codec* c, Slot& s, cudaStream_t st, const BatchReqDesc* tab, size_t nreq, int64_t total_full,
-                                int64_t nslots, int64_t max_nb, const BatchCopyParams& cp, cudaEvent_t ev_encoded) {
+// The PUT layout of a merged batch on slot `s` of codec `c`, in request order: every request's full blocks contiguous from s.src
+// (from block full0 on), the short last blocks behind all of them at 256-byte-rounded offsets (block tail_slot, byte tail_src_off);
+// parity rows [block][m][pitch] in s.out, digests [block][n][32] in s.dig.  A request is r->len object bytes for the frames in
+// r->files.  Sizes those buffers and fills request q's row of the BatchReqDesc table in s.hreq (`rows`) and / or its EncChunk
+// r->ch, whose digests come back to s.hdig (`chunks`).
+struct PutLayout {
+  int64_t total_full = 0, nslots = 0, max_nb = 0;  // full blocks, all blocks, the most blocks of one request
+};
+static int put_layout(mec_codec* c, Slot& s, const std::vector<BatchReq*>& reqs, bool rows, bool chunks, PutLayout& lay) {
+  const int m = c->m, n = c->n;
+  const int64_t bs = c->block_size, pitch = round_up(c->S(), 16);
+  int64_t ntails = 0, tail_bytes = 0;
+  for (const BatchReq* r : reqs) {
+    lay.total_full += r->len / bs;
+    if (r->len % bs) { ntails++; tail_bytes += round_up(r->len % bs, 256); }
+  }
+  lay.nslots = lay.total_full + ntails;
+  const int64_t nb1 = std::max<int64_t>(lay.nslots, 1);
+  int rc;
+  if ((rc = s.src.ensure(static_cast<size_t>(lay.total_full * bs + tail_bytes + 512)))) return rc;
+  if ((rc = s.out.ensure(static_cast<size_t>(nb1 * std::max(m, 1) * pitch)))) return rc;
+  if ((rc = s.dig.ensure(static_cast<size_t>(nb1 * n * 32)))) return rc;
+  if (chunks && (rc = s.hdig.ensure(static_cast<size_t>(nb1 * n * 32)))) return rc;
+  if (rows && (rc = s.hreq.ensure(reqs.size() * sizeof(BatchReqDesc)))) return rc;
+  if (rows && (rc = s.dreq.ensure(reqs.size() * sizeof(BatchReqDesc)))) return rc;
+  uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
+  uint8_t* dout = static_cast<uint8_t*>(s.out.p);
+  const uint8_t* hdig = static_cast<const uint8_t*>(s.hdig.p);
+  BatchReqDesc* tab = static_cast<BatchReqDesc*>(s.hreq.p);
+  int64_t fb = 0, tb = lay.total_full, toff = lay.total_full * bs;
+  for (size_t q = 0; q < reqs.size(); q++) {
+    BatchReq* r = reqs[q];
+    const int64_t nf = r->len / bs, tl = r->len % bs;
+    if (rows) {
+      BatchReqDesc& d = tab[q];
+      memset(&d, 0, sizeof(d));
+      d.src = r->src; d.len = r->len; d.data_digests = r->data_digests; d.with_data = r->with_data ? 1 : 0;
+      for (int i = 0; i < n; i++) d.files[i] = r->files[i];
+      d.full0 = fb; d.tail_slot = tl ? tb : -1; d.tail_src_off = tl ? toff : 0;
+    }
+    if (chunks) {
+      EncChunk& ch = r->ch;
+      ch = EncChunk();
+      ch.nfull = nf; ch.tail = tl; ch.nb = nf + (tl ? 1 : 0);
+      ch.s = &s; ch.st = s.st; ch.pitch = pitch;
+      ch.d_src = dsrc + fb * bs; ch.d_out = dout + fb * m * pitch; ch.h_dig = hdig + fb * n * 32;
+      if (tl) { ch.d_src_tail = dsrc + toff; ch.d_out_tail = dout + tb * m * pitch; ch.h_dig_tail = hdig + tb * n * 32; }
+    }
+    fb += nf;
+    if (tl) { tb++; toff += round_up(tl, 256); }
+    lay.max_nb = std::max(lay.max_nb, nf + (tl ? 1 : 0));
+  }
+  return MEC_OK;
+}
+
+// Encode and frame scatter of a staged batch in the PUT layout (`tab`, `lay`: put_layout; `cp` describes the staging): ONE latency
+// launch with a per-block geometry table when the batch fits one, otherwise one launch over all full blocks plus one per short
+// block; then the scatter kernel writes every frame into every caller's part-file images.  Used by merged PUTs on the batcher's
+// codec and by merged transcodes on the destination codec (slot `s` of codec `c`, enqueued on stream `st`).  `ev_encoded` (may be
+// null) is recorded between the encode and the scatter.
+static int batch_encode_scatter(mec_codec* c, Slot& s, cudaStream_t st, const BatchReqDesc* tab, size_t nreq, const PutLayout& lay,
+                                const BatchCopyParams& cp, cudaEvent_t ev_encoded) {
   const int k = c->k, m = c->m, n = c->n;
   const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
+  const int64_t total_full = lay.total_full, nslots = lay.nslots;
   uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
   uint8_t* dout = static_cast<uint8_t*>(s.out.p);
   uint8_t* ddig = static_cast<uint8_t*>(s.dig.p);
@@ -2402,7 +2456,7 @@ static int batch_encode_scatter(mec_codec* c, Slot& s, cudaStream_t st, const Ba
         return rc;
   }
   if (ev_encoded) cudaEventRecord(ev_encoded, st);
-  batch_scatter_kernel<<<dim3(static_cast<unsigned>(std::min<int64_t>(max_nb, 16)), static_cast<unsigned>(n), static_cast<unsigned>(nreq)), 128, 0, st>>>(cp);
+  batch_scatter_kernel<<<dim3(static_cast<unsigned>(std::min<int64_t>(lay.max_nb, 16)), static_cast<unsigned>(n), static_cast<unsigned>(nreq)), 128, 0, st>>>(cp);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
   return MEC_OK;
@@ -2414,52 +2468,27 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   const int k = c->k, m = c->m, n = c->n;
   const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
   *needs_retire = true;
-  bool all_mapped = n <= kBatchMaxFiles && getenv("MEC_BATCHER_MEMCPY") == nullptr;
+  bool all_mapped = n <= kBatchMaxFiles && !b->sw.memcpy;
   for (BatchReq* r : reqs) all_mapped &= r->mapped;
-  int64_t total_full = 0, ntails = 0, tail_bytes = 0;
-  for (BatchReq* r : reqs) {
-    total_full += r->len / bs;
-    if (r->len % bs) { ntails++; tail_bytes += round_up(r->len % bs, 256); }
-  }
-  const int64_t nslots = total_full + ntails;
-  *nblocks = nslots;
+  PutLayout lay;
   int rc;
-  if ((rc = s.src.ensure(static_cast<size_t>(total_full * bs + tail_bytes + 512)))) return rc;
-  if ((rc = s.out.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * std::max(m, 1) * pitch)))) return rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * n * 32)))) return rc;
-  if ((rc = s.hdig.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * n * 32)))) return rc;
+  if ((rc = put_layout(c, s, reqs, all_mapped, true, lay))) return rc;
+  const int64_t nslots = lay.nslots;
+  *nblocks = nslots;
   uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
   uint8_t* dout = static_cast<uint8_t*>(s.out.p);
   uint8_t* ddig = static_cast<uint8_t*>(s.dig.p);
-  const uint8_t* hdig = static_cast<const uint8_t*>(s.hdig.p);
-  int64_t fb = 0, tb = total_full, toff = total_full * bs;
   if (all_mapped) {
     // gather kernel -> ONE fused launch over all full blocks (+ one per tail) -> scatter kernel: a handful of launches and one
     // small table copy per batch, whatever the number of requests
-    if ((rc = s.hreq.ensure(reqs.size() * sizeof(BatchReqDesc)))) return rc;
-    if ((rc = s.dreq.ensure(reqs.size() * sizeof(BatchReqDesc)))) return rc;
-    BatchReqDesc* tab = static_cast<BatchReqDesc*>(s.hreq.p);
-    int64_t max_len = 0, max_nb = 0;
-    for (size_t q = 0; q < reqs.size(); q++) {
-      BatchReq* r = reqs[q];
-      BatchReqDesc& d = tab[q];
-      memset(&d, 0, sizeof(d));
+    const BatchReqDesc* tab = static_cast<const BatchReqDesc*>(s.hreq.p);
+    for (const BatchReq* r : reqs) {
       const int64_t nf = r->len / bs, tl = r->len % bs;
-      d.src = r->src; d.len = r->len; d.data_digests = r->data_digests; d.with_data = r->with_data ? 1 : 0;
-      for (int i = 0; i < n; i++) d.files[i] = r->files[i];
-      d.full0 = fb; d.tail_slot = tl ? tb : -1; d.tail_src_off = tl ? toff : 0;
-      r->ch = EncChunk();
-      r->ch.nfull = nf; r->ch.tail = tl; r->ch.s = &s;
-      r->ch.d_src = dsrc + fb * bs; r->ch.d_src_tail = dsrc + toff; r->ch.d_out_tail = dout + tb * m * pitch; r->ch.h_dig_tail = hdig + tb * n * 32;
-      fb += nf;
-      if (tl) { tb++; toff += round_up(tl, 256); }
-      max_len = std::max(max_len, r->len);
-      max_nb = std::max(max_nb, nf + (tl ? 1 : 0));
       c->st_h2d += r->len;
       c->st_d2h += (nf * S + (tl ? ceil_frac(tl, k) : 0)) * (r->with_data ? n : m);
     }
-    const int phase_slot = static_cast<int>(&s - c->slots);
-    if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
+    const int si = static_cast<int>(&s - c->slots);
+    mark_phase(b, s, 0);
     MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, reqs.size() * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
     CrcSegParams crc;
     if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
@@ -2469,13 +2498,11 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     cp.staged = dsrc; cp.parity = dout; cp.digests = ddig;
     // staging: the copy engines are the faster reader of host memory (one call per request); the gather kernel (SM loads over
     // PCIe, no per-request call at all) is kept for hosts where the worker thread is the bottleneck
-    static const bool use_gather = getenv("MEC_BATCHER_GATHER") != nullptr;
     // requests [0, ndma) go through the copy engine, [ndma, nreq) through the gather kernel on the aux stream, concurrently
-    size_t ndma = use_gather ? 0 : reqs.size();
-    if (!use_gather && b->gather_pct > 0 && b->aux && reqs.size() >= 8)
-      ndma = reqs.size() - reqs.size() * static_cast<size_t>(b->gather_pct) / 100;
+    size_t ndma = b->sw.gather ? 0 : reqs.size();
+    if (!b->sw.gather && b->sw.gather_pct > 0 && b->aux && reqs.size() >= 8)
+      ndma = reqs.size() - reqs.size() * static_cast<size_t>(b->sw.gather_pct) / 100;
     if (ndma < reqs.size()) {
-      const int si = static_cast<int>(&s - c->slots);
       cudaStream_t gs = s.st;
       if (ndma > 0) {
         gs = b->aux;
@@ -2506,28 +2533,14 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
       }
       if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
     }
-    if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[static_cast<int>(&s - c->slots)], 0));
-    if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
+    if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[si], 0));
+    mark_phase(b, s, 1);
     if ((rc = batcher_crc_launch(b, s, crc))) return rc;
-    if ((rc = batch_encode_scatter(c, s, s.st, tab, reqs.size(), total_full, nslots, max_nb, cp, b->trace ? b->ev_ph[phase_slot][2] : nullptr)))
-      return rc;
-    if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][3], s.st);
+    if ((rc = batch_encode_scatter(c, s, s.st, tab, reqs.size(), lay, cp, b->sw.trace ? b->ev_ph[si][2] : nullptr))) return rc;
+    mark_phase(b, s, 3);
     *needs_retire = false;
     c->st_blocks_encoded += nslots;
     return MEC_OK;
-  }
-  for (BatchReq* r : reqs) {
-    EncChunk& ch = r->ch;
-    ch = EncChunk();
-    ch.b0 = 0; ch.nfull = r->len / bs; ch.tail = r->len % bs; ch.nb = ch.nfull + (ch.tail ? 1 : 0);
-    ch.s = &s; ch.st = s.st; ch.pitch = pitch;
-    ch.d_src = dsrc + fb * bs; ch.d_out = dout + fb * m * pitch; ch.h_dig = hdig + fb * n * 32;
-    if (ch.tail > 0) {
-      ch.d_src_tail = dsrc + toff; ch.d_out_tail = dout + tb * m * pitch; ch.h_dig_tail = hdig + tb * n * 32;
-      toff += round_up(ch.tail, 256);
-      tb++;
-    }
-    fb += ch.nfull;
   }
   CrcSegParams crc;
   if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
@@ -2540,7 +2553,8 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     c->st_h2d += r->len;
   }
   if ((rc = batcher_crc_launch(b, s, crc))) return rc;
-  if (total_full > 0 && (rc = encode_device_locked(c, dsrc, total_full * bs, dout, pitch, ddig, s.st))) return rc;  // ONE launch for every caller's full blocks
+  if (lay.total_full > 0 && (rc = encode_device_locked(c, dsrc, lay.total_full * bs, dout, pitch, ddig, s.st))) return rc;  // ONE launch for every caller's full blocks
+  const uint8_t* hdig = static_cast<const uint8_t*>(s.hdig.p);
   for (BatchReq* r : reqs) {
     const EncChunk& ch = r->ch;
     if (ch.tail > 0 && (rc = encode_device_locked(c, ch.d_src_tail, ch.tail, ch.d_out_tail, pitch,
@@ -2573,7 +2587,7 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
   mec_codec* c = b->codec;
   const int k = c->k, n = c->n;
   const int64_t bs = c->block_size, S = c->S();
-  const bool heal = reqs.front()->kind == 2;
+  const bool heal = reqs.front()->kind == ReqKind::Heal;
   const size_t nreq = reqs.size();
   if (b->patterns.size() + nreq > kMaxCachedPatterns) b->patterns.clear();  // pointers into the cache stay valid for this batch
   std::vector<const BatchPattern*> pats;
@@ -2652,14 +2666,11 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
     lay.max_nb = std::max(lay.max_nb, d.nblocks);
     rq->get_nblocks = d.nblocks;
   }
-  static const int64_t dma_blocks = getenv("MEC_BATCHER_DMA_BLOCKS") ? atoll(getenv("MEC_BATCHER_DMA_BLOCKS")) : 1;
   for (size_t q = 0; q < nreq; q++) {
-    tab[q].dma = tab[q].nblocks >= dma_blocks ? 1 : 0;
+    tab[q].dma = tab[q].nblocks >= b->sw.dma_blocks ? 1 : 0;
     if (tab[q].tail_slot >= 0) tab[q].tail_slot += lay.nfull_slots;
     reqs[q]->get_slot0 = tab[q].slot0;
     reqs[q]->get_tail_slot = tab[q].tail_slot;
-    reqs[q]->ch = EncChunk();
-    reqs[q]->ch.s = &s;
   }
   if (heal) {
     uint8_t** outs = reinterpret_cast<uint8_t**>(tab + nreq);
@@ -2691,8 +2702,7 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
   const int64_t stride = round_up(nslots * P + 512, 256);
-  const int phase_slot = static_cast<int>(&s - c->slots);
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][0], s.st);
+  mark_phase(b, s, 0);
   MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, lay.table_bytes, cudaMemcpyHostToDevice, s.st));
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
@@ -2734,7 +2744,7 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
   }
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][1], s.st);
+  mark_phase(b, s, 1);
   MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
   const int32_t* block_len = nullptr;
   const bool mixed = lay.npat > 1;
@@ -2778,7 +2788,7 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
       if (tab[q].tail_slot >= 0 && (rc = launch(tab[q].tail_slot, 1, tab[q].last_len))) return rc;
   }
   MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
-  if (b->trace) cudaEventRecord(b->ev_ph[phase_slot][2], s.st);
+  mark_phase(b, s, 2);
   b->st_patterns += lay.npat;
   if (mixed) b->st_mixed++;
   int64_t rebuilt = 0;
@@ -2802,7 +2812,7 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   // writeDataBlocks: 0 = the scatter kernel assembles every object in device memory and ONE copy per request takes it to the caller
   // (fewest driver-side copy descriptors), 1 = the scatter kernel stores straight into the callers' buffers over PCIe, 2 = the copy
   // engine moves every (request, shard, block) piece itself
-  static const int out_mode = getenv("MEC_BATCHER_GET_OUT") ? atoi(getenv("MEC_BATCHER_GET_OUT")) : 0;
+  const int out_mode = b->sw.get_out;
   std::vector<int64_t> asm_off(reqs.size(), 0);
   if (out_mode == 0) {
     int64_t total = 0;
@@ -2849,7 +2859,7 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
       if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
     }
   }
-  if (b->trace) cudaEventRecord(b->ev_ph[&s - c->slots][3], s.st);
+  mark_phase(b, s, 3);
   *nblocks = nslots;
   return MEC_OK;
 }
@@ -2874,7 +2884,7 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
   }
-  if (b->trace) cudaEventRecord(b->ev_ph[&s - c->slots][3], s.st);
+  mark_phase(b, s, 3);
   *nblocks = nslots;
   return MEC_OK;
 }
@@ -2887,42 +2897,22 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
 static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
   mec_codec* e = b->dst;
-  const int si = static_cast<int>(&s - c->slots);
-  Slot& d = e->slots[si];
+  Slot& d = e->slots[&s - c->slots];
   BatchGetParams gp;
   ReadLayout lay;
   int rc = batch_read_plan(b, s, reqs, gp, lay);
   if (rc) return rc;
+  PutLayout put;  // every request's destination side: a PUT of the part (mec_batcher_transcode)
+  if ((rc = put_layout(e, d, reqs, true, false, put))) return rc;
   const size_t nreq = reqs.size();
   const int ek = e->k, en = e->n;
   const int64_t bs = e->block_size, eS = e->S(), epitch = round_up(eS, 16);
-  int64_t total_full = 0, ntails = 0, tail_bytes = 0;
-  for (BatchReq* r : reqs) {
-    total_full += r->total / bs;
-    if (r->total % bs) { ntails++; tail_bytes += round_up(r->total % bs, 256); }
-  }
-  const int64_t nslots = total_full + ntails;
-  if ((rc = d.src.ensure(static_cast<size_t>(total_full * bs + tail_bytes + 512)))) return rc;
-  if ((rc = d.out.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * std::max(e->m, 1) * epitch)))) return rc;
-  if ((rc = d.dig.ensure(static_cast<size_t>(std::max<int64_t>(nslots, 1) * en * 32)))) return rc;
-  if ((rc = d.hreq.ensure(nreq * sizeof(BatchReqDesc)))) return rc;
-  if ((rc = d.dreq.ensure(nreq * sizeof(BatchReqDesc)))) return rc;
-  BatchReqDesc* dt = static_cast<BatchReqDesc*>(d.hreq.p);
-  int64_t fb = 0, tb = total_full, toff = total_full * bs, max_nb = 0;
-  for (size_t q = 0; q < nreq; q++) {
-    const BatchReq* r = reqs[q];
-    BatchReqDesc& w = dt[q];
-    memset(&w, 0, sizeof(w));
+  for (const BatchReq* r : reqs) {
     const int64_t nf = r->total / bs, tl = r->total % bs;
-    w.len = r->total; w.with_data = 1;
-    for (int i = 0; i < en; i++) w.files[i] = r->outs[i];
-    w.full0 = fb; w.tail_slot = tl ? tb : -1; w.tail_src_off = tl ? toff : 0;
-    fb += nf;
-    if (tl) { tb++; toff += round_up(tl, 256); }
-    max_nb = std::max(max_nb, nf + (tl ? 1 : 0));
     c->st_h2d += static_cast<int64_t>(c->k) * mec_bitrot_shard_file_size(mec_shard_file_size(c, r->total), c->S(), MEC_HIGHWAYHASH256S);
     e->st_d2h += (nf * eS + (tl ? ceil_frac(tl, ek) : 0)) * en;
   }
+  const BatchReqDesc* dt = static_cast<const BatchReqDesc*>(d.hreq.p);
   if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, lay, false))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(d.dreq.p, dt, nreq * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
   BatchCopyParams cp;
@@ -2933,9 +2923,9 @@ static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchRe
   batch_transcode_resplit_kernel<<<dim3(gx, static_cast<unsigned>(c->k), static_cast<unsigned>(nreq)), 128, 0, s.st>>>(gp, cp);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
-  if ((rc = batch_encode_scatter(e, d, s.st, dt, nreq, total_full, nslots, max_nb, cp, nullptr))) return rc;
-  if (b->trace) cudaEventRecord(b->ev_ph[si][3], s.st);
-  e->st_blocks_encoded += nslots;
+  if ((rc = batch_encode_scatter(e, d, s.st, dt, nreq, put, cp, nullptr))) return rc;
+  mark_phase(b, s, 3);
+  e->st_blocks_encoded += put.nslots;
   *nblocks = lay.nslots();
   return MEC_OK;
 }
@@ -2958,9 +2948,9 @@ static void batcher_main(mec_batcher* b) {
       if (!b->queue.empty() && nbusy < kSlots) {
         // gather: whatever is queued now; when nothing is in flight, give concurrent callers max_wait_us to join
         auto req_blocks = [&](const BatchReq* r) -> int64_t {
-          return r->kind == 0 ? ceil_frac(r->len, c->block_size)
-                 : r->kind >= 2 ? ceil_frac(r->total, c->block_size)
-                                : (r->length / c->block_size + 2);
+          return r->kind == ReqKind::Put   ? ceil_frac(r->len, c->block_size)
+                 : r->kind == ReqKind::Get ? r->length / c->block_size + 2
+                                           : ceil_frac(r->total, c->block_size);  // heal, transcode: the whole part
         };
         auto blocks_queued = [&] {
           int64_t nb = 0;
@@ -2977,7 +2967,7 @@ static void batcher_main(mec_batcher* b) {
         // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.45 ms however few
         // blocks it is given (one warp walks one erasure block), so the copy of one batch has to overlap the kernel of another —
         // otherwise a closed loop of callers falls into a convoy (all of them in one batch, the GPU idle while they wake up)
-        static const int depth = getenv("MEC_BATCHER_DEPTH") ? atoi(getenv("MEC_BATCHER_DEPTH")) : 4;
+        const int depth = b->sw.depth;
         int64_t cap = b->max_blocks;
         if (depth > 0 && nbusy < depth - 1) {
           const int64_t q = blocks_queued();
@@ -2986,7 +2976,7 @@ static void batcher_main(mec_batcher* b) {
         int64_t nb = 0, nread = 0;
         bool mixed = false;
         const BatchReq* lead = b->queue.front();
-        const bool mix = b->mix && lead->kind != 0;
+        const bool mix = b->mix && is_read(lead->kind);
         const int64_t limit = std::min<int64_t>(c->eng->small_limit(c->opt), 1 << 16);  // block_pattern holds uint16_t indices
         for (auto it = b->queue.begin(); it != b->queue.end();) {
           BatchReq* r = *it;
@@ -3009,35 +2999,31 @@ static void batcher_main(mec_batcher* b) {
     if (!reqs.empty()) {
       Slot& s = c->slots[head];
       InflightBatch& fb = inflight[head];
-      int rc;
+      int rc = MEC_OK;
       int64_t nblocks = 0;
       const auto t_submit = clk::now();
+      fb.kind = reqs.front()->kind;
       {
         std::lock_guard<std::mutex> lk(c->mu);
-        fb.is_get = reqs.front()->kind != 0;
-        fb.get_k = c->k;
-        if (reqs.front()->kind == 3) {
-          std::lock_guard<std::mutex> lk_dst(b->dst->mu);  // source, then destination: mec_transcode's order
-          rc = batcher_submit_transcode(b, s, reqs, &nblocks);
-          if (rc != MEC_OK)
-            for (BatchReq* r : reqs) r->ch.s = &s;
-        } else if (fb.is_get) {
-          rc = reqs.front()->kind == 2 ? batcher_submit_heal(b, s, reqs, &nblocks) : batcher_submit_get(b, s, reqs, &nblocks);
-          if (rc != MEC_OK)
-            for (BatchReq* r : reqs) r->ch.s = &s;  // batcher_finish looks the slot up through the first request
-        } else {
-          rc = batcher_submit(b, s, reqs, &fb.needs_retire, &nblocks);
+        switch (fb.kind) {
+          case ReqKind::Put: rc = batcher_submit(b, s, reqs, &fb.needs_retire, &nblocks); break;
+          case ReqKind::Get: rc = batcher_submit_get(b, s, reqs, &nblocks); break;
+          case ReqKind::Heal: rc = batcher_submit_heal(b, s, reqs, &nblocks); break;
+          case ReqKind::Transcode: {
+            std::lock_guard<std::mutex> lk_dst(b->dst->mu);  // source, then destination: mec_transcode's order
+            rc = batcher_submit_transcode(b, s, reqs, &nblocks);
+            break;
+          }
         }
       }
       b->us_submit += us_since(t_submit);
       fb.reqs = reqs;
-      fb.busy = true;
-      // a batch the kernels carry end to end: every GET or heal batch, a PUT batch unless it took the memcpy path
-      const bool kernel_batch = fb.is_get || !fb.needs_retire;
-      fb.traced = b->trace && rc == MEC_OK && kernel_batch;
+      // a batch the kernels carry end to end: every read batch, a PUT batch unless it took the memcpy path
+      const bool kernel_batch = is_read(fb.kind) || !fb.needs_retire;
+      fb.traced = b->sw.trace && rc == MEC_OK && kernel_batch;
       if (rc != MEC_OK) {  // drain what was enqueued before the failure, then fail the whole batch
         cudaStreamSynchronize(s.st);
-        batcher_finish(b, fb, rc);
+        batcher_finish(b, fb, s, rc);
       } else {
         b->st_batches++;
         if (kernel_batch) b->st_kernel_batches++;
@@ -3065,7 +3051,7 @@ static void batcher_main(mec_batcher* b) {
         b->us_stage += static_cast<int64_t>(a * 1000); b->us_kernel += static_cast<int64_t>(k2 * 1000); b->us_scatter += static_cast<int64_t>(sc * 1000);
       }
       const auto t_fin = clk::now();
-      batcher_finish(b, inflight[tail], e == cudaSuccess ? MEC_OK : MEC_ERR_CUDA);
+      batcher_finish(b, inflight[tail], c->slots[tail], e == cudaSuccess ? MEC_OK : MEC_ERR_CUDA);
       b->us_finish += us_since(t_fin);
       tail = (tail + 1) % kSlots;
       nbusy--;
@@ -3073,6 +3059,28 @@ static void batcher_main(mec_batcher* b) {
   }
 }
 }  // namespace
+
+// The environment switches of a new batcher (BatcherSwitches)
+static BatcherSwitches batcher_switches() {
+  BatcherSwitches w;
+  const char* e;
+  w.memcpy = getenv("MEC_BATCHER_MEMCPY") != nullptr;
+  w.gather = getenv("MEC_BATCHER_GATHER") != nullptr;
+  if ((e = getenv("MEC_BATCHER_GATHER_PCT"))) w.gather_pct = std::max(0, std::min(100, atoi(e)));
+  if ((e = getenv("MEC_BATCHER_DMA_BLOCKS"))) w.dma_blocks = atoll(e);
+  if ((e = getenv("MEC_BATCHER_GET_OUT"))) w.get_out = atoi(e);
+  if ((e = getenv("MEC_BATCHER_DEPTH"))) w.depth = atoi(e);
+  w.trace = getenv("MEC_BATCHER_TRACE") != nullptr;
+  return w;
+}
+
+// Slot `s` of codec `c` sized up front for a merged PUT batch of `blocks` blocks: object bytes, parity rows, digests
+static int size_put_slot(const mec_codec* c, Slot& s, int64_t blocks) {
+  int rc;
+  if ((rc = s.src.ensure(static_cast<size_t>(blocks * c->block_size)))) return rc;
+  if ((rc = s.out.ensure(static_cast<size_t>(blocks * std::max(c->m, 1) * round_up(c->S(), 16))))) return rc;
+  return s.dig.ensure(static_cast<size_t>(blocks * c->n * 32));
+}
 
 // mec_batcher_new_ex, and with `dst` (a codec of the destination geometry without an engine yet, owned from here on, freed on
 // failure) mec_batcher_new_transcode: the destination's engine and slots are set up before the worker starts
@@ -3094,6 +3102,7 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
   mec_batcher* b = new mec_batcher;
   b->codec = c;
   b->dst = dst;
+  b->sw = batcher_switches();
   b->mix = (flags & MEC_BATCHER_MIX_PATTERNS) && c->eng->small_ok(c->opt, 1);  // per-block decode plans exist in the latency kernel only
   if (max_batch_blocks > 0) b->max_blocks = max_batch_blocks;
   // a merged batch stages at most 1 GiB of object bytes: six slots are sized for a full batch up front (below)
@@ -3106,11 +3115,9 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
-    const int64_t S = c->S(), pitch = round_up(S, 16), P = round_up(32 + S, 16), slots = b->max_blocks + std::min<int64_t>(64, b->max_blocks / 8 + 4);
+    const int64_t P = round_up(32 + c->S(), 16), slots = b->max_blocks + std::min<int64_t>(64, b->max_blocks / 8 + 4);
     for (Slot& s : c->slots) {
-      if (rc == MEC_OK) rc = s.src.ensure(static_cast<size_t>(slots * block_size));
-      if (rc == MEC_OK) rc = s.out.ensure(static_cast<size_t>(slots * std::max(m, 1) * pitch));
-      if (rc == MEC_OK) rc = s.dig.ensure(static_cast<size_t>(slots * c->n * 32));
+      if (rc == MEC_OK) rc = size_put_slot(c, s, slots);
       if (rc == MEC_OK) rc = s.hdig.ensure(static_cast<size_t>(slots * c->n * 32));
       if (rc == MEC_OK) rc = s.aux.ensure(static_cast<size_t>(k * round_up(slots * P + 512, 256)));
       if (rc == MEC_OK) rc = s.flags.ensure(static_cast<size_t>(slots * k));
@@ -3136,11 +3143,8 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
       // the destination side of a merged transcode batch, laid out as a merged PUT batch of the destination geometry: object bytes,
       // parity rows, digests, the PUT request table and the latency kernel's block table
       std::lock_guard<std::mutex> lk_dst(dst->mu);
-      const int64_t epitch = round_up(dst->S(), 16);
       for (Slot& s : dst->slots) {
-        if (rc == MEC_OK) rc = s.src.ensure(static_cast<size_t>(slots * block_size));
-        if (rc == MEC_OK) rc = s.out.ensure(static_cast<size_t>(slots * std::max(dst->m, 1) * epitch));
-        if (rc == MEC_OK) rc = s.dig.ensure(static_cast<size_t>(slots * dst->n * 32));
+        if (rc == MEC_OK) rc = size_put_slot(dst, s, slots);
         if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
         if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
         if (rc == MEC_OK) rc = s.blk.ensure(static_cast<size_t>(slots) * sizeof(SmallBlock));
@@ -3150,18 +3154,16 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     cudaSetDevice(cur);
   }
   if (rc) { mec_codec_free(c); mec_codec_free(dst); delete b; return rc; }
-  b->trace = getenv("MEC_BATCHER_TRACE") != nullptr;
-  if (b->trace) {
+  if (b->sw.trace) {
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
     for (int i = 0; i < kSlots; i++)
       for (int j = 0; j < 4; j++)
-        if (cudaEventCreate(&b->ev_ph[i][j]) != cudaSuccess) { cudaGetLastError(); b->trace = false; }
+        if (cudaEventCreate(&b->ev_ph[i][j]) != cudaSuccess) { cudaGetLastError(); b->sw.trace = false; }
     cudaSetDevice(cur);
   }
-  if (const char* e = getenv("MEC_BATCHER_GATHER_PCT")) b->gather_pct = std::max(0, std::min(100, atoi(e)));
-  if (b->gather_pct > 0) {
+  if (b->sw.gather_pct > 0) {
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
@@ -3170,7 +3172,7 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
       ok = cudaEventCreateWithFlags(&b->ev_table[i], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&b->ev_gather[i], cudaEventDisableTiming) == cudaSuccess;
     cudaSetDevice(cur);
-    if (!ok) { cudaGetLastError(); b->gather_pct = 0; }
+    if (!ok) { cudaGetLastError(); b->sw.gather_pct = 0; }
   }
   b->worker = std::thread(batcher_main, b);
   *out = b;
@@ -3223,12 +3225,12 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
 }
 
 // Queues `r` for the worker and waits until its batch is done.  A PUT wakes the worker only as the first arrival or as the one that
-// fills a batch, not as every caller; a GET or heal always wakes it.
+// fills a batch, not as every caller; a GET, heal or transcode always wakes it.
 static int64_t batcher_enqueue_wait(mec_batcher* b, BatchReq& r) {
   std::unique_lock<std::mutex> lk(b->mu);
   if (b->stop) return MEC_ERR_INVALID_ARGUMENT;
   b->queue.push_back(&r);
-  if (r.kind != 0 || b->queue.size() == 1 ||
+  if (r.kind != ReqKind::Put || b->queue.size() == 1 ||
       static_cast<int64_t>(b->queue.size()) * std::max<int64_t>(1, r.len / b->codec->block_size) >= b->max_blocks)
     b->cv_work.notify_one();
   r.cv.wait(lk, [&] { return r.done; });
@@ -3272,6 +3274,20 @@ extern "C" int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, in
   if (which && !out3) return MEC_ERR_INVALID_ARGUMENT;
   return batcher_call(b, src, len, files, data_digests, data_digests == nullptr, write_quorum, which, out3);
 }
+// The k readers parallelReader picks for a read or move (choose_readers on r.gfiles, r.prefer), chosen on the caller's thread: equal
+// reader sets share a batch.  Sets their bits in r.alive_mask and clears *mapped unless every one of them is page-locked.
+static int batch_readers(const mec_codec* c, BatchReq& r, bool* mapped) {
+  uint8_t alive[kBatchMaxFiles];
+  int chosen[kBatchMaxFiles];
+  for (int i = 0; i < c->n; i++) alive[i] = r.gfiles[i] != nullptr;
+  if (choose_readers(c, r.gfiles, alive, r.prefer, chosen) < c->k) return MEC_ERR_READ_QUORUM;
+  for (int t = 0; t < c->k; t++) {
+    r.alive_mask |= 1ull << chosen[t];
+    *mapped = *mapped && mec_is_pinned(r.gfiles[chosen[t]]) != 0;
+  }
+  return MEC_OK;
+}
+
 // Erasure.Decode through the coalescer: GETs that are queued together and read the same drives are merged into one launch — without
 // `prefer` the same drives online, with it the same k readers parallelReader picks; with MEC_BATCHER_MIX_PATTERNS any reads.
 // Calls whose buffers are not page-locked, and calls that meet bitrot, run on their own through a private handle.
@@ -3282,24 +3298,15 @@ extern "C" int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* cons
   if (offset < 0 || length < 0 || offset + length > total) return MEC_ERR_INVALID_ARGUMENT;  // cmd/erasure-decode.go:240-245
   if (length == 0) return 0;
   if (!dst) return MEC_ERR_INVALID_ARGUMENT;
-  mec_codec* c = b->codec;
-  const int n = c->n, k = c->k;
+  const int n = b->codec->n, k = b->codec->k;
   BatchReq r;
-  r.kind = 1; r.gfiles = files; r.offset = offset; r.length = length; r.total = total; r.dst = dst; r.heal_hint = heal_hint;
+  r.kind = ReqKind::Get; r.gfiles = files; r.offset = offset; r.length = length; r.total = total; r.dst = dst; r.heal_hint = heal_hint;
   r.prefer = prefer;
-  bool mapped = n <= kBatchMaxFiles && n <= 64 && k <= 32 && mec_is_pinned(dst) != 0;
+  bool mapped = !b->sw.memcpy && n <= kBatchMaxFiles && n <= 64 && k <= 32 && mec_is_pinned(dst) != 0;
   if (prefer && n <= kBatchMaxFiles) {
-    // the readers parallelReader picks (preferReaders, cmd/erasure-decode.go:92-123), chosen here on the caller's thread: the
-    // request's key is that reader set (a k-bit mask equals an alive mask only when exactly those k drives are online)
-    uint8_t alive[kBatchMaxFiles];
-    int chosen[kBatchMaxFiles];
-    for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
-    const int nch = choose_readers(c, files, alive, prefer, chosen);
-    if (nch < k) return MEC_ERR_READ_QUORUM;
-    for (int t = 0; t < k; t++) {
-      r.alive_mask |= 1ull << chosen[t];
-      mapped = mapped && mec_is_pinned(files[chosen[t]]) != 0;
-    }
+    // with preferReaders (cmd/erasure-decode.go:92-123): a k-bit mask equals an alive mask only when exactly those k drives are online
+    const int rc = batch_readers(b->codec, r, &mapped);
+    if (rc) return rc;
   } else {
     int online = 0;
     for (int i = 0; i < n; i++) {
@@ -3312,11 +3319,7 @@ extern "C" int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* cons
     for (int i = 0, cnt = 0; i < n && cnt < k && mapped; i++)
       if (files[i]) { mapped = mec_is_pinned(files[i]) != 0; cnt++; }
   }
-  if (!mapped || getenv("MEC_BATCHER_MEMCPY") != nullptr) {
-    mec_codec* sc = batcher_serial(b);
-    return sc ? mec_decode_prefer(sc, files, prefer, offset, length, total, dst, heal_hint) : MEC_ERR_UNEXPECTED;
-  }
-  return batcher_enqueue_wait(b, r);
+  return mapped ? batcher_enqueue_wait(b, r) : batcher_run_alone(b, r);
 }
 extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* files, int64_t offset, int64_t length, int64_t total,
                                       uint8_t* dst, int* heal_hint) {
@@ -3330,28 +3333,16 @@ extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* file
 extern "C" int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
                                 uint8_t* const* out_files, uint8_t* corrupt) {
   if (!b || !files || !out_files) return MEC_ERR_INVALID_ARGUMENT;
-  mec_codec* c = b->codec;
-  const int n = c->n, k = c->k;
-  auto serial = [&]() -> int {
-    mec_codec* sc = batcher_serial(b);
-    return sc ? mec_heal_prefer(sc, files, prefer, total, out_files, corrupt) : MEC_ERR_UNEXPECTED;
-  };
-  if (n > kBatchMaxFiles || n > 64) return serial();
+  const int n = b->codec->n;
+  BatchReq r;
+  r.kind = ReqKind::Heal; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
+  r.prefer = prefer; r.outs = out_files; r.corrupt = corrupt;
+  if (n > kBatchMaxFiles || n > 64) return static_cast<int>(batcher_run_alone(b, r));
   if (corrupt) memset(corrupt, 0, static_cast<size_t>(n));
   if (total <= 0) return MEC_OK;
-  // the readers parallelReader would pick, chosen here on the caller's thread: equal reader sets share a launch
-  uint8_t alive[kBatchMaxFiles];
-  int chosen[kBatchMaxFiles];
-  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
-  if (choose_readers(c, files, alive, prefer, chosen) < k) return MEC_ERR_READ_QUORUM;
-  BatchReq r;
-  r.kind = 2; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
-  r.prefer = prefer; r.outs = out_files; r.corrupt = corrupt;
-  bool mapped = getenv("MEC_BATCHER_MEMCPY") == nullptr;
-  for (int t = 0; t < k; t++) {
-    r.alive_mask |= 1ull << chosen[t];
-    mapped = mapped && mec_is_pinned(files[chosen[t]]) != 0;
-  }
+  bool mapped = !b->sw.memcpy;
+  const int rc = batch_readers(b->codec, r, &mapped);
+  if (rc) return rc;
   int nstale = 0;
   for (int i = 0; i < n; i++)
     if (out_files[i]) {
@@ -3360,7 +3351,7 @@ extern "C" int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, con
       mapped = mapped && mec_is_pinned(out_files[i]) != 0;
     }
   // a drive that is read and also rewritten is passed through unchanged by reconstruct_range: the serial path does that
-  if (!mapped || (r.alive_mask & r.stale_mask) != 0 || nstale > kMaxR) return serial();
+  if (!mapped || (r.alive_mask & r.stale_mask) != 0 || nstale > kMaxR) return static_cast<int>(batcher_run_alone(b, r));
   return static_cast<int>(batcher_enqueue_wait(b, r));
 }
 
@@ -3378,25 +3369,17 @@ extern "C" int64_t mec_batcher_transcode(mec_batcher* b, const uint8_t* const* f
   for (int i = 0; i < e->n; i++) online += out_files[i] != nullptr;
   if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
   if (total == 0) return 0;
-  const int n = c->n, k = c->k;
-  auto serial = [&]() -> int64_t { return batcher_transcode_serial(b, files, prefer, total, out_files, write_quorum, heal_hint); };
-  if (n > kBatchMaxFiles || e->n > kBatchMaxFiles) return serial();
-  // the readers parallelReader would pick, chosen here on the caller's thread: equal reader sets share a batch
-  uint8_t alive[kBatchMaxFiles];
-  int chosen[kBatchMaxFiles];
-  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
-  if (choose_readers(c, files, alive, prefer, chosen) < k) return MEC_ERR_READ_QUORUM;
   BatchReq r;
-  r.kind = 3; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
-  r.prefer = prefer; r.outs = out_files; r.heal_hint = heal_hint;
-  bool mapped = getenv("MEC_BATCHER_MEMCPY") == nullptr;
-  for (int t = 0; t < k; t++) {
-    r.alive_mask |= 1ull << chosen[t];
-    mapped = mapped && mec_is_pinned(files[chosen[t]]) != 0;
-  }
+  r.kind = ReqKind::Transcode; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
+  r.prefer = prefer; r.heal_hint = heal_hint;
+  r.len = total; r.files = out_files; r.with_data = true;  // the destination side, a PUT of the part
+  if (c->n > kBatchMaxFiles || e->n > kBatchMaxFiles) return batcher_run_alone(b, r);
+  bool mapped = !b->sw.memcpy;
+  const int rc = batch_readers(c, r, &mapped);
+  if (rc) return rc;
   for (int i = 0; i < e->n && mapped; i++)
     if (out_files[i]) mapped = mec_is_pinned(out_files[i]) != 0;
-  if (!mapped || ceil_frac(total, c->block_size) > b->max_blocks) return serial();
+  if (!mapped || ceil_frac(total, c->block_size) > b->max_blocks) return batcher_run_alone(b, r);
   return batcher_enqueue_wait(b, r);
 }
 
