@@ -95,12 +95,22 @@ int mec_encode_blocks_device(mec_codec* c, const uint8_t* d_src, int64_t len, ui
  * digest check of streamingBitrotReader.ReadAt (cmd/bitrot-streaming.go:186-196).
  *   frames[i]   : host pointer to shard file i in streaming-bitrot layout ([32B digest][shard])*,
  *                 or NULL when the drive is offline.  All `nblocks` blocks are full blocks except
- *                 that the last block's shard length is `last_shard_len` (0 => shard_size).
- *   want[i]     : 1 = rebuild shard i into out[i] (same frame layout, digests recomputed)
- *   data_only   : ReconstructData semantics (parity never rebuilt)
- *   corrupt[i]  : set to 1 when any frame of file i fails its digest
- * The first k readable files in index order are used (parallelReader.Read, cmd/erasure-decode.go:127);
- * a file with a corrupt frame is dropped for the whole call and the next one is tried. */
+ *                 that the last block's shard length is `last_shard_len` (0 => shard_size; a value
+ *                 below 0 or above shard_size is MEC_ERR_INVALID_ARGUMENT, checked before any device work).
+ *   want[i]     : 1 = out[i] receives shard file i (same frame layout): copied from frames[i] when
+ *                 file i is one of the readers, otherwise rebuilt with recomputed digests
+ *   data_only   : ReconstructData semantics (parity never rebuilt: out[i] of a wanted parity shard
+ *                 that is not read is left as it was)
+ *   corrupt[i]  : (optional, n bytes, cleared on entry) set to 1 when a frame of file i that was read
+ *                 fails its digest.  Only the files read are checked; the others are never looked at.
+ * The first k readable files in index order are read (parallelReader.Read, cmd/erasure-decode.go:127).
+ * A reader whose frame fails its digest is dropped for the rest of the call: the blocks before that
+ * frame stand, and the call resumes at it with the next readable file.  A wanted reader that is
+ * dropped is passed through up to the bad frame and, unless it is parity under data_only, rebuilt
+ * from there.  When the readable files run out (initially, or after drops) the call returns
+ * MEC_ERR_READ_QUORUM; corrupt[] then names every reader it dropped, so a caller that handed over
+ * only k files can drop those and call again with the next ones (include/minio_erasure.hpp,
+ * readAndReconstruct).  The out[] files are complete only when the call returns MEC_OK. */
 int mec_reconstruct_frames(mec_codec* c, const uint8_t* const* frames, int64_t nblocks,
                            int64_t last_shard_len, const uint8_t* want, int data_only,
                            uint8_t* const* out, uint8_t* corrupt);

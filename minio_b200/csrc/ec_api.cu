@@ -1214,6 +1214,7 @@ extern "C" int mec_reconstruct_device(mec_codec* c, const uint8_t* const* d_fram
 extern "C" int mec_reconstruct_frames(mec_codec* c, const uint8_t* const* frames, int64_t nblocks, int64_t last_shard_len,
                                       const uint8_t* want, int data_only, uint8_t* const* out, uint8_t* corrupt) {
   if (!c || !frames || !want || !out || nblocks < 0) return MEC_ERR_INVALID_ARGUMENT;
+  if (last_shard_len < 0 || last_shard_len > c->S()) return MEC_ERR_INVALID_ARGUMENT;
   int rc = require_streaming(c);
   if (rc) return rc;
   if (c->n > kMaxShards) return MEC_ERR_UNSUPPORTED;
@@ -1221,7 +1222,6 @@ extern "C" int mec_reconstruct_frames(mec_codec* c, const uint8_t* const* frames
   if (corrupt) memset(corrupt, 0, static_cast<size_t>(c->n));
   if (nblocks == 0) return MEC_OK;
   FrameGeom g{nblocks, c->S(), last_shard_len > 0 ? last_shard_len : c->S()};
-  if (g.last_len > g.S) return MEC_ERR_INVALID_ARGUMENT;
   std::vector<uint8_t> alive(c->n);
   for (int i = 0; i < c->n; i++) alive[i] = frames[i] != nullptr;
   RangeSink sk;
