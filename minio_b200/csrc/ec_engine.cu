@@ -617,6 +617,11 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
   // warps (ec_small.cuh).  The throughput kernel needs ~0.45 ms for a 1 MiB block however few there are (one warp walks it);
   // this one ~0.16 ms up to one block per SM (RS(12,4), H100 80GB HBM3 at a 400 W power limit); a few blocks per SM later both are
   // bound by the same instruction count and the throughput kernel's occupancy wins.
+  // Every geometry the engine accepts fits it: otherwise a legal launch would silently fall through to the throughput kernel, and
+  // one that only the latency kernel can run (per-block geometry or decode plans) would fail with MEC_ERR_UNSUPPORTED.
+  static_assert(small_smem_bytes(kMaxK, kMaxR, true, 4) <= 227 * 1024, "widest latency-kernel launch exceeds shared memory");
+  static_assert(32 * small_hash_warps(kMaxK + kMaxR) + 32 * small_gf_warps(kMaxK + kMaxR) <= 256,
+                "widest latency-kernel launch exceeds its __launch_bounds__");
   {
     if (small_ok(opt, d.nblocks) && d.S > 0 && (d.contiguous || d.in_ptr[0] != nullptr)) {
       for (int t = 0; t < d.k; t++) p.in_ptr[t] = d.contiguous ? d.in_base + static_cast<int64_t>(t) * d.S : d.in_ptr[t];

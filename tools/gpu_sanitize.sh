@@ -128,3 +128,64 @@ PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
 echo "== racecheck"; timeout 1200 compute-sanitizer --tool racecheck --print-limit 20 python /tmp/san_case.py > gpurun_out/racecheck.txt 2>&1; echo rc=$?; grep -E "RACECHECK SUMMARY|sanitizer case ok|hazard" gpurun_out/racecheck.txt | head -12
 echo "== synccheck"; timeout 1200 compute-sanitizer --tool synccheck --print-limit 20 python /tmp/san_case.py > gpurun_out/synccheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Barrier" gpurun_out/synccheck.txt | head -8
+
+# The latency kernel (ec_small.cuh) at its pipeline edges: one stage + 1 and seven stages on one 3- and one 4-GF-warp geometry,
+# 1-byte shards, a 1-byte last block, and RS(8,8) rebuilding 8 shards.  Every object has an allocation of exactly its length
+# (PYTORCH_NO_CUDA_MEMORY_CACHING=1), so that memcheck sees any read past its last byte, including the zero-byte cp.async of a
+# shard row that is all padding.
+cat > /tmp/san_small.py <<'PY'
+import sys, numpy as np, torch
+sys.path.insert(0, '.'); sys.path.insert(0, 'tests')
+import minio_b200 as mb, oracle_lib as o
+st = torch.cuda.current_stream().cuda_stream
+g = torch.Generator(device="cuda:0"); g.manual_seed(5)
+rnd = lambda n: torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda:0", generator=g)
+for k, m, sup in ((12, 4, 768), (16, 4, 1024)):
+    for S in (1, sup + 1, 6 * sup + 29):
+        bs = k * S if k * S % 2 else k * S - 1
+        for length in (3 * bs + 1, 2 * bs + bs // 2):
+            nb, pitch = -(-length // bs), (S + 15) // 16 * 16
+            src = rnd(length)
+            par = torch.zeros((nb * m, pitch), dtype=torch.uint8, device="cuda:0")
+            dig = torch.zeros((nb, k + m, 32), dtype=torch.uint8, device="cuda:0")
+            c = mb.Codec(k, m, bs)
+            c.encode_blocks_device(src.data_ptr(), length, par.data_ptr(), pitch, dig.data_ptr(), st)
+            torch.cuda.synchronize()
+            assert c.stat("form_small") == c.launches == 1, (k, m, S, length)
+            h, hp, hd = src.cpu().numpy(), par.cpu().numpy(), dig.cpu().numpy()
+            for b in range(nb):
+                sh = o.encode_data(k, m, h[b * bs:(b + 1) * bs])
+                assert all(np.array_equal(hp[b * m + j, :sh[0].size], sh[k + j]) for j in range(m)), (k, m, S, length, b)
+                assert all(hd[b, i].tobytes() == o.hh256(sh[i]) for i in range(k + m)), (k, m, S, length, b)
+            c.close()
+k, m, S, nb = 8, 8, 769, 3
+erased = [0, 2, 4, 6, 9, 11, 13, 15]
+src = np.random.default_rng(6).integers(0, 256, nb * k * S, dtype=np.uint8)
+shards = [o.encode_data(k, m, src[b * k * S:(b + 1) * k * S]) for b in range(nb)]
+fp = (32 + S + 15) // 16 * 16
+frames = {}
+for i in range(k + m):
+    if i in erased: continue
+    f = np.zeros((nb, fp), dtype=np.uint8)
+    for b in range(nb):
+        f[b, :32] = np.frombuffer(o.hh256(shards[b][i]), dtype=np.uint8); f[b, 32:32 + S] = shards[b][i]
+    frames[i] = torch.from_numpy(f).to("cuda:0")
+out = torch.zeros((nb * 8, (S + 15) // 16 * 16), dtype=torch.uint8, device="cuda:0")
+dig = torch.zeros((nb, k + 8, 32), dtype=torch.uint8, device="cuda:0")
+cor = torch.zeros((nb, k), dtype=torch.uint8, device="cuda:0")
+c = mb.Codec(k, m, k * S)
+c.reconstruct_device([frames[i].data_ptr() if i in frames else 0 for i in range(k + m)], fp, nb, [int(i in erased) for i in range(k + m)],
+                     0, out.data_ptr(), out.shape[1], dig.data_ptr(), cor.data_ptr(), st)
+torch.cuda.synchronize()
+assert c.stat("form_small") == c.launches == 1 and int(cor.sum()) == 0
+ho = out.cpu().numpy()
+assert all(np.array_equal(ho[b * 8 + q, :S], shards[b][i]) for b in range(nb) for q, i in enumerate(erased))
+c.close()
+print("latency-kernel sanitizer case ok")
+PY
+logs=${SANITIZE_LOGS:-/tmp}   # full sanitizer reports of this stanza: small_<tool>.txt
+for tool in memcheck racecheck synccheck; do
+  echo "== $tool (latency kernel): $logs/small_$tool.txt"
+  PYTORCH_NO_CUDA_MEMORY_CACHING=1 timeout 1200 compute-sanitizer --tool $tool --print-limit 20 python /tmp/san_small.py > "$logs/small_$tool.txt" 2>&1
+  echo rc=$?; grep -E "ERROR SUMMARY|RACECHECK SUMMARY|sanitizer case ok|Invalid|out of bounds|hazard|Barrier" "$logs/small_$tool.txt" | head -12
+done
