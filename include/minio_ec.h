@@ -189,9 +189,14 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
  * the rest of the call, the part resuming at that block with the next reader.  out_files / write_quorum as mec_encode (complete
  * part.N images of dst's geometry, NULL = offline writer).  Returns total_length, or a negative MEC_ERR_*; *heal_hint =
  * MEC_ERR_FILE_CORRUPT when a source frame failed its digest but the part was still moved.
+ * dst's block size may be src's or a whole fraction of it: src block_size = R x dst block_size for an integer R >= 1 (a legacy
+ * part written with blockSizeV1 = 10 MiB, cmd/object-api-common.go:34, moved into a pool that writes blockSizeV2 = 1 MiB blocks).
+ * The part is still read, verified and failed over in source blocks; each source block becomes R destination blocks.
  * Refused before any device work: src == dst or a NULL src / dst / files / out_files (MEC_ERR_INVALID_ARGUMENT; for the same
- * geometry use a second handle), different block sizes or devices or an algorithm other than HighwayHash256S on either side
- * (MEC_ERR_UNSUPPORTED), fewer than write_quorum non-NULL out_files (MEC_ERR_WRITE_QUORUM).  total_length == 0 returns 0 and
+ * geometry use a second handle), a dst block size that does not divide src's (larger ones included), different devices, or an
+ * algorithm other than HighwayHash256S on either side (MEC_ERR_UNSUPPORTED: whole-file bitrot chains one digest over the whole
+ * shard file, so such parts move through mec_decode_whole + mec_encode_sg), fewer than write_quorum non-NULL out_files
+ * (MEC_ERR_WRITE_QUORUM).  total_length == 0 returns 0 and
  * writes nothing.  Fewer than k readable source files is MEC_ERR_READ_QUORUM.  Both codecs are held for the call.  Counters:
  * "blocks_read" and "bytes_h2d" grow on src, "blocks_encoded" and "bytes_d2h" on dst. */
 int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, const uint8_t* prefer, int64_t total_length,
@@ -270,6 +275,19 @@ int mec_batcher_heal(mec_batcher* b, const uint8_t* const* files, const uint8_t*
  * blocks and max_batch_blocks = 512. */
 int mec_batcher_new_transcode(int k, int m, int dst_k, int dst_m, int64_t block_size, int device, int64_t max_batch_blocks,
                               int max_wait_us, int flags, mec_batcher** out);
+/* mec_batcher_new_transcode with a destination block size of its own: moves from (k, m, block_size) to (dst_k, dst_m,
+ * dst_block_size), where block_size = R x dst_block_size for an integer R >= 1 (mec_transcode's rule; mec_batcher_new_transcode is
+ * dst_block_size = block_size).  Refusals in this order: the source geometry's errors, then the destination's, as mec_codec_new
+ * reports them; unknown flags (MEC_ERR_INVALID_ARGUMENT); block_size % dst_block_size != 0 (MEC_ERR_UNSUPPORTED).
+ * max_batch_blocks, the private-path threshold and the 1 GiB cap on a merged batch's staging count source blocks.  The destination
+ * codec's six slots are sized for the object bytes of a full source batch: B x R destination blocks each (B as above), i.e.
+ * B x R x (dst_block_size + dst_m x round_up(S', 16) + (dst_k + dst_m) x 32) bytes plus small tables (S' = ceil(dst_block_size /
+ * dst_k)) — per object byte what an R = 1 batcher spends.  Example: RS(12,4) at 10 MiB into RS(6,2) at 1 MiB (R = 10),
+ * max_batch_blocks = 16: B = 16 + 6 = 22, so each destination slot holds 220 blocks, 220 MiB of object bytes plus 73 MiB of
+ * parity rows, about 1.7 GiB for all six; the source side's six slots (staging, survivor arena, rebuilt rows) take about 3 GiB
+ * more. */
+int mec_batcher_new_transcode_ex(int k, int m, int64_t block_size, int dst_k, int dst_m, int64_t dst_block_size, int device,
+                                 int64_t max_batch_blocks, int max_wait_us, int flags, mec_batcher** out);
 /* mec_transcode through the coalescer: arguments, results, heal_hint and refusals of mec_transcode (files / prefer / total_length
  * of the source, out_files / write_quorum of the destination).  Checked on the caller's thread before anything is queued: a NULL
  * batcher, files or out_files, total_length < 0 or a batcher not made by mec_batcher_new_transcode (MEC_ERR_INVALID_ARGUMENT), fewer

@@ -76,6 +76,7 @@ def lib():
     L.mec_batcher_decode_prefer.argtypes = [vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_batcher_heal.argtypes = [vp, vp, vp, i64, vp, vp]
     L.mec_batcher_new_transcode.argtypes = [i32, i32, i32, i32, i64, i32, i64, i32, i32, C.POINTER(vp)]
+    L.mec_batcher_new_transcode_ex.argtypes = [i32, i32, i64, i32, i32, i64, i32, i64, i32, i32, C.POINTER(vp)]
     L.mec_batcher_transcode.restype = i64
     L.mec_batcher_transcode.argtypes = [vp, vp, vp, i64, vp, i32, C.POINTER(i32)]
     L.mec_batcher_stat.restype = i64
@@ -446,21 +447,25 @@ class Batcher:
     """mec_batcher: concurrent PutObject calls of one geometry merged into shared launches.  encode() may be called from many
     threads at once (ctypes releases the GIL for the duration of the call).  mix_patterns=True (MEC_BATCHER_MIX_PATTERNS): GETs
     and heals of different erasure patterns (reader sets, stale sets) share batches.  dst=(k2, m2) (mec_batcher_new_transcode): the
-    batcher also moves parts of its geometry to RS(k2, m2) of the same block size (transcode())."""
+    batcher also moves parts of its geometry to RS(k2, m2) of the same block size (transcode()); dst=(k2, m2, dst_block_size)
+    (mec_batcher_new_transcode_ex): to RS(k2, m2) with a block size that divides block_size (legacy 10 MiB parts into 1 MiB)."""
 
     def __init__(self, k, m, block_size=1 << 20, device=0, max_batch_blocks=256, max_wait_us=200, mix_patterns=False, dst=None):
         h = C.c_void_p()
         flags = MIX_PATTERNS if mix_patterns else 0
         if dst is None:
             rc = lib().mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, flags, C.byref(h))
-        else:
+        elif len(dst) == 2:
             rc = lib().mec_batcher_new_transcode(k, m, dst[0], dst[1], block_size, device, max_batch_blocks, max_wait_us, flags,
                                                  C.byref(h))
+        else:
+            rc = lib().mec_batcher_new_transcode_ex(k, m, block_size, dst[0], dst[1], dst[2], device, max_batch_blocks, max_wait_us,
+                                                    flags, C.byref(h))
         if rc:
             raise MecError(rc, "mec_batcher_new_ex" if dst is None else "mec_batcher_new_transcode")
         self.h, self.k, self.m, self.n, self.block_size = h, k, m, k + m, block_size
         self._sizes = Codec(k, m, block_size, device=device)
-        self._dst_sizes = None if dst is None else Codec(dst[0], dst[1], block_size, device=device)
+        self._dst_sizes = None if dst is None else Codec(dst[0], dst[1], dst[2] if len(dst) > 2 else block_size, device=device)
 
     def _encode_crc(self, src, files, dd, write_quorum, checksums):
         """mec_batcher_encode_crc -> (CRC32, CRC32C, CRC64NVME), 0 where not asked for"""

@@ -259,11 +259,15 @@ __global__ void __launch_bounds__(128) transcode_resplit_kernel(const __grid_con
 // grid (block stride, k source data shards, nreq), 128 threads: the batched form of transcode_resplit_kernel for a merged batch of
 // moves (mec_batcher_transcode).  Request z's decode plan (chosen readers, rebuilt data shards) and its source slots come from the
 // read table p.reqs[z], which covers the whole part (start_block 0); where its object bytes go comes from the PUT table d.reqs[z]
-// (len = total): full blocks at d.staged + (full0 + b) * bs, the short last block at d.staged + tail_src_off.  CTA (x, i, z) copies
-// the object bytes of data shard i of every block of request z, never Split's zero padding.  Both geometries share the block size,
-// so source block b is destination block b; the source's short last slot (shard length last_len) may still hold a short object
-// block when ceil(tail / k) == S, so each block's byte count is taken from the part length.  Source rows are read up to one word
-// past their end, inside the arena's padding and the slack behind the rebuilt rows (see transcode_resplit_kernel).
+// (len = total): full destination blocks at d.staged + full0 * d.bs onwards, the short last destination block at d.staged +
+// tail_src_off.  CTA (x, i, z) copies the object bytes of data shard i of every source block of request z, never Split's zero
+// padding.  Source block b (source block size p.bs) holds object bytes [b * p.bs, (b + 1) * p.bs); the destination block size d.bs
+// divides p.bs, so those bytes are whole destination blocks, except at the end of the part.  A shard's run of object bytes
+// [o, o + have) lies in the contiguous full destination blocks below edge = (len / d.bs) * d.bs and in the short last destination
+// block above it; a run that straddles the edge is copied in two pieces.  The source's short last slot (shard length last_len) may
+// still hold a short object block when ceil(tail / k) == S, so each block's byte count is taken from the part length.  Source rows
+// are read up to one word past their end, inside the arena's padding and the slack behind the rebuilt rows (see
+// transcode_resplit_kernel).
 __global__ void __launch_bounds__(128) batch_transcode_resplit_kernel(const BatchGetParams p, const BatchCopyParams d) {
   const BatchGetDesc& r = p.reqs[blockIdx.z];
   const BatchReqDesc& w = d.reqs[blockIdx.z];
@@ -272,7 +276,8 @@ __global__ void __launch_bounds__(128) batch_transcode_resplit_kernel(const Batc
   for (int x = 0; x < p.k; x++) if (r.chosen[x] == i) t = x;
   for (int x = 0; x < r.r; x++) if (r.targets[x] == i) q = x;
   if (t < 0 && q < 0) return;
-  const int64_t nfull = w.len / p.bs;
+  const int64_t edge = w.len / d.bs * d.bs;
+  uint8_t* const full = d.staged + w.full0 * d.bs;
   for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
     const bool is_tail = r.tail_slot >= 0 && b == r.nblocks - 1;
     const int64_t cur = is_tail ? r.last_len : p.S, slot = get_slot(r, b);
@@ -281,8 +286,10 @@ __global__ void __launch_bounds__(128) batch_transcode_resplit_kernel(const Batc
     have = have > cur ? cur : have;
     if (have <= 0) continue;
     const uint8_t* src = t >= 0 ? p.arena + t * p.arena_stride + slot * p.P + 32 : p.rebuilt + (slot * p.r + q) * p.pitch;
-    uint8_t* dst = d.staged + (b < nfull ? (w.full0 + b) * p.bs : w.tail_src_off) + static_cast<int64_t>(i) * cur;
-    cta_copy(dst, src, have, false);
+    const int64_t o = b * p.bs + static_cast<int64_t>(i) * cur;
+    const int64_t lo = o < edge ? (edge - o < have ? edge - o : have) : 0;  // bytes below the edge
+    if (lo > 0) cta_copy(full + o, src, lo, false);
+    if (lo < have) cta_copy(d.staged + w.tail_src_off + (o + lo - edge), src + lo, have - lo, false);
   }
 }
 

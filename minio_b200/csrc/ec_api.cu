@@ -1012,7 +1012,8 @@ static int emit_frames(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
 // Transcode sink of one chunk (whole part, so chunk block b is part block ch.b0 + b): the chunk's data shards, read or rebuilt,
 // re-split by ONE launch into the object bytes of its blocks in the destination codec's slot `si` (the same index as the source
 // slot, whose stream carries everything), then encoded there and queued as destination frames like mec_encode's.  *out is what
-// frames_retire needs once the chunk is accepted.
+// frames_retire needs once the chunk is accepted.  The destination block size divides the source's (R = bs / ebs): the re-split
+// runs in source blocks, and the chunk's object bytes are destination blocks [ch.b0 * R, ...), the part's short last one included.
 static_assert(kMaxK <= kBatchMaxFiles, "ResplitParams::src holds one entry per source data shard");
 static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk, const RChunk& ch, int si, int64_t stride,
                           int64_t pitch, EncChunk* out) {
@@ -1021,12 +1022,12 @@ static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk,
   Slot& d = e->slots[si];
   const int k = c->k;
   const int64_t bs = sk.bs, bytes = std::min(sk.total - ch.b0 * bs, ch.nb * bs);
-  const int64_t epitch = round_up(e->S(), 16);
+  const int64_t ebs = e->block_size, enb = ceil_frac(bytes, ebs), epitch = round_up(e->S(), 16);
   int rc;
   if ((rc = d.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
-  if ((rc = d.out.ensure(static_cast<size_t>(ch.nb * std::max(e->m, 1) * epitch)))) return rc;
-  if ((rc = d.dig.ensure(static_cast<size_t>(ch.nb * e->n * 32)))) return rc;
-  if ((rc = d.hdig.ensure(static_cast<size_t>(ch.nb * e->n * 32)))) return rc;
+  if ((rc = d.out.ensure(static_cast<size_t>(enb * std::max(e->m, 1) * epitch)))) return rc;
+  if ((rc = d.dig.ensure(static_cast<size_t>(enb * e->n * 32)))) return rc;
+  if ((rc = d.hdig.ensure(static_cast<size_t>(enb * e->n * 32)))) return rc;
   ResplitParams p;
   p.obj = static_cast<uint8_t*>(d.src.p);
   p.arena = static_cast<const uint8_t*>(s.aux.p); p.arena_stride = stride; p.P = g.dpitch();
@@ -1042,10 +1043,10 @@ static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk,
   if ((rc = encode_device_locked(e, p.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.p), s.st))) return rc;
   EncChunk& ec = *out;
   ec = EncChunk{};
-  ec.b0 = ch.b0; ec.nb = ch.nb; ec.nfull = p.nfull; ec.tail = p.tail; ec.s = &d; ec.pitch = epitch; ec.st = s.st;
-  ec.d_src = p.obj; ec.d_src_tail = p.obj + p.nfull * bs;
-  ec.d_out = static_cast<uint8_t*>(d.out.p); ec.d_out_tail = ec.d_out + p.nfull * e->m * epitch;
-  ec.h_dig = static_cast<const uint8_t*>(d.hdig.p); ec.h_dig_tail = ec.h_dig + p.nfull * e->n * 32;
+  ec.b0 = ch.b0 * (bs / ebs); ec.nb = enb; ec.nfull = bytes / ebs; ec.tail = bytes % ebs; ec.s = &d; ec.pitch = epitch; ec.st = s.st;
+  ec.d_src = p.obj; ec.d_src_tail = p.obj + ec.nfull * ebs;
+  ec.d_out = static_cast<uint8_t*>(d.out.p); ec.d_out_tail = ec.d_out + ec.nfull * e->m * epitch;
+  ec.h_dig = static_cast<const uint8_t*>(d.hdig.p); ec.h_dig_tail = ec.h_dig + ec.nfull * e->n * 32;
   return frames_enqueue_chunk(e, ec, sk.enc_files, true, nullptr);
 }
 
@@ -1070,6 +1071,9 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
   int64_t chunk = std::max<int64_t>(1, (32ll << 20) / std::max<int64_t>(1, g.S * k));
   chunk = std::max(chunk, std::min(4 * chunk, g.nblocks / 12));
   if (g.nblocks < 2 * chunk) chunk = std::max<int64_t>(4, ceil_frac(g.nblocks, 4));  // short ranges: ~four pieces, copies overlap (see encode_pipeline)
+  // a move from larger source blocks (legacy 10 MiB parts into 1 MiB blocks): one source block already carries R destination blocks
+  // and ~3 of them are the 32 MiB above, so a 64 MiB part would be three chunks; at least four keep its copies overlapping
+  if (sk.enc && sk.enc->block_size < sk.bs) chunk = std::min(chunk, ceil_frac(g.nblocks, 4));
   if (c->opt.chunk_blocks > 0) chunk = c->opt.chunk_blocks;
   chunk = std::min(chunk, g.nblocks);
   const int64_t stride = round_up(chunk * P + 512, 256);
@@ -1151,9 +1155,11 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     }
     if (good > 0 && sk.enc) {  // destination digests of the accepted blocks only; a redo rewrites every frame from the bad block on
       EncChunk acc = enc_inflight[si];
-      if (good < acc.nb) { acc.nb = acc.nfull = good; acc.tail = 0; }  // the short last block, if any, is the chunk's last: not accepted
+      // `good` whole source blocks are good * R full destination blocks; the part's short last destination block is the chunk's
+      // last: accepted only with the whole chunk
+      if (good < ch.nb) { acc.nb = acc.nfull = good * (sk.bs / sk.enc->block_size); acc.tail = 0; }
       frames_retire(sk.enc, acc, sk.enc_files, true, nullptr);
-      sk.enc->st_blocks_encoded += good;
+      sk.enc->st_blocks_encoded += acc.nb;
     }
     c->st_blocks_read += good;
     c->st_shards_rebuilt += good * ch.r;
@@ -1320,13 +1326,16 @@ extern "C" int mec_heal(mec_codec* c, const uint8_t* const* files, int64_t total
 // cmd/erasure-server-pool-rebalance.go:848): Erasure.Decode of a whole part on `src` piped into Erasure.Encode on `dst`.  The
 // reconstruct pipeline of mec_decode_prefer runs with the transcode sink, so the object bytes never leave the device: each chunk
 // is read, verified (and rebuilt where readers are missing), re-split, encoded and written out as dst's frames on one stream.
+// dst's block size may be a whole fraction of src's (a legacy blockSizeV1 = 10 MiB part re-PUT with blockSizeV2 = 1 MiB blocks,
+// cmd/object-api-common.go:34, cmd/storage-datatypes.go:393): chunks still run in source blocks, each re-split into R = src / dst
+// destination blocks.
 extern "C" int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, const uint8_t* prefer, int64_t total,
                                  mec_codec* dst, uint8_t* const* out_files, int write_quorum, int* heal_hint) {
   NvtxRange nvtx("mec_transcode");
   if (heal_hint) *heal_hint = 0;
   // one handle cannot be both ends: the source slots hold the survivors while the destination slots hold the re-split bytes
   if (!src || !dst || src == dst || !files || !out_files || total < 0) return MEC_ERR_INVALID_ARGUMENT;
-  if (src->block_size != dst->block_size || src->device != dst->device || src->algo != MEC_HIGHWAYHASH256S ||
+  if (src->block_size % dst->block_size != 0 || src->device != dst->device || src->algo != MEC_HIGHWAYHASH256S ||
       dst->algo != MEC_HIGHWAYHASH256S)
     return MEC_ERR_UNSUPPORTED;
   int online = 0;
@@ -3141,14 +3150,16 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     if (rc == MEC_OK) rc = ensure_crc(c);
     if (dst) {
       // the destination side of a merged transcode batch, laid out as a merged PUT batch of the destination geometry: object bytes,
-      // parity rows, digests, the PUT request table and the latency kernel's block table
+      // parity rows, digests, the PUT request table and the latency kernel's block table.  A batch of `slots` source blocks holds
+      // the object bytes of slots x R destination blocks (R = block_size / dst block size); it has at most `slots` requests.
       std::lock_guard<std::mutex> lk_dst(dst->mu);
+      const int64_t dslots = slots * (block_size / dst->block_size);
       for (Slot& s : dst->slots) {
-        if (rc == MEC_OK) rc = size_put_slot(dst, s, slots);
+        if (rc == MEC_OK) rc = size_put_slot(dst, s, dslots);
         if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
         if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
-        if (rc == MEC_OK) rc = s.blk.ensure(static_cast<size_t>(slots) * sizeof(SmallBlock));
-        if (rc == MEC_OK) rc = s.hblk.ensure(static_cast<size_t>(slots) * sizeof(SmallBlock));
+        if (rc == MEC_OK) rc = s.blk.ensure(static_cast<size_t>(dslots) * sizeof(SmallBlock));
+        if (rc == MEC_OK) rc = s.hblk.ensure(static_cast<size_t>(dslots) * sizeof(SmallBlock));
       }
     }
     cudaSetDevice(cur);
@@ -3185,18 +3196,26 @@ extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, 
   if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;
   return batcher_create(k, m, block_size, device, max_batch_blocks, max_wait_us, flags, nullptr, out);
 }
-extern "C" int mec_batcher_new_transcode(int k, int m, int dst_k, int dst_m, int64_t block_size, int device, int64_t max_batch_blocks,
-                                         int max_wait_us, int flags, mec_batcher** out) {
+extern "C" int mec_batcher_new_transcode_ex(int k, int m, int64_t block_size, int dst_k, int dst_m, int64_t dst_block_size, int device,
+                                            int64_t max_batch_blocks, int max_wait_us, int flags, mec_batcher** out) {
   if (!out) return MEC_ERR_INVALID_ARGUMENT;
   *out = nullptr;
-  if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;
   mec_codec* probe = nullptr;
   int rc = mec_codec_new(k, m, block_size, MEC_HIGHWAYHASH256S, device, &probe);  // the source geometry's errors come first
   mec_codec_free(probe);
   if (rc) return rc;
-  mec_codec* dst = nullptr;
-  if ((rc = mec_codec_new(dst_k, dst_m, block_size, MEC_HIGHWAYHASH256S, device, &dst))) return rc;
+  if ((rc = mec_codec_new(dst_k, dst_m, dst_block_size, MEC_HIGHWAYHASH256S, device, &probe))) return rc;
+  mec_codec* dst = probe;
+  if (flags & ~MEC_BATCHER_MIX_PATTERNS) { mec_codec_free(dst); return MEC_ERR_INVALID_ARGUMENT; }
+  if (block_size % dst_block_size != 0) { mec_codec_free(dst); return MEC_ERR_UNSUPPORTED; }  // as mec_transcode
   return batcher_create(k, m, block_size, device, max_batch_blocks, max_wait_us, flags, dst, out);
+}
+extern "C" int mec_batcher_new_transcode(int k, int m, int dst_k, int dst_m, int64_t block_size, int device, int64_t max_batch_blocks,
+                                         int max_wait_us, int flags, mec_batcher** out) {
+  if (!out) return MEC_ERR_INVALID_ARGUMENT;
+  *out = nullptr;
+  if (flags & ~MEC_BATCHER_MIX_PATTERNS) return MEC_ERR_INVALID_ARGUMENT;  // this call has always refused unknown flags first
+  return mec_batcher_new_transcode_ex(k, m, block_size, dst_k, dst_m, block_size, device, max_batch_blocks, max_wait_us, flags, out);
 }
 extern "C" int mec_batcher_new(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, mec_batcher** out) {
   return mec_batcher_new_ex(k, m, block_size, device, max_batch_blocks, max_wait_us, 0, out);

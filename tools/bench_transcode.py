@@ -1,12 +1,13 @@
 #!/usr/bin/env python
 """Data movement between pools: mec_transcode against mec_decode_prefer + mec_encode_sg on the same pinned, NUMA-local buffers.
 
-Workloads: RS(12,4) -> RS(6,2) and RS(12,4) -> RS(12,4), parts of 64 MiB and 1 MiB, source healthy and with two data drives offline.
+Workloads: RS(12,4) -> RS(6,2) and RS(12,4) -> RS(12,4) at 1 MiB blocks, and legacy parts written with 10 MiB blocks (blockSizeV1)
+moved from RS(12,4) into RS(6,2) at 1 MiB; parts of 64 MiB and 1 MiB, source healthy and with two data drives offline.
 After a warm-up the two modes run alternately, three timed runs each.  Prints one JSON line: GiB/s of part bytes and calls/s per
 mode, bytes moved per direction per call (from the codecs' counters), the card with its power limit and clock ceiling, and, from a
 separate profiled run, the kernel time per chunk of reconstruct, re-split and encode (CUDA activity trace).
 
-    python tools/bench_transcode.py [--out DIR]
+    python tools/bench_transcode.py [--out DIR] [--legacy-only]
 """
 import argparse
 import ctypes as C
@@ -42,12 +43,13 @@ def ptrs(arrs):
 
 
 class Workload:
-    def __init__(self, k1, m1, k2, m2, total, offline):
+    def __init__(self, k1, m1, k2, m2, total, offline, bs1=MiB, bs2=MiB):
         L = capi.lib()
         self.pinned = []
         pin = lambda n: self.pinned.append(mb.pinned_array(n, device=DEV)) or self.pinned[-1]
         self.k1, self.m1, self.k2, self.m2, self.total, self.offline = k1, m1, k2, m2, total, offline
-        self.src, self.dst = mb.Codec(k1, m1, MiB, device=DEV), mb.Codec(k2, m2, MiB, device=DEV)
+        self.bs1, self.bs2 = bs1, bs2
+        self.src, self.dst = mb.Codec(k1, m1, bs1, device=DEV), mb.Codec(k2, m2, bs2, device=DEV)
         data = pin(total)
         data[:] = np.random.default_rng(total + k2).integers(0, 256, total, dtype=np.uint8)
         fsz = self.src.bitrot_file_size(total)
@@ -63,7 +65,7 @@ class Workload:
         self.sg_files = [pin(dsz) if i >= k2 else None for i in range(k2 + m2)]
         self.marker = np.zeros(1, dtype=np.uint8)
         self.sg_ptrs = ptrs([f if f is not None else self.marker for f in self.sg_files])
-        nb = -(-total // MiB)
+        nb = -(-total // bs2)
         self.dd = pin(nb * k2 * 32)
         self.hint = C.c_int(0)
 
@@ -87,7 +89,7 @@ class Workload:
     def same_outputs(self):
         """parity drives byte for byte, data drives' digests: both modes wrote the same part files"""
         k2, S = self.k2, self.dst.shard_size()
-        nb = -(-self.total // MiB)
+        nb = -(-self.total // self.bs2)
         dd = self.dd.reshape(nb, k2, 32)
         for i in range(k2, k2 + self.m2):
             if not np.array_equal(self.outs[i], self.sg_files[i]):
@@ -102,7 +104,8 @@ class Workload:
         return {d: self.src.stat("bytes_" + d) + self.dst.stat("bytes_" + d) for d in ("h2d", "d2h")}
 
     def name(self):
-        return (f"RS({self.k1},{self.m1})->RS({self.k2},{self.m2}) {self.total // MiB} MiB "
+        bs = "" if self.bs1 == self.bs2 else f" {self.bs1 // MiB} MiB blocks -> {self.bs2 // MiB} MiB blocks,"
+        return (f"RS({self.k1},{self.m1})->RS({self.k2},{self.m2}){bs} {self.total // MiB} MiB "
                 + ("healthy" if not self.offline else f"data drives {sorted(self.offline)} offline"))
 
 
@@ -114,7 +117,7 @@ def timed(fn, calls):
 
 
 def measure(w, calls):
-    row = {"workload": w.name(), "part_bytes": w.total, "calls_per_run": calls}
+    row = {"workload": w.name(), "part_bytes": w.total, "src_block_size": w.bs1, "dst_block_size": w.bs2, "calls_per_run": calls}
     modes = {"transcode": w.transcode, "decode_encode_sg": w.decode_encode_sg}
     for fn in modes.values():
         for _ in range(3):
@@ -179,14 +182,17 @@ def kernel_times(w, calls, out_dir):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="directory for the profiler trace (default: a temporary one, removed)")
+    ap.add_argument("--legacy-only", action="store_true", help="only the workloads whose source block size differs")
     args = ap.parse_args()
     assert mb.device_count() > 0, "no CUDA device"
     capi.lib().mec_bind_thread_to_device(DEV)
-    result = {"card": card(), "block_size": MiB, "runs": 3, "results": [], "kernel_times": []}
-    for (k1, m1, k2, m2) in ((12, 4, 6, 2), (12, 4, 12, 4)):
+    result = {"card": card(), "runs": 3, "results": [], "kernel_times": []}
+    # (k1, m1, source block size, k2, m2, destination block size): equal pools, and a decommissioned pool's legacy 10 MiB-block parts
+    pairs = [(12, 4, MiB, 6, 2, MiB), (12, 4, MiB, 12, 4, MiB), (12, 4, 10 * MiB, 6, 2, MiB)]
+    for (k1, m1, bs1, k2, m2, bs2) in pairs[2:] if args.legacy_only else pairs:
         for total, calls in ((64 * MiB, 24), (MiB, 400)):
             for offline in ((), (0, 1)):
-                w = Workload(k1, m1, k2, m2, total, set(offline))
+                w = Workload(k1, m1, k2, m2, total, set(offline), bs1, bs2)
                 result["results"].append(measure(w, calls))
                 if total == 64 * MiB and (k1, m1, k2, m2) == (12, 4, 6, 2):
                     result["kernel_times"].append(kernel_times(w, 4, args.out))

@@ -11,7 +11,8 @@
 //                  the drives (hashOrder, cmd/erasure-metadata-utils.go:178), and ONE physical drive (drive 0) is offline (GET) or
 //                  stale (heal) — so the shard it held rotates from object to object: n erasure patterns in every round of requests
 //   mode btranscode : moves of whole parts from RS(12,4) to the destination geometry DST="k2,m2" (default 6,2; decommission and
-//                  rebalance, mec_batcher_transcode) through ONE transcode batcher (mec_batcher_new_transcode)
+//                  rebalance, mec_batcher_transcode) through ONE transcode batcher (mec_batcher_new_transcode_ex); block sizes in bytes
+//                  SRC_BS (source) and DST_BS (destination), default 1 MiB each (legacy 10 MiB-block parts: SRC_BS=10485760)
 //   mode transcode : the same moves, each a mec_transcode call on the handle pair t % P (source and destination codec)
 //   btranscode_rot / transcode_rot : as bget_rot, drive 0 offline and thread t's object rotated by t % n
 //                  (after the timed window every thread's out files are compared with a plain mec_encode on the destination geometry)
@@ -72,18 +73,19 @@ int main(int argc, char** argv) {
   const int P = argc > 5 ? atoi(argv[5]) : 8;
   const int device = argc > 6 ? atoi(argv[6]) : 0;
   const int k = 12, m = 4, n = k + m;
-  const int64_t bs = 1 << 20;
+  const bool move = mode == "btranscode" || mode == "transcode";
+  const int64_t bs = move && getenv("SRC_BS") ? atoll(getenv("SRC_BS")) : 1 << 20;
+  const int64_t bs2 = move && getenv("DST_BS") ? atoll(getenv("DST_BS")) : 1 << 20;
   const bool gpu = mode != "cpu";
   mec_codec* probe = nullptr;
   mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &probe);
   const int64_t S = mec_shard_size(probe), fsz = mec_bitrot_shard_file_size(mec_shard_file_size(probe, osize), S, MEC_HIGHWAYHASH256S);
   const int64_t nb = (osize + bs - 1) / bs;
-  const bool move = mode == "btranscode" || mode == "transcode";
   int k2 = 6, m2 = 2;
   if (const char* e = getenv("DST")) sscanf(e, "%d,%d", &k2, &m2);
   const int n2 = k2 + m2;
   mec_codec* probe2 = nullptr;
-  mec_codec_new(k2, m2, bs, MEC_HIGHWAYHASH256S, device, &probe2);
+  mec_codec_new(k2, m2, bs2, MEC_HIGHWAYHASH256S, device, &probe2);
   const int64_t fsz2 = mec_bitrot_shard_file_size(mec_shard_file_size(probe2, osize), mec_shard_size(probe2), MEC_HIGHWAYHASH256S);
   if (gpu) mec_bind_thread_to_device(device);
   auto alloc = [&](size_t b) -> uint8_t* { return gpu ? static_cast<uint8_t*>(mec_alloc_pinned_on(device, b)) : static_cast<uint8_t*>(malloc(b)); };
@@ -138,11 +140,11 @@ int main(int argc, char** argv) {
     }
     mec_codec_free(c0);
     if (mode == "btranscode") {
-      int rc = mec_batcher_new_transcode(k, m, k2, m2, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
-                                         getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
+      int rc = mec_batcher_new_transcode_ex(k, m, bs, k2, m2, bs2, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
+                                            getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
       if (rc) { fprintf(stderr, "transcode batcher: %d %s\n", rc, mec_last_error()); return 1; }
     } else {
-      for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k2, m2, bs, MEC_HIGHWAYHASH256S, device, &c); pool2.push_back(c); }
+      for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k2, m2, bs2, MEC_HIGHWAYHASH256S, device, &c); pool2.push_back(c); }
     }
   }
   if (mode == "get" || mode == "heal") {  // every thread's part files must exist first
@@ -248,7 +250,8 @@ int main(int argc, char** argv) {
            (long long)mec_batcher_stat(bat, "us_submit"), (long long)mec_batcher_stat(bat, "us_sync"), (long long)mec_batcher_stat(bat, "us_finish"),
            (long long)mec_batcher_stat(bat, "us_idle"), (long long)mec_batcher_stat(bat, "us_stage"), (long long)mec_batcher_stat(bat, "us_kernel"),
            (long long)mec_batcher_stat(bat, "us_scatter"));
-  if (move) printf(", \"dst\": \"%d,%d\"", k2, m2);
+  if (move) printf(", \"dst\": \"%d,%d\", \"src_block_size\": %lld, \"dst_block_size\": %lld", k2, m2, static_cast<long long>(bs),
+                  static_cast<long long>(bs2));
   if (mode == "btranscode")
     printf(", \"transcodes\": %lld, \"transcodes_serial\": %lld, \"redone\": %lld", static_cast<long long>(mec_batcher_stat(bat, "transcodes")),
            static_cast<long long>(mec_batcher_stat(bat, "transcodes_serial")), static_cast<long long>(mec_batcher_stat(bat, "redone")));

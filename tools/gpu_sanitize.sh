@@ -123,6 +123,28 @@ th = [threading.Thread(target=move, args=(t,)) for t in range(4)]
 assert all(r[1] == 0 and all(np.array_equal(x, y) for x, y in zip(r[0], tw[t])) for t, r in enumerate(res))
 assert bat.stat("batches") == 1 and bat.stat("transcodes") == 4
 bat.close()
+# legacy parts: RS(12,4) at 10 MiB blocks -> RS(6,2) at 1 MiB blocks, one merged batch of two moves (a source block run that
+# straddles the edge between full and short destination blocks) and one mec_transcode with source drive 1 offline
+lbs = 10 << 20
+ldat = [np.random.default_rng(40 + t).integers(0, 256, n, dtype=np.uint8) for t, n in enumerate((lbs + (1 << 19) + 7, 3 << 19))]
+lsrc = []
+for a in ldat:
+    fs = o.erasure_encode(k, m, lbs, 3, a)[0]
+    pf = [mb.pinned_array(f.size) for f in fs]
+    for x, f in zip(pf, fs): x[:] = f
+    lsrc.append(pf)
+ltw = [o.erasure_encode(6, 2, 1 << 20, 3, a)[0] for a in ldat]
+bat = mb.Batcher(k, m, lbs, max_batch_blocks=3, max_wait_us=500000, dst=(6, 2, 1 << 20))
+res = [None] * 2
+def lmove(t): res[t] = bat.transcode(lsrc[t], ldat[t].size, pinned=True)
+th = [threading.Thread(target=lmove, args=(t,)) for t in range(2)]
+[x.start() for x in th]; [x.join() for x in th]
+assert all(r[1] == 0 and all(np.array_equal(x, y) for x, y in zip(r[0], ltw[t])) for t, r in enumerate(res))
+assert bat.stat("batches") == 1 and bat.stat("transcodes") == 2
+bat.close()
+lc, ld = mb.Codec(k, m, lbs), mb.Codec(6, 2, 1 << 20)
+outs, hint = lc.transcode([None if i == 1 else f for i, f in enumerate(lsrc[0])], ldat[0].size, ld)
+assert hint == 0 and all(np.array_equal(x, y) for x, y in zip(outs, ltw[0]))
 print("sanitizer case ok")
 PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
