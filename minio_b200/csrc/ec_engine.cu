@@ -737,8 +737,9 @@ int Engine::launch_fused(const FusedDesc& d, const EngineOptions& opt, cudaStrea
       p.in_ptr[t] = d.in_ptr[t];
       if (!use_tma) continue;
       const int64_t off = d.in_ptr[t] - d.map_base[t];  // offset of the shard inside its block row
+      // TMA fills a box outside the map with zeros: the shard must lie inside the row the map covers, for one block as for many
       if ((reinterpret_cast<uintptr_t>(d.map_base[t]) & 15) || off < 0 || off + ntiles * kTile + 64 >= (1ll << 31) ||
-          d.nblocks >= (1ll << 31) || row_bytes >= (1ll << 33) || (d.nblocks > 1 && off + d.S > d.in_block_stride)) {
+          d.nblocks >= (1ll << 31) || row_bytes >= (1ll << 33) || off + d.S > row_bytes) {
         use_tma = false;
       } else {
         p.in_c0[t] = static_cast<int32_t>(off & ~15ll);
