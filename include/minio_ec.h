@@ -212,7 +212,8 @@ int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, const uint8_t
  * device staging for all six is allocated here (about 2.4 x max_batch_blocks x block_size each).
  * mec_batcher_stat: "batches", "requests", "blocks", "kernel_batches" (batches moved by the gather / scatter kernels), "redone"
  * (merged GETs and heals that met a frame failing its digest check and were redone on their own), "crc_requests" (PUTs through
- * mec_batcher_encode_crc with a non-empty mask that got their checksums), "launches", "patterns" (distinct erasure patterns — reader
+ * mec_batcher_encode_crc / _sums with a non-empty CRC mask that got their checksums), "sum_requests" (PUTs through
+ * mec_batcher_encode_sums that got at least one MD5 / SHA-1 / SHA-256 digest), "launches", "patterns" (distinct erasure patterns — reader
  * set plus rebuilt shards — summed over GET and heal batches) and "mixed_batches" (GET and heal batches of more than one pattern);
  * with MEC_BATCHER_TRACE=1 in the environment also the worker's and the streams' accumulated phase times "us_submit", "us_sync",
  * "us_finish", "us_idle", "us_stage", "us_kernel", "us_scatter".  Any other name is answered by mec_get_stat on the batcher's own
@@ -245,6 +246,19 @@ int64_t mec_batcher_encode_sg(mec_batcher* b, const uint8_t* src, int64_t len, u
  * mask share batches. */
 int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
                                int write_quorum, int which, uint64_t* out3);
+/* mec_batcher_encode_crc plus the hashes hash.Reader computes over a PutObject body that cannot be merged from parts: MD5 for the
+ * ETag (internal/etag/reader.go), SHA-256 of a signed payload (x-amz-content-sha256) and SHA-1 / SHA-256 of x-amz-checksum-sha1 /
+ * -sha256 (internal/hash/reader.go:267-310).  Outputs and return value are those of mec_batcher_encode_crc (data_digests == NULL:
+ * complete part files; non-NULL: the scatter-gather outputs).  `which` is any subset of MEC_CRC* and MEC_SUM_* (below); any other
+ * bit returns MEC_ERR_INVALID_ARGUMENT.  crc3 receives the CRCs as mec_batcher_encode_crc's out3 does; sums (MEC_SUM_BYTES bytes)
+ * receives the asked-for digests at their offsets, the other bytes are left as they were.  A set bit with a NULL destination returns
+ * MEC_ERR_INVALID_ARGUMENT before anything is queued.  Outputs are written only when the call returns >= 0; len == 0 gives the
+ * digests of the empty message without device work.  Each batch that holds requests with MEC_SUM_* bits adds ONE stream_sums_kernel
+ * launch (one thread per request and algorithm, on a second stream of the batch's slot, forked once the batch is staged so the
+ * encode does not wait for it) and one small copy back; the batch completes when both are done.  Requests with and without hashes
+ * share batches. */
+int64_t mec_batcher_encode_sums(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
+                                int write_quorum, int which, uint64_t* crc3, uint8_t* sums);
 /* Erasure.Decode through the coalescer (arguments and results of mec_decode): GETs queued together that see the same drives online
  * share one reader set and are merged into one fused launch (gather kernel, reconstruct, scatter into every caller's dst).  A request
  * that meets a corrupt frame is redone on its own with parallelReader's exact fail-over; pageable buffers take the same private path. */
@@ -324,6 +338,23 @@ int mec_checksums_device(mec_codec* c, const uint8_t* d_src, int64_t len, int wh
 int mec_checksums(mec_codec* c, const uint8_t* src, int64_t len, int which, uint64_t* out3);
 uint64_t mec_checksum_combine(int type, uint64_t crc1, uint64_t crc2, int64_t len2);
 int64_t mec_last_checksums(const mec_codec* c, uint64_t* out3);
+
+/* ---- object hashes of many messages at once (MD5, SHA-1, SHA-256) ----------------------------------------------------------
+ * MD5 (the ETag), SHA-1 and SHA-256 are chains that cannot be split: one GPU thread hashes one message, far slower than a CPU core
+ * does, so this pays only for many independent messages at once (one thread per message and algorithm, one launch).
+ * mec_sums_device: message i is d_base[offsets[i], offsets[i] + lens[i]) (offsets and lens are host arrays, read before the call
+ * returns; any byte alignment); its record is d_sums + i * MEC_SUM_BYTES: MD5 at +0 (16 bytes), SHA-1 at +32 (20 bytes), SHA-256 at
+ * +64 (32 bytes), each in the byte order of Go's Sum(nil).  Slots of algorithms not asked for, and the padding bytes, are left as
+ * they were.  `which` must be a non-empty subset of MEC_SUM_*; any other value, count < 0, a negative offset or length, or NULL
+ * offsets / lens / d_sums with count > 0 (or d_base with a non-empty message) return MEC_ERR_INVALID_ARGUMENT before any device
+ * work.  A zero-length message yields the digest of the empty message.  Asynchronous on `cuda_stream`; calls on one handle share
+ * its work table, so a call first waits on the host until the previous call's kernel has finished. */
+#define MEC_SUM_MD5 8
+#define MEC_SUM_SHA1 16
+#define MEC_SUM_SHA256 32
+#define MEC_SUM_BYTES 96 /* MD5 at +0 (16 B), SHA-1 at +32 (20 B), SHA-256 at +64 (32 B) */
+int mec_sums_device(mec_codec* c, int which, const uint8_t* d_base, const int64_t* offsets, const int64_t* lens, int64_t count,
+                    uint8_t* d_sums, void* cuda_stream);
 
 /* ---- legacy whole-file bitrot (cmd/bitrot-whole.go, BitrotAlgorithm SHA256 / BLAKE2b512 / HighwayHash256) ----
  * Erasure.Encode with wholeBitrotWriters (cmd/bitrot-whole.go:35-45): files[i] receives the raw shard file

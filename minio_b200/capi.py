@@ -11,6 +11,10 @@ ERRORS = {-1: "ErrInvShardNum", -2: "ErrMaxShardNum", -3: "ErrTooFewShards", -4:
           -11: "errErasureWriteQuorum", -12: "errInvalidArgument", -100: "CUDA error", -101: "no CUDA device",
           -102: "unsupported on the GPU path"}
 MIX_PATTERNS = 1  # MEC_BATCHER_MIX_PATTERNS
+CRC32, CRC32C, CRC64NVME = 1, 2, 4  # MEC_CRC*
+SUM_MD5, SUM_SHA1, SUM_SHA256 = 8, 16, 32  # MEC_SUM_*
+SUM_BYTES = 96  # MEC_SUM_BYTES: one record of mec_sums_device / mec_batcher_encode_sums
+SUM_SLOTS = {"md5": (SUM_MD5, 0, 16), "sha1": (SUM_SHA1, 32, 20), "sha256": (SUM_SHA256, 64, 32)}  # name -> (bit, offset, length)
 
 _LIB = None
 
@@ -70,6 +74,9 @@ def lib():
     L.mec_batcher_encode_sg.argtypes = [vp, vp, i64, vp, vp, i32]
     L.mec_batcher_encode_crc.restype = i64
     L.mec_batcher_encode_crc.argtypes = [vp, vp, i64, vp, vp, i32, i32, vp]
+    L.mec_batcher_encode_sums.restype = i64
+    L.mec_batcher_encode_sums.argtypes = [vp, vp, i64, vp, vp, i32, i32, vp, vp]
+    L.mec_sums_device.argtypes = [vp, i32, vp, vp, vp, i64, vp, vp]
     L.mec_batcher_decode.restype = i64
     L.mec_batcher_decode.argtypes = [vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_batcher_decode_prefer.restype = i64
@@ -259,6 +266,17 @@ class Codec:
         if rc:
             raise MecError(rc, "mec_checksums_device")
         return tuple(int(v) for v in out)
+
+    def sums_device(self, d_base, offsets, lens, which, d_sums, stream=0):
+        """mec_sums_device: MD5 / SHA-1 / SHA-256 (a mask of SUM_*) of the messages d_base[offsets[i], offsets[i] + lens[i]) in device
+        memory; record i (SUM_BYTES bytes, see SUM_SLOTS) at d_sums + i * SUM_BYTES.  Asynchronous on `stream`."""
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        ln = np.ascontiguousarray(lens, dtype=np.int64)
+        if off.size != ln.size:
+            raise ValueError("offsets and lens differ in length")
+        rc = lib().mec_sums_device(self.h, which, d_base, off.ctypes.data, ln.ctypes.data, off.size, d_sums, stream)
+        if rc:
+            raise MecError(rc, "mec_sums_device")
 
     def last_checksums(self):
         out = (C.c_uint64 * 3)()
@@ -476,16 +494,30 @@ class Batcher:
             raise MecError(rc, "mec_batcher_encode_crc")
         return tuple(int(v) for v in out)
 
-    def encode(self, src, online=None, write_quorum=0, pinned=False, checksums=0):
+    def _encode_sums(self, src, files, dd, write_quorum, checksums, hashes):
+        """mec_batcher_encode_sums -> ((CRC32, CRC32C, CRC64NVME), {"md5": ..., "sha1": ..., "sha256": ...} for the bits of hashes)"""
+        out = (C.c_uint64 * 3)()
+        rec = (C.c_uint8 * SUM_BYTES)()
+        rc = lib().mec_batcher_encode_sums(self.h, src.ctypes.data if src.size else None, src.size, _ptrs(files),
+                                           None if dd is None else dd.ctypes.data, write_quorum, checksums | hashes, out, rec)
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_encode_sums")
+        return tuple(int(v) for v in out), {name: bytes(rec[o:o + n]) for name, (bit, o, n) in SUM_SLOTS.items() if hashes & bit}
+
+    def encode(self, src, online=None, write_quorum=0, pinned=False, checksums=0, hashes=0):
         """pinned=True: the part files are allocated page-locked (and `src` must be, e.g. a pinned_array) — the batch then moves
         through the gather / scatter kernels instead of per-request copies.  The caller owns (and should free) those arrays.
         checksums: a mask of CRC32 / CRC32C / CRC64NVME; non-zero returns (files, (crc32, crc32c, crc64nvme)) computed on the
-        bytes the batch staged (mec_batcher_encode_crc)."""
+        bytes the batch staged (mec_batcher_encode_crc).  hashes: a mask of SUM_MD5 / SUM_SHA1 / SUM_SHA256; non-zero appends
+        {"md5": bytes, "sha1": bytes, "sha256": bytes} with the keys asked for (mec_batcher_encode_sums)."""
         src = _u8(src)
         fsz = self._sizes.bitrot_file_size(src.size)
         online = [True] * self.n if online is None else online
         mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
         files = [mk(fsz) if online[i] else None for i in range(self.n)]
+        if hashes:
+            crcs, sums = self._encode_sums(src, files, None, write_quorum, checksums, hashes)
+            return (files, crcs, sums) if checksums else (files, sums)
         if checksums:
             return files, self._encode_crc(src, files, None, write_quorum, checksums)
         rc = lib().mec_batcher_encode(self.h, src.ctypes.data if src.size else None, src.size, _ptrs(files), write_quorum)
@@ -493,10 +525,11 @@ class Batcher:
             raise MecError(rc, "mec_batcher_encode")
         return files
 
-    def encode_sg(self, src, online=None, write_quorum=0, pinned=False, checksums=0):
+    def encode_sg(self, src, online=None, write_quorum=0, pinned=False, checksums=0, hashes=0):
         """mec_batcher_encode_sg: -> (files, data_digests) shaped like Codec.encode_sg.  pinned=True: the parity images and the
         [block][k][32] digest array are page-locked (and `src` must be), so the scatter kernel writes both; the caller owns them.
-        checksums: as for encode(); non-zero returns (files, data_digests, (crc32, crc32c, crc64nvme))."""
+        checksums: as for encode(); non-zero returns (files, data_digests, (crc32, crc32c, crc64nvme)).  hashes: as for encode();
+        non-zero appends the digest dict."""
         src = _u8(src)
         fsz = self._sizes.bitrot_file_size(src.size)
         nb = -(-src.size // self.block_size)
@@ -505,6 +538,10 @@ class Batcher:
         marker = np.zeros(1, dtype=np.uint8)  # data drives: only NULL / non-NULL is looked at
         files = [(mk(fsz) if i >= self.k else marker) if online[i] else None for i in range(self.n)]
         dd = mk(max(nb, 1) * self.k * 32).reshape(max(nb, 1), self.k, 32)
+        if hashes:
+            crcs, sums = self._encode_sums(src, files, dd, write_quorum, checksums, hashes)
+            files = [f if i >= self.k else None for i, f in enumerate(files)]
+            return (files, dd[:nb], crcs, sums) if checksums else (files, dd[:nb], sums)
         if checksums:
             crcs = self._encode_crc(src, files, dd, write_quorum, checksums)
             return [f if i >= self.k else None for i, f in enumerate(files)], dd[:nb], crcs

@@ -15,6 +15,7 @@
 #include "ec_engine.h"
 #include "whole_hash.cuh"
 #include "crc.cuh"
+#include "obj_hash.cuh"
 #include "batch_copy.cuh"
 #include <nvtx3/nvToolsExt.h>
 
@@ -65,7 +66,8 @@ struct Slot {
   DevBuf crc_tab;                    // checksum work table of a merged batch ([CrcReq nreq][CrcWork nwork], crc.cuh)
   DevBuf dreq;                       // request table of a merged batch (batch_copy.cuh)
   DevBuf blk;                        // per-block geometry of a merged launch (SmallBlock / per-frame lengths)
-  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab;
+  DevBuf sum_tab, sum_out;           // object hashes of a merged batch: SumWork table, one kSumRecord record per request (obj_hash.cuh)
+  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum;
   cudaStream_t st = nullptr;
 };
 
@@ -83,6 +85,10 @@ struct mec_codec {
   int checksums = 0;                    // option "checksums": MEC_CRC32 | MEC_CRC32C | MEC_CRC64NVME computed by the host-buffer encode calls
   uint64_t last_crc[kCrcTypes] = {0, 0, 0};
   int64_t last_crc_len = 0;
+  // mec_sums_device: the work table of the last call, and an event behind its kernel (the next call refills the table after it)
+  DevBuf sum_tab;
+  PinBuf hsum_tab;
+  cudaEvent_t sum_ev = nullptr;
   // boundary counters (mec_get_stat)
   int64_t st_blocks_encoded = 0, st_blocks_read = 0, st_shards_rebuilt = 0, st_corrupt = 0, st_h2d = 0, st_d2h = 0;
   int64_t S() const { return ceil_frac(block_size, k); }
@@ -204,10 +210,13 @@ extern "C" void mec_codec_free(mec_codec* c) {
     if (s.st) { cudaStreamSynchronize(s.st); cudaStreamDestroy(s.st); }
     s.src.release(); s.out.release(); s.dig.release(); s.aux.release(); s.flags.release();
     s.hdig.release(); s.hflags.release(); s.hcrc.release(); s.crc_part.release(); s.crc_out.release(); s.dreq.release(); s.hreq.release(); s.blk.release(); s.hblk.release();
-    s.crc_tab.release(); s.hcrc_tab.release();
+    s.crc_tab.release(); s.hcrc_tab.release(); s.sum_tab.release(); s.sum_out.release(); s.hsum_tab.release(); s.hsum.release();
   }
   c->flags.release();
   c->crc_tables.release();
+  if (c->sum_ev) cudaEventDestroy(c->sum_ev);
+  c->sum_tab.release();
+  c->hsum_tab.release();
   delete c;
 }
 
@@ -375,6 +384,64 @@ extern "C" int mec_checksums_device(mec_codec* c, const uint8_t* d_src, int64_t 
   if ((rc = checksums_enqueue(c, d_src, len, which, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), st))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(out3, s.crc_out.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   MEC_CUDA_OK(cudaStreamSynchronize(st));
+  return MEC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// object hashes (obj_hash.cuh): MD5 / SHA-1 / SHA-256 of many two-segment messages in device memory, one thread per (message,
+// algorithm).  The host writes the work table, sorted by (algorithm, length descending) so that a warp runs one algorithm over
+// similar lengths; mec_sums_device and the coalescer's PUT batches share this table code and the launch.
+constexpr int kSumMask = MEC_SUM_MD5 | MEC_SUM_SHA1 | MEC_SUM_SHA256;
+static_assert(MEC_SUM_BYTES == kSumRecord && MEC_SUM_MD5 << 1 == MEC_SUM_SHA1 && MEC_SUM_MD5 << 2 == MEC_SUM_SHA256, "obj_hash.cuh");
+
+// appends the items of one message (segments at off0 / off1 of the base buffer) whose record is at byte `rec` of the output
+static int64_t sum_items(SumWork* t, int64_t w, int which, int64_t rec, int64_t off0, int64_t len0, int64_t off1, int64_t len1) {
+  for (int a = 0; a < kSumAlgos; a++)
+    if (which & (MEC_SUM_MD5 << a)) t[w++] = SumWork{off0, len0, off1, len1, rec + 32 * a, a, 0};
+  return w;
+}
+static void sum_sort(SumWork* t, int64_t n) {
+  std::sort(t, t + n, [](const SumWork& x, const SumWork& y) {
+    return x.algo != y.algo ? x.algo < y.algo : x.len0 + x.len1 > y.len0 + y.len1;
+  });
+}
+// enqueue: ONE stream_sums_kernel over the nwork items of the device table `work`
+static int sum_launch(mec_codec* c, const uint8_t* base, const SumWork* work, int64_t nwork, uint8_t* out, cudaStream_t st) {
+  SumParams p;
+  p.base = base; p.work = work; p.nwork = nwork; p.out = out;
+  stream_sums_kernel<<<static_cast<unsigned>(ceil_frac(nwork, kSumThreads)), kSumThreads, 0, st>>>(p);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  return MEC_OK;
+}
+
+extern "C" int mec_sums_device(mec_codec* c, int which, const uint8_t* d_base, const int64_t* offsets, const int64_t* lens,
+                               int64_t count, uint8_t* d_sums, void* stream) {
+  if (!c || which <= 0 || (which & ~kSumMask) || count < 0) return MEC_ERR_INVALID_ARGUMENT;
+  if (count == 0) return MEC_OK;
+  if (!offsets || !lens || !d_sums) return MEC_ERR_INVALID_ARGUMENT;
+  for (int64_t i = 0; i < count; i++)
+    if (offsets[i] < 0 || lens[i] < 0 || (lens[i] > 0 && !d_base)) return MEC_ERR_INVALID_ARGUMENT;
+  const int per = __builtin_popcount(static_cast<unsigned>(which));
+  if (count > (int64_t{1} << 36) / per) return MEC_ERR_UNSUPPORTED;  // the grid's x dimension
+  std::lock_guard<std::mutex> lk(c->mu);
+  int rc;
+  if ((rc = ensure_engine(c))) return rc;
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  if (!c->sum_ev) MEC_CUDA_OK(cudaEventCreateWithFlags(&c->sum_ev, cudaEventDisableTiming));
+  MEC_CUDA_OK(cudaEventSynchronize(c->sum_ev));  // the previous call's kernel has read its table
+  const int64_t nwork = count * per;
+  const size_t bytes = static_cast<size_t>(nwork) * sizeof(SumWork);
+  if ((rc = c->hsum_tab.ensure(bytes))) return rc;
+  if ((rc = c->sum_tab.ensure(bytes))) return rc;
+  SumWork* t = static_cast<SumWork*>(c->hsum_tab.p);
+  int64_t w = 0;
+  for (int64_t i = 0; i < count; i++) w = sum_items(t, w, which, i * kSumRecord, offsets[i], lens[i], 0, 0);
+  sum_sort(t, nwork);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MEC_CUDA_OK(cudaMemcpyAsync(c->sum_tab.p, t, bytes, cudaMemcpyHostToDevice, st));
+  if ((rc = sum_launch(c, d_base, static_cast<const SumWork*>(c->sum_tab.p), nwork, d_sums, st))) return rc;
+  MEC_CUDA_OK(cudaEventRecord(c->sum_ev, st));
   return MEC_OK;
 }
 
@@ -2153,8 +2220,10 @@ struct BatchReq {
   uint8_t* data_digests = nullptr;
   bool with_data = false;
   bool mapped = false;   // every buffer of the call is page-locked (device-addressable): eligible for the gather / scatter kernels
-  int crc_which = 0;          // MEC_CRC* mask of mec_batcher_encode_crc; the results go to crc_out[0..3)
+  int crc_which = 0;          // MEC_CRC* mask of mec_batcher_encode_crc / _sums; the results go to crc_out[0..3)
   uint64_t* crc_out = nullptr;
+  int sum_which = 0;          // MEC_SUM_* mask of mec_batcher_encode_sums; the digests go to their slots of sums[0..MEC_SUM_BYTES)
+  uint8_t* sums = nullptr;
   int64_t result = 0;
   bool done = false;
   std::condition_variable cv;  // one per request: a finished batch wakes its own callers, not every thread parked in the batcher
@@ -2193,6 +2262,11 @@ struct mec_batcher {
   std::atomic<int64_t> st_batches{0}, st_requests{0}, st_blocks{0}, st_kernel_batches{0};
   std::atomic<int64_t> st_redone{0};  // merged GETs and heals that met a frame failing its digest and were redone on their own
   std::atomic<int64_t> st_crc_requests{0};  // PUTs that got their object checksums (mec_batcher_encode_crc)
+  std::atomic<int64_t> st_sum_requests{0};  // PUTs that got at least one object hash (mec_batcher_encode_sums)
+  // object hashes of a PUT batch run on a second stream per slot, forked once the batch is staged (ev_staged) and joined before the
+  // slot's stream ends (ev_summed), so the batch's encode is not queued behind them
+  cudaStream_t sum_st[kSlots] = {};
+  cudaEvent_t ev_staged[kSlots] = {}, ev_summed[kSlots] = {};
   // MEC_BATCHER_MIX_PATTERNS (and a codec whose options allow the latency kernel): GETs merge with GETs and heals with heals
   // whatever their reader and stale sets, as long as a batch of several erasure patterns fits one latency launch
   bool mix = false;
@@ -2282,6 +2356,12 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
         for (int ty = 0; ty < kCrcTypes; ty++) r->crc_out[ty] = h[ty];
         b->st_crc_requests++;
       }
+      if (rc == MEC_OK && r->sum_which) {  // batcher_sums_fork's records, record q of the slot's pinned mirror
+        const uint8_t* h = static_cast<const uint8_t*>(s.hsum.p) + q * kSumRecord;
+        for (int a = 0; a < kSumAlgos; a++)
+          if (r->sum_which & (MEC_SUM_MD5 << a)) memcpy(r->sums + 32 * a, h + 32 * a, static_cast<size_t>(sum_digest_len(a)));
+        b->st_sum_requests++;
+      }
       r->result = rc == MEC_OK ? r->len : rc;
     }
   }
@@ -2362,6 +2442,54 @@ static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
   MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, static_cast<size_t>(p.nreq) * kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
+  return MEC_OK;
+}
+
+// Object hashes of the PUTs of a batch that asked for them (mec_batcher_encode_sums): one work item per (request, algorithm) over
+// the request's two segments of s.src (full blocks at ch.d_src, short last block at ch.d_src_tail), record q of s.sum_out for
+// request q.  batcher_sums_table writes the table and enqueues its copy ahead of the staging, as batcher_crc_table does, and
+// returns the number of items (0: the batch enqueues nothing for hashes).  batcher_sums_fork, enqueued once the batch is staged,
+// runs ONE stream_sums_kernel on the slot's second stream; batcher_sums_join makes the slot's stream wait for it and copies the
+// records to s.hsum, where batcher_finish reads them.  The buffers were sized by mec_batcher_new; they only grow here for a batch led
+// by a request larger than max_batch_blocks.
+static int batcher_sums_table(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t* nwork) {
+  *nwork = 0;
+  for (BatchReq* r : reqs) *nwork += __builtin_popcount(static_cast<unsigned>(r->sum_which));
+  if (*nwork == 0) return MEC_OK;
+  const int64_t bs = b->codec->block_size;
+  const size_t bytes = static_cast<size_t>(*nwork) * sizeof(SumWork);
+  int rc;
+  if ((rc = s.hsum_tab.ensure(bytes))) return rc;
+  if ((rc = s.sum_tab.ensure(bytes))) return rc;
+  if ((rc = s.sum_out.ensure(reqs.size() * kSumRecord))) return rc;
+  if ((rc = s.hsum.ensure(reqs.size() * kSumRecord))) return rc;
+  const uint8_t* base = static_cast<const uint8_t*>(s.src.p);
+  SumWork* t = static_cast<SumWork*>(s.hsum_tab.p);
+  int64_t w = 0;
+  for (size_t q = 0; q < reqs.size(); q++) {
+    const EncChunk& ch = reqs[q]->ch;
+    w = sum_items(t, w, reqs[q]->sum_which, static_cast<int64_t>(q) * kSumRecord, ch.nfull ? ch.d_src - base : 0, ch.nfull * bs,
+                  ch.tail ? ch.d_src_tail - base : 0, ch.tail);
+  }
+  sum_sort(t, w);
+  MEC_CUDA_OK(cudaMemcpyAsync(s.sum_tab.p, t, bytes, cudaMemcpyHostToDevice, s.st));
+  return MEC_OK;
+}
+static int batcher_sums_fork(mec_batcher* b, Slot& s, int64_t nwork) {
+  if (nwork == 0) return MEC_OK;
+  const int si = static_cast<int>(&s - b->codec->slots);
+  MEC_CUDA_OK(cudaEventRecord(b->ev_staged[si], s.st));
+  MEC_CUDA_OK(cudaStreamWaitEvent(b->sum_st[si], b->ev_staged[si], 0));
+  int rc = sum_launch(b->codec, static_cast<const uint8_t*>(s.src.p), static_cast<const SumWork*>(s.sum_tab.p), nwork,
+                      static_cast<uint8_t*>(s.sum_out.p), b->sum_st[si]);
+  if (rc) return rc;
+  MEC_CUDA_OK(cudaEventRecord(b->ev_summed[si], b->sum_st[si]));
+  return MEC_OK;
+}
+static int batcher_sums_join(mec_batcher* b, Slot& s, size_t nreq, int64_t nwork) {
+  if (nwork == 0) return MEC_OK;
+  MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_summed[&s - b->codec->slots], 0));
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hsum.p, s.sum_out.p, nreq * kSumRecord, cudaMemcpyDeviceToHost, s.st));
   return MEC_OK;
 }
 
@@ -2501,6 +2629,8 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, reqs.size() * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
     CrcSegParams crc;
     if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
+    int64_t nsum;
+    if ((rc = batcher_sums_table(b, s, reqs, &nsum))) return rc;
     BatchCopyParams cp;
     cp.reqs = static_cast<const BatchReqDesc*>(s.dreq.p);
     cp.nreq = static_cast<int>(reqs.size()); cp.k = k; cp.m = m; cp.bs = bs; cp.S = S; cp.pitch = pitch;
@@ -2544,15 +2674,19 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     }
     if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[si], 0));
     mark_phase(b, s, 1);
+    if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
     if ((rc = batcher_crc_launch(b, s, crc))) return rc;
     if ((rc = batch_encode_scatter(c, s, s.st, tab, reqs.size(), lay, cp, b->sw.trace ? b->ev_ph[si][2] : nullptr))) return rc;
     mark_phase(b, s, 3);
+    if ((rc = batcher_sums_join(b, s, reqs.size(), nsum))) return rc;
     *needs_retire = false;
     c->st_blocks_encoded += nslots;
     return MEC_OK;
   }
   CrcSegParams crc;
   if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
+  int64_t nsum;
+  if ((rc = batcher_sums_table(b, s, reqs, &nsum))) return rc;
   for (BatchReq* r : reqs) {
     const EncChunk& ch = r->ch;
     if (ch.nfull > 0)
@@ -2561,6 +2695,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
       MEC_CUDA_OK(cudaMemcpyAsync(const_cast<uint8_t*>(ch.d_src_tail), r->src + ch.nfull * bs, static_cast<size_t>(ch.tail), cudaMemcpyHostToDevice, s.st));
     c->st_h2d += r->len;
   }
+  if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
   if ((rc = batcher_crc_launch(b, s, crc))) return rc;
   if (lay.total_full > 0 && (rc = encode_device_locked(c, dsrc, lay.total_full * bs, dout, pitch, ddig, s.st))) return rc;  // ONE launch for every caller's full blocks
   const uint8_t* hdig = static_cast<const uint8_t*>(s.hdig.p);
@@ -2573,6 +2708,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   MEC_CUDA_OK(cudaMemcpyAsync(s.hdig.p, s.dig.p, static_cast<size_t>(nslots * n * 32), cudaMemcpyDeviceToHost, s.st));
   for (BatchReq* r : reqs)
     if ((rc = frames_enqueue(c, r->ch, r->files, r->with_data, r->data_digests))) return rc;
+  if ((rc = batcher_sums_join(b, s, reqs.size(), nsum))) return rc;
   c->st_blocks_encoded += nslots;
   return MEC_OK;
 }
@@ -3032,6 +3168,7 @@ static void batcher_main(mec_batcher* b) {
       fb.traced = b->sw.trace && rc == MEC_OK && kernel_batch;
       if (rc != MEC_OK) {  // drain what was enqueued before the failure, then fail the whole batch
         cudaStreamSynchronize(s.st);
+        if (b->sum_st[head]) cudaStreamSynchronize(b->sum_st[head]);
         batcher_finish(b, fb, s, rc);
       } else {
         b->st_batches++;
@@ -3091,6 +3228,14 @@ static int size_put_slot(const mec_codec* c, Slot& s, int64_t blocks) {
   return s.dig.ensure(static_cast<size_t>(blocks * c->n * 32));
 }
 
+static void batcher_destroy_streams(mec_batcher* b) {
+  for (int i = 0; i < kSlots; i++) {
+    if (b->ev_staged[i]) cudaEventDestroy(b->ev_staged[i]);
+    if (b->ev_summed[i]) cudaEventDestroy(b->ev_summed[i]);
+    if (b->sum_st[i]) cudaStreamDestroy(b->sum_st[i]);
+  }
+}
+
 // mec_batcher_new_ex, and with `dst` (a codec of the destination geometry without an engine yet, owned from here on, freed on
 // failure) mec_batcher_new_transcode: the destination's engine and slots are set up before the worker starts
 static int batcher_create(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
@@ -3146,7 +3291,19 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
       if (rc == MEC_OK) rc = s.crc_part.ensure(static_cast<size_t>(nwork) * kCrcTypes * sizeof(uint64_t));
       if (rc == MEC_OK) rc = s.crc_out.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
       if (rc == MEC_OK) rc = s.hcrc.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
+      // object hashes (batcher_sums_table): at most `slots` requests, each with up to kSumAlgos items and one record
+      if (rc == MEC_OK) rc = s.sum_tab.ensure(static_cast<size_t>(slots) * kSumAlgos * sizeof(SumWork));
+      if (rc == MEC_OK) rc = s.hsum_tab.ensure(static_cast<size_t>(slots) * kSumAlgos * sizeof(SumWork));
+      if (rc == MEC_OK) rc = s.sum_out.ensure(static_cast<size_t>(slots) * kSumRecord);
+      if (rc == MEC_OK) rc = s.hsum.ensure(static_cast<size_t>(slots) * kSumRecord);
     }
+    for (int i = 0; i < kSlots && rc == MEC_OK; i++)
+      if (cudaStreamCreateWithFlags(&b->sum_st[i], cudaStreamNonBlocking) != cudaSuccess ||
+          cudaEventCreateWithFlags(&b->ev_staged[i], cudaEventDisableTiming) != cudaSuccess ||
+          cudaEventCreateWithFlags(&b->ev_summed[i], cudaEventDisableTiming) != cudaSuccess) {
+        set_last_error(std::string("object-hash stream: ") + cudaGetErrorString(cudaGetLastError()));
+        rc = MEC_ERR_CUDA;
+      }
     if (rc == MEC_OK) rc = ensure_crc(c);
     if (dst) {
       // the destination side of a merged transcode batch, laid out as a merged PUT batch of the destination geometry: object bytes,
@@ -3164,7 +3321,7 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     }
     cudaSetDevice(cur);
   }
-  if (rc) { mec_codec_free(c); mec_codec_free(dst); delete b; return rc; }
+  if (rc) { batcher_destroy_streams(b); mec_codec_free(c); mec_codec_free(dst); delete b; return rc; }
   if (b->sw.trace) {
     int cur = 0;
     cudaGetDevice(&cur);
@@ -3236,6 +3393,7 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
       if (b->ev_ph[i][j]) cudaEventDestroy(b->ev_ph[i][j]);
   }
   if (b->aux) cudaStreamDestroy(b->aux);
+  batcher_destroy_streams(b);
   mec_codec_free(b->serial);
   mec_codec_free(b->serial_dst);
   mec_codec_free(b->dst);
@@ -3257,7 +3415,7 @@ static int64_t batcher_enqueue_wait(mec_batcher* b, BatchReq& r) {
 }
 
 static int64_t batcher_call(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests, bool with_data,
-                            int write_quorum, int crc_which = 0, uint64_t* crc_out = nullptr) {
+                            int write_quorum, int crc_which = 0, uint64_t* crc_out = nullptr, int sum_which = 0, uint8_t* sums = nullptr) {
   if (!b || len < 0 || !files || (len > 0 && !src)) return MEC_ERR_INVALID_ARGUMENT;
   int online = 0;
   for (int i = 0; i < b->codec->n; i++) online += files[i] != nullptr;
@@ -3267,11 +3425,21 @@ static int64_t batcher_call(mec_batcher* b, const uint8_t* src, int64_t len, uin
       for (int ty = 0; ty < kCrcTypes; ty++) crc_out[ty] = 0;
       b->st_crc_requests++;
     }
+    if (sum_which) {  // the digests of the empty message
+      static const uint8_t kEmpty[kSumAlgos][32] = {
+          {0xd4, 0x1d, 0x8c, 0xd9, 0x8f, 0x00, 0xb2, 0x04, 0xe9, 0x80, 0x09, 0x98, 0xec, 0xf8, 0x42, 0x7e},
+          {0xda, 0x39, 0xa3, 0xee, 0x5e, 0x6b, 0x4b, 0x0d, 0x32, 0x55, 0xbf, 0xef, 0x95, 0x60, 0x18, 0x90, 0xaf, 0xd8, 0x07, 0x09},
+          {0xe3, 0xb0, 0xc4, 0x42, 0x98, 0xfc, 0x1c, 0x14, 0x9a, 0xfb, 0xf4, 0xc8, 0x99, 0x6f, 0xb9, 0x24,
+           0x27, 0xae, 0x41, 0xe4, 0x64, 0x9b, 0x93, 0x4c, 0xa4, 0x95, 0x99, 0x1b, 0x78, 0x52, 0xb8, 0x55}};
+      for (int a = 0; a < kSumAlgos; a++)
+        if (sum_which & (MEC_SUM_MD5 << a)) memcpy(sums + 32 * a, kEmpty[a], static_cast<size_t>(sum_digest_len(a)));
+      b->st_sum_requests++;
+    }
     return 0;
   }
   BatchReq r;
   r.src = src; r.len = len; r.files = files; r.data_digests = data_digests; r.with_data = with_data;
-  r.crc_which = crc_which; r.crc_out = crc_out;
+  r.crc_which = crc_which; r.crc_out = crc_out; r.sum_which = sum_which; r.sums = sums;
   // page-locked buffers (mec_alloc_pinned*, or anything cudaHostRegister'ed) are moved by the gather / scatter kernels; checked here,
   // on the caller's thread, so the worker does not pay for it
   r.mapped = mec_is_pinned(src) && (!data_digests || mec_is_pinned(data_digests));
@@ -3292,6 +3460,14 @@ extern "C" int64_t mec_batcher_encode_crc(mec_batcher* b, const uint8_t* src, in
   which &= 7;
   if (which && !out3) return MEC_ERR_INVALID_ARGUMENT;
   return batcher_call(b, src, len, files, data_digests, data_digests == nullptr, write_quorum, which, out3);
+}
+extern "C" int64_t mec_batcher_encode_sums(mec_batcher* b, const uint8_t* src, int64_t len, uint8_t* const* files, uint8_t* data_digests,
+                                           int write_quorum, int which, uint64_t* crc3, uint8_t* sums) {
+  constexpr int kCrcMask = MEC_CRC32 | MEC_CRC32C | MEC_CRC64NVME;
+  if (which & ~(kCrcMask | kSumMask)) return MEC_ERR_INVALID_ARGUMENT;
+  if (((which & kCrcMask) && !crc3) || ((which & kSumMask) && !sums)) return MEC_ERR_INVALID_ARGUMENT;
+  return batcher_call(b, src, len, files, data_digests, data_digests == nullptr, write_quorum, which & kCrcMask, crc3, which & kSumMask,
+                      sums);
 }
 // The k readers parallelReader picks for a read or move (choose_readers on r.gfiles, r.prefer), chosen on the caller's thread: equal
 // reader sets share a batch.  Sets their bits in r.alive_mask and clears *mapped unless every one of them is page-locked.
@@ -3410,6 +3586,7 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "kernel_batches")) return b->st_kernel_batches.load();
   if (!strcmp(name, "redone")) return b->st_redone.load();
   if (!strcmp(name, "crc_requests")) return b->st_crc_requests.load();
+  if (!strcmp(name, "sum_requests")) return b->st_sum_requests.load();
   if (!strcmp(name, "patterns")) return b->st_patterns.load();
   if (!strcmp(name, "mixed_batches")) return b->st_mixed.load();
   if (!strcmp(name, "launches")) return b->codec->eng ? b->codec->eng->launches() : 0;

@@ -3,6 +3,9 @@
 //   mode batcher : every PUT goes through ONE mec_batcher (cross-request coalescing into merged launches)
 //   mode batcher_crc : the same PUTs, each also asking for its CRC32, CRC32C and CRC64NVME (mec_batcher_encode_crc); after the timed
 //                  window every thread's last checksums are checked against a table CRC computed here on the host
+//   mode batcher_sums : the same PUTs, each also asking for the object hashes of the mask SUMS (default 8 = MEC_SUM_MD5, the ETag;
+//                  40 = MD5 | SHA-256) through mec_batcher_encode_sums; after the timed window every thread's last digests are checked
+//                  against an MD5 written out here and the oracle's SHA-256
 //   mode pool    : every thread picks a codec handle from a pool of P (no coalescing: one launch per call)
 //   mode get     : degraded GETs (4 data drives offline) through the pool
 //   mode bheal   : heals of one stale data drive (Erasure.Heal, the MRF / new-disk traffic) through ONE mec_batcher
@@ -34,6 +37,7 @@
 #include <vector>
 #include "minio_ec.h"
 extern "C" void orc_encode_hash_blocks_st(int k, int m, int64_t bs, const uint8_t* src, int64_t nblocks, uint8_t* parity, uint8_t* digests);
+extern "C" void orc_sha256(const uint8_t* p, size_t n, uint8_t out[32]);
 
 // byte-at-a-time table CRC (reflected, init and xorout all ones): CRC32, CRC32C, CRC64NVME as Go's hash/crc32 and hash/crc64 give them
 static uint64_t host_crc(const uint8_t* p, int64_t n, uint64_t poly, int bits) {
@@ -47,6 +51,44 @@ static uint64_t host_crc(const uint8_t* p, int64_t n, uint64_t poly, int bits) {
   uint64_t c = mask;
   for (int64_t i = 0; i < n; i++) c = tab[(c ^ p[i]) & 0xff] ^ (c >> 8);
   return c ^ mask;
+}
+
+// MD5 (RFC 1321), a byte-at-a-time host reference for the batcher_sums check
+static void host_md5(const uint8_t* p, int64_t n, uint8_t out[16]) {
+  static const uint32_t K[64] = {
+      0xd76aa478, 0xe8c7b756, 0x242070db, 0xc1bdceee, 0xf57c0faf, 0x4787c62a, 0xa8304613, 0xfd469501, 0x698098d8, 0x8b44f7af, 0xffff5bb1,
+      0x895cd7be, 0x6b901122, 0xfd987193, 0xa679438e, 0x49b40821, 0xf61e2562, 0xc040b340, 0x265e5a51, 0xe9b6c7aa, 0xd62f105d, 0x02441453,
+      0xd8a1e681, 0xe7d3fbc8, 0x21e1cde6, 0xc33707d6, 0xf4d50d87, 0x455a14ed, 0xa9e3e905, 0xfcefa3f8, 0x676f02d9, 0x8d2a4c8a, 0xfffa3942,
+      0x8771f681, 0x6d9d6122, 0xfde5380c, 0xa4beea44, 0x4bdecfa9, 0xf6bb4b60, 0xbebfbc70, 0x289b7ec6, 0xeaa127fa, 0xd4ef3085, 0x04881d05,
+      0xd9d4d039, 0xe6db99e5, 0x1fa27cf8, 0xc4ac5665, 0xf4292244, 0x432aff97, 0xab9423a7, 0xfc93a039, 0x655b59c3, 0x8f0ccc92, 0xffeff47d,
+      0x85845dd1, 0x6fa87e4f, 0xfe2ce6e0, 0xa3014314, 0x4e0811a1, 0xf7537e82, 0xbd3af235, 0x2ad7d2bb, 0xeb86d391};
+  static const int R[16] = {7, 12, 17, 22, 5, 9, 14, 20, 4, 11, 16, 23, 6, 10, 15, 21};
+  uint32_t h[4] = {0x67452301, 0xefcdab89, 0x98badcfe, 0x10325476};
+  const int64_t nblk = (n + 8) / 64 + 1;  // message, 0x80, zeros, 8-byte length
+  for (int64_t b = 0; b < nblk; b++) {
+    uint32_t w[16] = {};
+    for (int i = 0; i < 64; i++) {
+      const int64_t pos = b * 64 + i;
+      uint32_t v = pos < n ? p[pos] : pos == n ? 0x80 : 0;
+      if (b == nblk - 1 && i >= 56) v = static_cast<uint8_t>(static_cast<uint64_t>(n) * 8 >> (8 * (i - 56)));
+      w[i / 4] |= v << (8 * (i % 4));
+    }
+    uint32_t a = h[0], bb = h[1], c = h[2], d = h[3];
+    for (int i = 0; i < 64; i++) {
+      uint32_t f;
+      int g;
+      if (i < 16) { f = (bb & c) | (~bb & d); g = i; }
+      else if (i < 32) { f = (d & bb) | (~d & c); g = (5 * i + 1) % 16; }
+      else if (i < 48) { f = bb ^ c ^ d; g = (3 * i + 5) % 16; }
+      else { f = c ^ (bb | ~d); g = (7 * i) % 16; }
+      const uint32_t x = a + f + K[i] + w[g];
+      const int r = R[(i / 16) * 4 + i % 4];
+      a = d; d = c; c = bb;
+      bb = bb + ((x << r) | (x >> (32 - r)));
+    }
+    h[0] += a; h[1] += bb; h[2] += c; h[3] += d;
+  }
+  for (int i = 0; i < 16; i++) out[i] = static_cast<uint8_t>(h[i / 4] >> (8 * (i % 4)));
 }
 
 static void on_segv(int sig) {
@@ -90,7 +132,9 @@ int main(int argc, char** argv) {
   if (gpu) mec_bind_thread_to_device(device);
   auto alloc = [&](size_t b) -> uint8_t* { return gpu ? static_cast<uint8_t*>(mec_alloc_pinned_on(device, b)) : static_cast<uint8_t*>(malloc(b)); };
   // per-thread buffers: object, 16 part files, digests, destination, the healed part file
+  const int sums_mask = getenv("SUMS") ? atoi(getenv("SUMS")) : MEC_SUM_MD5;
   struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; uint64_t crc[3];
+              uint8_t sums[MEC_SUM_BYTES];
               std::vector<uint8_t*> outs; };  // outs: the destination part files of the transcode modes
   std::vector<TB> tb(T);
   uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
@@ -114,7 +158,7 @@ int main(int argc, char** argv) {
   }
   mec_batcher* bat = nullptr;
   std::vector<mec_codec*> pool, pool2;
-  if (mode == "batcher" || mode == "batcher_crc") {
+  if (mode == "batcher" || mode == "batcher_crc" || mode == "batcher_sums") {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
@@ -162,6 +206,7 @@ int main(int argc, char** argv) {
     TB& b = tb[t];
     if (mode == "batcher") return mec_batcher_encode_sg(bat, b.obj, osize, b.files.data(), b.dd, k + 1);
     if (mode == "batcher_crc") return mec_batcher_encode_crc(bat, b.obj, osize, b.files.data(), b.dd, k + 1, MEC_CRC32 | MEC_CRC32C | MEC_CRC64NVME, b.crc);
+    if (mode == "batcher_sums") return mec_batcher_encode_sums(bat, b.obj, osize, b.files.data(), b.dd, k + 1, sums_mask, nullptr, b.sums);
     if (mode == "pool") return mec_encode_sg(pool[t % P], b.obj, osize, b.files.data(), b.dd, k + 1);
     if (mode == "bget") {
       const uint8_t* f[64];
@@ -231,6 +276,12 @@ int main(int argc, char** argv) {
       if (tb[t].crc[0] != host_crc(tb[t].obj, osize, 0xEDB88320ull, 32) || tb[t].crc[1] != host_crc(tb[t].obj, osize, 0x82F63B78ull, 32) ||
           tb[t].crc[2] != host_crc(tb[t].obj, osize, 0x9A6C9329AC4BC9B5ull, 64))
         errors++;
+  if (mode == "batcher_sums")  // every thread's digests equal the host's
+    for (int t = 0; t < T; t++) {
+      uint8_t want[32];
+      if (sums_mask & MEC_SUM_MD5) { host_md5(tb[t].obj, osize, want); if (memcmp(tb[t].sums, want, 16)) errors++; }
+      if (sums_mask & MEC_SUM_SHA256) { orc_sha256(tb[t].obj, static_cast<size_t>(osize), want); if (memcmp(tb[t].sums + 64, want, 32)) errors++; }
+    }
   std::vector<double> all;
   for (auto& v : lat) all.insert(all.end(), v.begin(), v.end());
   std::sort(all.begin(), all.end());
@@ -240,6 +291,8 @@ int main(int argc, char** argv) {
          mode_name.c_str(), T, static_cast<long long>(osize >> 20), static_cast<long long>(osize), all.size(), sec, total / sec / (1 << 30), all.size() / sec, all[all.size() / 2],
          all[static_cast<size_t>(all.size() * 0.99)], static_cast<long long>(errors.load()));
   if (mode == "batcher_crc") printf(", \"crc_requests\": %lld", static_cast<long long>(mec_batcher_stat(bat, "crc_requests")));
+  if (mode == "batcher_sums")
+    printf(", \"sums_mask\": %d, \"sum_requests\": %lld", sums_mask, static_cast<long long>(mec_batcher_stat(bat, "sum_requests")));
   if (bat) printf(", \"mix\": %d, \"batches\": %lld, \"blocks_per_batch\": %.1f, \"launches\": %lld, \"patterns\": %lld, \"mixed_batches\": %lld",
                   bflags ? 1 : 0, static_cast<long long>(mec_batcher_stat(bat, "batches")),
                   static_cast<double>(mec_batcher_stat(bat, "blocks")) / std::max<int64_t>(1, mec_batcher_stat(bat, "batches")),
