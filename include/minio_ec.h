@@ -195,7 +195,7 @@ int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobjects, const ui
  * Refused before any device work: src == dst or a NULL src / dst / files / out_files (MEC_ERR_INVALID_ARGUMENT; for the same
  * geometry use a second handle), a dst block size that does not divide src's (larger ones included), different devices, or an
  * algorithm other than HighwayHash256S on either side (MEC_ERR_UNSUPPORTED: whole-file bitrot chains one digest over the whole
- * shard file, so such parts move through mec_decode_whole + mec_encode_sg), fewer than write_quorum non-NULL out_files
+ * shard file, so such parts move through mec_transcode_whole), fewer than write_quorum non-NULL out_files
  * (MEC_ERR_WRITE_QUORUM).  total_length == 0 returns 0 and
  * writes nothing.  Fewer than k readable source files is MEC_ERR_READ_QUORUM.  Both codecs are held for the call.  Counters:
  * "blocks_read" and "bytes_h2d" grow on src, "blocks_encoded" and "bytes_d2h" on dst. */
@@ -388,6 +388,28 @@ int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const uint8_t* sum
                    uint8_t* const* out_files, uint8_t* out_sums, uint8_t* corrupt);
 int mec_digest_size(int algo);
 
+/* mec_transcode for a part written with a whole-file bitrot algorithm (the oldest parts, mostly with blockSizeV1 = 10 MiB blocks,
+ * which decommission and rebalance drain): the source side has mec_decode_whole's meaning over the whole part — files[i] the raw
+ * shard file of drive i (NULL = offline), sums + i*64 its expected digest (erasure.GetChecksumInfo(part.Number).Hash) — with
+ * mec_decode_prefer's `prefer` (readers with prefer[i] != 0 first, as parallelReader.preferReaders orders them).  A reader whose
+ * whole-file digest does not match is dropped and the next one in that order takes its place; the call then still moves the part
+ * and sets *heal_hint = MEC_ERR_FILE_CORRUPT.  out_files / write_quorum as mec_transcode: complete streaming-bitrot part.N images of
+ * dst's geometry.  Returns total_length, or a negative MEC_ERR_*.
+ * Refused before any device work: src == dst or a NULL src / dst / files / sums / out_files, total_length < 0
+ * (MEC_ERR_INVALID_ARGUMENT); a src algorithm other than SHA256, BLAKE2b512 or HighwayHash256 (a streaming part moves through
+ * mec_transcode), a dst algorithm other than HighwayHash256S, a dst block size that does not divide src's, or different devices
+ * (MEC_ERR_UNSUPPORTED); fewer than write_quorum non-NULL out_files (MEC_ERR_WRITE_QUORUM).  total_length == 0 returns 0 and writes
+ * nothing.  The chosen readers are staged and verified before anything is written: fewer than k verified readers is
+ * MEC_ERR_READ_QUORUM with every out file untouched.  The readers of a round are hashed by ONE whole_hash_kernel launch (one thread
+ * per file: on a move with no corrupt reader the only hash launch of the call), the missing data shards are rebuilt from the raw
+ * shard rows, and the part is re-split, encoded and written in chunks of about 32 MiB of object bytes through both codecs' slots.
+ * Device memory: the staged source, k x (round_up(mec_shard_file_size(total_length), 16) + 256) bytes in src's slot 0 (as
+ * mec_decode_whole), the rebuilt data-shard rows of the chunks in flight on src, and dst's chunk buffers (object bytes, parity rows
+ * and digests of a chunk per slot).  Counters: "blocks_read", "bytes_h2d" (k x the shard file size when no reader is dropped) and
+ * "corrupt_shards" grow on src, "blocks_encoded" and "bytes_d2h" on dst; src's "bytes_d2h" does not grow. */
+int64_t mec_transcode_whole(mec_codec* src, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
+                            int64_t total_length, mec_codec* dst, uint8_t* const* out_files, int write_quorum, int* heal_hint);
+
 /* bitrotVerify (cmd/bitrot.go:164) for the streaming algorithm: scans a whole shard file. */
 int mec_bitrot_verify(mec_codec* c, const uint8_t* file, int64_t file_len, int64_t part_len);
 /* The same for many shard files at once (the deep scan of the data scanner visits every part on every drive): results[f] = MEC_OK or
@@ -421,7 +443,7 @@ int mec_selftest(int device);
  *   decoupled from the GF warps: ~0.16 ms for a 1 MiB block instead of ~0.45 ms on an H100); -1 (default) = five per SM, 0 = never. */
 int mec_set_option(mec_codec* c, const char* name, int64_t value);
 /* Boundary counters (SURVEY §5 metrics row): name is one of "launches", "blocks_encoded", "blocks_read",
- * "shards_rebuilt", "corrupt_shards", "bytes_h2d", "bytes_d2h", "jit_compiles", "jit_ms", "jit_disk_hits" (process-wide), "jit_launches",
+ * "shards_rebuilt", "corrupt_shards", "bytes_h2d", "bytes_d2h", "whole_hash_launches" (whole-file hash kernel launches), "jit_compiles", "jit_ms", "jit_disk_hits" (process-wide), "jit_launches",
  * "small_launches" (launches that took the latency form).  -1 for unknown names.
  * Kernel dispatch (which form of the fused kernel ran, for tests and diagnosis): "form_<f>" counts the launches of form f, one of
  *   small (latency kernel), fast3d, fast3d_auto, fast3d_semi, fast, fast_auto, aligned, aligned_auto, runtime, bytewise (the

@@ -111,6 +111,8 @@ def lib():
     L.mec_decode_prefer.argtypes = [vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_transcode.restype = i64
     L.mec_transcode.argtypes = [vp, vp, vp, i64, vp, vp, i32, C.POINTER(i32)]
+    L.mec_transcode_whole.restype = i64
+    L.mec_transcode_whole.argtypes = [vp, vp, vp, vp, i64, vp, vp, i32, C.POINTER(i32)]
     L.mec_jit_compile_check.restype = i64
     L.mec_jit_compile_check.argtypes = [i32, i32, vp, i32, i32, i32, i32]
     L.mec_jit_prewarm.argtypes = [vp]
@@ -390,6 +392,29 @@ class Codec:
         if rc < 0:
             raise MecError(rc, "mec_decode_whole")
         return dst[:length], hint.value
+
+    def transcode_whole(self, files, sums, total, dst, prefer=None, online=None, write_quorum=0):
+        """mec_transcode_whole: move a whole part of `total` bytes written with this codec's whole-file bitrot algorithm — raw shard
+        files (None = offline) and their expected digests `sums` — to the geometry of the streaming Codec `dst` without the object
+        bytes leaving the device.  online = dst's writers (None = all).  -> (out_files, heal_hint) as Codec.transcode: heal_hint is
+        -7 when a reader failed its whole-file digest and the next one took its place."""
+        files = [None if f is None else _u8(f) for f in files]
+        sm = np.zeros((self.n, 64), dtype=np.uint8)
+        for i, d in enumerate(sums):
+            if d is not None:
+                sm[i, :len(d)] = np.frombuffer(bytes(d), dtype=np.uint8)
+        fsz = dst.bitrot_file_size(total)
+        online = [True] * dst.n if online is None else online
+        outs = [np.zeros(fsz, dtype=np.uint8) if online[i] else None for i in range(dst.n)]
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        marker = np.zeros(1, dtype=np.uint8)  # an empty part's online writers still count against the quorum
+        optrs = _ptrs([(o if o.size else marker) if o is not None else None for o in outs])
+        rc = lib().mec_transcode_whole(self.h, _ptrs(files), sm.ctypes.data, None if pf is None else pf.ctypes.data, total, dst.h,
+                                       optrs, write_quorum, C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_transcode_whole")
+        return outs, hint.value
 
     def heal_whole(self, files, sums, stale, total):
         """-> (out_files, out_sums, rc, corrupt): rc is 0 or -7 (healed, bitrot met in a source)."""

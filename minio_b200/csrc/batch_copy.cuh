@@ -256,6 +256,39 @@ __global__ void __launch_bounds__(128) transcode_resplit_kernel(const __grid_con
   cta_copy(p.obj + b * p.bs + static_cast<int64_t>(i) * per, src, have, false);
 }
 
+// ---- mec_transcode_whole: a part of a whole-file bitrot algorithm has no frames; its verified shard files sit raw on the device ----
+struct WholeResplitParams {
+  uint8_t* obj;                 // device: object bytes of the chunk's source blocks, chunk block b at b*bs
+  const uint8_t* arena;         // verified raw shard files: arena position t at arena + t*fpitch, part block B's shard at + B*S
+  int64_t fpitch;               // >= round_up(shard file size, 16) + 256 (the padding the copy may read into)
+  const uint8_t* rebuilt;       // rebuilt data shards of the chunk: chunk block b, row q at (b*r + q)*pitch
+  int64_t pitch;
+  int64_t b0;                   // part block of the chunk's first block
+  int64_t bs, S, total;         // source block size, full shard length, part length
+  int k, r;
+  int8_t src[kBatchMaxFiles];   // data shard i: read at arena position src[i] >= 0, or rebuilt row -1 - src[i]
+};
+
+// grid (source blocks of the chunk, k source data shards), 128 threads: writeDataBlocks (cmd/erasure-utils.go:42) into device
+// memory.  CTA (b, i) copies the object bytes of data shard i of part block B = b0 + b to obj + b*bs + i*S_B, where S_B =
+// ceil(blen / k) and blen = min(bs, total - B*bs): the byte count comes from the part length, so Split's zero padding is never
+// copied, even when the short last block's shards are S long.  Raw shards lie at B*S inside a shard file, any byte offset (S =
+// 87382 for RS(12,4) at 1 MiB), and land at any offset: cta_copy stores destination-aligned 16-byte vectors built from 4-byte
+// loads and funnel shifts, reading at most one word past a shard, which stays inside a file's 256 bytes of padding and inside
+// the 256 bytes the caller allocates behind the last rebuilt row.
+__global__ void __launch_bounds__(128) whole_resplit_kernel(const __grid_constant__ WholeResplitParams p) {
+  const int64_t b = blockIdx.x, B = p.b0 + b;
+  const int i = blockIdx.y;
+  const int64_t blen = p.total - B * p.bs < p.bs ? p.total - B * p.bs : p.bs;
+  const int64_t per = (blen + p.k - 1) / p.k;
+  int64_t have = blen - static_cast<int64_t>(i) * per;
+  have = have < 0 ? 0 : (have > per ? per : have);
+  if (have == 0) return;
+  const int t = p.src[i];
+  const uint8_t* src = t >= 0 ? p.arena + t * p.fpitch + B * p.S : p.rebuilt + (b * p.r + (-1 - t)) * p.pitch;
+  cta_copy(p.obj + b * p.bs + static_cast<int64_t>(i) * per, src, have, false);
+}
+
 // grid (block stride, k source data shards, nreq), 128 threads: the batched form of transcode_resplit_kernel for a merged batch of
 // moves (mec_batcher_transcode).  Request z's decode plan (chosen readers, rebuilt data shards) and its source slots come from the
 // read table p.reqs[z], which covers the whole part (start_block 0); where its object bytes go comes from the PUT table d.reqs[z]

@@ -91,6 +91,7 @@ struct mec_codec {
   cudaEvent_t sum_ev = nullptr;
   // boundary counters (mec_get_stat)
   int64_t st_blocks_encoded = 0, st_blocks_read = 0, st_shards_rebuilt = 0, st_corrupt = 0, st_h2d = 0, st_d2h = 0;
+  int64_t st_whole_hash = 0;  // whole_hash_kernel launches
   int64_t S() const { return ceil_frac(block_size, k); }
 };
 
@@ -247,6 +248,7 @@ extern "C" int64_t mec_get_stat(const mec_codec* c, const char* name) {
   if (!strcmp(name, "corrupt_shards")) return c->st_corrupt;
   if (!strcmp(name, "bytes_h2d")) return c->st_h2d;
   if (!strcmp(name, "bytes_d2h")) return c->st_d2h;
+  if (!strcmp(name, "whole_hash_launches")) return c->st_whole_hash;
   if (!strcmp(name, "jit_compiles")) return c->eng ? c->eng->jit_compiles() : 0;
   if (!strcmp(name, "jit_launches")) return c->eng ? c->eng->jit_launches() : 0;
   if (!strcmp(name, "small_launches")) return c->eng ? c->eng->small_launches() : 0;
@@ -1617,7 +1619,7 @@ static int whole_hash_device(mec_codec* c, int algo, const uint8_t* d_data, int6
   const int64_t nthreads = hp.algo == MEC_HIGHWAYHASH256 ? 2 * count : count;
   whole_hash_kernel<<<static_cast<unsigned>((nthreads + threads - 1) / threads), threads, 0, st>>>(hp);
   MEC_CUDA_OK(cudaGetLastError());
-  (void)c;
+  c->st_whole_hash++;
   return MEC_OK;
 }
 
@@ -1742,9 +1744,13 @@ static int require_whole(mec_codec* c) {
   return ensure_engine(c);
 }
 
-// stage + verify: on return chosen[0..k) (ascending) name k verified files, file chosen[t] at s.aux + pos[t]*fpitch
+// stage + verify: on return chosen[0..k) (ascending) name k verified files, file chosen[t] at s.aux + pos[t]*fpitch.  Readers are
+// taken as parallelReader takes them (`prefer` first, see choose_readers).  one_launch: the files of a round are hashed by ONE
+// launch over the span of arena positions that holds them (verified files inside the span are hashed again: one thread per file,
+// so the launch takes no longer); otherwise one launch per file.
 static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const uint8_t* sums, int64_t sfs, uint8_t* alive,
-                                uint8_t* corrupt, int* chosen, int* pos, int64_t fpitch, Slot& s) {
+                                uint8_t* corrupt, int* chosen, int* pos, int64_t fpitch, Slot& s, const uint8_t* prefer = nullptr,
+                                bool one_launch = false) {
   const int k = c->k, n = c->n, ds = mec_digest_size(c->algo);
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * fpitch + 256)))) return rc;
@@ -1754,10 +1760,8 @@ static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const
   for (int i = 0; i < n; i++) slot_of[i] = -1;
   bool verified[kMaxShards] = {};
   for (;;) {
-    int want[kMaxShards], nw = 0;
-    for (int i = 0; i < n && nw < k; i++)
-      if (alive[i]) want[nw++] = i;
-    if (nw < k) return MEC_ERR_READ_QUORUM;
+    int want[kMaxShards];
+    if (choose_readers(c, files, alive, prefer, want) < k) return MEC_ERR_READ_QUORUM;
     // arena positions: keep verified files where they are, give the newcomers the free positions
     bool used[kMaxK] = {};
     for (int q = 0; q < k; q++)
@@ -1776,12 +1780,21 @@ static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const
       c->st_h2d += sfs;
     }
     if (nf == 0) break;
-    for (int q = 0; q < nf; q++) {  // one launch per newcomer keeps the arena positions arbitrary; these files are few and the hash is serial anyway
-      const int pos = slot_of[fresh[q]];
-      if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p) + pos * fpitch, fpitch, sfs, 1,
-                                  static_cast<uint8_t*>(s.dig.p) + pos * 64, s.st)))
+    if (one_launch) {
+      int lo = k, hi = -1;
+      for (int q = 0; q < nf; q++) { lo = std::min(lo, slot_of[fresh[q]]); hi = std::max(hi, slot_of[fresh[q]]); }
+      if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p) + lo * fpitch, fpitch, sfs, hi - lo + 1,
+                                  static_cast<uint8_t*>(s.dig.p) + lo * 64, s.st)))
         return rc;
       c->eng->count_launch();
+    } else {
+      for (int q = 0; q < nf; q++) {  // one launch per newcomer keeps the arena positions arbitrary; these files are few and the hash is serial anyway
+        const int pos = slot_of[fresh[q]];
+        if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p) + pos * fpitch, fpitch, sfs, 1,
+                                    static_cast<uint8_t*>(s.dig.p) + pos * 64, s.st)))
+          return rc;
+        c->eng->count_launch();
+      }
     }
     MEC_CUDA_OK(cudaMemcpyAsync(s.hdig.p, s.dig.p, static_cast<size_t>(k * 64), cudaMemcpyDeviceToHost, s.st));
     MEC_CUDA_OK(cudaStreamSynchronize(s.st));
@@ -1808,10 +1821,10 @@ static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const
   return MEC_OK;
 }
 
-// launch the rebuild of `targets` over blocks [first, first + nb) of raw shard files (stride S between blocks, no frames); the
-// last of those blocks has shards of last_len bytes
-static int launch_whole_rebuild(mec_codec* c, Slot& s, const int* pos, int64_t fpitch, int64_t S, int64_t last_len, int64_t first,
-                                int64_t nb, const uint8_t* rows, int r, int64_t pitch) {
+// launch the rebuild of `targets` over blocks [first, first + nb) of raw shard files (arena position t at arena + t*fpitch, stride S
+// between blocks, no frames) into out (block b, row q at (b*r + q)*pitch); the last of those blocks has shards of last_len bytes
+static int launch_whole_rebuild(mec_codec* c, const uint8_t* arena, uint8_t* out, cudaStream_t st, const int* pos, int64_t fpitch,
+                                int64_t S, int64_t last_len, int64_t first, int64_t nb, const uint8_t* rows, int r, int64_t pitch) {
   const int k = c->k;
   FusedDesc d;
   d.k = k; d.r = r; d.coef = rows; d.static_encode = false; d.contiguous = false; d.hash_outputs = false;
@@ -1824,13 +1837,13 @@ static int launch_whole_rebuild(mec_codec* c, Slot& s, const int* pos, int64_t f
     d.nblocks = cnt;
     d.S = static_cast<int32_t>(pass == 0 ? S : last_len);
     for (int t = 0; t < k; t++) {
-      const uint8_t* base = static_cast<const uint8_t*>(s.aux.p) + pos[t] * fpitch;
+      const uint8_t* base = arena + pos[t] * fpitch;
       d.in_ptr[t] = base + (first + f0) * S;
       d.map_base[t] = base;
       d.map_len[t] = fpitch;
     }
-    d.out = static_cast<uint8_t*>(s.out.p) + f0 * r * pitch;
-    int rc = c->eng->launch_fused(d, c->opt, s.st);
+    d.out = out + f0 * r * pitch;
+    int rc = c->eng->launch_fused(d, c->opt, st);
     if (rc) return rc;
   }
   return MEC_OK;
@@ -1866,7 +1879,9 @@ extern "C" int64_t mec_decode_whole(mec_codec* c, const uint8_t* const* files, c
   const int r = p.r;
   if (r > 0) {
     if ((rc = s.out.ensure(static_cast<size_t>(nb * r * pitch)))) return rc;
-    if ((rc = launch_whole_rebuild(c, s, pos, fpitch, S, rr.last_len, rr.start_block, nb, p.rows.data(), r, pitch))) return rc;
+    if ((rc = launch_whole_rebuild(c, static_cast<const uint8_t*>(s.aux.p), static_cast<uint8_t*>(s.out.p), s.st, pos, fpitch, S,
+                                   rr.last_len, rr.start_block, nb, p.rows.data(), r, pitch)))
+      return rc;
   }
   // writeDataBlocks by DMA: data shard i of block B sits in a verified shard file (stride S) or in a rebuilt row
   for (int i = 0; i < k; i++) {
@@ -1921,7 +1936,9 @@ extern "C" int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const u
   const int* targets = p.targets;
   if (r > 0) {
     if ((rc = s.out.ensure(static_cast<size_t>(nblocks * r * pitch)))) return rc;
-    if ((rc = launch_whole_rebuild(c, s, pos, fpitch, S, last_len, 0, nblocks, p.rows.data(), r, pitch))) return rc;
+    if ((rc = launch_whole_rebuild(c, static_cast<const uint8_t*>(s.aux.p), static_cast<uint8_t*>(s.out.p), s.st, pos, fpitch, S,
+                                   last_len, 0, nblocks, p.rows.data(), r, pitch)))
+      return rc;
     // rebuilt rows -> contiguous shard files on the device (for the whole-file hash), then files and sums go home
     if ((rc = s.src.ensure(static_cast<size_t>(r * fpitch + 256)))) return rc;
     if ((rc = s.dig.ensure(static_cast<size_t>((k + r) * 64)))) return rc;
@@ -1958,6 +1975,105 @@ extern "C" int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const u
   bool any = false;
   for (int i = 0; i < n; i++) { any |= corrupt[i] != 0; if (corrupt_out) corrupt_out[i] = corrupt[i]; }
   return any ? MEC_ERR_FILE_CORRUPT : MEC_OK;  // Heal's derr (cmd/erasure-decode.go:338-341,366)
+}
+
+// Data movement between pools for a part written with a whole-file bitrot algorithm: Erasure.Decode over wholeBitrotReaders on
+// `src` (as mec_decode_whole, with mec_decode_prefer's `prefer`) piped into Erasure.Encode on `dst` (as mec_transcode), without
+// the object leaving the device.  wholeBitrotReader verifies a file before it hands out any byte of it (cmd/bitrot-whole.go:66-81),
+// so the chosen readers' shard files are staged in slot 0's arena and hashed first — ONE whole_hash_kernel launch per round of
+// readers — and nothing is written until k of them have verified.  The part then runs in chunks of source blocks through the
+// codecs' slots, each on the source slot's stream: the missing data shards are rebuilt from the raw shard rows, whole_resplit_kernel
+// re-splits the chunk into dst's object bytes, dst encodes them and its frames go out, so the copy back of chunk c overlaps the
+// rebuild, re-split and encode of chunk c+1.
+extern "C" int64_t mec_transcode_whole(mec_codec* src, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
+                                       int64_t total, mec_codec* dst, uint8_t* const* out_files, int write_quorum, int* heal_hint) {
+  NvtxRange nvtx("mec_transcode_whole");
+  if (heal_hint) *heal_hint = 0;
+  if (!src || !dst || src == dst || !files || !sums || !out_files || total < 0) return MEC_ERR_INVALID_ARGUMENT;
+  const bool whole_src = src->algo == MEC_SHA256 || src->algo == MEC_HIGHWAYHASH256 || src->algo == MEC_BLAKE2B512;
+  if (!whole_src || dst->algo != MEC_HIGHWAYHASH256S || src->block_size % dst->block_size != 0 || src->device != dst->device)
+    return MEC_ERR_UNSUPPORTED;
+  int online = 0;
+  for (int i = 0; i < dst->n; i++) online += out_files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  if (total == 0) return 0;
+  const int k = src->k, n = src->n;
+  if (k > kMaxK || n > kMaxShards || src->S() >= (1ll << 31) || dst->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
+  int rc;
+  if ((rc = require_streaming(dst))) return rc;
+  std::scoped_lock lk(src->mu, dst->mu);  // two threads moving parts in opposite directions lock in the same order
+  if ((rc = require_whole(src))) return rc;
+  MEC_CUDA_OK(cudaSetDevice(src->device));
+  const int64_t bs = src->block_size, S = src->S(), sfs = mec_shard_file_size(src, total);
+  const int64_t nblocks = ceil_frac(total, bs), last_len = sfs - (nblocks - 1) * S;
+  const int64_t fpitch = round_up(sfs, 16) + 256, pitch = round_up(S, 16);
+  SlotDrain drain(src);
+  Slot& s0 = src->slots[0];
+  std::vector<uint8_t> alive(n), corrupt(n, 0);
+  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
+  int chosen[kMaxShards], pos[kMaxK];
+  if ((rc = stage_verified_whole(src, files, sums, sfs, alive.data(), corrupt.data(), chosen, pos, fpitch, s0, prefer, true)))
+    return rc;
+  DecodePlan p;
+  if ((rc = plan_decode(src, chosen, k, nullptr, 1, &p))) return rc;
+  const int r = p.r;
+  WholeResplitParams rp = {};
+  rp.arena = static_cast<const uint8_t*>(s0.aux.p); rp.fpitch = fpitch; rp.pitch = pitch;
+  rp.bs = bs; rp.S = S; rp.total = total; rp.k = k; rp.r = r;
+  for (int t = 0; t < k; t++)
+    if (chosen[t] < k) rp.src[chosen[t]] = static_cast<int8_t>(pos[t]);
+  for (int q = 0; q < r; q++) rp.src[p.targets[q]] = static_cast<int8_t>(-1 - q);
+  // ~32 MiB of object bytes per chunk; a shorter part is cut into about four chunks so that its copies back still overlap
+  int64_t chunk = std::max<int64_t>(1, (32ll << 20) / bs);
+  if (nblocks < 4 * chunk) chunk = ceil_frac(nblocks, 4);
+  if (src->opt.chunk_blocks > 0) chunk = src->opt.chunk_blocks;
+  const int64_t ebs = dst->block_size, epitch = round_up(dst->S(), 16);
+  EncChunk inflight[kSlots];
+  SlotRing ring(src, [&](int q) {
+    frames_retire(dst, inflight[q], out_files, true, nullptr);
+    dst->st_blocks_encoded += inflight[q].nb;
+  });
+  for (int64_t b0 = 0; b0 < nblocks; b0 += chunk) {
+    if ((rc = ring.acquire())) return rc;
+    const int si = ring.si;
+    Slot& s = src->slots[si];
+    Slot& d = dst->slots[si];
+    const int64_t nb = std::min(chunk, nblocks - b0), bytes = std::min(total - b0 * bs, nb * bs), enb = ceil_frac(bytes, ebs);
+    if (r > 0) {
+      if ((rc = s.out.ensure(static_cast<size_t>(nb * r * pitch + 256)))) return rc;  // whole_resplit_kernel reads past the last row
+      const int64_t chunk_last = b0 + nb == nblocks ? last_len : S;
+      if ((rc = launch_whole_rebuild(src, rp.arena, static_cast<uint8_t*>(s.out.p), s.st, pos, fpitch, S, chunk_last, b0, nb,
+                                     p.rows.data(), r, pitch)))
+        return rc;
+    }
+    if ((rc = d.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
+    if ((rc = d.out.ensure(static_cast<size_t>(enb * std::max(dst->m, 1) * epitch)))) return rc;
+    if ((rc = d.dig.ensure(static_cast<size_t>(enb * dst->n * 32)))) return rc;
+    if ((rc = d.hdig.ensure(static_cast<size_t>(enb * dst->n * 32)))) return rc;
+    rp.obj = static_cast<uint8_t*>(d.src.p);
+    rp.rebuilt = static_cast<const uint8_t*>(s.out.p);
+    rp.b0 = b0;
+    whole_resplit_kernel<<<dim3(static_cast<unsigned>(nb), static_cast<unsigned>(k)), 128, 0, s.st>>>(rp);
+    MEC_CUDA_OK(cudaGetLastError());
+    src->eng->count_launch();
+    if ((rc = encode_device_locked(dst, rp.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.p), s.st)))
+      return rc;
+    EncChunk& ec = inflight[si];
+    ec = EncChunk{};
+    ec.b0 = b0 * (bs / ebs); ec.nb = enb; ec.nfull = bytes / ebs; ec.tail = bytes % ebs; ec.s = &d; ec.pitch = epitch; ec.st = s.st;
+    ec.d_src = rp.obj; ec.d_src_tail = rp.obj + ec.nfull * ebs;
+    ec.d_out = static_cast<uint8_t*>(d.out.p); ec.d_out_tail = ec.d_out + ec.nfull * dst->m * epitch;
+    ec.h_dig = static_cast<const uint8_t*>(d.hdig.p); ec.h_dig_tail = ec.h_dig + ec.nfull * dst->n * 32;
+    if ((rc = frames_enqueue_chunk(dst, ec, out_files, true, nullptr))) return rc;
+    ring.submitted();
+  }
+  if ((rc = ring.finish())) return rc;
+  src->st_blocks_read += nblocks;
+  src->st_shards_rebuilt += nblocks * r;
+  if (heal_hint)
+    for (int i = 0; i < n; i++)
+      if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
+  return total;
 }
 
 // ------------------------------------------------------------------------------------------------
