@@ -319,6 +319,38 @@ int mec_batcher_new_transcode_ex(int k, int m, int64_t block_size, int dst_k, in
  * "blocks_encoded" and "bytes_d2h" on the destination codec. */
 int64_t mec_batcher_transcode(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t total_length,
                               uint8_t* const* out_files, int write_quorum, int* heal_hint);
+/* mec_transcode_whole through the coalescer, on any batcher made by mec_batcher_new_transcode or mec_batcher_new_transcode_ex: the
+ * source geometry (k, m, block_size) is the batcher's, the destination its destination codec (whose block size may divide the
+ * source's, as for mec_batcher_transcode).  algo is the part's whole-file algorithm (MEC_SHA256, MEC_BLAKE2B512 or
+ * MEC_HIGHWAYHASH256), files[i] the raw shard file of source drive i (NULL = offline), sums + i*64 its expected digest
+ * (erasure.GetChecksumInfo(part.Number).Hash); prefer, out_files, write_quorum, heal_hint and the result as mec_transcode_whole.
+ * Checked on the caller's thread before anything is queued, in this order: a NULL batcher, files, sums or out_files,
+ * total_length < 0, a batcher not made for transcoding, or an algo that is no MEC_* bitrot value (MEC_ERR_INVALID_ARGUMENT,
+ * *heal_hint = 0); MEC_HIGHWAYHASH256S (MEC_ERR_UNSUPPORTED: a streaming part moves through mec_batcher_transcode); fewer than
+ * write_quorum non-NULL out_files (MEC_ERR_WRITE_QUORUM); total_length == 0 (returns 0, writes nothing); fewer than k non-NULL
+ * source files (MEC_ERR_READ_QUORUM).  The k readers are chosen there as parallelReader chooses them (`prefer` first, then index
+ * order).  A merged batch holds whole-file moves of one algorithm only, never other kinds of requests; without
+ * MEC_BATCHER_MIX_PATTERNS its moves share one reader set, with it reader sets mix and the batch is cut at one latency launch.
+ * A batch stages the chosen readers' shard files of all its moves in one batched copy, hashes all of them in ONE whole_hash_kernel
+ * launch (one thread per file, two for HighwayHash256: a batch waits for its longest file), rebuilds the missing data shards from
+ * the raw rows in one merged reconstruct, and re-splits, encodes and scatters as mec_batcher_transcode does.  A move whose chosen
+ * readers all match their sums is done (heal_hint = 0, counted in "transcodes_whole").  A move with any mismatching reader is
+ * redone alone on the private pair, which applies the exact fail-over (the next reader in `prefer` order, heal_hint =
+ * MEC_ERR_FILE_CORRUPT, every out file rewritten; counted in "redone" and "transcodes_whole_serial").  Moves with a chosen reader
+ * or an out file that is not page-locked, geometries of more than 32 drives, MEC_BATCHER_MEMCPY in the environment and parts of
+ * more than max_batch_blocks source blocks take that private path directly: mec_transcode_whole on a private source handle of the
+ * request's algorithm (up to three, each created on first use) and the private destination handle.  As for mec_batcher_transcode,
+ * the out files' contents are unspecified when the call returns an error.
+ * Counters (mec_batcher_stat): "transcodes_whole" (moves completed by merged batches), "transcodes_whole_serial" (moves of the
+ * private path, redos included); "whole_hash_launches" grows by one per merged whole-file batch; "blocks_read" and "bytes_h2d"
+ * (k x mec_shard_file_size(total_length) per clean move) grow on the source side, "dst_blocks_encoded" and "dst_bytes_d2h" on the
+ * destination side.  Device memory: the file arena of a batch (its object bytes plus at most 272 x k bytes per request) is the
+ * source slot's PUT staging buffer, which mec_batcher_new_transcode* sizes up front for a full batch: max_batch_blocks +
+ * min(64, max_batch_blocks / 8 + 4) blocks of block_size + 272 x k bytes (at 1 MiB blocks within the slack the PUT staging
+ * already has), plus a 16-byte stream-table entry and a 64-byte digest per staged file. */
+int64_t mec_batcher_transcode_whole(mec_batcher* b, int algo, const uint8_t* const* files, const uint8_t* sums,
+                                    const uint8_t* prefer, int64_t total_length, uint8_t* const* out_files, int write_quorum,
+                                    int* heal_hint);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------

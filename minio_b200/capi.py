@@ -86,6 +86,8 @@ def lib():
     L.mec_batcher_new_transcode_ex.argtypes = [i32, i32, i64, i32, i32, i64, i32, i64, i32, i32, C.POINTER(vp)]
     L.mec_batcher_transcode.restype = i64
     L.mec_batcher_transcode.argtypes = [vp, vp, vp, i64, vp, i32, C.POINTER(i32)]
+    L.mec_batcher_transcode_whole.restype = i64
+    L.mec_batcher_transcode_whole.argtypes = [vp, i32, vp, vp, vp, i64, vp, i32, C.POINTER(i32)]
     L.mec_batcher_stat.restype = i64
     L.mec_batcher_stat.argtypes = [vp, C.c_char_p]
     L.mec_checksums.argtypes = [vp, vp, i64, i32, vp]
@@ -626,6 +628,31 @@ class Batcher:
                                          C.byref(hint))
         if rc < 0:
             raise MecError(rc, "mec_batcher_transcode")
+        return outs, hint.value
+
+    def transcode_whole(self, files, sums, total, algo, prefer=None, online=None, write_quorum=0, pinned=False):
+        """mec_batcher_transcode_whole (a batcher made with dst=): move a whole part of `total` bytes written with the whole-file
+        bitrot algorithm `algo` (SHA256, BLAKE2B512 or HIGHWAYHASH256) — raw shard files (None = offline) and their expected digests
+        `sums` — to the destination geometry.  online / write_quorum / pinned as transcode(): page-locked shard files and pinned=True
+        let the move ride in merged batches.  -> (out_files, heal_hint) as Codec.transcode_whole."""
+        files = [None if f is None else _u8(f) for f in files]
+        sm = np.zeros((self.n, 64), dtype=np.uint8)
+        for i, d in enumerate(sums):
+            if d is not None:
+                sm[i, :len(d)] = np.frombuffer(bytes(d), dtype=np.uint8)
+        n2 = self._dst_sizes.n if self._dst_sizes is not None else 0
+        fsz = self._dst_sizes.bitrot_file_size(total) if self._dst_sizes is not None else 0
+        online = [True] * n2 if online is None else online
+        mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
+        outs = [mk(fsz) if online[i] else None for i in range(n2)]
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        marker = np.zeros(1, dtype=np.uint8)  # an empty part's online writers still count against the quorum
+        optrs = _ptrs([(o if o.size else marker) if o is not None else None for o in outs]) if n2 else (C.c_void_p * 1)()
+        rc = lib().mec_batcher_transcode_whole(self.h, algo, _ptrs(files), sm.ctypes.data, None if pf is None else pf.ctypes.data,
+                                               total, optrs, write_quorum, C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_transcode_whole")
         return outs, hint.value
 
     def stat(self, name):

@@ -10,6 +10,7 @@
 // (whole 128-byte PCIe writes per warp) and the source is re-aligned in registers.
 #pragma once
 #include <cstdint>
+#include "whole_hash.cuh"  // WholeStream
 
 namespace mec {
 
@@ -323,6 +324,22 @@ __global__ void __launch_bounds__(128) batch_transcode_resplit_kernel(const Batc
     const int64_t lo = o < edge ? (edge - o < have ? edge - o : have) : 0;  // bytes below the edge
     if (lo > 0) cta_copy(full + o, src, lo, false);
     if (lo < have) cta_copy(d.staged + w.tail_src_off + (o + lo - edge), src + lo, have - lo, false);
+  }
+}
+
+// grid (block stride, k reader positions, nreq), 128 threads: a merged batch of whole-file moves (mec_batcher_transcode_whole).
+// Its parts have no frames: the chosen readers' raw shard files sit in a device file arena, file (z, t) = reader position t of
+// request z at files + streams[z * k + t].off (16-byte aligned, at least 256 readable bytes behind it), block b's shard at + b * S.
+// This lays every shard into the frame arena slot a GET batch would have staged it in (shard at + 32, the digest bytes are left
+// as they are), so the merged reconstruct and batch_transcode_resplit_kernel run on it unchanged.  Sources sit at any byte
+// offset (S = 87382 for RS(12,4) at 1 MiB); cta_copy reads at most one word past a shard, inside the file's padding.
+__global__ void __launch_bounds__(128) batch_whole_rows_kernel(const BatchGetParams p, const uint8_t* files, const WholeStream* streams) {
+  const BatchGetDesc& r = p.reqs[blockIdx.z];
+  const int t = blockIdx.y;
+  const uint8_t* f = files + streams[static_cast<int64_t>(blockIdx.z) * p.k + t].off;
+  for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
+    const bool is_tail = r.tail_slot >= 0 && b == r.nblocks - 1;
+    cta_copy(p.arena + t * p.arena_stride + get_slot(r, b) * p.P + 32, f + (r.start_block + b) * p.S, is_tail ? r.last_len : p.S, false);
   }
 }
 

@@ -67,7 +67,8 @@ struct Slot {
   DevBuf dreq;                       // request table of a merged batch (batch_copy.cuh)
   DevBuf blk;                        // per-block geometry of a merged launch (SmallBlock / per-frame lengths)
   DevBuf sum_tab, sum_out;           // object hashes of a merged batch: SumWork table, one kSumRecord record per request (obj_hash.cuh)
-  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum;
+  DevBuf wtab;                       // merged whole-file moves: the WholeStream of every staged shard file (whole_hash.cuh)
+  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum, hwtab;
   cudaStream_t st = nullptr;
 };
 
@@ -212,6 +213,7 @@ extern "C" void mec_codec_free(mec_codec* c) {
     s.src.release(); s.out.release(); s.dig.release(); s.aux.release(); s.flags.release();
     s.hdig.release(); s.hflags.release(); s.hcrc.release(); s.crc_part.release(); s.crc_out.release(); s.dreq.release(); s.hreq.release(); s.blk.release(); s.hblk.release();
     s.crc_tab.release(); s.hcrc_tab.release(); s.sum_tab.release(); s.sum_out.release(); s.hsum_tab.release(); s.hsum.release();
+    s.wtab.release(); s.hwtab.release();
   }
   c->flags.release();
   c->crc_tables.release();
@@ -1608,10 +1610,12 @@ extern "C" int mec_digest_size(int algo) {
   return -1;
 }
 
+// `count` streams at d_data + s*pitch of `len` bytes each, or, with a device stream table, at d_data + streams[s].off of
+// streams[s].len bytes
 static int whole_hash_device(mec_codec* c, int algo, const uint8_t* d_data, int64_t pitch, int64_t len, int64_t count,
-                             uint8_t* d_out, cudaStream_t st) {
+                             uint8_t* d_out, cudaStream_t st, const WholeStream* streams = nullptr) {
   WholeHashParams hp;
-  hp.data = d_data; hp.pitch = pitch; hp.len = len; hp.nstreams = static_cast<int>(count);
+  hp.data = d_data; hp.pitch = pitch; hp.len = len; hp.streams = streams; hp.nstreams = static_cast<int>(count);
   hp.algo = algo == MEC_HIGHWAYHASH256S ? MEC_HIGHWAYHASH256 : algo;
   hp.out = d_out;
   memcpy(hp.key, kMagicKey, 32);
@@ -2311,9 +2315,12 @@ extern "C" int mec_selftest(int device) {
 #include <deque>
 #include <unordered_map>
 
-enum class ReqKind { Put, Get, Heal, Transcode };  // PutObject (encode), GetObject (decode), Heal, a move between pools
-// a GET, heal or transcode: stages survivor frames, and per-frame digest verdicts decide which of its requests are done
+// PutObject (encode), GetObject (decode), Heal, a move between pools, a move of a part written with a whole-file bitrot algorithm
+enum class ReqKind { Put, Get, Heal, Transcode, TranscodeWhole };
+// a GET, heal or move: stages its readers, and digest verdicts (per frame; per shard file for a whole-file move) decide which of
+// its requests are done
 static inline bool is_read(ReqKind k) { return k != ReqKind::Put; }
+static inline bool is_move(ReqKind k) { return k == ReqKind::Transcode || k == ReqKind::TranscodeWhole; }
 
 struct BatchReq {
   ReqKind kind = ReqKind::Put;
@@ -2325,6 +2332,9 @@ struct BatchReq {
   uint64_t alive_mask = 0;           // bit i = reader i is online (heal, GET with `prefer`: one of the k chosen readers)
   int64_t get_slot0 = 0, get_tail_slot = -1, get_nblocks = 0;  // placement of the request's blocks in the merged batch
   const uint8_t* prefer = nullptr;   // preferReaders (cmd/erasure-decode.go:92-123), for the redo of a request that met bitrot
+  // whole-file move: the part's algorithm (0 for every other request: a batch holds one algorithm) and expected digests (+ i*64)
+  int whole_algo = 0;
+  const uint8_t* whole_sums = nullptr;
   // heal
   uint8_t* const* outs = nullptr;
   uint8_t* corrupt = nullptr;
@@ -2401,6 +2411,10 @@ struct mec_batcher {
   mec_codec* dst = nullptr;
   mec_codec* serial_dst = nullptr;
   std::atomic<int64_t> st_transcodes{0}, st_transcodes_serial{0};  // moves completed by merged batches / by the private pair
+  // mec_batcher_transcode_whole: the source halves of the private pair, one per whole-file algorithm (SHA256, HighwayHash256,
+  // BLAKE2b512), each created on first use, and the moves completed by merged batches / by the private pair
+  mec_codec* serial_whole[3] = {};
+  std::atomic<int64_t> st_transcodes_whole{0}, st_transcodes_whole_serial{0};
 };
 
 namespace {
@@ -2411,21 +2425,30 @@ struct InflightBatch {
   bool traced = false;
 };
 
-// The private handle `h` of `g`'s geometry, created on first use
-static mec_codec* batcher_private(mec_batcher* b, const mec_codec* g, mec_codec*& h) {
+// The private handle `h` of `g`'s geometry and bitrot algorithm `algo`, created on first use
+static mec_codec* batcher_private(mec_batcher* b, const mec_codec* g, mec_codec*& h, int algo = MEC_HIGHWAYHASH256S) {
   std::lock_guard<std::mutex> lk(b->serial_mu);
   if (!h) {
     mec_codec* p = nullptr;
-    if (mec_codec_new(g->k, g->m, g->block_size, MEC_HIGHWAYHASH256S, g->device, &p) == MEC_OK) h = p;
+    if (mec_codec_new(g->k, g->m, g->block_size, algo, g->device, &p) == MEC_OK) h = p;
   }
   return h;
 }
+// index of a whole-file algorithm in mec_batcher::serial_whole
+static inline int whole_index(int algo) { return algo == MEC_SHA256 ? 0 : algo == MEC_HIGHWAYHASH256 ? 1 : 2; }
 
 // A read or move on its own, through the private handles: a call the merged path cannot take, or the redo of a merged one that met
 // a frame failing its digest, which applies parallelReader's block-sequential fail-over exactly (a heal rewrites every out file in
 // full and reports the failing readers; a transcode rewrites every out file in full through mec_transcode on the private pair, its
-// write quorum already checked on the caller's thread)
+// write quorum already checked on the caller's thread; a whole-file move does the same through mec_transcode_whole, whose source
+// handle carries the part's algorithm)
 static int64_t batcher_run_alone(mec_batcher* b, const BatchReq& r) {
+  if (r.kind == ReqKind::TranscodeWhole) {
+    b->st_transcodes_whole_serial++;
+    mec_codec* sc = batcher_private(b, b->codec, b->serial_whole[whole_index(r.whole_algo)], r.whole_algo);
+    mec_codec* sd = batcher_private(b, b->dst, b->serial_dst);
+    return sc && sd ? mec_transcode_whole(sc, r.gfiles, r.whole_sums, r.prefer, r.total, sd, r.files, 0, r.heal_hint) : MEC_ERR_UNEXPECTED;
+  }
   if (r.kind == ReqKind::Transcode) b->st_transcodes_serial++;
   mec_codec* sc = batcher_private(b, b->codec, b->serial);
   if (r.kind == ReqKind::Transcode) {
@@ -2443,13 +2466,21 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
   if (is_read(fb.kind)) {
     // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own; the others are done
     // (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
+    // (a whole-file move: the digests of its k staged shard files, request q's at s.hdig + q*k*64, against its expected sums)
     const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
+    const uint8_t* wd = static_cast<const uint8_t*>(s.hdig.p);
     const int k = c->k;
-    for (BatchReq* r : fb.reqs) {
-      int64_t res = rc != MEC_OK ? rc : r->kind == ReqKind::Heal ? MEC_OK : r->kind == ReqKind::Transcode ? r->total : r->length;
+    for (size_t q = 0; q < fb.reqs.size(); q++) {
+      BatchReq* r = fb.reqs[q];
+      int64_t res = rc != MEC_OK ? rc : r->kind == ReqKind::Heal ? MEC_OK : is_move(r->kind) ? r->total : r->length;
       if (rc == MEC_OK) {
         bool bad = false;
-        for (int64_t bb = 0; bb < r->get_nblocks && !bad; bb++) {
+        if (r->kind == ReqKind::TranscodeWhole) {
+          const size_t ds = static_cast<size_t>(mec_digest_size(r->whole_algo));
+          for (int i = 0, t = 0; i < c->n && !bad; i++)  // stream t of the request is its t-th chosen reader, ascending
+            if ((r->alive_mask >> i) & 1) bad = memcmp(wd + (q * k + t++) * 64, r->whole_sums + static_cast<size_t>(i) * 64, ds) != 0;
+        }
+        for (int64_t bb = 0; bb < r->get_nblocks && !bad && r->kind != ReqKind::TranscodeWhole; bb++) {
           const int64_t slot = (r->get_tail_slot >= 0 && bb == r->get_nblocks - 1) ? r->get_tail_slot : r->get_slot0 + bb;
           for (int t = 0; t < k; t++) bad |= fl[slot * k + t] != 0;
         }
@@ -2459,6 +2490,7 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
         } else {
           if (r->heal_hint) *r->heal_hint = 0;
           if (r->kind == ReqKind::Transcode) b->st_transcodes++;
+          if (r->kind == ReqKind::TranscodeWhole) b->st_transcodes_whole++;
         }
       }
       r->result = res;
@@ -2953,31 +2985,46 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
   return MEC_OK;
 }
 
+// The raw shard files of a merged batch of whole-file moves, staged and hashed by batch_whole_stage: file (z, t) at files +
+// streams[z * k + t].off on the device
+struct WholeFiles {
+  const uint8_t* files;
+  const WholeStream* streams;
+};
+
 // The request table to the device, survivor frames of every block of every request -> the slot's arena, the fused reconstruct of
 // every request's targets over all of them, and the per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table
 // gp.reqs points at; gp holds the geometry and gets the arena and rebuilt rows here.  A batch of several erasure patterns is ONE
-// latency launch with a decode plan per block (batcher_main only merges such a batch when its blocks fit one).
+// latency launch with a decode plan per block (batcher_main only merges such a batch when its blocks fit one).  `raw` (a batch of
+// whole-file moves): the arena is filled from the staged raw shard files by batch_whole_rows_kernel instead, and the reconstruct
+// neither hashes nor verifies anything (those files were hashed whole; s.dig holds their digests and is left alone).
 static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* tab, BatchGetParams& gp, const ReadLayout& lay,
-                                  bool hash_outputs) {
+                                  bool hash_outputs, const WholeFiles* raw = nullptr) {
   mec_codec* c = b->codec;
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
   const int64_t stride = round_up(nslots * P + 512, 256);
-  mark_phase(b, s, 0);
+  if (!raw) mark_phase(b, s, 0);  // a whole-file batch marks the start of its staging (batch_whole_stage)
   MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, lay.table_bytes, cudaMemcpyHostToDevice, s.st));
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(nslots * std::max(r, 1) * pitch)))) return rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(nslots * (k + r) * 32)))) return rc;
-  if ((rc = s.flags.ensure(static_cast<size_t>(nslots * k)))) return rc;
-  if ((rc = s.hflags.ensure(static_cast<size_t>(nslots * k)))) return rc;
+  if (!raw) {
+    if ((rc = s.dig.ensure(static_cast<size_t>(nslots * (k + r) * 32)))) return rc;
+    if ((rc = s.flags.ensure(static_cast<size_t>(nslots * k)))) return rc;
+    if ((rc = s.hflags.ensure(static_cast<size_t>(nslots * k)))) return rc;
+  }
   gp.arena = static_cast<uint8_t*>(s.aux.p); gp.arena_stride = stride;
   gp.rebuilt = static_cast<const uint8_t*>(s.out.p);
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
   // long ranges are staged by the copy engines (k strided copies per request are cheap next to megabytes of frames); short ones by
   // the gather kernel (no per-request driver call at all)
   const int64_t fstride = 32 + S;
-  {
+  if (raw) {
+    batch_whole_rows_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp, raw->files, raw->streams);
+    MEC_CUDA_OK(cudaGetLastError());
+    c->eng->count_launch();
+  } else {
     // one 1-D copy per (request, survivor, block) frame — the arena pads frames to a 16-byte pitch — all of them in ONE batched call
     std::vector<void*> dsts, srcs;
     std::vector<size_t> sizes;
@@ -2997,16 +3044,16 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
       }
     }
     if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
-  }
-  bool any_gather = false;
-  for (int q = 0; q < gp.nreq; q++) any_gather |= !tab[q].dma;
-  if (any_gather) {
-    batch_get_gather_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp);
-    MEC_CUDA_OK(cudaGetLastError());
-    c->eng->count_launch();
+    bool any_gather = false;
+    for (int q = 0; q < gp.nreq; q++) any_gather |= !tab[q].dma;
+    if (any_gather) {
+      batch_get_gather_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp);
+      MEC_CUDA_OK(cudaGetLastError());
+      c->eng->count_launch();
+    }
   }
   mark_phase(b, s, 1);
-  MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
+  if (!raw) MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
   const int32_t* block_len = nullptr;
   const bool mixed = lay.npat > 1;
   const uint8_t* dtab = static_cast<const uint8_t*>(s.dreq.p);
@@ -3025,12 +3072,16 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
       d.map_base[t] = base; d.map_len[t] = stride - slot0 * P; d.expect_ptr[t] = base; d.in_ptr[t] = base + 32;
     }
     d.out = static_cast<uint8_t*>(s.out.p) + slot0 * r * pitch;
-    d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * (k + r) * 32;
-    d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0 * k;
+    if (!raw) {
+      d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * (k + r) * 32;
+      d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0 * k;
+    }
     return c->eng->launch_fused(d, c->opt, s.st);
   };
   if (mixed && !c->eng->small_ok(c->opt, nslots)) return MEC_ERR_UNSUPPORTED;
-  if (mixed && lay.ntails == 0) {
+  if (raw && r == 0) {
+    // nothing to rebuild and nothing to verify: every request reads its k data drives
+  } else if (mixed && lay.ntails == 0) {
     if ((rc = launch(0, nslots, S))) return rc;
   } else if (lay.ntails > 0 && c->eng->small_ok(c->opt, nslots)) {
     // ONE launch for every block of every caller, the short last ones included (per-block shard lengths in the latency kernel)
@@ -3048,7 +3099,7 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     for (int q = 0; q < gp.nreq; q++)
       if (tab[q].tail_slot >= 0 && (rc = launch(tab[q].tail_slot, 1, tab[q].last_len))) return rc;
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
+  if (!raw) MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
   mark_phase(b, s, 2);
   b->st_patterns += lay.npat;
   if (mixed) b->st_mixed++;
@@ -3150,15 +3201,63 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
   return MEC_OK;
 }
 
+// The staging of a merged batch of whole-file moves (mec_batcher_transcode_whole), on the slot's stream: the raw shard files of
+// every request's k chosen readers (tab[z].chosen) -> the file arena in s.src (file (z, t) 16-byte aligned with 256 readable bytes
+// behind it, as stage_verified_whole lays files out) in ONE batched copy, then ONE whole_hash_kernel launch over all nreq x k files
+// with a stream table, and their digests back to s.hdig (file (z, t) at + (z * k + t) * 64), where batcher_finish compares them
+// with every request's expected sums.  s.src of a transcode batcher's slot is sized up front for a full batch (batcher_create).
+static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const BatchGetDesc* tab, WholeFiles* wf) {
+  mec_codec* c = b->codec;
+  const int k = c->k;
+  const size_t nreq = reqs.size(), nfiles = nreq * static_cast<size_t>(k);
+  int rc;
+  if ((rc = s.hwtab.ensure(nfiles * sizeof(WholeStream)))) return rc;
+  if ((rc = s.wtab.ensure(nfiles * sizeof(WholeStream)))) return rc;
+  if ((rc = s.dig.ensure(nfiles * 64))) return rc;
+  if ((rc = s.hdig.ensure(nfiles * 64))) return rc;
+  WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+  int64_t arena = 0;
+  for (size_t z = 0; z < nreq; z++) {
+    const int64_t sfs = mec_shard_file_size(c, reqs[z]->total);
+    for (int t = 0; t < k; t++) {
+      ws[z * k + t] = WholeStream{arena, sfs};
+      arena += round_up(sfs, 16) + 256;
+    }
+    c->st_h2d += static_cast<int64_t>(k) * sfs;
+  }
+  if ((rc = s.src.ensure(static_cast<size_t>(arena)))) return rc;
+  uint8_t* files = static_cast<uint8_t*>(s.src.p);
+  mark_phase(b, s, 0);
+  MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, nfiles * sizeof(WholeStream), cudaMemcpyHostToDevice, s.st));
+  std::vector<void*> dsts, srcs;
+  std::vector<size_t> sizes;
+  for (size_t z = 0; z < nreq; z++)
+    for (int t = 0; t < k; t++) {
+      const WholeStream& w = ws[z * k + t];
+      dsts.push_back(files + w.off); srcs.push_back(const_cast<uint8_t*>(tab[z].files[tab[z].chosen[t]])); sizes.push_back(static_cast<size_t>(w.len));
+    }
+  if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
+  const WholeStream* dws = static_cast<const WholeStream*>(s.wtab.p);
+  if ((rc = whole_hash_device(c, reqs.front()->whole_algo, files, 0, 0, static_cast<int64_t>(nfiles), static_cast<uint8_t*>(s.dig.p), s.st, dws)))
+    return rc;
+  c->eng->count_launch();
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hdig.p, s.dig.p, nfiles * 64, cudaMemcpyDeviceToHost, s.st));
+  *wf = WholeFiles{files, dws};
+  return MEC_OK;
+}
+
 // one merged batch of moves between pools (mec_batcher_transcode), everything on the source slot's stream: survivor frames staged and
 // the missing data shards rebuilt as for whole-part GETs (not hashed: they are consumed here) -> batch_transcode_resplit_kernel
 // writes every request's object bytes into the destination slot's staging in the PUT layout -> the destination codec's encode and
 // frame scatter of a merged PUT batch into every caller's out files.  The destination codec's slot with the same index holds the
-// destination side (as emit_transcode uses it), so the six batches in flight never share staging.
+// destination side (as emit_transcode uses it), so the six batches in flight never share staging.  A batch of whole-file moves
+// (mec_batcher_transcode_whole) is staged and hashed by batch_whole_stage and its raw shard rows laid into the frame arena; from the
+// rebuild on it runs exactly as a batch of streaming moves.
 static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
   mec_codec* e = b->dst;
   Slot& d = e->slots[&s - c->slots];
+  const bool whole = reqs.front()->kind == ReqKind::TranscodeWhole;
   BatchGetParams gp;
   ReadLayout lay;
   int rc = batch_read_plan(b, s, reqs, gp, lay);
@@ -3170,11 +3269,15 @@ static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchRe
   const int64_t bs = e->block_size, eS = e->S(), epitch = round_up(eS, 16);
   for (const BatchReq* r : reqs) {
     const int64_t nf = r->total / bs, tl = r->total % bs;
-    c->st_h2d += static_cast<int64_t>(c->k) * mec_bitrot_shard_file_size(mec_shard_file_size(c, r->total), c->S(), MEC_HIGHWAYHASH256S);
+    if (!whole)
+      c->st_h2d += static_cast<int64_t>(c->k) * mec_bitrot_shard_file_size(mec_shard_file_size(c, r->total), c->S(), MEC_HIGHWAYHASH256S);
     e->st_d2h += (nf * eS + (tl ? ceil_frac(tl, ek) : 0)) * en;
   }
   const BatchReqDesc* dt = static_cast<const BatchReqDesc*>(d.hreq.p);
-  if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, lay, false))) return rc;
+  const BatchGetDesc* rt = static_cast<const BatchGetDesc*>(s.hreq.p);
+  WholeFiles wf;
+  if (whole && (rc = batch_whole_stage(b, s, reqs, rt, &wf))) return rc;
+  if ((rc = batch_read_reconstruct(b, s, rt, gp, lay, false, whole ? &wf : nullptr))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(d.dreq.p, dt, nreq * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
   BatchCopyParams cp;
   cp.reqs = static_cast<const BatchReqDesc*>(d.dreq.p);
@@ -3224,7 +3327,7 @@ static void batcher_main(mec_batcher* b) {
           b->cv_work.wait_for(lk, std::chrono::microseconds(b->max_wait_us), [&] { return b->stop || blocks_queued() >= b->max_blocks; });
         // a batch = the oldest request plus everything queued behind it of the same kind (and, for GETs, heals and transcodes, the same reader
         // set; for heals also the same stale drives — unless b->mix: then reads of other patterns join while the batch's blocks fit
-        // one latency launch, and a batch of several patterns is cut at that limit)
+        // one latency launch, and a batch of several patterns is cut at that limit; whole-file moves also share their algorithm)
         // a shallow pipeline is filled with several smaller batches rather than one big one: the fused kernel takes ~0.45 ms however few
         // blocks it is given (one warp walks one erasure block), so the copy of one batch has to overlap the kernel of another —
         // otherwise a closed loop of callers falls into a convoy (all of them in one batch, the GPU idle while they wake up)
@@ -3242,7 +3345,7 @@ static void batcher_main(mec_batcher* b) {
         for (auto it = b->queue.begin(); it != b->queue.end();) {
           BatchReq* r = *it;
           const bool same = r->alive_mask == lead->alive_mask && r->stale_mask == lead->stale_mask;
-          if (r->kind != lead->kind || (!same && !mix)) { ++it; continue; }
+          if (r->kind != lead->kind || r->whole_algo != lead->whole_algo || (!same && !mix)) { ++it; continue; }
           const int64_t rb = req_blocks(r);
           if (!reqs.empty() && nb + rb > cap) break;
           if (mix) {  // the exact blocks of the read
@@ -3270,7 +3373,8 @@ static void batcher_main(mec_batcher* b) {
           case ReqKind::Put: rc = batcher_submit(b, s, reqs, &fb.needs_retire, &nblocks); break;
           case ReqKind::Get: rc = batcher_submit_get(b, s, reqs, &nblocks); break;
           case ReqKind::Heal: rc = batcher_submit_heal(b, s, reqs, &nblocks); break;
-          case ReqKind::Transcode: {
+          case ReqKind::Transcode:
+          case ReqKind::TranscodeWhole: {
             std::lock_guard<std::mutex> lk_dst(b->dst->mu);  // source, then destination: mec_transcode's order
             rc = batcher_submit_transcode(b, s, reqs, &nblocks);
             break;
@@ -3421,6 +3525,17 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
         rc = MEC_ERR_CUDA;
       }
     if (rc == MEC_OK) rc = ensure_crc(c);
+    if (dst)
+      // merged whole-file moves (batch_whole_stage): the raw shard files of a batch in s.src.  Request z of NB_z source blocks
+      // stages k files of at most NB_z x S bytes (k x S < block_size + k), each padded by at most 15 + 256 bytes, so a batch of at
+      // most `slots` blocks and requests fits slots x (block_size + 272 x k) bytes; one stream-table entry and one digest per file
+      for (Slot& s : c->slots) {
+        if (rc == MEC_OK) rc = s.src.ensure(static_cast<size_t>(slots * (block_size + 272 * k)));
+        if (rc == MEC_OK) rc = s.wtab.ensure(static_cast<size_t>(slots * k) * sizeof(WholeStream));
+        if (rc == MEC_OK) rc = s.hwtab.ensure(static_cast<size_t>(slots * k) * sizeof(WholeStream));
+        if (rc == MEC_OK) rc = s.dig.ensure(static_cast<size_t>(slots * std::max(c->n * 32, k * 64)));
+        if (rc == MEC_OK) rc = s.hdig.ensure(static_cast<size_t>(slots * std::max(c->n * 32, k * 64)));
+      }
     if (dst) {
       // the destination side of a merged transcode batch, laid out as a merged PUT batch of the destination geometry: object bytes,
       // parity rows, digests, the PUT request table and the latency kernel's block table.  A batch of `slots` source blocks holds
@@ -3512,6 +3627,7 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
   batcher_destroy_streams(b);
   mec_codec_free(b->serial);
   mec_codec_free(b->serial_dst);
+  for (mec_codec* h : b->serial_whole) mec_codec_free(h);
   mec_codec_free(b->dst);
   mec_codec_free(b->codec);
   delete b;
@@ -3694,6 +3810,36 @@ extern "C" int64_t mec_batcher_transcode(mec_batcher* b, const uint8_t* const* f
   return batcher_enqueue_wait(b, r);
 }
 
+// mec_transcode_whole through the coalescer: whole-file moves of one algorithm queued together that read the same k drives (any,
+// with MEC_BATCHER_MIX_PATTERNS) are merged into one batch, staged in one batched copy and hashed in one launch (batch_whole_stage),
+// then rebuilt, re-split, encoded and scattered as a batch of streaming moves.  The private path is mec_batcher_transcode's, through
+// mec_transcode_whole on a private pair whose source handle carries the request's algorithm.
+extern "C" int64_t mec_batcher_transcode_whole(mec_batcher* b, int algo, const uint8_t* const* files, const uint8_t* sums,
+                                               const uint8_t* prefer, int64_t total, uint8_t* const* out_files, int write_quorum,
+                                               int* heal_hint) {
+  if (heal_hint) *heal_hint = 0;
+  if (!b || !b->dst || !files || !sums || !out_files || total < 0 || mec_digest_size(algo) < 0) return MEC_ERR_INVALID_ARGUMENT;
+  if (algo == MEC_HIGHWAYHASH256S) return MEC_ERR_UNSUPPORTED;  // a streaming part moves through mec_batcher_transcode
+  mec_codec* c = b->codec;
+  mec_codec* e = b->dst;
+  int online = 0;
+  for (int i = 0; i < e->n; i++) online += out_files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  if (total == 0) return 0;
+  BatchReq r;
+  r.kind = ReqKind::TranscodeWhole; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
+  r.prefer = prefer; r.heal_hint = heal_hint; r.whole_algo = algo; r.whole_sums = sums;
+  r.len = total; r.files = out_files; r.with_data = true;  // the destination side, a PUT of the part
+  if (c->n > kBatchMaxFiles || e->n > kBatchMaxFiles) return batcher_run_alone(b, r);
+  bool mapped = !b->sw.memcpy;
+  const int rc = batch_readers(c, r, &mapped);
+  if (rc) return rc;
+  for (int i = 0; i < e->n && mapped; i++)
+    if (out_files[i]) mapped = mec_is_pinned(out_files[i]) != 0;
+  if (!mapped || ceil_frac(total, c->block_size) > b->max_blocks) return batcher_run_alone(b, r);
+  return batcher_enqueue_wait(b, r);
+}
+
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!b || !name) return -1;
   if (!strcmp(name, "batches")) return b->st_batches.load();
@@ -3715,6 +3861,8 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "us_scatter")) return b->us_scatter.load();
   if (!strcmp(name, "transcodes")) return b->st_transcodes.load();
   if (!strcmp(name, "transcodes_serial")) return b->st_transcodes_serial.load();
+  if (!strcmp(name, "transcodes_whole")) return b->st_transcodes_whole.load();
+  if (!strcmp(name, "transcodes_whole_serial")) return b->st_transcodes_whole_serial.load();
   if (!strncmp(name, "dst_", 4)) return b->dst ? mec_get_stat(b->dst, name + 4) : -1;  // the destination codec of merged moves
   return mec_get_stat(b->codec, name);  // the batcher's codec: which kernel forms its merged launches ran ("form_*", "last_*", ...)
 }

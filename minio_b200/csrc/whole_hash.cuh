@@ -110,13 +110,23 @@ __device__ inline void blake2b_compress(uint64_t (&h)[8], const uint64_t (&m)[16
 }
 
 // ---- one thread per stream; streams are contiguous, 16-byte aligned, padded with >= 128 readable bytes ------
+// One stream of a launch with a stream table: data + off, len bytes (a merged batch of shard files of different lengths)
+struct WholeStream {
+  int64_t off, len;
+};
+
 struct WholeHashParams {
   const uint8_t* data;   // stream s at data + s*pitch
   int64_t pitch, len;    // every stream has the same length
+  const WholeStream* streams;  // device, optional: stream s is data + streams[s].off, streams[s].len bytes (pitch, len unused)
   int nstreams, algo;    // MEC_SHA256 = 1, MEC_HIGHWAYHASH256 = 2, MEC_BLAKE2B512 = 4
   uint8_t* out;          // digest of stream s at out + s*64
   uint64_t key[4];
 };
+
+__device__ __forceinline__ WholeStream whole_stream(const WholeHashParams& p, int s) {
+  return p.streams ? p.streams[s] : WholeStream{static_cast<int64_t>(s) * p.pitch, p.len};
+}
 
 __global__ void whole_hash_kernel(const WholeHashParams p) {
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
@@ -124,11 +134,12 @@ __global__ void whole_hash_kernel(const WholeHashParams p) {
     // HighwayHash-256: two threads per stream, exactly the half-state code of the fused kernel
     const int s = tid >> 1, h = tid & 1;
     const bool live = s < p.nstreams;
-    const uint8_t* d = p.data + static_cast<int64_t>(live ? s : 0) * p.pitch;
+    const WholeStream ws = whole_stream(p, live ? s : 0);
+    const uint8_t* d = p.data + ws.off;
     HHHalf hs;
     hh_init(hs, p.key, h);
-    const int64_t npk = p.len >> 5;
-    const int rem = static_cast<int>(p.len & 31);
+    const int64_t npk = ws.len >> 5;
+    const int rem = static_cast<int>(ws.len & 31);
     if (live) {
       for (int64_t q = 0; q < npk; q++) {
         const uint4 v = *reinterpret_cast<const uint4*>(d + q * 32 + 16 * h);
@@ -148,12 +159,14 @@ __global__ void whole_hash_kernel(const WholeHashParams p) {
     return;
   }
   if (tid >= p.nstreams) return;
-  const uint8_t* d = p.data + static_cast<int64_t>(tid) * p.pitch;
+  const WholeStream ws = whole_stream(p, tid);
+  const uint8_t* d = p.data + ws.off;
+  const int64_t len = ws.len;
   uint8_t* o = p.out + static_cast<int64_t>(tid) * 64;
   if (p.algo == 1) {
     uint32_t h[8] = {0x6a09e667, 0xbb67ae85, 0x3c6ef372, 0xa54ff53a, 0x510e527f, 0x9b05688c, 0x1f83d9ab, 0x5be0cd19};
     uint32_t w[16];
-    const int64_t nfull = p.len >> 6;
+    const int64_t nfull = len >> 6;
     for (int64_t b = 0; b < nfull; b++) {
 #pragma unroll
       for (int q = 0; q < 4; q++) {
@@ -163,13 +176,13 @@ __global__ void whole_hash_kernel(const WholeHashParams p) {
       sha256_compress(h, w);
     }
     // padding: 0x80, zeros, 64-bit big-endian bit length
-    const int r = static_cast<int>(p.len & 63);
+    const int r = static_cast<int>(len & 63);
     uint8_t blk[128];
     for (int i = 0; i < 128; i++) blk[i] = 0;
     for (int i = 0; i < r; i++) blk[i] = d[nfull * 64 + i];
     blk[r] = 0x80;
     const int total = r < 56 ? 64 : 128;
-    const uint64_t bits = static_cast<uint64_t>(p.len) * 8;
+    const uint64_t bits = static_cast<uint64_t>(len) * 8;
     for (int i = 0; i < 8; i++) blk[total - 1 - i] = static_cast<uint8_t>(bits >> (8 * i));
     for (int bb = 0; bb < total; bb += 64) {
       for (int q = 0; q < 16; q++)
@@ -187,10 +200,10 @@ __global__ void whole_hash_kernel(const WholeHashParams p) {
     h[0] ^= 0x01010000ull ^ 64;
     uint64_t m[16];
     // all blocks but the last are full 128-byte blocks; the last block (1..128 bytes, or the empty message) is final
-    const int64_t nblk = p.len == 0 ? 1 : (p.len + 127) / 128;
+    const int64_t nblk = len == 0 ? 1 : (len + 127) / 128;
     for (int64_t b = 0; b < nblk; b++) {
       const bool last = b == nblk - 1;
-      const int64_t have = last ? p.len - b * 128 : 128;
+      const int64_t have = last ? len - b * 128 : 128;
       if (have == 128) {
 #pragma unroll
         for (int q = 0; q < 8; q++) {

@@ -18,6 +18,10 @@
 //                  SRC_BS (source) and DST_BS (destination), default 1 MiB each (legacy 10 MiB-block parts: SRC_BS=10485760)
 //   mode transcode : the same moves, each a mec_transcode call on the handle pair t % P (source and destination codec)
 //   btranscode_rot / transcode_rot : as bget_rot, drive 0 offline and thread t's object rotated by t % n
+//   mode btranscode_whole / transcode_whole (and their _rot forms): the same moves of parts written with the whole-file bitrot
+//                  algorithm ALGO (1 = SHA256, 2 = HighwayHash256 (default), 4 = BLAKE2b512), their raw shard files and sums made
+//                  once by mec_encode_whole: through ONE transcode batcher (mec_batcher_transcode_whole), or each a
+//                  mec_transcode_whole call on the handle pair t % P (source codecs of that algorithm)
 //                  (after the timed window every thread's out files are compared with a plain mec_encode on the destination geometry)
 //   MIX=1        : the batcher of the b* modes is created with MEC_BATCHER_MIX_PATTERNS (reads of different patterns share batches)
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
@@ -103,7 +107,8 @@ int main(int argc, char** argv) {
   signal(SIGSEGV, on_segv);
   signal(SIGABRT, on_segv);
   std::string mode = argc > 1 ? argv[1] : "batcher";
-  const bool rot = mode == "bget_rot" || mode == "bheal_rot" || mode == "btranscode_rot" || mode == "transcode_rot";
+  const bool rot = mode == "bget_rot" || mode == "bheal_rot" || mode == "btranscode_rot" || mode == "transcode_rot" ||
+                   mode == "btranscode_whole_rot" || mode == "transcode_whole_rot";
   if (rot) mode.resize(mode.size() - 4);
   const std::string mode_name = rot ? mode + "_rot" : mode;
   const int bflags = getenv("MIX") && atoi(getenv("MIX")) ? MEC_BATCHER_MIX_PATTERNS : 0;
@@ -115,7 +120,10 @@ int main(int argc, char** argv) {
   const int P = argc > 5 ? atoi(argv[5]) : 8;
   const int device = argc > 6 ? atoi(argv[6]) : 0;
   const int k = 12, m = 4, n = k + m;
-  const bool move = mode == "btranscode" || mode == "transcode";
+  const bool whole = mode == "btranscode_whole" || mode == "transcode_whole";
+  const bool bmove = mode == "btranscode" || mode == "btranscode_whole";  // through the transcode batcher
+  const bool move = bmove || mode == "transcode" || mode == "transcode_whole";
+  const int walgo = getenv("ALGO") ? atoi(getenv("ALGO")) : MEC_HIGHWAYHASH256;
   const int64_t bs = move && getenv("SRC_BS") ? atoll(getenv("SRC_BS")) : 1 << 20;
   const int64_t bs2 = move && getenv("DST_BS") ? atoll(getenv("DST_BS")) : 1 << 20;
   const bool gpu = mode != "cpu";
@@ -135,6 +143,7 @@ int main(int argc, char** argv) {
   const int sums_mask = getenv("SUMS") ? atoi(getenv("SUMS")) : MEC_SUM_MD5;
   struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; uint64_t crc[3];
               uint8_t sums[MEC_SUM_BYTES];
+              std::vector<uint8_t> wsums;  // whole-file modes: the expected digest of every source shard file, n x 64
               std::vector<uint8_t*> outs; };  // outs: the destination part files of the transcode modes
   std::vector<TB> tb(T);
   uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
@@ -162,8 +171,8 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
-  } else if (gpu && mode != "bget" && mode != "bheal" && mode != "btranscode") {
-    for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
+  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove) {
+    for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, whole ? walgo : MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
   }
   if (mode == "bget" || mode == "bheal") {  // coalesced GETs / heals: part files through a temporary handle, then everything goes through the batcher
     mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c0);
@@ -177,13 +186,15 @@ int main(int argc, char** argv) {
     if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
   }
   if (move) {  // source part files through a temporary handle; the transcode batcher, or the pool's destination handles
-    mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c0);
+    mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, whole ? walgo : MEC_HIGHWAYHASH256S, device, &c0);
     for (int t = 0; t < T; t++) {
       std::vector<uint8_t*> f(tb[t].files);
-      if (mec_encode(c0, tb[t].obj, osize, f.data(), k) != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
+      tb[t].wsums.assign(static_cast<size_t>(n) * 64, 0);
+      const int64_t rc = whole ? mec_encode_whole(c0, tb[t].obj, osize, f.data(), tb[t].wsums.data(), k) : mec_encode(c0, tb[t].obj, osize, f.data(), k);
+      if (rc != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
     }
     mec_codec_free(c0);
-    if (mode == "btranscode") {
+    if (bmove) {
       int rc = mec_batcher_new_transcode_ex(k, m, bs, k2, m2, bs2, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
                                             getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
       if (rc) { fprintf(stderr, "transcode batcher: %d %s\n", rc, mec_last_error()); return 1; }
@@ -234,6 +245,9 @@ int main(int argc, char** argv) {
       const uint8_t* f[64];
       for (int i = 0; i < n; i++) f[i] = rot && i == drive0_shard(t) ? nullptr : b.files[i];
       int hint = 0;
+      if (mode == "btranscode_whole") return mec_batcher_transcode_whole(bat, walgo, f, b.wsums.data(), nullptr, osize, b.outs.data(), k2, &hint);
+      if (mode == "transcode_whole")
+        return mec_transcode_whole(pool[t % P], f, b.wsums.data(), nullptr, osize, pool2[t % P], b.outs.data(), k2, &hint);
       return mode == "btranscode" ? mec_batcher_transcode(bat, f, nullptr, osize, b.outs.data(), k2, &hint)
                                   : mec_transcode(pool[t % P], f, nullptr, osize, pool2[t % P], b.outs.data(), k2, &hint);
     }
@@ -305,10 +319,15 @@ int main(int argc, char** argv) {
            (long long)mec_batcher_stat(bat, "us_scatter"));
   if (move) printf(", \"dst\": \"%d,%d\", \"src_block_size\": %lld, \"dst_block_size\": %lld", k2, m2, static_cast<long long>(bs),
                   static_cast<long long>(bs2));
+  if (whole) printf(", \"algo\": %d", walgo);
   if (mode == "btranscode")
     printf(", \"transcodes\": %lld, \"transcodes_serial\": %lld, \"redone\": %lld", static_cast<long long>(mec_batcher_stat(bat, "transcodes")),
            static_cast<long long>(mec_batcher_stat(bat, "transcodes_serial")), static_cast<long long>(mec_batcher_stat(bat, "redone")));
-  if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode") printf(", \"pool\": %d", P);
+  if (mode == "btranscode_whole")
+    printf(", \"transcodes_whole\": %lld, \"transcodes_whole_serial\": %lld, \"redone\": %lld, \"whole_hash_launches\": %lld",
+           static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole")), static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole_serial")),
+           static_cast<long long>(mec_batcher_stat(bat, "redone")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
+  if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode" || mode == "transcode_whole") printf(", \"pool\": %d", P);
   printf("}\n");
   if (bat) mec_batcher_free(bat);
   for (auto c : pool) mec_codec_free(c);

@@ -145,6 +145,30 @@ bat.close()
 lc, ld = mb.Codec(k, m, lbs), mb.Codec(6, 2, 1 << 20)
 outs, hint = lc.transcode([None if i == 1 else f for i, f in enumerate(lsrc[0])], ldat[0].size, ld)
 assert hint == 0 and all(np.array_equal(x, y) for x, y in zip(outs, ltw[0]))
+# whole-file moves (mec_batcher_transcode_whole): four RS(12,4) parts written with SHA256 -> RS(6,2) in one merged batch with
+# source drive 1 offline (one batched staging copy, ONE whole_hash_kernel launch over shard files of four lengths,
+# batch_whole_rows_kernel, the merged reconstruct without digests, re-split, encode and scatter), then a fifth move whose chosen
+# reader 5 has a flipped byte: its merged batch fails the digest check and it is redone on the private pair
+wdat = [np.random.default_rng(60 + t).integers(0, 256, n, dtype=np.uint8) for t, n in enumerate((1 << 19, (1 << 20) + 5, 77, 2 * (1 << 20) + 999, 300001))]
+wsrc, wsum = [], []
+for a in wdat:
+    fs, ss = o.erasure_encode(k, m, bs, 1, a)
+    pf = [mb.pinned_array(f.size) for f in fs]
+    for x, f in zip(pf, fs): x[:] = f
+    wsrc.append(pf); wsum.append(ss)
+wsrc[4][5][100] ^= 1
+wtw = [o.erasure_encode(6, 2, bs, 3, a)[0] for a in wdat]
+bat = mb.Batcher(k, m, bs, max_batch_blocks=8, max_wait_us=500000, dst=(6, 2))
+res = [None] * 5
+def wmove(t): res[t] = bat.transcode_whole([None if i == 1 else f for i, f in enumerate(wsrc[t])], wsum[t], wdat[t].size, 1, pinned=True)
+th = [threading.Thread(target=wmove, args=(t,)) for t in range(4)]
+[x.start() for x in th]; [x.join() for x in th]
+assert all(r[1] == 0 and all(np.array_equal(x, y) for x, y in zip(r[0], wtw[t])) for t, r in enumerate(res[:4]))
+assert bat.stat("batches") == 1 and bat.stat("transcodes_whole") == 4 and bat.stat("whole_hash_launches") == 1
+res[4] = bat.transcode_whole(wsrc[4], wsum[4], wdat[4].size, 1, pinned=True)
+assert res[4][1] == -7 and all(np.array_equal(x, y) for x, y in zip(res[4][0], wtw[4]))
+assert bat.stat("redone") == 1 and bat.stat("transcodes_whole_serial") == 1
+bat.close()
 print("sanitizer case ok")
 PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
