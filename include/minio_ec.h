@@ -413,7 +413,8 @@ int mec_whole_hash_device(mec_codec* c, int algo, const uint8_t* d_msgs, int64_t
  * mec_decode_whole returns bytes written (*heal_hint = MEC_ERR_FILE_CORRUPT when a reader was dropped but the read succeeded).
  * mec_heal_whole rebuilds every shard file with out_files[i] != NULL, writes its digest to out_sums + i*64 (optional) and returns
  * MEC_OK, or MEC_ERR_FILE_CORRUPT when it healed but met bitrot in a source (corrupt[i], optional, names the readers).
- * The codec's algorithm must be SHA256, BLAKE2b512 or HighwayHash256. */
+ * The codec's algorithm must be SHA256, BLAKE2b512 or HighwayHash256.  mec_heal_whole writes the legacy format (raw shard files
+ * and whole-file sums); healObject heals into the streaming format, which is what mec_heal_mixed writes. */
 int64_t mec_decode_whole(mec_codec* c, const uint8_t* const* files, const uint8_t* sums, int64_t offset, int64_t length,
                          int64_t total_length, uint8_t* dst, int* heal_hint);
 int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const uint8_t* sums, int64_t total_length,
@@ -441,6 +442,43 @@ int mec_digest_size(int algo);
  * "corrupt_shards" grow on src, "blocks_encoded" and "bytes_d2h" on dst; src's "bytes_d2h" does not grow. */
 int64_t mec_transcode_whole(mec_codec* src, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
                             int64_t total_length, mec_codec* dst, uint8_t* const* out_files, int write_quorum, int* heal_hint);
+
+/* Erasure.Decode / Erasure.Heal over a part whose drives mix bitrot formats: a legacy part (whole-file algorithm) of which some
+ * drives were healed.  healObject heals into HighwayHash256S frames (cmd/erasure-healing.go:593-596) and leaves the healed drive no
+ * checksum entry, so it reads as streaming (cmd/erasure-metadata.go:43-51); every GET opens each drive with its own algorithm
+ * (cmd/erasure-object.go:381-384) and parallelReader mixes the two reader kinds in one decode.
+ *   c          : a HighwayHash256S codec of the part's geometry (another algorithm: MEC_ERR_UNSUPPORTED)
+ *   algos[i]   : drive i's bitrot algorithm, read only where files[i] != NULL (heal: and out_files[i] == NULL)
+ *                MEC_HIGHWAYHASH256S: files[i] is the drive's part.N image from its first frame, as mec_decode_prefer takes it;
+ *                MEC_SHA256, MEC_BLAKE2B512, MEC_HIGHWAYHASH256: files[i] is the raw shard file (mec_shard_file_size(total) bytes),
+ *                sums + i*64 its expected digest
+ *   prefer     : as mec_decode_prefer; NULL = index order
+ * Fail-over is parallelReader's over both kinds.  Readers are chosen as mec_decode_prefer chooses them, preferred ones first, then
+ * index order.  A whole-file reader is verified when it is first chosen, before any block is read through it (xlStorage.ReadFile
+ * hashes the whole file on the first ReadAt, cmd/xl-storage.go:1931-1950): the whole-file readers that join the set in one round
+ * are staged and hashed by ONE whole_hash_kernel launch, and one whose digest does not match is dropped for the rest of the call,
+ * corrupt[i] set, and the next reader chosen.  A streaming reader is checked frame by frame; when one fails at block b it is
+ * dropped and the call resumes at b with the next reader, which, if it is whole-file, is hashed first.  Whole-file readers that are
+ * never chosen are never staged, hashed or reported.  Verified files stay on the device for the whole call:
+ * k x (round_up(mec_shard_file_size(total_length), 16) + 256) bytes in a buffer of the codec's own.
+ * mec_decode_mixed has mec_decode_prefer's argument checks, in its order (MEC_ERR_SHORT_DATA included), and its results:
+ * *heal_hint = MEC_ERR_FILE_CORRUPT when a reader was dropped.
+ * mec_heal_mixed: out_files[i] != NULL marks a stale drive, which is never read whatever files[i] holds (healObject opens no reader
+ * on a drive it heals, cmd/erasure-healing.go:572-575); it receives the complete HighwayHash256S part.N image, byte for byte what
+ * mec_encode writes for drive i.  Returns MEC_OK, MEC_ERR_FILE_CORRUPT (healed, but a reader was dropped; corrupt[i], optional,
+ * names them) or MEC_ERR_READ_QUORUM; out files are complete only on the first two.  No whole-file sums come back: a healed drive
+ * has none.
+ * Refused before any device work: a NULL c, algos or files, for heal a NULL out_files, an algos[i] that is no MEC_* bitrot value on a
+ * read drive, a NULL sums while a read drive is whole-file (MEC_ERR_INVALID_ARGUMENT); two different whole-file algorithms among the
+ * read drives (MEC_ERR_UNSUPPORTED).  length == 0 returns 0; heal with total_length <= 0 returns MEC_OK.
+ * With every drive HighwayHash256S (and no stale drive among the readers) the calls equal mec_decode_prefer / mec_heal_prefer; with
+ * every drive whole-file and prefer == NULL, mec_decode_mixed equals mec_decode_whole.
+ * Counters: "blocks_read", "shards_rebuilt", "corrupt_shards" and "bytes_d2h" as the streaming calls; "bytes_h2d" = frame bytes of
+ * streaming readers + one shard file per whole-file reader hashed; "whole_hash_launches" + 1 per round with whole-file newcomers. */
+int64_t mec_decode_mixed(mec_codec* c, const int* algos, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
+                         int64_t offset, int64_t length, int64_t total_length, uint8_t* dst, int* heal_hint);
+int mec_heal_mixed(mec_codec* c, const int* algos, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
+                   int64_t total_length, uint8_t* const* out_files, uint8_t* corrupt);
 
 /* bitrotVerify (cmd/bitrot.go:164) for the streaming algorithm: scans a whole shard file. */
 int mec_bitrot_verify(mec_codec* c, const uint8_t* file, int64_t file_len, int64_t part_len);

@@ -99,6 +99,9 @@ def lib():
     L.mec_decode_whole.restype = i64
     L.mec_decode_whole.argtypes = [vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
     L.mec_heal_whole.argtypes = [vp, vp, vp, i64, vp, vp, vp]
+    L.mec_decode_mixed.restype = i64
+    L.mec_decode_mixed.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
+    L.mec_heal_mixed.argtypes = [vp, vp, vp, vp, vp, i64, vp, vp]
     L.mec_encode_blocks.argtypes = [vp, vp, i64, vp, vp]
     L.mec_encode_blocks_device.argtypes = [vp, vp, i64, vp, i64, vp, vp]
     L.mec_reconstruct_frames.argtypes = [vp, vp, i64, i64, vp, i32, vp, vp]
@@ -434,6 +437,53 @@ class Codec:
             raise MecError(rc, "mec_heal_whole")
         ds = lib().mec_digest_size(self.algo)
         return outs, [osum[i, :ds].tobytes() if stale[i] else None for i in range(self.n)], rc, corrupt
+
+    def _mixed_args(self, algos, sums):
+        al = (C.c_int32 * self.n)(*[int(a) for a in algos])
+        if sums is None:
+            return al, None
+        sm = np.zeros((self.n, 64), dtype=np.uint8)
+        for i, d in enumerate(sums):
+            if d is not None:
+                sm[i, :len(d)] = np.frombuffer(bytes(d), dtype=np.uint8)
+        return al, sm
+
+    def decode_mixed(self, files, algos, sums, offset, length, total, prefer=None):
+        """Erasure.Decode over a part whose drives mix bitrot formats (this codec is HighwayHash256S): algos[i] is drive i's
+        algorithm; files[i] its part.N image (HIGHWAYHASH256S) or raw shard file (a whole-file algorithm, expected digest sums[i]);
+        None = offline.  sums: list of bytes / None, or None.  -> (bytes, heal_hint) as Codec.decode."""
+        files = [None if f is None else _u8(f) for f in files]
+        al, sm = self._mixed_args(algos, sums)
+        dst = np.zeros(max(length, 1), dtype=np.uint8)
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        rc = lib().mec_decode_mixed(self.h, al, _ptrs(files), None if sm is None else sm.ctypes.data,
+                                    None if pf is None else pf.ctypes.data, offset, length, total, dst.ctypes.data, C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_decode_mixed")
+        return dst[:length], hint.value
+
+    def heal_mixed(self, files, algos, sums, stale, total, prefer=None, report=False):
+        """Erasure.Heal as healObject runs it on a part whose drives mix bitrot formats: the stale drives are rebuilt as
+        HighwayHash256S part.N images whatever format the readers have (files / algos / sums as decode_mixed; a stale drive is never
+        read).  report as Codec.heal."""
+        files = [None if f is None else _u8(f) for f in files]
+        al, sm = self._mixed_args(algos, sums)
+        fsz = self.bitrot_file_size(total)
+        outs = [np.zeros(fsz, dtype=np.uint8) if stale[i] else None for i in range(self.n)]
+        corrupt = np.zeros(self.n, dtype=np.uint8)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        marker = np.zeros(1, dtype=np.uint8)  # an empty part's stale drives are still marked
+        optrs = _ptrs([(o if o.size else marker) if o is not None else None for o in outs])
+        rc = lib().mec_heal_mixed(self.h, al, _ptrs(files), None if sm is None else sm.ctypes.data,
+                                  None if pf is None else pf.ctypes.data, total, optrs, corrupt.ctypes.data)
+        if report:
+            if rc and rc != -7:
+                raise MecError(rc, "mec_heal_mixed")
+            return outs, rc, corrupt
+        if rc:
+            raise MecError(rc, "mec_heal_mixed")
+        return outs
 
     def whole_hash(self, algo, msgs, msg_len, count):
         msgs = _u8(msgs)

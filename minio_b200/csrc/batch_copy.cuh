@@ -343,4 +343,29 @@ __global__ void __launch_bounds__(128) batch_whole_rows_kernel(const BatchGetPar
   }
 }
 
+// ---- mec_decode_mixed / mec_heal_mixed: whole-file readers beside streaming ones in the reconstruct pipeline --------------------
+struct WholeFramesParams {
+  uint8_t* arena;               // chunk arena: reader position t at arena + t*arena_stride, chunk block b's frame at + b*P
+  int64_t arena_stride, P;
+  const uint8_t* files;         // verified raw shard files: file slot f at files + f*fpitch (at least 256 readable bytes behind it)
+  int64_t fpitch;
+  int64_t S, first;             // full shard length; file block of the chunk's first block
+  int64_t nb, last_len;         // blocks of the chunk; shard length of its last block
+  int ncols;                    // whole-file positions of the chunk
+  int8_t pos[kBatchMaxFiles];   // column y: arena position pos[y], file slot file[y]
+  int8_t file[kBatchMaxFiles];
+};
+
+// grid (blocks of the chunk, whole-file positions), 128 threads: the single-request form of batch_whole_rows_kernel.  CTA (b, y)
+// lays row first + b of file file[y] into frame slot b of arena position pos[y] (shard at + 32; the digest bytes are left as they
+// are, the reconstruct does not check them), so the fused reconstruct and both sinks run on the chunk arena unchanged.  Rows sit
+// at any byte offset (S = 87382 for RS(12,4) at 1 MiB, 873814 at 10 MiB); cta_copy reads at most one word past a row, inside the
+// file's padding for its last row.
+__global__ void __launch_bounds__(128) whole_rows_frames_kernel(const __grid_constant__ WholeFramesParams p) {
+  const int64_t b = blockIdx.x;
+  const int y = blockIdx.y;
+  const uint8_t* row = p.files + p.file[y] * p.fpitch + (p.first + b) * p.S;
+  cta_copy(p.arena + p.pos[y] * p.arena_stride + b * p.P + 32, row, b == p.nb - 1 ? p.last_len : p.S, false);
+}
+
 }  // namespace mec

@@ -93,6 +93,10 @@ struct mec_codec {
   // boundary counters (mec_get_stat)
   int64_t st_blocks_encoded = 0, st_blocks_read = 0, st_shards_rebuilt = 0, st_corrupt = 0, st_h2d = 0, st_d2h = 0;
   int64_t st_whole_hash = 0;  // whole_hash_kernel launches
+  // mec_decode_mixed / mec_heal_mixed: the verified whole-file readers of the call (k files at a pitch of round_up(sfs, 16) + 256)
+  // and their digests; they stay on the device for the whole call while the slot arenas cycle through the chunks
+  DevBuf whole, whole_dig;
+  PinBuf hwhole_dig;
   int64_t S() const { return ceil_frac(block_size, k); }
 };
 
@@ -217,6 +221,7 @@ extern "C" void mec_codec_free(mec_codec* c) {
   }
   c->flags.release();
   c->crc_tables.release();
+  c->whole.release(); c->whole_dig.release(); c->hwhole_dig.release();
   if (c->sum_ev) cudaEventDestroy(c->sum_ev);
   c->sum_tab.release();
   c->hsum_tab.release();
@@ -913,8 +918,10 @@ struct RChunk : DecodePlan {
 static inline uint8_t* arena_ptr(Slot& s, int64_t stride, int t) { return static_cast<uint8_t*>(s.aux.p) + t * stride; }
 
 // Rebuild `ch.targets` for the chunk from the staged survivor frames.  d_out rows: (b*r + q); digests [b][k + r]; flags [b][k].
+// raw[t] (optional): position t holds rows of a verified whole-file reader laid into frame slots, with no digest to check — its
+// expected-digest pointer is null, so the kernel leaves its flags at 0.
 static int launch_reconstruct(mec_codec* c, const FrameGeom& g, const RChunk& ch, Slot& s, int64_t stride, const uint8_t* rows,
-                              int64_t pitch, bool hash_outputs) {
+                              int64_t pitch, bool hash_outputs, const bool* raw = nullptr) {
   const int k = c->k, r = ch.r;
   FusedDesc d;
   d.k = k; d.r = r; d.coef = rows; d.static_encode = false; d.contiguous = false; d.hash_outputs = hash_outputs;
@@ -928,7 +935,7 @@ static int launch_reconstruct(mec_codec* c, const FrameGeom& g, const RChunk& ch
     d.tail_block = nfull; d.tail_S = static_cast<int32_t>(g.last_len);
     for (int t = 0; t < k; t++) {
       const uint8_t* base = arena_ptr(s, stride, t);
-      d.map_base[t] = base; d.map_len[t] = stride; d.expect_ptr[t] = base; d.in_ptr[t] = base + 32;
+      d.map_base[t] = base; d.map_len[t] = stride; d.expect_ptr[t] = (raw && raw[t]) ? nullptr : base; d.in_ptr[t] = base + 32;
     }
     d.out = static_cast<uint8_t*>(s.out.p);
     d.digests = static_cast<uint8_t*>(s.dig.p);
@@ -945,7 +952,7 @@ static int launch_reconstruct(mec_codec* c, const FrameGeom& g, const RChunk& ch
       const uint8_t* base = arena_ptr(s, stride, t) + first * g.dpitch();
       d.map_base[t] = base;
       d.map_len[t] = stride - first * g.dpitch();
-      d.expect_ptr[t] = base;
+      d.expect_ptr[t] = (raw && raw[t]) ? nullptr : base;
       d.in_ptr[t] = base + 32;
     }
     d.out = static_cast<uint8_t*>(s.out.p) + first * r * pitch;
@@ -1121,6 +1128,80 @@ static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk,
   return frames_enqueue_chunk(e, ec, sk.enc_files, true, nullptr);
 }
 
+// Whole-file readers of a call (wholeBitrotReader, cmd/bitrot-whole.go:66-81): a reader hashes its WHOLE shard file on its first
+// read, whatever the offset (xlStorage.ReadFile with a verifier, cmd/xl-storage.go:1931-1950).  Verified files stay on the device
+// for the whole call: file i at arena + slot_of[i]*fpitch (k positions, fpitch >= round_up(sfs, 16) + 256), -1 = not staged.
+struct WholeSet {
+  const uint8_t* const* files;  // raw shard files (host), mec_shard_file_size(total) bytes each
+  const uint8_t* sums;          // expected digest of file i at + i*64
+  const uint8_t* whole;         // n flags: reader i is whole-file; NULL = every reader
+  int algo;
+  int64_t sfs, fpitch;
+  uint8_t* arena;               // device: k * fpitch + 256 bytes
+  uint8_t* dig;                 // device: k x 64 digest slots
+  uint8_t* hdig;                // pinned host: k x 64
+  int slot_of[kMaxShards];
+  bool is_whole(int i) const { return !whole || whole[i]; }
+};
+
+static int whole_hash_device(mec_codec* c, int algo, const uint8_t* d_data, int64_t pitch, int64_t len, int64_t count,
+                             uint8_t* d_out, cudaStream_t st, const WholeStream* streams);
+
+// One round of whole-file verification over the reader set want[0..nwant): the whole-file readers in it that are not staged yet
+// are copied into free arena positions and hashed — by ONE launch over the span of positions that holds them (one_launch; verified
+// files inside the span are hashed again, one thread per file, so the launch takes no longer), otherwise one launch per file — and
+// a reader whose digest does not match is dropped for the rest of the call (errFileCorrupt: alive[i] = 0, corrupt[i] = 1).
+// *dropped tells the caller to choose its readers again.  Drains `st`.
+static int whole_round(mec_codec* c, WholeSet& w, const int* want, int nwant, uint8_t* alive, uint8_t* corrupt, bool one_launch,
+                       cudaStream_t st, bool* dropped) {
+  const int k = c->k, n = c->n, ds = mec_digest_size(w.algo);
+  *dropped = false;
+  bool used[kMaxK] = {};  // positions held by verified files (every one of them is still a chosen reader)
+  for (int i = 0; i < n; i++)
+    if (w.slot_of[i] >= 0) used[w.slot_of[i]] = true;
+  int fresh[kMaxK], nf = 0;
+  for (int q = 0; q < nwant; q++) {
+    const int i = want[q];
+    if (!w.is_whole(i) || w.slot_of[i] >= 0) continue;
+    int pos = 0;
+    while (pos < k && used[pos]) pos++;
+    if (pos == k) return MEC_ERR_UNEXPECTED;
+    used[pos] = true;
+    w.slot_of[i] = pos;
+    fresh[nf++] = i;
+    if (w.sfs > 0)
+      MEC_CUDA_OK(cudaMemcpyAsync(w.arena + pos * w.fpitch, w.files[i], static_cast<size_t>(w.sfs), cudaMemcpyHostToDevice, st));
+    c->st_h2d += w.sfs;
+  }
+  if (nf == 0) return MEC_OK;
+  int rc;
+  if (one_launch) {
+    int lo = k, hi = -1;
+    for (int q = 0; q < nf; q++) { lo = std::min(lo, w.slot_of[fresh[q]]); hi = std::max(hi, w.slot_of[fresh[q]]); }
+    if ((rc = whole_hash_device(c, w.algo, w.arena + lo * w.fpitch, w.fpitch, w.sfs, hi - lo + 1, w.dig + lo * 64, st, nullptr))) return rc;
+    c->eng->count_launch();
+  } else {
+    for (int q = 0; q < nf; q++) {  // one launch per newcomer keeps the arena positions arbitrary; these files are few and the hash is serial anyway
+      const int pos = w.slot_of[fresh[q]];
+      if ((rc = whole_hash_device(c, w.algo, w.arena + pos * w.fpitch, w.fpitch, w.sfs, 1, w.dig + pos * 64, st, nullptr))) return rc;
+      c->eng->count_launch();
+    }
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(w.hdig, w.dig, static_cast<size_t>(k * 64), cudaMemcpyDeviceToHost, st));
+  MEC_CUDA_OK(cudaStreamSynchronize(st));
+  for (int q = 0; q < nf; q++) {
+    const int i = fresh[q];
+    if (memcmp(w.hdig + w.slot_of[i] * 64, w.sums + static_cast<size_t>(i) * 64, static_cast<size_t>(ds)) != 0) {
+      alive[i] = 0;
+      if (corrupt) corrupt[i] = 1;
+      c->st_corrupt++;
+      w.slot_of[i] = -1;
+      *dropped = true;
+    }
+  }
+  return MEC_OK;
+}
+
 // Core of Decode / Heal: frames[i] point at the first frame of the range (host).  The range is cut into chunks that run through
 // the codec's six slots — while chunk c is in the kernel, chunk c+1 is being staged and chunk c-1 is on its way back — each
 // slot with its own stream, survivor arena, output and flag buffers.  Chunks retire in order: the per-frame digest verdicts
@@ -1128,9 +1209,14 @@ static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk,
 // for the rest of the call (parallelReader.Read: p.readers[i] = nil, cmd/erasure-decode.go:196-199), everything submitted
 // behind the bad block is discarded and the range resumes AT the bad block with the next readers in order — exactly the
 // block-sequential fail-over of the reference, without giving up the pipelining in the common clean case.
+// `whole` (optional) makes the readers it flags whole-file readers, the two kinds mixed as parallelReader mixes them: such a
+// reader's frames[i] is only tested for NULL, its rows come from the verified file in whole->arena (block sk.first_block + b of
+// the range at row b).  A reader set that holds an unverified whole-file reader is verified first (whole_round), and chosen again
+// while readers drop — at the first chunk and at the resume after a streaming reader failed.  Whole-file positions are laid into
+// the chunk arena on the device, not staged from the host, and carry no per-frame digest.
 static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const FrameGeom& g, const uint8_t* want,
                              int data_only, const RangeSink& sk, uint8_t* corrupt, uint8_t* alive /*n, in/out*/,
-                             const uint8_t* prefer = nullptr, bool hash_outputs = true) {
+                             const uint8_t* prefer = nullptr, bool hash_outputs = true, WholeSet* whole = nullptr) {
   NvtxRange nvtx("mec_reconstruct_range");
   const int k = c->k, n = c->n;
   if (k > kMaxK) return MEC_ERR_UNSUPPORTED;
@@ -1161,9 +1247,27 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     Slot& s = c->slots[si];
     RChunk& ch = inflight[si];
     ch.b0 = b0; ch.nb = std::min(chunk, g.nblocks - b0); ch.epoch = epoch;
-    const int nch = choose_readers(c, frames, alive, prefer, ch.chosen);
-    int e = plan_decode(c, ch.chosen, nch, want, data_only, &ch);
-    if (e) return e;
+    int nch = choose_readers(c, frames, alive, prefer, ch.chosen);
+    int e;
+    // Only the first submit and the first after a resume can meet a newcomer: every other slot is idle then, so the arena
+    // positions a round fills are read by no chunk in flight.
+    while (whole && nch >= k) {
+      bool dropped = false;
+      if ((e = whole_round(c, *whole, ch.chosen, k, alive, corrupt, true, s.st, &dropped))) return e;
+      if (!dropped) break;
+      nch = choose_readers(c, frames, alive, prefer, ch.chosen);
+    }
+    if ((e = plan_decode(c, ch.chosen, nch, want, data_only, &ch))) return e;
+    bool raw[kMaxK] = {};
+    WholeFramesParams wp;
+    wp.ncols = 0;
+    if (whole)
+      for (int t = 0; t < k; t++)
+        if (whole->is_whole(ch.chosen[t])) {
+          raw[t] = true;
+          wp.pos[wp.ncols] = static_cast<int8_t>(t);
+          wp.file[wp.ncols++] = static_cast<int8_t>(whole->slot_of[ch.chosen[t]]);
+        }
     if ((e = s.aux.ensure(static_cast<size_t>(k * stride)))) return e;
     if ((e = s.out.ensure(static_cast<size_t>(ch.nb * std::max(ch.r, 1) * pitch)))) return e;
     if ((e = s.dig.ensure(static_cast<size_t>(ch.nb * (k + ch.r) * 32)))) return e;
@@ -1178,16 +1282,24 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     CopyList list;
     if (batched) {
       for (int t = 0; t < k; t++)
-        for (int64_t j = 0; j < ch.nb; j++)
+        for (int64_t j = 0; j < ch.nb && !raw[t]; j++)
           list.add(arena_ptr(s, stride, t) + j * P, frames[ch.chosen[t]] + (b0 + j) * fstride, 32 + (j == ch.nb - 1 ? sub.last_len : g.S));
       if ((e = list.flush(s.st))) return e;
     } else {
       for (int t = 0; t < k; t++)
-        if ((e = stage_frames(frames[ch.chosen[t]] + b0 * fstride, arena_ptr(s, stride, t), sub, s.st))) return e;
+        if (!raw[t] && (e = stage_frames(frames[ch.chosen[t]] + b0 * fstride, arena_ptr(s, stride, t), sub, s.st))) return e;
     }
-    c->st_h2d += sub.file_bytes() * k;
+    c->st_h2d += sub.file_bytes() * (k - wp.ncols);
+    if (wp.ncols > 0) {  // whole-file positions: their rows of the chunk's blocks, from the verified files into the frame slots
+      wp.arena = static_cast<uint8_t*>(s.aux.p); wp.arena_stride = stride; wp.P = P;
+      wp.files = whole->arena; wp.fpitch = whole->fpitch;
+      wp.S = g.S; wp.first = sk.first_block + b0; wp.nb = ch.nb; wp.last_len = sub.last_len;
+      whole_rows_frames_kernel<<<dim3(static_cast<unsigned>(ch.nb), static_cast<unsigned>(wp.ncols)), 128, 0, s.st>>>(wp);
+      MEC_CUDA_OK(cudaGetLastError());
+      c->eng->count_launch();
+    }
     MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(ch.nb * k), s.st));
-    if ((e = launch_reconstruct(c, g, ch, s, stride, ch.rows.data(), pitch, hash_outputs))) return e;
+    if ((e = launch_reconstruct(c, g, ch, s, stride, ch.rows.data(), pitch, hash_outputs, whole ? raw : nullptr))) return e;
     MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(ch.nb * k), cudaMemcpyDeviceToHost, s.st));
     if (sk.enc) { if ((e = emit_transcode(c, g, sk, ch, si, stride, pitch, &enc_inflight[si]))) return e; }
     else if (sk.dst) { if ((e = emit_object(c, g, sk, ch, s, stride, pitch, batched ? &list : nullptr))) return e; }
@@ -1749,78 +1861,27 @@ static int require_whole(mec_codec* c) {
 }
 
 // stage + verify: on return chosen[0..k) (ascending) name k verified files, file chosen[t] at s.aux + pos[t]*fpitch.  Readers are
-// taken as parallelReader takes them (`prefer` first, see choose_readers).  one_launch: the files of a round are hashed by ONE
-// launch over the span of arena positions that holds them (verified files inside the span are hashed again: one thread per file,
-// so the launch takes no longer); otherwise one launch per file.
+// taken as parallelReader takes them (`prefer` first, see choose_readers), in rounds of whole_round until k have verified.
 static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const uint8_t* sums, int64_t sfs, uint8_t* alive,
                                 uint8_t* corrupt, int* chosen, int* pos, int64_t fpitch, Slot& s, const uint8_t* prefer = nullptr,
                                 bool one_launch = false) {
-  const int k = c->k, n = c->n, ds = mec_digest_size(c->algo);
+  const int k = c->k, n = c->n;
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * fpitch + 256)))) return rc;
   if ((rc = s.dig.ensure(static_cast<size_t>(k * 64)))) return rc;
   if ((rc = s.hdig.ensure(static_cast<size_t>(k * 64)))) return rc;
-  int slot_of[kMaxShards];  // which arena position holds file i (-1 = not staged)
-  for (int i = 0; i < n; i++) slot_of[i] = -1;
-  bool verified[kMaxShards] = {};
-  for (;;) {
+  WholeSet w{files, sums, nullptr, c->algo, sfs, fpitch, static_cast<uint8_t*>(s.aux.p), static_cast<uint8_t*>(s.dig.p),
+             static_cast<uint8_t*>(s.hdig.p), {}};
+  for (int i = 0; i < n; i++) w.slot_of[i] = -1;
+  for (bool dropped = true; dropped;) {
     int want[kMaxShards];
     if (choose_readers(c, files, alive, prefer, want) < k) return MEC_ERR_READ_QUORUM;
-    // arena positions: keep verified files where they are, give the newcomers the free positions
-    bool used[kMaxK] = {};
-    for (int q = 0; q < k; q++)
-      if (slot_of[want[q]] >= 0) used[slot_of[want[q]]] = true;
-    int fresh[kMaxK], nf = 0;
-    for (int q = 0; q < k; q++) {
-      const int i = want[q];
-      if (slot_of[i] >= 0) continue;
-      int pos = 0;
-      while (used[pos]) pos++;
-      used[pos] = true;
-      slot_of[i] = pos;
-      fresh[nf++] = i;
-      if (sfs > 0)
-        MEC_CUDA_OK(cudaMemcpyAsync(static_cast<uint8_t*>(s.aux.p) + pos * fpitch, files[i], static_cast<size_t>(sfs), cudaMemcpyHostToDevice, s.st));
-      c->st_h2d += sfs;
-    }
-    if (nf == 0) break;
-    if (one_launch) {
-      int lo = k, hi = -1;
-      for (int q = 0; q < nf; q++) { lo = std::min(lo, slot_of[fresh[q]]); hi = std::max(hi, slot_of[fresh[q]]); }
-      if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p) + lo * fpitch, fpitch, sfs, hi - lo + 1,
-                                  static_cast<uint8_t*>(s.dig.p) + lo * 64, s.st)))
-        return rc;
-      c->eng->count_launch();
-    } else {
-      for (int q = 0; q < nf; q++) {  // one launch per newcomer keeps the arena positions arbitrary; these files are few and the hash is serial anyway
-        const int pos = slot_of[fresh[q]];
-        if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p) + pos * fpitch, fpitch, sfs, 1,
-                                    static_cast<uint8_t*>(s.dig.p) + pos * 64, s.st)))
-          return rc;
-        c->eng->count_launch();
-      }
-    }
-    MEC_CUDA_OK(cudaMemcpyAsync(s.hdig.p, s.dig.p, static_cast<size_t>(k * 64), cudaMemcpyDeviceToHost, s.st));
-    MEC_CUDA_OK(cudaStreamSynchronize(s.st));
-    bool dropped = false;
-    for (int q = 0; q < nf; q++) {
-      const int i = fresh[q], pos = slot_of[i];
-      if (memcmp(static_cast<const uint8_t*>(s.hdig.p) + pos * 64, sums + static_cast<size_t>(i) * 64, static_cast<size_t>(ds)) != 0) {
-        alive[i] = 0;                 // errFileCorrupt: the reader is gone for the rest of the call
-        if (corrupt) corrupt[i] = 1;
-        c->st_corrupt++;
-        slot_of[i] = -1;
-        dropped = true;
-      } else {
-        verified[i] = true;
-      }
-    }
-    if (!dropped) break;
+    if ((rc = whole_round(c, w, want, k, alive, corrupt, one_launch, s.st, &dropped))) return rc;
   }
   // compact into ascending order: position t must hold the t-th chosen file (decode rows are defined on ascending indices)
   int nch = 0;
   for (int i = 0; i < n && nch < k; i++)
-    if (alive[i] && verified[i]) { chosen[nch] = i; pos[nch++] = slot_of[i]; }
+    if (alive[i] && w.slot_of[i] >= 0) { chosen[nch] = i; pos[nch++] = w.slot_of[i]; }
   if (nch < k) return MEC_ERR_READ_QUORUM;
   return MEC_OK;
 }
@@ -2078,6 +2139,122 @@ extern "C" int64_t mec_transcode_whole(mec_codec* src, const uint8_t* const* fil
     for (int i = 0; i < n; i++)
       if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
   return total;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Decode / Heal over a part whose drives mix bitrot formats.  healObject heals a legacy part into the streaming format
+// (cmd/erasure-healing.go:593-596, a healed drive has no checksum entry and reads as HighwayHash256S, cmd/erasure-metadata.go:43-51),
+// so after the first heal some drives hold [digest][shard] frames and the others raw shard files with whole-file sums, and every
+// reader is opened with its own drive's algorithm (cmd/erasure-object.go:381-384, cmd/bitrot.go:112-117).  Both kinds run through
+// reconstruct_range: streaming readers are staged and checked frame by frame, whole-file readers are hashed when first chosen.
+
+// The read drives' formats.  Refuses an algos[i] that is no MEC_* value and a NULL sums beside a whole-file read drive
+// (MEC_ERR_INVALID_ARGUMENT), and two whole-file algorithms (MEC_ERR_UNSUPPORTED: one legacy part has one).  *walgo = that
+// algorithm, 0 when every read drive streams.  A drive is read where files[i] != NULL and, for heal, out_files[i] == NULL.
+static int mixed_formats(const mec_codec* c, const int* algos, const uint8_t* const* files, uint8_t* const* out_files, const uint8_t* sums,
+                         int* walgo) {
+  int wa = 0;
+  bool two = false;
+  for (int i = 0; i < c->n; i++) {
+    if (!files[i] || (out_files && out_files[i])) continue;
+    const int a = algos[i];
+    if (a < MEC_SHA256 || a > MEC_BLAKE2B512) return MEC_ERR_INVALID_ARGUMENT;
+    if (a == MEC_HIGHWAYHASH256S) continue;
+    if (wa && a != wa) two = true;
+    if (!wa) wa = a;
+  }
+  if (wa && !sums) return MEC_ERR_INVALID_ARGUMENT;
+  if (two) return MEC_ERR_UNSUPPORTED;
+  *walgo = wa;
+  return MEC_OK;
+}
+
+// reconstruct_range with the whole-file side when a read drive is whole-file (walgo != 0): its verified files sit in the codec's
+// own buffer (c->whole) for the whole call.  alive[] must be set: only alive drives are ever read.
+static int mixed_range(mec_codec* c, const int* algos, const uint8_t* const* files, const uint8_t* sums, int walgo, int64_t total,
+                       const uint8_t* const* frames, const FrameGeom& g, const uint8_t* want, int data_only, const RangeSink& sk,
+                       uint8_t* corrupt, uint8_t* alive, const uint8_t* prefer, bool hash_outputs) {
+  if (!walgo) return reconstruct_range(c, frames, g, want, data_only, sk, corrupt, alive, prefer, hash_outputs);
+  const int k = c->k, n = c->n;
+  if (k > kMaxK || n > kMaxShards) return MEC_ERR_UNSUPPORTED;
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  const int64_t sfs = mec_shard_file_size(c, total), fpitch = round_up(sfs, 16) + 256;
+  int rc;
+  if ((rc = c->whole.ensure(static_cast<size_t>(k * fpitch + 256)))) return rc;
+  if ((rc = c->whole_dig.ensure(static_cast<size_t>(k * 64)))) return rc;
+  if ((rc = c->hwhole_dig.ensure(static_cast<size_t>(k * 64)))) return rc;
+  uint8_t whole[kMaxShards] = {};
+  for (int i = 0; i < n; i++) whole[i] = alive[i] && algos[i] != MEC_HIGHWAYHASH256S;
+  WholeSet w{files, sums, whole, walgo, sfs, fpitch, static_cast<uint8_t*>(c->whole.p), static_cast<uint8_t*>(c->whole_dig.p),
+             static_cast<uint8_t*>(c->hwhole_dig.p), {}};
+  for (int i = 0; i < n; i++) w.slot_of[i] = -1;
+  return reconstruct_range(c, frames, g, want, data_only, sk, corrupt, alive, prefer, hash_outputs, &w);
+}
+
+extern "C" int64_t mec_decode_mixed(mec_codec* c, const int* algos, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
+                                    int64_t offset, int64_t length, int64_t total, uint8_t* dst, int* heal_hint) {
+  NvtxRange nvtx("mec_decode_mixed");
+  if (heal_hint) *heal_hint = 0;
+  if (!c || !algos || !files) return MEC_ERR_INVALID_ARGUMENT;
+  if (offset < 0 || length < 0) return MEC_ERR_INVALID_ARGUMENT;      // cmd/erasure-decode.go:240-242
+  if (offset + length > total) return MEC_ERR_INVALID_ARGUMENT;       // :243-245
+  if (length == 0) return 0;                                          // :247-249
+  if (!dst) return MEC_ERR_INVALID_ARGUMENT;
+  int walgo = 0;
+  int rc = mixed_formats(c, algos, files, nullptr, sums, &walgo);
+  if (rc) return rc;
+  if ((rc = require_streaming(c))) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const int k = c->k, n = c->n;
+  const int64_t bs = c->block_size, S = c->S();
+  const ReadRange rr = read_range(c, offset, length, total);
+  const FrameGeom g{rr.nblocks, S, rr.last_len};
+  if (static_cast<int64_t>(k) * g.last_len < std::min(offset + length, total) - rr.last_block * bs) return MEC_ERR_SHORT_DATA;
+  const int64_t foff = rr.start_block * (32 + S);
+  std::vector<const uint8_t*> in(n);
+  std::vector<uint8_t> alive(n), want(n, 0), corrupt(n, 0);
+  for (int i = 0; i < n; i++) {
+    alive[i] = files[i] != nullptr;
+    in[i] = files[i] && algos[i] == MEC_HIGHWAYHASH256S ? files[i] + foff : files[i];  // a whole-file reader's pointer is only tested for NULL
+  }
+  for (int i = 0; i < k; i++) want[i] = 1;
+  RangeSink sk;
+  sk.dst = dst; sk.first_block = rr.start_block; sk.lo = offset; sk.hi = offset + length; sk.bs = bs; sk.total = total;
+  rc = mixed_range(c, algos, files, sums, walgo, total, in.data(), g, want.data(), 1, sk, corrupt.data(), alive.data(), prefer, false);
+  if (rc) return rc;
+  if (heal_hint)
+    for (int i = 0; i < n; i++)
+      if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
+  return length;
+}
+
+extern "C" int mec_heal_mixed(mec_codec* c, const int* algos, const uint8_t* const* files, const uint8_t* sums, const uint8_t* prefer,
+                              int64_t total, uint8_t* const* out_files, uint8_t* corrupt) {
+  NvtxRange nvtx("mec_heal_mixed");
+  if (!c || !algos || !files || !out_files) return MEC_ERR_INVALID_ARGUMENT;
+  if (corrupt) memset(corrupt, 0, static_cast<size_t>(c->n));
+  int walgo = 0;
+  int rc = mixed_formats(c, algos, files, out_files, sums, &walgo);
+  if (rc) return rc;
+  if (total <= 0) return MEC_OK;
+  if ((rc = require_streaming(c))) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const int n = c->n;
+  const int64_t S = c->S(), sfs = mec_shard_file_size(c, total);
+  FrameGeom g;
+  g.nblocks = ceil_frac(total, c->block_size);
+  g.S = S;
+  g.last_len = sfs - (g.nblocks - 1) * S;
+  std::vector<uint8_t> alive(n), want(n, 0), bad(n, 0);
+  // healObject opens no reader on a drive it heals (cmd/erasure-healing.go:572-575): a stale drive is never read
+  for (int i = 0; i < n; i++) { alive[i] = files[i] != nullptr && out_files[i] == nullptr; want[i] = out_files[i] != nullptr; }
+  RangeSink sk;
+  sk.out = out_files;
+  rc = mixed_range(c, algos, files, sums, walgo, total, files, g, want.data(), 0, sk, bad.data(), alive.data(), prefer, true);
+  if (rc) return rc;
+  bool any = false;
+  for (int i = 0; i < n; i++) { any |= bad[i] != 0; if (corrupt) corrupt[i] = bad[i]; }
+  return any ? MEC_ERR_FILE_CORRUPT : MEC_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
