@@ -351,6 +351,40 @@ int64_t mec_batcher_transcode(mec_batcher* b, const uint8_t* const* files, const
 int64_t mec_batcher_transcode_whole(mec_batcher* b, int algo, const uint8_t* const* files, const uint8_t* sums,
                                     const uint8_t* prefer, int64_t total_length, uint8_t* const* out_files, int write_quorum,
                                     int* heal_hint);
+/* mec_decode_mixed / mec_heal_mixed through the coalescer, on any batcher (its codec is the HighwayHash256S codec of the part's
+ * geometry): the arguments of those calls with the batcher in place of the codec, and their results, heal_hint and corrupt[].
+ * Checked on the caller's thread before anything is queued, in the single-codec calls' order: a NULL batcher, algos or files (heal:
+ * out_files) (MEC_ERR_INVALID_ARGUMENT, *heal_hint = 0); for decode the range checks, length == 0 (returns 0), a NULL dst and
+ * MEC_ERR_SHORT_DATA; the drive formats (an algos[i] that is no MEC_* value, or a NULL sums beside a whole-file read drive:
+ * MEC_ERR_INVALID_ARGUMENT; two whole-file algorithms: MEC_ERR_UNSUPPORTED); heal with total_length <= 0 (MEC_OK); fewer than k
+ * readable drives (MEC_ERR_READ_QUORUM).  The k readers are chosen there as mec_decode_mixed chooses them: drives with files[i] !=
+ * NULL (heal: and out_files[i] == NULL), `prefer` first, then index order.
+ * A call whose k chosen readers all stream is an ordinary merged GET or heal: it shares batches with mec_batcher_decode_prefer /
+ * mec_batcher_heal requests under their rules.  A call with a whole-file reader among them joins batches of such calls of the same
+ * whole-file algorithm only (without MEC_BATCHER_MIX_PATTERNS of the same reader set — and, for heals, stale set — with it of any,
+ * cut at one latency launch).  Such a batch stages the streaming readers' frames of every range as GET batches do and the
+ * whole-file readers' entire shard files into a file arena, hashes all those files in ONE whole_hash_kernel launch, lays their raw
+ * rows into the frame arena and runs the merged reconstruct and scatters unchanged (a GET batch in which no call reads frames skips
+ * the frame digests, and launches nothing more when nothing is rebuilt).  A call whose streaming frames pass their digests and whose
+ * whole-file readers match their sums is done (counted in "reads_whole" when it has a whole-file reader); any other is redone alone
+ * through mec_decode_mixed / mec_heal_mixed with the same `prefer` on the batcher's private handle, which applies parallelReader's
+ * exact fail-over (counted in "redone" and "reads_whole_serial"), and its batch neighbours complete as merged.  Calls with a chosen
+ * reader, dst or out file that is not page-locked, more than 32 drives, MEC_BATCHER_MEMCPY in the environment, more stale drives
+ * than a merged heal rebuilds, or a whole-file reader and a part of more than max_batch_blocks blocks take that private path
+ * directly (counted in "reads_whole_serial").
+ * Counters: "whole_hash_launches" grows by one per merged batch with whole-file readers; such a batch adds to "bytes_h2d" what
+ * mec_decode_mixed would (the frame bytes of every streaming reader plus one shard file per whole-file reader), and to
+ * "blocks_read" and "shards_rebuilt" what every merged read batch adds.
+ * Device memory: a slot's first batch with whole-file readers sizes its file arena for a full batch — B x (block_size + 272 x k)
+ * bytes in the PUT staging buffer (B = max_batch_blocks + min(64, max_batch_blocks / 8 + 4)), plus 84 bytes of stream table,
+ * digest and pinned mirrors per file slot, B x k of them — and later batches allocate nothing.  Transcode batchers have it from
+ * the start; a batcher that never sees a whole-file reader allocates nothing more.  GET batches with whole-file readers scatter
+ * straight into the callers' buffers, since the file arena takes the staging buffer the GET assembly would use. */
+int64_t mec_batcher_decode_mixed(mec_batcher* b, const int* algos, const uint8_t* const* files, const uint8_t* sums,
+                                 const uint8_t* prefer, int64_t offset, int64_t length, int64_t total_length, uint8_t* dst,
+                                 int* heal_hint);
+int mec_batcher_heal_mixed(mec_batcher* b, const int* algos, const uint8_t* const* files, const uint8_t* sums,
+                           const uint8_t* prefer, int64_t total_length, uint8_t* const* out_files, uint8_t* corrupt);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------

@@ -88,6 +88,9 @@ def lib():
     L.mec_batcher_transcode.argtypes = [vp, vp, vp, i64, vp, i32, C.POINTER(i32)]
     L.mec_batcher_transcode_whole.restype = i64
     L.mec_batcher_transcode_whole.argtypes = [vp, i32, vp, vp, vp, i64, vp, i32, C.POINTER(i32)]
+    L.mec_batcher_decode_mixed.restype = i64
+    L.mec_batcher_decode_mixed.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, vp, C.POINTER(i32)]
+    L.mec_batcher_heal_mixed.argtypes = [vp, vp, vp, vp, vp, i64, vp, vp]
     L.mec_batcher_stat.restype = i64
     L.mec_batcher_stat.argtypes = [vp, C.c_char_p]
     L.mec_checksums.argtypes = [vp, vp, i64, i32, vp]
@@ -704,6 +707,45 @@ class Batcher:
         if rc < 0:
             raise MecError(rc, "mec_batcher_transcode_whole")
         return outs, hint.value
+
+    def decode_mixed(self, files, algos, sums, offset, length, total, dst=None, prefer=None):
+        """mec_batcher_decode_mixed: Codec.decode_mixed through the coalescer (files / algos / sums / prefer as there; page-locked
+        readers and a page-locked dst let the call ride in merged batches).  -> (bytes, heal_hint)"""
+        files = [None if f is None else _u8(f) for f in files]
+        al, sm = self._sizes._mixed_args(algos, sums)
+        if dst is None:
+            dst = np.zeros(max(length, 1), dtype=np.uint8)
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        rc = lib().mec_batcher_decode_mixed(self.h, al, _ptrs(files), None if sm is None else sm.ctypes.data,
+                                            None if pf is None else pf.ctypes.data, offset, length, total, dst.ctypes.data,
+                                            C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_decode_mixed")
+        return dst[:length], hint.value
+
+    def heal_mixed(self, files, algos, sums, stale, total, prefer=None, report=False, pinned=False):
+        """mec_batcher_heal_mixed: Codec.heal_mixed through the coalescer (arguments, report and results as there).  Page-locked
+        readers and pinned=True (the out files are allocated page-locked; the caller owns and should free them) let the heal ride
+        in merged batches."""
+        files = [None if f is None else _u8(f) for f in files]
+        al, sm = self._sizes._mixed_args(algos, sums)
+        fsz = self._sizes.bitrot_file_size(total)
+        mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
+        outs = [mk(fsz) if stale[i] else None for i in range(self.n)]
+        corrupt = np.zeros(self.n, dtype=np.uint8)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        marker = np.zeros(1, dtype=np.uint8)  # an empty part's stale drives are still marked
+        optrs = _ptrs([(o if o.size else marker) if o is not None else None for o in outs])
+        rc = lib().mec_batcher_heal_mixed(self.h, al, _ptrs(files), None if sm is None else sm.ctypes.data,
+                                          None if pf is None else pf.ctypes.data, total, optrs, corrupt.ctypes.data)
+        if report:
+            if rc and rc != -7:
+                raise MecError(rc, "mec_batcher_heal_mixed")
+            return outs, rc, corrupt
+        if rc:
+            raise MecError(rc, "mec_batcher_heal_mixed")
+        return outs
 
     def stat(self, name):
         return lib().mec_batcher_stat(self.h, name.encode())

@@ -142,7 +142,7 @@ struct BatchGetDesc {
   int64_t tail_slot;                     // slot of the part's short last block when the range reaches it, -1 otherwise
   int64_t last_len;                      // shard length of that block
   int32_t dma;                           // 1: the copy engines stage this request's frames (long ranges), the gather kernel skips it
-  int32_t pad;
+  uint32_t whole_pos;                    // bit t: arena position t is a whole-file reader, laid by batch_whole_rows_kernel (no frames)
   // the request's decode plan (a batch of one erasure pattern: the same for every request)
   int8_t chosen[32];                     // reader set (ascending shard indices), arena position t -> shard
   int8_t targets[16];                    // rebuilt shards (GET: the data shards not read; heal: the stale drives), output row q -> shard
@@ -164,11 +164,11 @@ __host__ __device__ __forceinline__ int64_t get_slot(const BatchGetDesc& r, int6
   return (r.tail_slot >= 0 && b == r.nblocks - 1) ? r.tail_slot : r.slot0 + b;
 }
 
-// grid (block stride, k reader positions, nreq): frames of the chosen readers -> arena
+// grid (block stride, k reader positions, nreq): frames of the chosen readers -> arena (whole-file positions have no frames)
 __global__ void __launch_bounds__(128) batch_get_gather_kernel(const BatchGetParams p) {
   const BatchGetDesc& r = p.reqs[blockIdx.z];
-  if (r.dma) return;
   const int t = blockIdx.y;
+  if (r.dma || ((r.whole_pos >> t) & 1)) return;
   const uint8_t* f = r.files[r.chosen[t]];
   const int64_t fstride = 32 + p.S;
   __shared__ __align__(16) uint8_t stage[kStageBytes + 32];
@@ -327,16 +327,20 @@ __global__ void __launch_bounds__(128) batch_transcode_resplit_kernel(const Batc
   }
 }
 
-// grid (block stride, k reader positions, nreq), 128 threads: a merged batch of whole-file moves (mec_batcher_transcode_whole).
-// Its parts have no frames: the chosen readers' raw shard files sit in a device file arena, file (z, t) = reader position t of
-// request z at files + streams[z * k + t].off (16-byte aligned, at least 256 readable bytes behind it), block b's shard at + b * S.
-// This lays every shard into the frame arena slot a GET batch would have staged it in (shard at + 32, the digest bytes are left
-// as they are), so the merged reconstruct and batch_transcode_resplit_kernel run on it unchanged.  Sources sit at any byte
+// grid (block stride, k reader positions, nreq), 128 threads: the whole-file readers of a merged batch — every reader of a whole-file
+// move (mec_batcher_transcode_whole), the whole-file readers of a mixed GET or heal (mec_batcher_decode_mixed / _heal_mixed).  Their
+// raw shard files sit in a device file arena, one stream-table entry per whole-file reader: position t of request z (bit t of
+// whole_pos) is stream first[z] + (whole-file positions of z below t), its file at files + streams[that].off (16-byte aligned, at
+// least 256 readable bytes behind it), block b's shard at + b * S.  This lays every such shard into the frame arena slot a GET batch
+// would have staged it in (shard at + 32, the digest bytes are left as they are), so the merged reconstruct, the scatters and
+// batch_transcode_resplit_kernel run on it unchanged.  Other positions are left to the frame staging.  Sources sit at any byte
 // offset (S = 87382 for RS(12,4) at 1 MiB); cta_copy reads at most one word past a shard, inside the file's padding.
-__global__ void __launch_bounds__(128) batch_whole_rows_kernel(const BatchGetParams p, const uint8_t* files, const WholeStream* streams) {
+__global__ void __launch_bounds__(128) batch_whole_rows_kernel(const BatchGetParams p, const uint8_t* files, const WholeStream* streams,
+                                                               const int32_t* first) {
   const BatchGetDesc& r = p.reqs[blockIdx.z];
   const int t = blockIdx.y;
-  const uint8_t* f = files + streams[static_cast<int64_t>(blockIdx.z) * p.k + t].off;
+  if (!((r.whole_pos >> t) & 1)) return;
+  const uint8_t* f = files + streams[first[blockIdx.z] + __popc(r.whole_pos & ((1u << t) - 1))].off;
   for (int64_t b = blockIdx.x; b < r.nblocks; b += gridDim.x) {
     const bool is_tail = r.tail_slot >= 0 && b == r.nblocks - 1;
     cta_copy(p.arena + t * p.arena_stride + get_slot(r, b) * p.P + 32, f + (r.start_block + b) * p.S, is_tail ? r.last_len : p.S, false);

@@ -67,8 +67,10 @@ struct Slot {
   DevBuf dreq;                       // request table of a merged batch (batch_copy.cuh)
   DevBuf blk;                        // per-block geometry of a merged launch (SmallBlock / per-frame lengths)
   DevBuf sum_tab, sum_out;           // object hashes of a merged batch: SumWork table, one kSumRecord record per request (obj_hash.cuh)
-  DevBuf wtab;                       // merged whole-file moves: the WholeStream of every staged shard file (whole_hash.cuh)
-  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum, hwtab;
+  // merged batches with whole-file readers (batch_whole_stage): the WholeStream of every staged shard file (whole_hash.cuh) and
+  // each request's first stream behind them; one 64-byte digest per staged file
+  DevBuf wtab, wdig;
+  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum, hwtab, hwdig;
   cudaStream_t st = nullptr;
 };
 
@@ -217,7 +219,7 @@ extern "C" void mec_codec_free(mec_codec* c) {
     s.src.release(); s.out.release(); s.dig.release(); s.aux.release(); s.flags.release();
     s.hdig.release(); s.hflags.release(); s.hcrc.release(); s.crc_part.release(); s.crc_out.release(); s.dreq.release(); s.hreq.release(); s.blk.release(); s.hblk.release();
     s.crc_tab.release(); s.hcrc_tab.release(); s.sum_tab.release(); s.sum_out.release(); s.hsum_tab.release(); s.hsum.release();
-    s.wtab.release(); s.hwtab.release();
+    s.wtab.release(); s.hwtab.release(); s.wdig.release(); s.hwdig.release();
   }
   c->flags.release();
   c->crc_tables.release();
@@ -2509,9 +2511,13 @@ struct BatchReq {
   uint64_t alive_mask = 0;           // bit i = reader i is online (heal, GET with `prefer`: one of the k chosen readers)
   int64_t get_slot0 = 0, get_tail_slot = -1, get_nblocks = 0;  // placement of the request's blocks in the merged batch
   const uint8_t* prefer = nullptr;   // preferReaders (cmd/erasure-decode.go:92-123), for the redo of a request that met bitrot
-  // whole-file move: the part's algorithm (0 for every other request: a batch holds one algorithm) and expected digests (+ i*64)
+  // whole-file move, or a mixed GET / heal with a whole-file reader among its k chosen: the part's algorithm (0 for every other
+  // request: a batch holds one algorithm), the expected digests (+ i*64) and the chosen whole-file readers (bit i = drive i)
   int whole_algo = 0;
   const uint8_t* whole_sums = nullptr;
+  uint64_t whole_drives = 0;
+  // mec_batcher_decode_mixed / _heal_mixed: every drive's bitrot algorithm; the private path is mec_decode_mixed / mec_heal_mixed
+  const int* algos = nullptr;
   // heal
   uint8_t* const* outs = nullptr;
   uint8_t* corrupt = nullptr;
@@ -2592,6 +2598,9 @@ struct mec_batcher {
   // BLAKE2b512), each created on first use, and the moves completed by merged batches / by the private pair
   mec_codec* serial_whole[3] = {};
   std::atomic<int64_t> st_transcodes_whole{0}, st_transcodes_whole_serial{0};
+  // mec_batcher_decode_mixed / _heal_mixed: calls with a whole-file reader completed by merged batches, and mixed calls of the
+  // private path (redos included)
+  std::atomic<int64_t> st_reads_whole{0}, st_reads_whole_serial{0};
 };
 
 namespace {
@@ -2628,6 +2637,12 @@ static int64_t batcher_run_alone(mec_batcher* b, const BatchReq& r) {
   }
   if (r.kind == ReqKind::Transcode) b->st_transcodes_serial++;
   mec_codec* sc = batcher_private(b, b->codec, b->serial);
+  if (r.algos) {  // a mixed read: fail-over may reach a drive of either format
+    b->st_reads_whole_serial++;
+    if (!sc) return MEC_ERR_UNEXPECTED;
+    if (r.kind == ReqKind::Heal) return mec_heal_mixed(sc, r.algos, r.gfiles, r.whole_sums, r.prefer, r.total, r.outs, r.corrupt);
+    return mec_decode_mixed(sc, r.algos, r.gfiles, r.whole_sums, r.prefer, r.offset, r.length, r.total, r.dst, r.heal_hint);
+  }
   if (r.kind == ReqKind::Transcode) {
     mec_codec* sd = batcher_private(b, b->dst, b->serial_dst);
     return sc && sd ? mec_transcode(sc, r.gfiles, r.prefer, r.total, sd, r.files, 0, r.heal_hint) : MEC_ERR_UNEXPECTED;
@@ -2642,24 +2657,28 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
   mec_codec* c = b->codec;
   if (is_read(fb.kind)) {
     // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own; the others are done
-    // (their bytes are in place; a heal's `corrupt` was zeroed when it was queued)
-    // (a whole-file move: the digests of its k staged shard files, request q's at s.hdig + q*k*64, against its expected sums)
+    // (their bytes are in place; a heal's `corrupt` was zeroed when it was queued).  A whole-file reader has no frames: the flags at
+    // its arena position mean nothing, and the digest of its staged shard file (batch_whole_stage: streams in request order, a
+    // request's in ascending position order, digest j at s.hwdig + j*64) is compared with its expected sum instead.
     const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
-    const uint8_t* wd = static_cast<const uint8_t*>(s.hdig.p);
+    const uint8_t* wd = static_cast<const uint8_t*>(s.hwdig.p);
+    const BatchGetDesc* tab = static_cast<const BatchGetDesc*>(s.hreq.p);
     const int k = c->k;
+    int64_t stream = 0;
     for (size_t q = 0; q < fb.reqs.size(); q++) {
       BatchReq* r = fb.reqs[q];
       int64_t res = rc != MEC_OK ? rc : r->kind == ReqKind::Heal ? MEC_OK : is_move(r->kind) ? r->total : r->length;
       if (rc == MEC_OK) {
         bool bad = false;
-        if (r->kind == ReqKind::TranscodeWhole) {
+        const uint32_t wpos = r->whole_algo ? tab[q].whole_pos : 0;
+        if (wpos) {
           const size_t ds = static_cast<size_t>(mec_digest_size(r->whole_algo));
-          for (int i = 0, t = 0; i < c->n && !bad; i++)  // stream t of the request is its t-th chosen reader, ascending
-            if ((r->alive_mask >> i) & 1) bad = memcmp(wd + (q * k + t++) * 64, r->whole_sums + static_cast<size_t>(i) * 64, ds) != 0;
+          for (int t = 0; t < k; t++)
+            if ((wpos >> t) & 1) bad |= memcmp(wd + stream++ * 64, r->whole_sums + static_cast<size_t>(tab[q].chosen[t]) * 64, ds) != 0;
         }
-        for (int64_t bb = 0; bb < r->get_nblocks && !bad && r->kind != ReqKind::TranscodeWhole; bb++) {
+        for (int64_t bb = 0; bb < r->get_nblocks && !bad; bb++) {
           const int64_t slot = (r->get_tail_slot >= 0 && bb == r->get_nblocks - 1) ? r->get_tail_slot : r->get_slot0 + bb;
-          for (int t = 0; t < k; t++) bad |= fl[slot * k + t] != 0;
+          for (int t = 0; t < k; t++) bad |= !((wpos >> t) & 1) && fl[slot * k + t] != 0;
         }
         if (bad) {
           b->st_redone++;
@@ -2668,6 +2687,7 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
           if (r->heal_hint) *r->heal_hint = 0;
           if (r->kind == ReqKind::Transcode) b->st_transcodes++;
           if (r->kind == ReqKind::TranscodeWhole) b->st_transcodes_whole++;
+          if (r->algos && r->whole_algo) b->st_reads_whole++;
         }
       }
       r->result = res;
@@ -3128,6 +3148,8 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
     for (int j = 0; j < pl.r; j++) d.targets[j] = static_cast<int8_t>(pl.targets[j]);
     d.r = pl.r;
     d.pattern = req_pat[q];
+    for (int t = 0; t < k; t++)
+      if ((rq->whole_drives >> d.chosen[t]) & 1) d.whole_pos |= 1u << t;
     const bool tail = rr.last_len != S;
     d.slot0 = lay.nfull_slots;
     lay.nfull_slots += d.nblocks - (tail ? 1 : 0);
@@ -3162,26 +3184,32 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
   return MEC_OK;
 }
 
-// The raw shard files of a merged batch of whole-file moves, staged and hashed by batch_whole_stage: file (z, t) at files +
-// streams[z * k + t].off on the device
+// The raw shard files of the whole-file readers of a merged batch, staged and hashed by batch_whole_stage: position t of request z
+// (bit t of its whole_pos) at files + streams[first[z] + whole-file positions of z below t].off on the device.  raw: no request
+// of the batch has a streaming reader and no digest is wanted (a GET or move batch), so the reconstruct neither hashes nor verifies.
 struct WholeFiles {
   const uint8_t* files;
   const WholeStream* streams;
+  const int32_t* first;
+  bool raw;
 };
+static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const BatchGetDesc* tab, WholeFiles* wf);
 
 // The request table to the device, survivor frames of every block of every request -> the slot's arena, the fused reconstruct of
 // every request's targets over all of them, and the per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table
 // gp.reqs points at; gp holds the geometry and gets the arena and rebuilt rows here.  A batch of several erasure patterns is ONE
-// latency launch with a decode plan per block (batcher_main only merges such a batch when its blocks fit one).  `raw` (a batch of
-// whole-file moves): the arena is filled from the staged raw shard files by batch_whole_rows_kernel instead, and the reconstruct
-// neither hashes nor verifies anything (those files were hashed whole; s.dig holds their digests and is left alone).
+// latency launch with a decode plan per block (batcher_main only merges such a batch when its blocks fit one).  `wf` (a batch with
+// whole-file readers, staged and hashed by batch_whole_stage): their positions are filled from the staged raw shard files by
+// batch_whole_rows_kernel, the frame staging skips them, and their verdict flags mean nothing (batcher_finish checks their file
+// digests instead).  wf->raw: the reconstruct neither hashes nor verifies anything.
 static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* tab, BatchGetParams& gp, const ReadLayout& lay,
-                                  bool hash_outputs, const WholeFiles* raw = nullptr) {
+                                  bool hash_outputs, const WholeFiles* wf = nullptr) {
   mec_codec* c = b->codec;
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
   const int64_t stride = round_up(nslots * P + 512, 256);
-  if (!raw) mark_phase(b, s, 0);  // a whole-file batch marks the start of its staging (batch_whole_stage)
+  const bool raw = wf && wf->raw;
+  if (!wf) mark_phase(b, s, 0);  // a batch with whole-file readers marks the start of its staging (batch_whole_stage)
   MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, lay.table_bytes, cudaMemcpyHostToDevice, s.st));
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
@@ -3197,19 +3225,24 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
   // long ranges are staged by the copy engines (k strided copies per request are cheap next to megabytes of frames); short ones by
   // the gather kernel (no per-request driver call at all)
   const int64_t fstride = 32 + S;
-  if (raw) {
-    batch_whole_rows_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp, raw->files, raw->streams);
+  if (wf) {
+    batch_whole_rows_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp, wf->files, wf->streams,
+                                                                                                                  wf->first);
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
-  } else {
+  }
+  if (!raw) {
     // one 1-D copy per (request, survivor, block) frame — the arena pads frames to a 16-byte pitch — all of them in ONE batched call
     std::vector<void*> dsts, srcs;
     std::vector<size_t> sizes;
+    bool any_gather = false;
     for (int q = 0; q < gp.nreq; q++) {
       const BatchGetDesc& d = tab[q];
-      if (!d.dma) continue;
+      const uint32_t frames = ~d.whole_pos & ((1ull << k) - 1);  // positions with frames to stage
+      if (!d.dma) { any_gather |= frames != 0; continue; }
       const int64_t nf = d.nblocks - (d.tail_slot >= 0 ? 1 : 0);
       for (int t = 0; t < k; t++) {
+        if (!((frames >> t) & 1)) continue;
         const uint8_t* f = d.files[d.chosen[t]] + d.start_block * fstride;
         uint8_t* a = gp.arena + t * stride;
         for (int64_t j = 0; j < nf; j++) {
@@ -3221,8 +3254,6 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
       }
     }
     if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
-    bool any_gather = false;
-    for (int q = 0; q < gp.nreq; q++) any_gather |= !tab[q].dma;
     if (any_gather) {
       batch_get_gather_kernel<<<dim3(gx, static_cast<unsigned>(k), static_cast<unsigned>(gp.nreq)), 128, 0, s.st>>>(gp);
       MEC_CUDA_OK(cudaGetLastError());
@@ -3301,7 +3332,10 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   // writeDataBlocks: 0 = the scatter kernel assembles every object in device memory and ONE copy per request takes it to the caller
   // (fewest driver-side copy descriptors), 1 = the scatter kernel stores straight into the callers' buffers over PCIe, 2 = the copy
   // engine moves every (request, shard, block) piece itself
-  const int out_mode = b->sw.get_out;
+  // A batch with whole-file readers stages their shard files in s.src (batch_whole_stage), so it scatters straight into the callers'
+  // buffers instead of assembling there.
+  const bool whole = reqs.front()->whole_algo != 0;
+  const int out_mode = whole && b->sw.get_out == 0 ? 1 : b->sw.get_out;
   std::vector<int64_t> asm_off(reqs.size(), 0);
   if (out_mode == 0) {
     int64_t total = 0;
@@ -3309,7 +3343,9 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
     if ((rc = s.src.ensure(static_cast<size_t>(total + 256)))) return rc;
     for (size_t q = 0; q < reqs.size(); q++) tab[q].dst = static_cast<uint8_t*>(s.src.p) + asm_off[q];
   }
-  if ((rc = batch_read_reconstruct(b, s, tab, gp, lay, false))) return rc;  // GetObject reads no digest of rebuilt data
+  WholeFiles wf;
+  if (whole && (rc = batch_whole_stage(b, s, reqs, tab, &wf))) return rc;
+  if ((rc = batch_read_reconstruct(b, s, tab, gp, lay, false, whole ? &wf : nullptr))) return rc;  // GetObject reads no digest of rebuilt data
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
   const int64_t stride = gp.arena_stride;
   if (out_mode == 2) {
@@ -3365,7 +3401,14 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
   if (rc) return rc;
   const int r = gp.r;
   const int64_t nslots = lay.nslots();
-  if ((rc = batch_read_reconstruct(b, s, static_cast<const BatchGetDesc*>(s.hreq.p), gp, lay, true))) return rc;
+  const BatchGetDesc* tab = static_cast<const BatchGetDesc*>(s.hreq.p);
+  const bool whole = reqs.front()->whole_algo != 0;
+  WholeFiles wf;
+  if (whole) {
+    if ((rc = batch_whole_stage(b, s, reqs, tab, &wf))) return rc;
+    wf.raw = false;  // the healed frames carry the digests of the rebuilt shards
+  }
+  if ((rc = batch_read_reconstruct(b, s, tab, gp, lay, true, whole ? &wf : nullptr))) return rc;
   if (r > 0) {
     const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
     batch_heal_scatter_kernel<<<dim3(gx, static_cast<unsigned>(r), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(
@@ -3378,48 +3421,85 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
   return MEC_OK;
 }
 
-// The staging of a merged batch of whole-file moves (mec_batcher_transcode_whole), on the slot's stream: the raw shard files of
-// every request's k chosen readers (tab[z].chosen) -> the file arena in s.src (file (z, t) 16-byte aligned with 256 readable bytes
-// behind it, as stage_verified_whole lays files out) in ONE batched copy, then ONE whole_hash_kernel launch over all nreq x k files
-// with a stream table, and their digests back to s.hdig (file (z, t) at + (z * k + t) * 64), where batcher_finish compares them
-// with every request's expected sums.  s.src of a transcode batcher's slot is sized up front for a full batch (batcher_create).
+// Device memory of a slot's batches with whole-file readers, for a batch of `slots` blocks and at most as many requests: request z
+// of NB_z blocks stages at most k files of at most NB_z x S bytes (k x S < block_size + k), each padded by at most 15 + 256 bytes, so
+// the file arena fits slots x (block_size + 272 x k) bytes; one stream-table entry, one first-stream index and one digest per file.
+// A transcode batcher sizes this up front (batcher_create); any other batcher on a slot's first batch with whole-file readers.
+static int size_whole_slot(const mec_codec* c, Slot& s, int64_t slots) {
+  const int k = c->k;
+  const size_t tab = static_cast<size_t>(slots * k) * sizeof(WholeStream) + static_cast<size_t>(slots) * sizeof(int32_t);
+  int rc;
+  if ((rc = s.src.ensure(static_cast<size_t>(slots * (c->block_size + 272 * k))))) return rc;
+  if ((rc = s.wtab.ensure(tab))) return rc;
+  if ((rc = s.hwtab.ensure(tab))) return rc;
+  if ((rc = s.wdig.ensure(static_cast<size_t>(slots * k * 64)))) return rc;
+  return s.hwdig.ensure(static_cast<size_t>(slots * k * 64));
+}
+// the blocks a batcher's slots are sized for (batcher_create)
+static int64_t batcher_slot_blocks(const mec_batcher* b) { return b->max_blocks + std::min<int64_t>(64, b->max_blocks / 8 + 4); }
+
+// The staging of the whole-file readers of a merged batch (every reader of a whole-file move, mec_batcher_transcode_whole; the
+// whole-file readers among a mixed GET's or heal's k chosen, mec_batcher_decode_mixed / _heal_mixed), on the slot's stream: the raw
+// shard files of every request's whole-file positions (bit t of tab[z].whole_pos: reader tab[z].chosen[t]) -> the file arena in
+// s.src (each 16-byte aligned with 256 readable bytes behind it, as stage_verified_whole lays files out) in ONE batched copy, then
+// ONE whole_hash_kernel launch over a stream table that holds only those files, in request order and ascending position order
+// within a request, and their digests back to s.hwdig, where batcher_finish compares them with every request's expected sums.
+// Request z's first stream is first[z], stored behind the stream table.  s.src is free: a heal or move batch does not stage object
+// bytes, and a GET batch with whole-file readers scatters straight into its callers' buffers (batcher_submit_get).  Counts
+// "bytes_h2d" as mec_decode_mixed does: the frames of every streaming reader plus one shard file per whole-file reader.
 static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const BatchGetDesc* tab, WholeFiles* wf) {
   mec_codec* c = b->codec;
   const int k = c->k;
-  const size_t nreq = reqs.size(), nfiles = nreq * static_cast<size_t>(k);
+  const size_t nreq = reqs.size();
   int rc;
-  if ((rc = s.hwtab.ensure(nfiles * sizeof(WholeStream)))) return rc;
-  if ((rc = s.wtab.ensure(nfiles * sizeof(WholeStream)))) return rc;
-  if ((rc = s.dig.ensure(nfiles * 64))) return rc;
-  if ((rc = s.hdig.ensure(nfiles * 64))) return rc;
+  if ((rc = size_whole_slot(c, s, batcher_slot_blocks(b)))) return rc;  // a no-op after the slot's first such batch
+  size_t nfiles = 0;
+  for (size_t z = 0; z < nreq; z++) nfiles += static_cast<size_t>(__builtin_popcount(tab[z].whole_pos));
+  const size_t tab_bytes = nfiles * sizeof(WholeStream) + nreq * sizeof(int32_t);
+  if ((rc = s.hwtab.ensure(tab_bytes))) return rc;  // a request larger than the slots' sizing leads its own batch
+  if ((rc = s.wtab.ensure(tab_bytes))) return rc;
+  if ((rc = s.wdig.ensure(nfiles * 64))) return rc;
+  if ((rc = s.hwdig.ensure(nfiles * 64))) return rc;
   WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+  int32_t* first = reinterpret_cast<int32_t*>(ws + nfiles);
   int64_t arena = 0;
+  size_t j = 0;
   for (size_t z = 0; z < nreq; z++) {
-    const int64_t sfs = mec_shard_file_size(c, reqs[z]->total);
-    for (int t = 0; t < k; t++) {
-      ws[z * k + t] = WholeStream{arena, sfs};
-      arena += round_up(sfs, 16) + 256;
-    }
-    c->st_h2d += static_cast<int64_t>(k) * sfs;
+    const BatchGetDesc& d = tab[z];
+    const int64_t sfs = mec_shard_file_size(c, d.total);
+    const int nw = __builtin_popcount(d.whole_pos);
+    first[z] = static_cast<int32_t>(j);
+    for (int t = 0; t < k; t++)
+      if ((d.whole_pos >> t) & 1) {
+        ws[j++] = WholeStream{arena, sfs};
+        arena += round_up(sfs, 16) + 256;
+      }
+    const FrameGeom g{d.nblocks, c->S(), d.last_len};
+    c->st_h2d += nw * sfs + (k - nw) * g.file_bytes();
   }
   if ((rc = s.src.ensure(static_cast<size_t>(arena)))) return rc;
   uint8_t* files = static_cast<uint8_t*>(s.src.p);
   mark_phase(b, s, 0);
-  MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, nfiles * sizeof(WholeStream), cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, tab_bytes, cudaMemcpyHostToDevice, s.st));
   std::vector<void*> dsts, srcs;
   std::vector<size_t> sizes;
+  j = 0;
   for (size_t z = 0; z < nreq; z++)
-    for (int t = 0; t < k; t++) {
-      const WholeStream& w = ws[z * k + t];
-      dsts.push_back(files + w.off); srcs.push_back(const_cast<uint8_t*>(tab[z].files[tab[z].chosen[t]])); sizes.push_back(static_cast<size_t>(w.len));
-    }
+    for (int t = 0; t < k; t++)
+      if ((tab[z].whole_pos >> t) & 1) {
+        const WholeStream& w = ws[j++];
+        if (w.len == 0) continue;
+        dsts.push_back(files + w.off); srcs.push_back(const_cast<uint8_t*>(tab[z].files[tab[z].chosen[t]])); sizes.push_back(static_cast<size_t>(w.len));
+      }
   if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
   const WholeStream* dws = static_cast<const WholeStream*>(s.wtab.p);
-  if ((rc = whole_hash_device(c, reqs.front()->whole_algo, files, 0, 0, static_cast<int64_t>(nfiles), static_cast<uint8_t*>(s.dig.p), s.st, dws)))
+  if ((rc = whole_hash_device(c, reqs.front()->whole_algo, files, 0, 0, static_cast<int64_t>(nfiles), static_cast<uint8_t*>(s.wdig.p), s.st, dws)))
     return rc;
   c->eng->count_launch();
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hdig.p, s.dig.p, nfiles * 64, cudaMemcpyDeviceToHost, s.st));
-  *wf = WholeFiles{files, dws};
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hwdig.p, s.wdig.p, nfiles * 64, cudaMemcpyDeviceToHost, s.st));
+  bool streaming = false;  // a request of the batch reads frames
+  for (size_t z = 0; z < nreq; z++) streaming |= tab[z].whole_pos != static_cast<uint32_t>((1ull << k) - 1);
+  *wf = WholeFiles{files, dws, reinterpret_cast<const int32_t*>(dws + nfiles), !streaming};
   return MEC_OK;
 }
 
@@ -3453,7 +3533,7 @@ static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchRe
   const BatchReqDesc* dt = static_cast<const BatchReqDesc*>(d.hreq.p);
   const BatchGetDesc* rt = static_cast<const BatchGetDesc*>(s.hreq.p);
   WholeFiles wf;
-  if (whole && (rc = batch_whole_stage(b, s, reqs, rt, &wf))) return rc;
+  if (whole && (rc = batch_whole_stage(b, s, reqs, rt, &wf))) return rc;  // every reader whole-file: wf.raw
   if ((rc = batch_read_reconstruct(b, s, rt, gp, lay, false, whole ? &wf : nullptr))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(d.dreq.p, dt, nreq * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
   BatchCopyParams cp;
@@ -3489,9 +3569,10 @@ static void batcher_main(mec_batcher* b) {
       if (!b->queue.empty() && nbusy < kSlots) {
         // gather: whatever is queued now; when nothing is in flight, give concurrent callers max_wait_us to join
         auto req_blocks = [&](const BatchReq* r) -> int64_t {
-          return r->kind == ReqKind::Put   ? ceil_frac(r->len, c->block_size)
-                 : r->kind == ReqKind::Get ? r->length / c->block_size + 2
-                                           : ceil_frac(r->total, c->block_size);  // heal, transcode: the whole part
+          // heal, transcode, a GET with a whole-file reader (its shard files are staged whole): the whole part
+          return r->kind == ReqKind::Put                      ? ceil_frac(r->len, c->block_size)
+                 : r->kind == ReqKind::Get && !r->whole_algo ? r->length / c->block_size + 2
+                                                              : ceil_frac(r->total, c->block_size);
         };
         auto blocks_queued = [&] {
           int64_t nb = 0;
@@ -3666,7 +3747,7 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
-    const int64_t P = round_up(32 + c->S(), 16), slots = b->max_blocks + std::min<int64_t>(64, b->max_blocks / 8 + 4);
+    const int64_t P = round_up(32 + c->S(), 16), slots = batcher_slot_blocks(b);
     for (Slot& s : c->slots) {
       if (rc == MEC_OK) rc = size_put_slot(c, s, slots);
       if (rc == MEC_OK) rc = s.hdig.ensure(static_cast<size_t>(slots * c->n * 32));
@@ -3703,16 +3784,9 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
       }
     if (rc == MEC_OK) rc = ensure_crc(c);
     if (dst)
-      // merged whole-file moves (batch_whole_stage): the raw shard files of a batch in s.src.  Request z of NB_z source blocks
-      // stages k files of at most NB_z x S bytes (k x S < block_size + k), each padded by at most 15 + 256 bytes, so a batch of at
-      // most `slots` blocks and requests fits slots x (block_size + 272 x k) bytes; one stream-table entry and one digest per file
-      for (Slot& s : c->slots) {
-        if (rc == MEC_OK) rc = s.src.ensure(static_cast<size_t>(slots * (block_size + 272 * k)));
-        if (rc == MEC_OK) rc = s.wtab.ensure(static_cast<size_t>(slots * k) * sizeof(WholeStream));
-        if (rc == MEC_OK) rc = s.hwtab.ensure(static_cast<size_t>(slots * k) * sizeof(WholeStream));
-        if (rc == MEC_OK) rc = s.dig.ensure(static_cast<size_t>(slots * std::max(c->n * 32, k * 64)));
-        if (rc == MEC_OK) rc = s.hdig.ensure(static_cast<size_t>(slots * std::max(c->n * 32, k * 64)));
-      }
+      // merged whole-file moves (batch_whole_stage): the raw shard files of a batch in s.src (size_whole_slot)
+      for (Slot& s : c->slots)
+        if (rc == MEC_OK) rc = size_whole_slot(c, s, slots);
     if (dst) {
       // the destination side of a merged transcode batch, laid out as a merged PUT batch of the destination geometry: object bytes,
       // parity rows, digests, the PUT request table and the latency kernel's block table.  A batch of `slots` source blocks holds
@@ -4011,10 +4085,104 @@ extern "C" int64_t mec_batcher_transcode_whole(mec_batcher* b, int algo, const u
   bool mapped = !b->sw.memcpy;
   const int rc = batch_readers(c, r, &mapped);
   if (rc) return rc;
+  r.whole_drives = r.alive_mask;  // every reader is whole-file
   for (int i = 0; i < e->n && mapped; i++)
     if (out_files[i]) mapped = mec_is_pinned(out_files[i]) != 0;
   if (!mapped || ceil_frac(total, c->block_size) > b->max_blocks) return batcher_run_alone(b, r);
   return batcher_enqueue_wait(b, r);
+}
+
+// The k readers of a mixed read (mec_batcher_decode_mixed / _heal_mixed), chosen on the caller's thread exactly as mec_decode_mixed /
+// mec_heal_mixed choose them: drives with alive[i] set, `prefer` first, then index order.  Sets r.whole_drives (the chosen readers
+// that are whole-file) and r.whole_algo (`walgo` when there is one, else 0), and clears *mapped unless every chosen reader is
+// page-locked.  Returns the chosen readers' mask, or 0 when fewer than k are alive (MEC_ERR_READ_QUORUM).
+static uint64_t mixed_readers(const mec_codec* c, BatchReq& r, const uint8_t* alive, int walgo, bool* mapped) {
+  int chosen[kBatchMaxFiles];
+  if (choose_readers(c, r.gfiles, alive, r.prefer, chosen) < c->k) return 0;
+  uint64_t mask = 0;
+  for (int t = 0; t < c->k; t++) {
+    const int i = chosen[t];
+    mask |= 1ull << i;
+    if (r.algos[i] != MEC_HIGHWAYHASH256S) r.whole_drives |= 1ull << i;
+    *mapped = *mapped && mec_is_pinned(r.gfiles[i]) != 0;
+  }
+  r.whole_algo = r.whole_drives ? walgo : 0;
+  return mask;
+}
+
+// mec_decode_mixed through the coalescer.  A GET whose k chosen readers all stream is an ordinary merged GET (the reader-set rules of
+// mec_batcher_decode_prefer); one with a whole-file reader among them joins batches of GETs of the same whole-file algorithm, whose
+// whole-file readers are staged whole and hashed in one launch (batch_whole_stage).  Either is redone through mec_decode_mixed on
+// the private handle when it meets bitrot.
+extern "C" int64_t mec_batcher_decode_mixed(mec_batcher* b, const int* algos, const uint8_t* const* files, const uint8_t* sums,
+                                            const uint8_t* prefer, int64_t offset, int64_t length, int64_t total, uint8_t* dst,
+                                            int* heal_hint) {
+  if (heal_hint) *heal_hint = 0;
+  if (!b || !algos || !files) return MEC_ERR_INVALID_ARGUMENT;
+  if (offset < 0 || length < 0) return MEC_ERR_INVALID_ARGUMENT;  // cmd/erasure-decode.go:240-242
+  if (offset + length > total) return MEC_ERR_INVALID_ARGUMENT;   // :243-245
+  if (length == 0) return 0;                                      // :247-249
+  if (!dst) return MEC_ERR_INVALID_ARGUMENT;
+  mec_codec* c = b->codec;
+  int walgo = 0;
+  int rc = mixed_formats(c, algos, files, nullptr, sums, &walgo);
+  if (rc) return rc;
+  const int n = c->n, k = c->k;
+  const ReadRange rr = read_range(c, offset, length, total);
+  if (static_cast<int64_t>(k) * rr.last_len < std::min(offset + length, total) - rr.last_block * c->block_size) return MEC_ERR_SHORT_DATA;
+  BatchReq r;
+  r.kind = ReqKind::Get; r.gfiles = files; r.offset = offset; r.length = length; r.total = total; r.dst = dst; r.heal_hint = heal_hint;
+  r.prefer = prefer; r.algos = algos; r.whole_sums = sums;
+  if (n > kBatchMaxFiles) return batcher_run_alone(b, r);
+  uint8_t alive[kBatchMaxFiles];
+  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr;
+  bool mapped = !b->sw.memcpy && mec_is_pinned(dst) != 0;
+  const uint64_t chosen = mixed_readers(c, r, alive, walgo, &mapped);
+  if (!chosen) return MEC_ERR_READ_QUORUM;
+  // the reader set batcher_main merges on: as mec_batcher_decode_prefer keys a streaming GET (the drives online without `prefer`),
+  // the chosen readers for a GET with a whole-file reader
+  if (prefer || r.whole_algo) {
+    r.alive_mask = chosen;
+  } else {
+    for (int i = 0; i < n; i++)
+      if (files[i]) r.alive_mask |= 1ull << i;
+  }
+  if (!mapped || (r.whole_algo && ceil_frac(total, c->block_size) > b->max_blocks)) return batcher_run_alone(b, r);
+  return batcher_enqueue_wait(b, r);
+}
+
+// mec_heal_mixed through the coalescer: as mec_batcher_decode_mixed, with mec_batcher_heal's rules for heals whose k chosen readers
+// all stream (the same readers and stale drives share a launch) and mec_heal_mixed as the private path.
+extern "C" int mec_batcher_heal_mixed(mec_batcher* b, const int* algos, const uint8_t* const* files, const uint8_t* sums,
+                                      const uint8_t* prefer, int64_t total, uint8_t* const* out_files, uint8_t* corrupt) {
+  if (!b || !algos || !files || !out_files) return MEC_ERR_INVALID_ARGUMENT;
+  mec_codec* c = b->codec;
+  const int n = c->n;
+  if (corrupt) memset(corrupt, 0, static_cast<size_t>(n));
+  int walgo = 0;
+  int rc = mixed_formats(c, algos, files, out_files, sums, &walgo);
+  if (rc) return rc;
+  if (total <= 0) return MEC_OK;
+  BatchReq r;
+  r.kind = ReqKind::Heal; r.gfiles = files; r.offset = 0; r.length = total; r.total = total;
+  r.prefer = prefer; r.outs = out_files; r.corrupt = corrupt; r.algos = algos; r.whole_sums = sums;
+  if (n > kBatchMaxFiles) return static_cast<int>(batcher_run_alone(b, r));
+  // healObject opens no reader on a drive it heals (cmd/erasure-healing.go:572-575): a stale drive is never read
+  uint8_t alive[kBatchMaxFiles];
+  for (int i = 0; i < n; i++) alive[i] = files[i] != nullptr && out_files[i] == nullptr;
+  bool mapped = !b->sw.memcpy;
+  r.alive_mask = mixed_readers(c, r, alive, walgo, &mapped);
+  if (!r.alive_mask) return MEC_ERR_READ_QUORUM;
+  int nstale = 0;
+  for (int i = 0; i < n; i++)
+    if (out_files[i]) {
+      r.stale_mask |= 1ull << i;
+      nstale++;
+      mapped = mapped && mec_is_pinned(out_files[i]) != 0;
+    }
+  if (!mapped || nstale > kMaxR || (r.whole_algo && ceil_frac(total, c->block_size) > b->max_blocks))
+    return static_cast<int>(batcher_run_alone(b, r));
+  return static_cast<int>(batcher_enqueue_wait(b, r));
 }
 
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
@@ -4040,6 +4208,8 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "transcodes_serial")) return b->st_transcodes_serial.load();
   if (!strcmp(name, "transcodes_whole")) return b->st_transcodes_whole.load();
   if (!strcmp(name, "transcodes_whole_serial")) return b->st_transcodes_whole_serial.load();
+  if (!strcmp(name, "reads_whole")) return b->st_reads_whole.load();
+  if (!strcmp(name, "reads_whole_serial")) return b->st_reads_whole_serial.load();
   if (!strncmp(name, "dst_", 4)) return b->dst ? mec_get_stat(b->dst, name + 4) : -1;  // the destination codec of merged moves
   return mec_get_stat(b->codec, name);  // the batcher's codec: which kernel forms its merged launches ran ("form_*", "last_*", ...)
 }

@@ -23,6 +23,12 @@
 //                  once by mec_encode_whole: through ONE transcode batcher (mec_batcher_transcode_whole), or each a
 //                  mec_transcode_whole call on the handle pair t % P (source codecs of that algorithm)
 //                  (after the timed window every thread's out files are compared with a plain mec_encode on the destination geometry)
+//   mode bget_mixed / bheal_mixed : GETs of whole objects / heals of one stale drive of legacy parts whose drives mix bitrot formats,
+//                  through ONE mec_batcher (mec_batcher_decode_mixed / mec_batcher_heal_mixed): drives [0, HEALED) were already healed
+//                  into HighwayHash256S frames (HEALED, default 8), the others hold raw shard files of the whole-file algorithm ALGO (as
+//                  above) with sums made once by mec_encode_whole; a heal rebuilds drive HEALED (the next legacy drive; drive n - 1 when
+//                  HEALED = n) from the others.  After the timed window every GET's bytes and every healed part file are checked.
+//   mode get_mixed / heal_mixed : the same calls, each a mec_decode_mixed / mec_heal_mixed call on a handle from the pool
 //   MIX=1        : the batcher of the b* modes is created with MEC_BATCHER_MIX_PATTERNS (reads of different patterns share batches)
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
 // Prints one JSON line: aggregate GiB/s, calls/s, p50/p99 latency.  Buffers are pinned (mec_alloc_pinned_on) for the GPU modes.
@@ -124,6 +130,11 @@ int main(int argc, char** argv) {
   const bool bmove = mode == "btranscode" || mode == "btranscode_whole";  // through the transcode batcher
   const bool move = bmove || mode == "transcode" || mode == "transcode_whole";
   const int walgo = getenv("ALGO") ? atoi(getenv("ALGO")) : MEC_HIGHWAYHASH256;
+  const bool bmixed = mode == "bget_mixed" || mode == "bheal_mixed";  // through the batcher
+  const bool mixed = bmixed || mode == "get_mixed" || mode == "heal_mixed";
+  const bool mixed_get = mode == "bget_mixed" || mode == "get_mixed";
+  const int healed = getenv("HEALED") ? std::max(0, std::min(k + m, atoi(getenv("HEALED")))) : 8;
+  const int mixed_stale = std::min(healed, k + m - 1);
   const int64_t bs = move && getenv("SRC_BS") ? atoll(getenv("SRC_BS")) : 1 << 20;
   const int64_t bs2 = move && getenv("DST_BS") ? atoll(getenv("DST_BS")) : 1 << 20;
   const bool gpu = mode != "cpu";
@@ -143,7 +154,8 @@ int main(int argc, char** argv) {
   const int sums_mask = getenv("SUMS") ? atoi(getenv("SUMS")) : MEC_SUM_MD5;
   struct TB { uint8_t* obj; std::vector<uint8_t*> files; uint8_t* dd; uint8_t* dst; uint8_t* parity; uint8_t* healed; uint64_t crc[3];
               uint8_t sums[MEC_SUM_BYTES];
-              std::vector<uint8_t> wsums;  // whole-file modes: the expected digest of every source shard file, n x 64
+              std::vector<uint8_t> wsums;  // whole-file and mixed modes: the expected digest of every source shard file, n x 64
+              std::vector<uint8_t*> wfiles;  // mixed modes: every drive's raw shard file of the whole-file algorithm
               std::vector<uint8_t*> outs; };  // outs: the destination part files of the transcode modes
   std::vector<TB> tb(T);
   uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
@@ -159,6 +171,11 @@ int main(int argc, char** argv) {
     tb[t].dst = take(osize);
     tb[t].parity = take(nb * m * S);
     tb[t].healed = take(fsz);
+    if (mixed)
+      for (int i = 0; i < n; i++) {
+        tb[t].wfiles.push_back(alloc(static_cast<size_t>(std::max<int64_t>(1, mec_shard_file_size(probe, osize)))));
+        if (!tb[t].wfiles.back()) { fprintf(stderr, "allocation failed\n"); return 1; }
+      }
     if (move)
       for (int i = 0; i < n2; i++) {
         tb[t].outs.push_back(alloc(static_cast<size_t>(fsz2)));
@@ -171,7 +188,7 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
-  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove) {
+  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove && !bmixed) {
     for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, whole ? walgo : MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
   }
   if (mode == "bget" || mode == "bheal") {  // coalesced GETs / heals: part files through a temporary handle, then everything goes through the batcher
@@ -184,6 +201,27 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
+  }
+  if (mixed) {  // both formats of every part through temporary handles; the batcher of the b*_mixed modes
+    mec_codec* cs = nullptr;
+    mec_codec* cw = nullptr;
+    mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &cs);
+    mec_codec_new(k, m, bs, walgo, device, &cw);
+    for (int t = 0; t < T; t++) {
+      std::vector<uint8_t*> f(tb[t].files), w(tb[t].wfiles);
+      tb[t].wsums.assign(static_cast<size_t>(n) * 64, 0);
+      if (mec_encode(cs, tb[t].obj, osize, f.data(), k) != osize || mec_encode_whole(cw, tb[t].obj, osize, w.data(), tb[t].wsums.data(), k) != osize) {
+        fprintf(stderr, "prep encode failed\n");
+        return 1;
+      }
+    }
+    mec_codec_free(cs);
+    mec_codec_free(cw);
+    if (bmixed) {
+      int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
+                                  getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
+      if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
+    }
   }
   if (move) {  // source part files through a temporary handle; the transcode batcher, or the pool's destination handles
     mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, whole ? walgo : MEC_HIGHWAYHASH256S, device, &c0);
@@ -241,6 +279,24 @@ int main(int argc, char** argv) {
       const int rc = mode == "bheal" ? mec_batcher_heal(bat, f, nullptr, osize, o, bad) : mec_heal_prefer(pool[t % P], f, nullptr, osize, o, bad);
       return rc == MEC_OK ? osize : rc;
     }
+    if (mixed) {  // drives [0, healed) stream, the others are raw shard files; a heal rebuilds drive mixed_stale
+      const uint8_t* f[64];
+      uint8_t* o[64] = {};
+      uint8_t bad[64];
+      int al[64];
+      for (int i = 0; i < n; i++) {
+        al[i] = i < healed ? MEC_HIGHWAYHASH256S : walgo;
+        f[i] = i < healed ? b.files[i] : b.wfiles[i];
+      }
+      int hint = 0;
+      if (mode == "bget_mixed") return mec_batcher_decode_mixed(bat, al, f, b.wsums.data(), nullptr, 0, osize, osize, b.dst, &hint);
+      if (mode == "get_mixed") return mec_decode_mixed(pool[t % P], al, f, b.wsums.data(), nullptr, 0, osize, osize, b.dst, &hint);
+      f[mixed_stale] = nullptr;
+      o[mixed_stale] = b.healed;
+      const int rc = bmixed ? mec_batcher_heal_mixed(bat, al, f, b.wsums.data(), nullptr, osize, o, bad)
+                            : mec_heal_mixed(pool[t % P], al, f, b.wsums.data(), nullptr, osize, o, bad);
+      return rc == MEC_OK ? osize : rc;
+    }
     if (move) {  // drive 0 offline in the _rot modes
       const uint8_t* f[64];
       for (int i = 0; i < n; i++) f[i] = rot && i == drive0_shard(t) ? nullptr : b.files[i];
@@ -275,6 +331,11 @@ int main(int argc, char** argv) {
   if (mode == "bheal" || mode == "heal")  // every healed part file equals the drive's original one
     for (int t = 0; t < T; t++)
       if (memcmp(tb[t].healed, tb[t].files[drive0_shard(t)], static_cast<size_t>(fsz)) != 0) errors++;
+  if (mixed)  // every GET's bytes equal the object, every healed part file the drive's streaming image
+    for (int t = 0; t < T; t++)
+      if (mixed_get ? memcmp(tb[t].dst, tb[t].obj, static_cast<size_t>(osize)) != 0
+                    : memcmp(tb[t].healed, tb[t].files[mixed_stale], static_cast<size_t>(fsz)) != 0)
+        errors++;
   if (move) {  // every destination part file equals what a plain mec_encode of the destination geometry writes
     std::vector<uint8_t*> want(n2);
     for (int i = 0; i < n2; i++) want[i] = static_cast<uint8_t*>(malloc(static_cast<size_t>(fsz2)));
@@ -319,7 +380,12 @@ int main(int argc, char** argv) {
            (long long)mec_batcher_stat(bat, "us_scatter"));
   if (move) printf(", \"dst\": \"%d,%d\", \"src_block_size\": %lld, \"dst_block_size\": %lld", k2, m2, static_cast<long long>(bs),
                   static_cast<long long>(bs2));
-  if (whole) printf(", \"algo\": %d", walgo);
+  if (whole || mixed) printf(", \"algo\": %d", walgo);
+  if (mixed) printf(", \"healed\": %d", healed);
+  if (bmixed)
+    printf(", \"reads_whole\": %lld, \"reads_whole_serial\": %lld, \"redone\": %lld, \"whole_hash_launches\": %lld",
+           static_cast<long long>(mec_batcher_stat(bat, "reads_whole")), static_cast<long long>(mec_batcher_stat(bat, "reads_whole_serial")),
+           static_cast<long long>(mec_batcher_stat(bat, "redone")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
   if (mode == "btranscode")
     printf(", \"transcodes\": %lld, \"transcodes_serial\": %lld, \"redone\": %lld", static_cast<long long>(mec_batcher_stat(bat, "transcodes")),
            static_cast<long long>(mec_batcher_stat(bat, "transcodes_serial")), static_cast<long long>(mec_batcher_stat(bat, "redone")));
@@ -327,7 +393,9 @@ int main(int argc, char** argv) {
     printf(", \"transcodes_whole\": %lld, \"transcodes_whole_serial\": %lld, \"redone\": %lld, \"whole_hash_launches\": %lld",
            static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole")), static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole_serial")),
            static_cast<long long>(mec_batcher_stat(bat, "redone")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
-  if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode" || mode == "transcode_whole") printf(", \"pool\": %d", P);
+  if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode" || mode == "transcode_whole" || mode == "get_mixed" ||
+      mode == "heal_mixed")
+    printf(", \"pool\": %d", P);
   printf("}\n");
   if (bat) mec_batcher_free(bat);
   for (auto c : pool) mec_codec_free(c);

@@ -169,6 +169,32 @@ res[4] = bat.transcode_whole(wsrc[4], wsum[4], wdat[4].size, 1, pinned=True)
 assert res[4][1] == -7 and all(np.array_equal(x, y) for x, y in zip(res[4][0], wtw[4]))
 assert bat.stat("redone") == 1 and bat.stat("transcodes_whole_serial") == 1
 bat.close()
+# mixed GETs and heals of half-healed SHA256 parts (mec_batcher_decode_mixed / mec_batcher_heal_mixed): even drives hold
+# HighwayHash256S frames, odd drives raw shard files.  Four GETs share one merged batch (frames of the streaming readers through the
+# gather kernel, the whole-file readers' shard files staged whole and hashed in ONE whole_hash_kernel launch over a stream table of
+# whole-file readers only, batch_whole_rows_kernel for their positions, the merged reconstruct with drive 2 offline, the GET scatter
+# straight into the callers' buffers), then four heals of drive 15 in one merged batch (heal frame scatter)
+hdat = [np.random.default_rng(80 + t).integers(0, 256, n, dtype=np.uint8) for t, n in enumerate((1 << 19, (1 << 20) + 5, 77, 2 * (1 << 20) + 999))]
+hsrc, hsum, hwant = [], [], []
+for a in hdat:
+    sf, _ = o.erasure_encode(k, m, bs, 3, a)
+    wf, ss = o.erasure_encode(k, m, bs, 1, a)
+    fs = [sf[i] if i % 2 == 0 else wf[i] for i in range(k + m)]
+    pf = [mb.pinned_array(max(f.size, 1))[:f.size] for f in fs]
+    for x, f in zip(pf, fs): x[:] = f
+    hsrc.append(pf); hsum.append([None if i % 2 == 0 else ss[i] for i in range(k + m)]); hwant.append(sf)
+halg = [3 if i % 2 == 0 else 1 for i in range(k + m)]
+bat = mb.Batcher(k, m, bs, max_batch_blocks=16, max_wait_us=500000)
+res = [None] * 8
+def hget(t): res[t] = bat.decode_mixed([None if i == 2 else f for i, f in enumerate(hsrc[t])], halg, hsum[t], 0, hdat[t].size, hdat[t].size, dst=mb.pinned_array(hdat[t].size))
+def hheal(t): res[4 + t] = bat.heal_mixed(hsrc[t], halg, hsum[t], [i == 15 for i in range(k + m)], hdat[t].size, pinned=True)
+for fn in (hget, hheal):
+    th = [threading.Thread(target=fn, args=(t,)) for t in range(4)]
+    [x.start() for x in th]; [x.join() for x in th]
+assert all(r[1] == 0 and np.array_equal(r[0], hdat[t]) for t, r in enumerate(res[:4]))
+assert all(np.array_equal(r[15], hwant[t][15]) for t, r in enumerate(res[4:]))
+assert bat.stat("batches") == 2 and bat.stat("reads_whole") == 8 and bat.stat("whole_hash_launches") == 2 and bat.stat("redone") == 0
+bat.close()
 print("sanitizer case ok")
 PY
 echo "== memcheck"; timeout 1200 compute-sanitizer --tool memcheck --print-limit 20 python /tmp/san_case.py > gpurun_out/memcheck.txt 2>&1; echo rc=$?; grep -E "ERROR SUMMARY|sanitizer case ok|Invalid|out of bounds|misaligned" gpurun_out/memcheck.txt | head -12
