@@ -385,6 +385,31 @@ int64_t mec_batcher_decode_mixed(mec_batcher* b, const int* algos, const uint8_t
                                  int* heal_hint);
 int mec_batcher_heal_mixed(mec_batcher* b, const int* algos, const uint8_t* const* files, const uint8_t* sums,
                            const uint8_t* prefer, int64_t total_length, uint8_t* const* out_files, uint8_t* corrupt);
+/* mec_bitrot_verify_parts through the coalescer (VerifyFile of one object on one drive, cmd/xl-storage.go:3100-3137; the deep-scan
+ * heals of the scanner, MRF and HealObject send many of them at once, cmd/erasure-healing-common.go:415-419), on any batcher
+ * (transcode batchers included): the arguments and results of mec_bitrot_verify_parts with the batcher in place of the codec; streaming
+ * parts use the batcher's shard size.  Checked on the caller's thread, before anything is queued and in this order: a NULL batcher,
+ * then mec_bitrot_verify_parts' refusals (MEC_ERR_INVALID_ARGUMENT, results untouched), then its per-part decisions (invalid parts,
+ * wrong streaming lengths, empty streaming parts); a call with nothing left to hash returns MEC_OK at once.
+ * Calls with a file to hash that is not page-locked, MEC_BATCHER_MEMCPY in the environment, more frames than one hash-only launch of
+ * the latency kernel takes (its "small_blocks" limit; B when the codec's options rule that kernel out), more staged bytes than
+ * B x block_size - 1024 (a frame pitch of round_up(32 + S, 16) per frame, round_up(file_len, 16) + 256 per whole-file part) or more
+ * whole-file parts than B x k (B = max_batch_blocks + min(64, max_batch_blocks / 8 + 4)) run through mec_bitrot_verify_parts on the
+ * batcher's private handle (counted in "verifies_serial").  Every other call joins a merged verify batch: verify calls only, and calls
+ * with a whole-file part only with such calls, whatever their algorithms (a frame-only scan never waits behind the chain hash of a
+ * long legacy file); a batch is cut at those same frame, byte and file limits.  A batch stages every frame and every whole file in
+ * ONE batched copy, hashes every frame in ONE hash-only launch with a per-frame length table (one launch per run of full frames and
+ * one per short frame when the options rule out the latency kernel) and every whole file in ONE whole_hash_kernel launch of up to
+ * three algorithm groups, and copies the verdicts and digests back once.  Nothing is redone: a corrupt part is a result and never
+ * affects its batch neighbours.
+ * Counters (mec_batcher_stat): "verifies" (calls completed by merged batches), "verifies_serial"; "batches", "requests" and "launches"
+ * as for other kinds; "blocks_read" grows by the frames hashed, "bytes_h2d" by the bytes staged (file_lens of every hashed part),
+ * "whole_hash_launches" by one per batch with whole-file parts.  Device memory: frames and files are staged in the slot's PUT
+ * staging buffer, which mec_batcher_new* sizes; a slot's first batch with whole-file parts sizes its file arena and stream table as
+ * mec_batcher_decode_mixed does (size shared with those batches), and the per-frame length table and verdict buffers grow to the
+ * largest batch; nothing more is allocated when the batcher is created. */
+int mec_batcher_verify(mec_batcher* b, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                       const int64_t* part_lens, const uint8_t* sums, int* results);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------
@@ -521,6 +546,28 @@ int mec_bitrot_verify(mec_codec* c, const uint8_t* file, int64_t file_len, int64
  * consecutive full frames — across files — share one hash-only launch.  Returns MEC_OK unless the call itself failed. */
 int mec_bitrot_verify_batch(mec_codec* c, int64_t nfiles, const uint8_t* const* files, const int64_t* file_lens,
                             const int64_t* part_lens, int* results);
+/* VerifyFile (cmd/xl-storage.go:3100-3137) in one call: bitrotVerify (cmd/bitrot.go:164-216) of every part of an object on one drive,
+ * each part with its own algorithm and sum (erasure.GetChecksumInfo(part.Number)), or of xl.meta inline data
+ * (cmd/erasure-healing-common.go:398-406).  Part p: algos[p] = checksumInfo.Algorithm, files[p] = file_lens[p] bytes of part.N as
+ * stored (or of the inline data), part_lens[p] = erasure.ShardFileSize(part.Size), sums + p*64 = checksumInfo.Hash (read only for
+ * whole-file algorithms).  The codec's own algorithm is not used.
+ *   streaming (MEC_HIGHWAYHASH256S): frames of the codec's shard size; results[p] is bitrotVerify's verdict: a file length other than
+ *     mec_bitrot_shard_file_size(part_lens[p]) or any frame failing its digest is MEC_ERR_FILE_CORRUPT (cmd/bitrot.go:183); an empty
+ *     part with an empty file is MEC_OK.
+ *   whole-file (MEC_SHA256, MEC_HIGHWAYHASH256, MEC_BLAKE2B512): the digest of all file_lens[p] bytes is compared with the first
+ *     mec_digest_size(algo) bytes of the sum (cmd/bitrot.go:165-174); part_lens[p] is not read.
+ * Refused before any device work with MEC_ERR_INVALID_ARGUMENT and results untouched, in this order: a NULL codec; nparts < 0; a NULL
+ * algos, files, file_lens, part_lens or results while nparts > 0; a NULL sums while a part is whole-file.  Per part, results[p] =
+ * MEC_ERR_INVALID_ARGUMENT for an algos[p] that is no MEC_* bitrot value, a negative file_lens[p] (or part_lens[p] of a streaming
+ * part), or a NULL files[p] with file_lens[p] > 0.  Returns MEC_OK unless the call itself failed.
+ * Streaming parts run through mec_bitrot_verify_batch's pipeline (hash-only launches over ~32 MiB chunks of frames through the codec's
+ * slots).  Whole-file parts are staged in input order in groups of at most 256 MiB of file bytes (a larger file alone), each group by
+ * ONE batched copy into slot 0's staging buffer (each file 16-byte aligned with 256 bytes behind it) and ONE whole_hash_kernel launch
+ * whose up to three algorithm groups hold its SHA256, HighwayHash256 and BLAKE2b512 parts ("whole_hash_launches" + 1 per group).
+ * Counters: "blocks_read" grows by the frames hashed, "bytes_h2d" by the file bytes staged.  mec_bitrot_verify_batch is this call
+ * with every part MEC_HIGHWAYHASH256S on a HighwayHash256S codec, except that it refuses a NULL file with part_lens[f] > 0 per file. */
+int mec_bitrot_verify_parts(mec_codec* c, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                            const int64_t* part_lens, const uint8_t* sums, int* results);
 
 /* ---- shard-shaped low-level calls (keep Erasure.EncodeData / reedsolomon.Encoder shapes) ---- */
 /* reedsolomon.Encoder.Encode: shards[0..k) in, shards[k..k+m) out, each shard_len bytes (host). */

@@ -132,6 +132,8 @@ def lib():
     L.mec_get_stat.argtypes = [vp, C.c_char_p]
     L.mec_bitrot_verify.argtypes = [vp, vp, i64, i64]
     L.mec_bitrot_verify_batch.argtypes = [vp, i64, vp, vp, vp, vp]
+    L.mec_bitrot_verify_parts.argtypes = [vp, i64, vp, vp, vp, vp, vp, C.POINTER(i32)]
+    L.mec_batcher_verify.argtypes = [vp, i64, vp, vp, vp, vp, vp, C.POINTER(i32)]
     L.mec_encode_whole.restype = i64
     L.mec_encode_whole.argtypes = [vp, vp, i64, vp, vp, i32]
     L.mec_whole_hash.argtypes = [vp, i32, vp, i64, i64, vp]
@@ -166,6 +168,26 @@ def _u8(a):
 
 def _ptrs(arrs):
     return (C.c_void_p * len(arrs))(*[(a.ctypes.data if (a is not None and a.size) else None) for a in arrs])
+
+
+def _verify_parts(fn, h, what, files, algos, part_lens, sums):
+    """the shared body of Codec.bitrot_verify_parts and Batcher.verify"""
+    files = [None if f is None else _u8(f) for f in files]
+    n = len(files)
+    al = (C.c_int32 * max(n, 1))(*[int(a) for a in algos])
+    fl = (C.c_int64 * max(n, 1))(*[0 if f is None else f.size for f in files])
+    pl = (C.c_int64 * max(n, 1))(*[int(x) for x in part_lens])
+    sm = None
+    if sums is not None:
+        sm = np.zeros((max(n, 1), 64), dtype=np.uint8)
+        for i, d in enumerate(sums):
+            if d is not None:
+                sm[i, :len(d)] = np.frombuffer(bytes(d), dtype=np.uint8)
+    res = (C.c_int32 * max(n, 1))()
+    rc = fn(h, n, al, _ptrs(files) if n else (C.c_void_p * 1)(), fl, pl, None if sm is None else sm.ctypes.data, res)
+    if rc:
+        raise MecError(rc, what)
+    return list(res)[:n]
 
 
 class Codec:
@@ -373,6 +395,12 @@ class Codec:
         if rc:
             raise MecError(rc, "mec_bitrot_verify_batch")
         return list(res)
+
+    def bitrot_verify_parts(self, files, algos, part_lens, sums=None):
+        """mec_bitrot_verify_parts (VerifyFile): part p is files[p] (bytes as stored, None = NULL), written with algos[p], of
+        part_lens[p] bytes (streaming parts; ShardFileSize(part.Size)), with the expected whole-file digest sums[p] (bytes or None;
+        read for whole-file algorithms only; sums=None passes NULL).  -> list of 0 / -7 / -12 per part."""
+        return _verify_parts(lib().mec_bitrot_verify_parts, self.h, "mec_bitrot_verify_parts", files, algos, part_lens, sums)
 
     # -- legacy whole-file bitrot
     def encode_whole(self, src, online=None, write_quorum=0):
@@ -746,6 +774,11 @@ class Batcher:
         if rc:
             raise MecError(rc, "mec_batcher_heal_mixed")
         return outs
+
+    def verify(self, files, algos, part_lens, sums=None):
+        """mec_batcher_verify: Codec.bitrot_verify_parts through the coalescer on this batcher's geometry (arguments and results as
+        there).  Page-locked files (pinned_array) let the call ride in merged batches."""
+        return _verify_parts(lib().mec_batcher_verify, self.h, "mec_batcher_verify", files, algos, part_lens, sums)
 
     def stat(self, name):
         return lib().mec_batcher_stat(self.h, name.encode())

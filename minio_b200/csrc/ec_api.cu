@@ -1583,11 +1583,61 @@ extern "C" int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobject
   return first_err.load();
 }
 
+// The hash-only check (k = 1, r = 0) of `nframes` frames staged in slot `s` at `base` (frame j at base + j*P: its 32-byte digest, then
+// lens[j] shard bytes; (arena_frames - j) * P + 512 readable bytes from frame j on), enqueued on the slot's stream.  `lens` is
+// page-locked host memory.  one_launch (the codec's options allow the latency kernel at this size): every frame, full or short,
+// hashes in ONE launch with a per-frame length table.  Otherwise one launch over each run of full frames and one per short frame
+// (a short frame's digest covers fewer bytes).  Verdicts come back to s.hflags[0, nframes).  Shared by bitrotVerify on a codec
+// (verify_files_locked) and merged verify batches (batcher_submit_verify).
+static int verify_frames(mec_codec* c, Slot& s, const uint8_t* base, int64_t arena_frames, int64_t nframes, const int32_t* lens, bool one_launch) {
+  const int64_t S = c->S(), P = round_up(32 + S, 16);
+  int rc;
+  if ((rc = s.dig.ensure(static_cast<size_t>(nframes * 32)))) return rc;
+  if ((rc = s.flags.ensure(static_cast<size_t>(nframes)))) return rc;
+  if ((rc = s.hflags.ensure(static_cast<size_t>(nframes)))) return rc;
+  MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nframes), s.st));
+  const int32_t* block_len = nullptr;
+  auto launch = [&](int64_t slot0, int64_t cnt, int64_t len) -> int {
+    FusedDesc d;
+    d.k = 1; d.r = 0; d.contiguous = false; d.key = kMagicKey;
+    d.block_len = block_len;
+    d.in_block_stride = P; d.expect_block_stride = P;
+    const uint8_t* at = base + slot0 * P;
+    d.nblocks = cnt; d.S = static_cast<int32_t>(len);
+    d.map_base[0] = at; d.map_len[0] = (arena_frames - slot0) * P + 512;
+    d.expect_ptr[0] = at; d.in_ptr[0] = at + 32;
+    d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * 32;
+    d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0;
+    return c->eng->launch_fused(d, c->opt, s.st);
+  };
+  if (one_launch) {
+    if ((rc = s.dreq.ensure(static_cast<size_t>(nframes) * sizeof(int32_t)))) return rc;
+    MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, lens, static_cast<size_t>(nframes) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
+    block_len = static_cast<const int32_t*>(s.dreq.p);
+    if ((rc = launch(0, nframes, S))) return rc;
+  } else {
+    // runs of full frames between the short ones
+    int64_t at = 0;
+    for (int64_t j = 0; j <= nframes; j++) {
+      if (j < nframes && lens[j] == S) continue;
+      if (j > at && (rc = launch(at, j - at, S))) return rc;
+      if (j < nframes && (rc = launch(j, 1, lens[j]))) return rc;
+      at = j + 1;
+    }
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nframes), cudaMemcpyDeviceToHost, s.st));
+  c->st_blocks_read += nframes;
+  return MEC_OK;
+}
+
+static inline bool is_whole_algo(int a) { return a == MEC_SHA256 || a == MEC_HIGHWAYHASH256 || a == MEC_BLAKE2B512; }
+
 // bitrotVerify (cmd/bitrot.go:164-215), streaming algorithm: every frame's digest is recomputed and compared.  The scan of one
 // or many shard files (the scanner's deep-scan visits every part of every drive of an object: cmd/xl-storage.go:2550-2600) is cut
-// into chunks of frames that run through the codec's slots: staging of chunk c+1 overlaps the hash-only launch (k = 1, r = 0) of
-// chunk c; a chunk's verdicts come back when its slot is reused.  result[f] = MEC_OK / MEC_ERR_FILE_CORRUPT per file.
-static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* const* files, const int64_t* file_lens, const int64_t* part_lens,
+// into chunks of frames that run through the codec's slots: staging of chunk c+1 overlaps the hash-only launch of chunk c
+// (verify_frames); a chunk's verdicts come back when its slot is reused.  Files with results[f] != MEC_OK, an empty part or (with
+// `algos`) a whole-file algorithm are skipped; result[f] = MEC_ERR_FILE_CORRUPT where a frame fails.
+static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* const* files, const int64_t* part_lens, const int* algos,
                                int* results) {
   const int64_t S = c->S(), fstride = 32 + S, P = round_up(32 + S, 16);
   MEC_CUDA_OK(cudaSetDevice(c->device));
@@ -1612,99 +1662,175 @@ static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* cons
     const int si = ring.si;
     Slot& s = c->slots[si];
     if ((rc = s.src.ensure(static_cast<size_t>(chunk * P + 512)))) return rc;
-    if ((rc = s.dig.ensure(static_cast<size_t>(chunk * 32)))) return rc;
-    if ((rc = s.flags.ensure(static_cast<size_t>(chunk)))) return rc;
-    if ((rc = s.hflags.ensure(static_cast<size_t>(chunk)))) return rc;
-    MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(chunk), s.st));
+    if ((rc = s.hreq.ensure(static_cast<size_t>(chunk) * sizeof(int32_t)))) return rc;
     int64_t used = 0;
     // fill the chunk with frames of consecutive files.  When the chunk is a launch the latency kernel takes (it is, unless options
-    // say otherwise: ~380 frames of a 1 MiB-block part file), every frame — full or short — hashes in ONE launch with a per-frame
-    // length table, and every frame is staged by ONE batched copy call: a scan over thousands of small part files costs two driver
-    // calls per 32 MiB, not two per file.  Otherwise: full frames in one launch, short last frames one launch each.
+    // say otherwise: ~380 frames of a 1 MiB-block part file), short runs of frames are staged by ONE batched copy call: a scan over
+    // thousands of small part files costs two driver calls per 32 MiB, not two per file.
     const bool one_launch = c->eng->small_ok(c->opt, chunk);
     CopyList list;
-    int32_t* lens = nullptr;
-    if (one_launch) {
-      if ((rc = s.hreq.ensure(static_cast<size_t>(chunk) * sizeof(int32_t)))) return rc;
-      if ((rc = s.dreq.ensure(static_cast<size_t>(chunk) * sizeof(int32_t)))) return rc;
-      lens = static_cast<int32_t*>(s.hreq.p);
-    }
-    struct Tail { int64_t slot, len; };
-    std::vector<Tail> tails;
+    int32_t* lens = static_cast<int32_t*>(s.hreq.p);
     while (f < nfiles && used < chunk) {
-      if (results[f] != MEC_OK || part_lens[f] == 0) { f++; b0 = 0; continue; }
+      if (results[f] != MEC_OK || part_lens[f] == 0 || (algos && algos[f] != MEC_HIGHWAYHASH256S)) { f++; b0 = 0; continue; }
       const int64_t nblocks = ceil_frac(part_lens[f], S), last_len = part_lens[f] - (nblocks - 1) * S;
       const int64_t take = std::min(chunk - used, nblocks - b0);
       FrameGeom sub{take, S, (b0 + take == nblocks) ? last_len : S};
-      if (one_launch) {  // every frame's length goes into the per-frame table; short runs of frames join the chunk's batched copy call
-        for (int64_t j = 0; j < take; j++) lens[used + j] = static_cast<int32_t>((j == take - 1) ? sub.last_len : S);
-      }
+      for (int64_t j = 0; j < take; j++) lens[used + j] = static_cast<int32_t>((j == take - 1) ? sub.last_len : S);
       if (one_launch && take < kBatchedCopyBlocks) {
         for (int64_t j = 0; j < take; j++)
           list.add(static_cast<uint8_t*>(s.src.p) + (used + j) * P, files[f] + (b0 + j) * fstride, 32 + lens[used + j]);
       } else if ((rc = stage_frames(files[f] + b0 * fstride, static_cast<uint8_t*>(s.src.p) + used * P, sub, s.st))) return rc;
       c->st_h2d += sub.file_bytes();
-      if (sub.last_len != S) tails.push_back(Tail{used + take - 1, sub.last_len});
       inflight[si].push_back(Piece{f, take});
       used += take;
       b0 += take;
       if (b0 == nblocks) { f++; b0 = 0; }
     }
     if (used == 0) break;
-    const int32_t* block_len = nullptr;
-    auto launch = [&](int64_t slot0, int64_t cnt, int64_t len) -> int {
-      FusedDesc d;
-      d.k = 1; d.r = 0; d.contiguous = false; d.key = kMagicKey;
-      d.block_len = block_len;
-      d.in_block_stride = P; d.expect_block_stride = P;
-      const uint8_t* base = static_cast<const uint8_t*>(s.src.p) + slot0 * P;
-      d.nblocks = cnt; d.S = static_cast<int32_t>(len);
-      d.map_base[0] = base; d.map_len[0] = (chunk - slot0) * P + 512;
-      d.expect_ptr[0] = base; d.in_ptr[0] = base + 32;
-      d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * 32;
-      d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0;
-      return c->eng->launch_fused(d, c->opt, s.st);
-    };
-    if (one_launch) {
-      if ((rc = list.flush(s.st))) return rc;
-      MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, lens, static_cast<size_t>(used) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
-      block_len = static_cast<const int32_t*>(s.dreq.p);
-      if ((rc = launch(0, used, S))) return rc;
-      tails.clear();
-    }
-    // runs of full frames between the short ones (a short frame's digest covers fewer bytes: its own launch)
-    int64_t at = one_launch ? used : 0;
-    for (size_t q = 0; q <= tails.size(); q++) {
-      const int64_t end = q < tails.size() ? tails[q].slot : used;
-      if (end > at && (rc = launch(at, end - at, S))) return rc;
-      if (q < tails.size()) {
-        if ((rc = launch(tails[q].slot, 1, tails[q].len))) return rc;
-        at = tails[q].slot + 1;
-      }
-    }
-    MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(used), cudaMemcpyDeviceToHost, s.st));
-    c->st_blocks_read += used;
+    if ((rc = list.flush(s.st))) return rc;
+    if ((rc = verify_frames(c, s, static_cast<const uint8_t*>(s.src.p), chunk, used, lens, one_launch))) return rc;
     ring.submitted();
   }
   return ring.finish();
 }
 
+// Legacy parts of a verify call (mec_bitrot_verify_parts): every part p with results[p] == MEC_OK and a whole-file algorithm is
+// hashed whole and compared with the first mec_digest_size bytes of sums + p*64 (cmd/bitrot.go:165-174).  Parts are staged in
+// input order in groups of at most kVerifyWholeGroupBytes file bytes (a larger file alone), each group by ONE batched copy into
+// slot 0 and ONE whole_hash_kernel launch whose algorithm groups hold its SHA256, HighwayHash256 and BLAKE2b512 parts.
+constexpr int64_t kVerifyWholeGroupBytes = 256ll << 20;
+static const int kWholeAlgos[kWholeGroups] = {MEC_SHA256, MEC_HIGHWAYHASH256, MEC_BLAKE2B512};
+static inline int whole_group(int algo) { return algo == MEC_SHA256 ? 0 : algo == MEC_HIGHWAYHASH256 ? 1 : 2; }
+
+static int whole_hash_groups(mec_codec* c, int ngroups, const int* algos, const int64_t* counts, const uint8_t* d_data, int64_t pitch,
+                             int64_t len, uint8_t* d_out, cudaStream_t st, const WholeStream* streams);
+static int verify_whole_locked(mec_codec* c, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                               const uint8_t* sums, int* results) {
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  Slot& s = c->slots[0];
+  SlotDrain drain(s);
+  int rc;
+  int64_t p = 0;
+  std::vector<int64_t> group[kWholeGroups];
+  while (p < nparts) {
+    for (auto& g : group) g.clear();
+    int64_t bytes = 0, nfiles = 0;
+    for (; p < nparts; p++) {
+      if (results[p] != MEC_OK || !is_whole_algo(algos[p])) continue;
+      if (nfiles > 0 && bytes + file_lens[p] > kVerifyWholeGroupBytes) break;
+      group[whole_group(algos[p])].push_back(p);
+      bytes += file_lens[p];
+      nfiles++;
+    }
+    if (nfiles == 0) break;
+    // the file arena as batch_whole_stage lays it out: each file 16-byte aligned with 256 readable bytes behind it
+    const size_t tab_bytes = static_cast<size_t>(nfiles) * sizeof(WholeStream);
+    if ((rc = s.hwtab.ensure(tab_bytes)) || (rc = s.wtab.ensure(tab_bytes))) return rc;
+    if ((rc = s.wdig.ensure(static_cast<size_t>(nfiles) * 64)) || (rc = s.hwdig.ensure(static_cast<size_t>(nfiles) * 64))) return rc;
+    WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+    int64_t arena = 0, j = 0, counts[kWholeGroups];
+    for (int g = 0; g < kWholeGroups; g++) {
+      counts[g] = static_cast<int64_t>(group[g].size());
+      for (int64_t q : group[g]) {
+        ws[j++] = WholeStream{arena, file_lens[q]};
+        arena += round_up(file_lens[q], 16) + 256;
+      }
+    }
+    if ((rc = s.src.ensure(static_cast<size_t>(arena)))) return rc;
+    uint8_t* d = static_cast<uint8_t*>(s.src.p);
+    MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, tab_bytes, cudaMemcpyHostToDevice, s.st));
+    CopyList list;
+    j = 0;
+    for (int g = 0; g < kWholeGroups; g++)
+      for (int64_t q : group[g]) list.add(d + ws[j++].off, files[q], file_lens[q]);
+    if ((rc = list.flush(s.st))) return rc;
+    if ((rc = whole_hash_groups(c, kWholeGroups, kWholeAlgos, counts, d, 0, 0, static_cast<uint8_t*>(s.wdig.p), s.st,
+                                static_cast<const WholeStream*>(s.wtab.p))))
+      return rc;
+    c->eng->count_launch();
+    MEC_CUDA_OK(cudaMemcpyAsync(s.hwdig.p, s.wdig.p, static_cast<size_t>(nfiles) * 64, cudaMemcpyDeviceToHost, s.st));
+    MEC_CUDA_OK(cudaStreamSynchronize(s.st));
+    c->st_h2d += bytes;
+    const uint8_t* got = static_cast<const uint8_t*>(s.hwdig.p);
+    j = 0;
+    for (int g = 0; g < kWholeGroups; g++)
+      for (int64_t q : group[g])
+        if (memcmp(got + 64 * j++, sums + q * 64, static_cast<size_t>(mec_digest_size(algos[q]))))
+          results[q] = MEC_ERR_FILE_CORRUPT;  // cmd/bitrot.go:171-173
+  }
+  return MEC_OK;
+}
+
+// The decisions of a verify call that need no device (mec_bitrot_verify_parts' per-part refusals, bitrotVerify's length check);
+// parts left at MEC_OK with bytes to hash are counted in *frames (streaming frames) and *whole (whole-file parts).
+static void verify_decide(int64_t S, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                          const int64_t* part_lens, int* results, int64_t* frames, int64_t* whole) {
+  *frames = *whole = 0;
+  for (int64_t p = 0; p < nparts; p++) {
+    const int a = algos[p];
+    const bool streaming = a == MEC_HIGHWAYHASH256S;
+    int r = MEC_OK;
+    if ((!streaming && !is_whole_algo(a)) || file_lens[p] < 0 || (streaming && part_lens[p] < 0) || (!files[p] && file_lens[p] > 0))
+      r = MEC_ERR_INVALID_ARGUMENT;
+    else if (streaming && file_lens[p] != mec_bitrot_shard_file_size(part_lens[p], S, a))
+      r = MEC_ERR_FILE_CORRUPT;  // cmd/bitrot.go:183
+    else if (streaming)
+      *frames += ceil_frac(part_lens[p], S);
+    else
+      (*whole)++;
+    results[p] = r;
+  }
+}
+
+// mec_bitrot_verify_parts' refusals before any device work
+static bool verify_args_ok(int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens, const int64_t* part_lens,
+                           const uint8_t* sums, const int* results) {
+  if (nparts < 0 || (nparts > 0 && (!algos || !files || !file_lens || !part_lens || !results))) return false;
+  if (!sums)
+    for (int64_t p = 0; p < nparts; p++)
+      if (is_whole_algo(algos[p])) return false;
+  return true;
+}
+
+// Device work of a verify call whose per-part decisions are made (results[p] == MEC_OK: hash it), on the locked codec
+static int verify_parts_locked(mec_codec* c, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                               const int64_t* part_lens, const uint8_t* sums, int* results, int64_t frames, int64_t whole) {
+  int rc;
+  if ((rc = ensure_engine(c))) return rc;
+  if (frames > 0 && (rc = verify_files_locked(c, nparts, files, part_lens, algos, results))) return rc;
+  if (whole > 0 && (rc = verify_whole_locked(c, nparts, algos, files, file_lens, sums, results))) return rc;
+  return MEC_OK;
+}
+
+extern "C" int mec_bitrot_verify_parts(mec_codec* c, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                                       const int64_t* part_lens, const uint8_t* sums, int* results) {
+  NvtxRange nvtx("mec_bitrot_verify_parts");
+  if (!c || !verify_args_ok(nparts, algos, files, file_lens, part_lens, sums, results)) return MEC_ERR_INVALID_ARGUMENT;
+  int64_t frames = 0, whole = 0;
+  verify_decide(c->S(), nparts, algos, files, file_lens, part_lens, results, &frames, &whole);
+  if (frames == 0 && whole == 0) return MEC_OK;
+  std::lock_guard<std::mutex> lk(c->mu);
+  return verify_parts_locked(c, nparts, algos, files, file_lens, part_lens, sums, results, frames, whole);
+}
+
+// bitrotVerify of streaming part files on a HighwayHash256S codec: mec_bitrot_verify_parts with every part HighwayHash256S, and the
+// call's own argument rules (a NULL file with a non-empty part is refused per file)
 extern "C" int mec_bitrot_verify_batch(mec_codec* c, int64_t nfiles, const uint8_t* const* files, const int64_t* file_lens,
                                        const int64_t* part_lens, int* results) {
   if (!c || nfiles < 0 || (nfiles > 0 && (!files || !file_lens || !part_lens || !results))) return MEC_ERR_INVALID_ARGUMENT;
   const int64_t S = c->S();
-  bool any = false;
+  int64_t frames = 0;
   for (int64_t f = 0; f < nfiles; f++) {
     results[f] = MEC_OK;
     if (!files[f] && part_lens[f] > 0) { results[f] = MEC_ERR_INVALID_ARGUMENT; continue; }
     if (file_lens[f] != mec_bitrot_shard_file_size(part_lens[f], S, c->algo)) results[f] = MEC_ERR_FILE_CORRUPT;  // cmd/bitrot.go:183
-    else if (part_lens[f] > 0) any = true;
+    else if (part_lens[f] > 0) frames += ceil_frac(part_lens[f], S);
   }
-  if (!any) return MEC_OK;
+  if (frames == 0) return MEC_OK;
   int rc = require_streaming(c);
   if (rc) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
-  return verify_files_locked(c, nfiles, files, file_lens, part_lens, results);
+  return verify_parts_locked(c, nfiles, nullptr, files, file_lens, part_lens, nullptr, results, frames, 0);
 }
 
 extern "C" int mec_bitrot_verify(mec_codec* c, const uint8_t* file, int64_t file_len, int64_t part_len) {
@@ -1724,21 +1850,37 @@ extern "C" int mec_digest_size(int algo) {
   return -1;
 }
 
-// `count` streams at d_data + s*pitch of `len` bytes each, or, with a device stream table, at d_data + streams[s].off of
-// streams[s].len bytes
-static int whole_hash_device(mec_codec* c, int algo, const uint8_t* d_data, int64_t pitch, int64_t len, int64_t count,
-                             uint8_t* d_out, cudaStream_t st, const WholeStream* streams = nullptr) {
+// ONE whole_hash_kernel launch over `ngroups` algorithm groups: group g is the next counts[g] streams, of algorithm algos[g], at
+// d_data + s*pitch of `len` bytes each or, with a device stream table, at d_data + streams[s].off of streams[s].len bytes.  Each
+// group starts on a warp boundary.  Empty groups are dropped.
+static int whole_hash_groups(mec_codec* c, int ngroups, const int* algos, const int64_t* counts, const uint8_t* d_data, int64_t pitch,
+                             int64_t len, uint8_t* d_out, cudaStream_t st, const WholeStream* streams) {
   WholeHashParams hp;
-  hp.data = d_data; hp.pitch = pitch; hp.len = len; hp.streams = streams; hp.nstreams = static_cast<int>(count);
-  hp.algo = algo == MEC_HIGHWAYHASH256S ? MEC_HIGHWAYHASH256 : algo;
-  hp.out = d_out;
+  memset(&hp, 0, sizeof(hp));
+  hp.data = d_data; hp.pitch = pitch; hp.len = len; hp.streams = streams; hp.out = d_out;
   memcpy(hp.key, kMagicKey, 32);
+  int64_t stream = 0, thread = 0;
+  for (int g = 0; g < ngroups; g++) {
+    if (counts[g] == 0) continue;
+    const int a = algos[g] == MEC_HIGHWAYHASH256S ? MEC_HIGHWAYHASH256 : algos[g];
+    const int q = hp.ngroups++;
+    thread = round_up(thread, 32);
+    hp.galgo[q] = a; hp.gstream[q] = static_cast<int>(stream); hp.gthread[q] = static_cast<int>(thread);
+    stream += counts[g];
+    thread += (a == MEC_HIGHWAYHASH256 ? 2 : 1) * counts[g];
+  }
+  hp.gstream[hp.ngroups] = static_cast<int>(stream);
+  if (hp.ngroups == 0) return MEC_OK;
   const int threads = 64;
-  const int64_t nthreads = hp.algo == MEC_HIGHWAYHASH256 ? 2 * count : count;
-  whole_hash_kernel<<<static_cast<unsigned>((nthreads + threads - 1) / threads), threads, 0, st>>>(hp);
+  whole_hash_kernel<<<static_cast<unsigned>((thread + threads - 1) / threads), threads, 0, st>>>(hp);
   MEC_CUDA_OK(cudaGetLastError());
   c->st_whole_hash++;
   return MEC_OK;
+}
+// `count` streams of one algorithm (whole_hash_groups with one group)
+static int whole_hash_device(mec_codec* c, int algo, const uint8_t* d_data, int64_t pitch, int64_t len, int64_t count,
+                             uint8_t* d_out, cudaStream_t st, const WholeStream* streams = nullptr) {
+  return whole_hash_groups(c, 1, &algo, &count, d_data, pitch, len, d_out, st, streams);
 }
 
 extern "C" int mec_whole_hash(mec_codec* c, int algo, const uint8_t* msgs, int64_t msg_len, int64_t count, uint8_t* digests) {
@@ -2494,11 +2636,12 @@ extern "C" int mec_selftest(int device) {
 #include <deque>
 #include <unordered_map>
 
-// PutObject (encode), GetObject (decode), Heal, a move between pools, a move of a part written with a whole-file bitrot algorithm
-enum class ReqKind { Put, Get, Heal, Transcode, TranscodeWhole };
+// PutObject (encode), GetObject (decode), Heal, a move between pools, a move of a part written with a whole-file bitrot algorithm,
+// bitrot verification of a drive's parts (VerifyFile)
+enum class ReqKind { Put, Get, Heal, Transcode, TranscodeWhole, Verify };
 // a GET, heal or move: stages its readers, and digest verdicts (per frame; per shard file for a whole-file move) decide which of
 // its requests are done
-static inline bool is_read(ReqKind k) { return k != ReqKind::Put; }
+static inline bool is_read(ReqKind k) { return k != ReqKind::Put && k != ReqKind::Verify; }
 static inline bool is_move(ReqKind k) { return k == ReqKind::Transcode || k == ReqKind::TranscodeWhole; }
 
 struct BatchReq {
@@ -2533,6 +2676,15 @@ struct BatchReq {
   uint64_t* crc_out = nullptr;
   int sum_which = 0;          // MEC_SUM_* mask of mec_batcher_encode_sums; the digests go to their slots of sums[0..MEC_SUM_BYTES)
   uint8_t* sums = nullptr;
+  // verify (mec_batcher_verify): the call's parts, decided on the caller's thread (verify_decide: results[p] == MEC_OK with bytes to
+  // hash marks a part the batch hashes); its streaming frames, whole-file parts and staged bytes (verify_staged)
+  int64_t vparts = 0, vframes = 0, vwhole = 0, vbytes = 0;
+  const int* valgos = nullptr;
+  const uint8_t* const* vfiles = nullptr;
+  const int64_t* vfile_lens = nullptr;
+  const int64_t* vpart_lens = nullptr;
+  const uint8_t* vsums = nullptr;
+  int* vresults = nullptr;
   int64_t result = 0;
   bool done = false;
   std::condition_variable cv;  // one per request: a finished batch wakes its own callers, not every thread parked in the batcher
@@ -2601,6 +2753,8 @@ struct mec_batcher {
   // mec_batcher_decode_mixed / _heal_mixed: calls with a whole-file reader completed by merged batches, and mixed calls of the
   // private path (redos included)
   std::atomic<int64_t> st_reads_whole{0}, st_reads_whole_serial{0};
+  // mec_batcher_verify: calls completed by merged batches / by the private handle
+  std::atomic<int64_t> st_verifies{0}, st_verifies_serial{0};
 };
 
 namespace {
@@ -2652,10 +2806,45 @@ static int64_t batcher_run_alone(mec_batcher* b, const BatchReq& r) {
   return mec_decode_prefer(sc, r.gfiles, r.prefer, r.offset, r.length, r.total, r.dst, r.heal_hint);
 }
 
+// The stream-table position of the first whole-file part of each algorithm group (whole_group) in a merged verify batch: the table
+// holds the SHA256 parts of every request, then the HighwayHash256 parts, then the BLAKE2b512 parts, each group in request order
+// and part order within a request
+static void verify_whole_firsts(const std::vector<BatchReq*>& reqs, int64_t (&first)[kWholeGroups]) {
+  int64_t counts[kWholeGroups] = {};
+  for (const BatchReq* r : reqs)
+    for (int64_t p = 0; p < r->vparts; p++)
+      if (r->vresults[p] == MEC_OK && is_whole_algo(r->valgos[p])) counts[whole_group(r->valgos[p])]++;
+  for (int g = 0, at = 0; g < kWholeGroups; g++) { first[g] = at; at += static_cast<int>(counts[g]); }
+}
+
 // Completes the batch that ran on slot `s` (rc: how its stream ended) and wakes its callers.
 static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int rc) {
   mec_codec* c = b->codec;
-  if (is_read(fb.kind)) {
+  if (fb.kind == ReqKind::Verify) {
+    // the frame verdicts in s.hflags and the whole-file digests in s.hwdig, both in batcher_submit_verify's order
+    const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
+    const uint8_t* wd = static_cast<const uint8_t*>(s.hwdig.p);
+    const int64_t S = c->S();
+    int64_t frame = 0, next[kWholeGroups];
+    verify_whole_firsts(fb.reqs, next);
+    for (BatchReq* r : fb.reqs) {
+      r->result = rc;
+      if (rc != MEC_OK) continue;
+      for (int64_t p = 0; p < r->vparts; p++) {
+        if (r->vresults[p] != MEC_OK) continue;
+        const int a = r->valgos[p];
+        bool bad = false;
+        if (a == MEC_HIGHWAYHASH256S) {
+          for (int64_t j = ceil_frac(r->vpart_lens[p], S); j > 0; j--) bad |= fl[frame++] != 0;
+        } else {
+          const int64_t q = next[whole_group(a)]++;
+          bad = memcmp(wd + q * 64, r->vsums + p * 64, static_cast<size_t>(mec_digest_size(a))) != 0;  // cmd/bitrot.go:171-173
+        }
+        if (bad) r->vresults[p] = MEC_ERR_FILE_CORRUPT;
+      }
+      b->st_verifies++;
+    }
+  } else if (is_read(fb.kind)) {
     // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own; the others are done
     // (their bytes are in place; a heal's `corrupt` was zeroed when it was queued).  A whole-file reader has no frames: the flags at
     // its arena position mean nothing, and the digest of its staged shard file (batch_whole_stage: streams in request order, a
@@ -3551,6 +3740,85 @@ static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchRe
   return MEC_OK;
 }
 
+// What one merged verify batch may hold: frames for one hash-only launch (the latency kernel's limit; with options that rule it out,
+// the blocks a slot is sized for), staged bytes within the slot's PUT staging buffer, whole-file parts within the stream table
+// size_whole_slot sizes.  A call beyond any of them takes the private path.
+struct VerifyLimits {
+  int64_t frames, bytes, files;
+};
+static VerifyLimits verify_limits(const mec_batcher* b) {
+  const mec_codec* c = b->codec;
+  const int64_t slots = batcher_slot_blocks(b);
+  return VerifyLimits{c->eng->small_ok(c->opt, 1) ? c->eng->small_limit(c->opt) : slots, slots * c->block_size - 1024, slots * c->k};
+}
+
+// One merged batch of verify calls (mec_batcher_verify), on the slot's stream: every frame of every streaming part (frame j at
+// s.src + j * P) and every whole-file part (from round_up(nframes * P + 512, 256) on, each 16-byte aligned with 256 readable bytes
+// behind it, as batch_whole_stage lays files out) in ONE batched copy; ONE hash-only launch over every frame with the per-frame
+// length table (verify_frames); ONE whole_hash_kernel launch whose algorithm groups hold every whole-file part (verify_whole_firsts'
+// order); the frame verdicts and file digests back to s.hflags and s.hwdig, where batcher_finish folds them into each caller's
+// results.  Nothing is redone: a corrupt part is a result.
+static int batcher_submit_verify(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t* nblocks) {
+  mec_codec* c = b->codec;
+  const int64_t S = c->S(), fstride = 32 + S, P = round_up(32 + S, 16);
+  int64_t nframes = 0, nwhole = 0, next[kWholeGroups], counts[kWholeGroups];
+  for (const BatchReq* r : reqs) { nframes += r->vframes; nwhole += r->vwhole; }
+  verify_whole_firsts(reqs, next);
+  for (int g = 0; g < kWholeGroups; g++) counts[g] = (g + 1 < kWholeGroups ? next[g + 1] : nwhole) - next[g];
+  int rc;
+  if (nwhole > 0 && (rc = size_whole_slot(c, s, batcher_slot_blocks(b)))) return rc;  // a no-op after the slot's first such batch
+  const int64_t woff = round_up(nframes * P + 512, 256);
+  int64_t end = woff;
+  for (const BatchReq* r : reqs) end += r->vbytes - r->vframes * P;  // the whole-file parts (verify_staged)
+  if ((rc = s.src.ensure(static_cast<size_t>(end)))) return rc;
+  if ((rc = s.hreq.ensure(static_cast<size_t>(nframes) * sizeof(int32_t) + 16))) return rc;
+  if ((rc = s.hwtab.ensure(static_cast<size_t>(nwhole) * sizeof(WholeStream) + 16)) || (rc = s.wtab.ensure(static_cast<size_t>(nwhole) * sizeof(WholeStream) + 16)))
+    return rc;
+  if ((rc = s.wdig.ensure(static_cast<size_t>(nwhole) * 64 + 64)) || (rc = s.hwdig.ensure(static_cast<size_t>(nwhole) * 64 + 64))) return rc;
+  uint8_t* arena = static_cast<uint8_t*>(s.src.p);
+  int32_t* lens = static_cast<int32_t*>(s.hreq.p);
+  WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+  CopyList list;
+  int64_t f = 0, wpos = woff;
+  for (const BatchReq* r : reqs)
+    for (int64_t p = 0; p < r->vparts; p++) {
+      if (r->vresults[p] != MEC_OK) continue;
+      const int a = r->valgos[p];
+      const uint8_t* file = r->vfiles[p];
+      if (a == MEC_HIGHWAYHASH256S) {
+        const int64_t nb = ceil_frac(r->vpart_lens[p], S), last = r->vpart_lens[p] - (nb - 1) * S;
+        for (int64_t j = 0; j < nb; j++, f++) {
+          lens[f] = static_cast<int32_t>(j == nb - 1 ? last : S);
+          list.add(arena + f * P, file + j * fstride, 32 + lens[f]);
+        }
+        c->st_h2d += r->vfile_lens[p];
+      } else {
+        const int64_t len = r->vfile_lens[p];
+        ws[next[whole_group(a)]++] = WholeStream{wpos, len};
+        list.add(arena + wpos, file, len);
+        wpos += round_up(len, 16) + 256;
+        c->st_h2d += len;
+      }
+    }
+  mark_phase(b, s, 0);
+  if (nwhole > 0)
+    MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, static_cast<size_t>(nwhole) * sizeof(WholeStream), cudaMemcpyHostToDevice, s.st));
+  if ((rc = list.flush(s.st))) return rc;
+  mark_phase(b, s, 1);
+  if (nframes > 0 && (rc = verify_frames(c, s, arena, nframes, nframes, lens, c->eng->small_ok(c->opt, nframes)))) return rc;
+  if (nwhole > 0) {
+    if ((rc = whole_hash_groups(c, kWholeGroups, kWholeAlgos, counts, arena, 0, 0, static_cast<uint8_t*>(s.wdig.p), s.st,
+                                static_cast<const WholeStream*>(s.wtab.p))))
+      return rc;
+    c->eng->count_launch();
+    MEC_CUDA_OK(cudaMemcpyAsync(s.hwdig.p, s.wdig.p, static_cast<size_t>(nwhole) * 64, cudaMemcpyDeviceToHost, s.st));
+  }
+  mark_phase(b, s, 2);
+  mark_phase(b, s, 3);
+  *nblocks = nframes;
+  return MEC_OK;
+}
+
 static void batcher_main(mec_batcher* b) {
   mec_codec* c = b->codec;
   cudaSetDevice(c->device);
@@ -3570,7 +3838,9 @@ static void batcher_main(mec_batcher* b) {
         // gather: whatever is queued now; when nothing is in flight, give concurrent callers max_wait_us to join
         auto req_blocks = [&](const BatchReq* r) -> int64_t {
           // heal, transcode, a GET with a whole-file reader (its shard files are staged whole): the whole part
+          // a verify: its staged bytes
           return r->kind == ReqKind::Put                      ? ceil_frac(r->len, c->block_size)
+                 : r->kind == ReqKind::Verify                 ? ceil_frac(r->vbytes, c->block_size)
                  : r->kind == ReqKind::Get && !r->whole_algo ? r->length / c->block_size + 2
                                                               : ceil_frac(r->total, c->block_size);
         };
@@ -3600,12 +3870,23 @@ static void batcher_main(mec_batcher* b) {
         const BatchReq* lead = b->queue.front();
         const bool mix = b->mix && is_read(lead->kind);
         const int64_t limit = std::min<int64_t>(c->eng->small_limit(c->opt), 1 << 16);  // block_pattern holds uint16_t indices
+        // verify batches: calls with a whole-file part only with such calls (a frame-only scan never waits behind the chain hash of a
+        // long legacy file), cut at verify_limits
+        const VerifyLimits vlim = verify_limits(b);
+        int64_t vframes = 0, vbytes = 0, vwhole = 0;
         for (auto it = b->queue.begin(); it != b->queue.end();) {
           BatchReq* r = *it;
           const bool same = r->alive_mask == lead->alive_mask && r->stale_mask == lead->stale_mask;
-          if (r->kind != lead->kind || r->whole_algo != lead->whole_algo || (!same && !mix)) { ++it; continue; }
+          if (r->kind != lead->kind || r->whole_algo != lead->whole_algo || (!same && !mix) || (r->vwhole > 0) != (lead->vwhole > 0)) {
+            ++it;
+            continue;
+          }
           const int64_t rb = req_blocks(r);
           if (!reqs.empty() && nb + rb > cap) break;
+          if (r->kind == ReqKind::Verify) {
+            if (!reqs.empty() && (vframes + r->vframes > vlim.frames || vbytes + r->vbytes > vlim.bytes || vwhole + r->vwhole > vlim.files)) break;
+            vframes += r->vframes; vbytes += r->vbytes; vwhole += r->vwhole;
+          }
           if (mix) {  // the exact blocks of the read
             const int64_t rs = read_range(c, r->offset, r->length, r->total).nblocks;
             if ((mixed || !same) && nread + rs > limit) break;
@@ -3631,6 +3912,7 @@ static void batcher_main(mec_batcher* b) {
           case ReqKind::Put: rc = batcher_submit(b, s, reqs, &fb.needs_retire, &nblocks); break;
           case ReqKind::Get: rc = batcher_submit_get(b, s, reqs, &nblocks); break;
           case ReqKind::Heal: rc = batcher_submit_heal(b, s, reqs, &nblocks); break;
+          case ReqKind::Verify: rc = batcher_submit_verify(b, s, reqs, &nblocks); break;
           case ReqKind::Transcode:
           case ReqKind::TranscodeWhole: {
             std::lock_guard<std::mutex> lk_dst(b->dst->mu);  // source, then destination: mec_transcode's order
@@ -3641,8 +3923,8 @@ static void batcher_main(mec_batcher* b) {
       }
       b->us_submit += us_since(t_submit);
       fb.reqs = reqs;
-      // a batch the kernels carry end to end: every read batch, a PUT batch unless it took the memcpy path
-      const bool kernel_batch = is_read(fb.kind) || !fb.needs_retire;
+      // a batch the kernels carry end to end: every read or verify batch, a PUT batch unless it took the memcpy path
+      const bool kernel_batch = fb.kind != ReqKind::Put || !fb.needs_retire;
       fb.traced = b->sw.trace && rc == MEC_OK && kernel_batch;
       if (rc != MEC_OK) {  // drain what was enqueued before the failure, then fail the whole batch
         cudaStreamSynchronize(s.st);
@@ -4185,6 +4467,45 @@ extern "C" int mec_batcher_heal_mixed(mec_batcher* b, const int* algos, const ui
   return static_cast<int>(batcher_enqueue_wait(b, r));
 }
 
+// The staged bytes of a verify call whose parts are decided (verify_decide): a frame pitch per streaming frame, a 16-byte-aligned file
+// and 256 bytes behind it per whole-file part (batcher_submit_verify's layout).  Clears *mapped unless every file to hash is page-locked.
+static int64_t verify_staged(const mec_codec* c, const BatchReq& r, bool* mapped) {
+  const int64_t S = c->S(), P = round_up(32 + S, 16);
+  int64_t bytes = 0;
+  for (int64_t p = 0; p < r.vparts; p++) {
+    if (r.vresults[p] != MEC_OK) continue;
+    const bool streaming = r.valgos[p] == MEC_HIGHWAYHASH256S;
+    bytes += streaming ? ceil_frac(r.vpart_lens[p], S) * P : round_up(r.vfile_lens[p], 16) + 256;
+    if (r.vfile_lens[p] > 0) *mapped = *mapped && mec_is_pinned(r.vfiles[p]) != 0;
+  }
+  return bytes;
+}
+
+// VerifyFile (cmd/xl-storage.go:3100-3137) through the coalescer: mec_bitrot_verify_parts on the batcher's geometry.  Refusals and the
+// per-part decisions that need no device are made on the caller's thread; the parts left to hash join a merged verify batch
+// (batcher_submit_verify), or run through mec_bitrot_verify_parts on the private handle when the call cannot ride in one.
+extern "C" int mec_batcher_verify(mec_batcher* b, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
+                                  const int64_t* part_lens, const uint8_t* sums, int* results) {
+  NvtxRange nvtx("mec_batcher_verify");
+  if (!b || !verify_args_ok(nparts, algos, files, file_lens, part_lens, sums, results)) return MEC_ERR_INVALID_ARGUMENT;
+  mec_codec* c = b->codec;
+  BatchReq r;
+  r.kind = ReqKind::Verify;
+  verify_decide(c->S(), nparts, algos, files, file_lens, part_lens, results, &r.vframes, &r.vwhole);
+  if (r.vframes == 0 && r.vwhole == 0) return MEC_OK;
+  r.vparts = nparts; r.valgos = algos; r.vfiles = files; r.vfile_lens = file_lens; r.vpart_lens = part_lens; r.vsums = sums;
+  r.vresults = results;
+  bool mapped = !b->sw.memcpy;
+  r.vbytes = verify_staged(c, r, &mapped);
+  const VerifyLimits lim = verify_limits(b);
+  if (!mapped || r.vframes > lim.frames || r.vbytes > lim.bytes || r.vwhole > lim.files) {
+    b->st_verifies_serial++;
+    mec_codec* sc = batcher_private(b, c, b->serial);
+    return sc ? mec_bitrot_verify_parts(sc, nparts, algos, files, file_lens, part_lens, sums, results) : MEC_ERR_UNEXPECTED;
+  }
+  return static_cast<int>(batcher_enqueue_wait(b, r));
+}
+
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!b || !name) return -1;
   if (!strcmp(name, "batches")) return b->st_batches.load();
@@ -4210,6 +4531,8 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "transcodes_whole_serial")) return b->st_transcodes_whole_serial.load();
   if (!strcmp(name, "reads_whole")) return b->st_reads_whole.load();
   if (!strcmp(name, "reads_whole_serial")) return b->st_reads_whole_serial.load();
+  if (!strcmp(name, "verifies")) return b->st_verifies.load();
+  if (!strcmp(name, "verifies_serial")) return b->st_verifies_serial.load();
   if (!strncmp(name, "dst_", 4)) return b->dst ? mec_get_stat(b->dst, name + 4) : -1;  // the destination codec of merged moves
   return mec_get_stat(b->codec, name);  // the batcher's codec: which kernel forms its merged launches ran ("form_*", "last_*", ...)
 }

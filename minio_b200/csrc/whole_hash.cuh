@@ -115,11 +115,20 @@ struct WholeStream {
   int64_t off, len;
 };
 
+// A launch hashes up to kWholeGroups algorithm groups: group g is streams [gstream[g], gstream[g+1]) of algorithm galgo[g], run by
+// the threads from gthread[g] on (a multiple of 32: no warp runs two algorithms, and HighwayHash lane pairs stay in one warp).  A
+// merged verification (mec_bitrot_verify_parts, mec_batcher_verify) mixes parts of every era in one launch, which then lasts as long
+// as its longest file rather than the sum of one launch per algorithm.
+constexpr int kWholeGroups = 3;
+
 struct WholeHashParams {
   const uint8_t* data;   // stream s at data + s*pitch
   int64_t pitch, len;    // every stream has the same length
   const WholeStream* streams;  // device, optional: stream s is data + streams[s].off, streams[s].len bytes (pitch, len unused)
-  int nstreams, algo;    // MEC_SHA256 = 1, MEC_HIGHWAYHASH256 = 2, MEC_BLAKE2B512 = 4
+  int ngroups;
+  int galgo[kWholeGroups];        // MEC_SHA256 = 1, MEC_HIGHWAYHASH256 = 2, MEC_BLAKE2B512 = 4
+  int gstream[kWholeGroups + 1];  // group g = streams [gstream[g], gstream[g + 1])
+  int gthread[kWholeGroups];      // first thread of group g
   uint8_t* out;          // digest of stream s at out + s*64
   uint64_t key[4];
 };
@@ -130,11 +139,19 @@ __device__ __forceinline__ WholeStream whole_stream(const WholeHashParams& p, in
 
 __global__ void whole_hash_kernel(const WholeHashParams p) {
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p.algo == 2) {
+  // the group of this thread's warp, from the warp's first thread
+  // (static indices only: a run-time index into the parameters would copy them to the stack)
+  const int warp0 = tid & ~31;
+  int algo = p.galgo[0], first = p.gstream[0], end = p.gstream[1], local = tid - p.gthread[0];
+#pragma unroll
+  for (int q = 1; q < kWholeGroups; q++)
+    if (q < p.ngroups && warp0 >= p.gthread[q]) { algo = p.galgo[q]; first = p.gstream[q]; end = p.gstream[q + 1]; local = tid - p.gthread[q]; }
+  const int count = end - first;
+  if (algo == 2) {
     // HighwayHash-256: two threads per stream, exactly the half-state code of the fused kernel
-    const int s = tid >> 1, h = tid & 1;
-    const bool live = s < p.nstreams;
-    const WholeStream ws = whole_stream(p, live ? s : 0);
+    const int s = first + (local >> 1), h = local & 1;
+    const bool live = local >= 0 && (local >> 1) < count;
+    const WholeStream ws = whole_stream(p, live ? s : first);
     const uint8_t* d = p.data + ws.off;
     HHHalf hs;
     hh_init(hs, p.key, h);
@@ -158,12 +175,13 @@ __global__ void whole_hash_kernel(const WholeHashParams p) {
     }
     return;
   }
-  if (tid >= p.nstreams) return;
-  const WholeStream ws = whole_stream(p, tid);
+  if (local < 0 || local >= count) return;
+  const int s = first + local;
+  const WholeStream ws = whole_stream(p, s);
   const uint8_t* d = p.data + ws.off;
   const int64_t len = ws.len;
-  uint8_t* o = p.out + static_cast<int64_t>(tid) * 64;
-  if (p.algo == 1) {
+  uint8_t* o = p.out + static_cast<int64_t>(s) * 64;
+  if (algo == 1) {
     uint32_t h[8] = {0x6a09e667, 0xbb67ae85, 0x3c6ef372, 0xa54ff53a, 0x510e527f, 0x9b05688c, 0x1f83d9ab, 0x5be0cd19};
     uint32_t w[16];
     const int64_t nfull = len >> 6;

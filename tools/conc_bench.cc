@@ -29,6 +29,10 @@
 //                  above) with sums made once by mec_encode_whole; a heal rebuilds drive HEALED (the next legacy drive; drive n - 1 when
 //                  HEALED = n) from the others.  After the timed window every GET's bytes and every healed part file are checked.
 //   mode get_mixed / heal_mixed : the same calls, each a mec_decode_mixed / mec_heal_mixed call on a handle from the pool
+//   mode bverify / verify : VerifyFile of one object on one drive (the deep-scan heal's per-drive check): each call verifies drive
+//                  t % n's shard file of the thread's object, written with ALGO (3 = HighwayHash256S frames; 1, 2, 4 = a raw shard file
+//                  with its whole-file sum made once by mec_encode_whole), through ONE mec_batcher (mec_batcher_verify) or each a
+//                  mec_bitrot_verify_parts call on a handle from the pool.  Every call must return MEC_OK with a clean result.
 //   MIX=1        : the batcher of the b* modes is created with MEC_BATCHER_MIX_PATTERNS (reads of different patterns share batches)
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
 // Prints one JSON line: aggregate GiB/s, calls/s, p50/p99 latency.  Buffers are pinned (mec_alloc_pinned_on) for the GPU modes.
@@ -135,6 +139,8 @@ int main(int argc, char** argv) {
   const bool mixed_get = mode == "bget_mixed" || mode == "get_mixed";
   const int healed = getenv("HEALED") ? std::max(0, std::min(k + m, atoi(getenv("HEALED")))) : 8;
   const int mixed_stale = std::min(healed, k + m - 1);
+  const bool bverify = mode == "bverify", verify = bverify || mode == "verify";
+  const bool vwhole = verify && walgo != MEC_HIGHWAYHASH256S;
   const int64_t bs = move && getenv("SRC_BS") ? atoll(getenv("SRC_BS")) : 1 << 20;
   const int64_t bs2 = move && getenv("DST_BS") ? atoll(getenv("DST_BS")) : 1 << 20;
   const bool gpu = mode != "cpu";
@@ -171,7 +177,7 @@ int main(int argc, char** argv) {
     tb[t].dst = take(osize);
     tb[t].parity = take(nb * m * S);
     tb[t].healed = take(fsz);
-    if (mixed)
+    if (mixed || vwhole)
       for (int i = 0; i < n; i++) {
         tb[t].wfiles.push_back(alloc(static_cast<size_t>(std::max<int64_t>(1, mec_shard_file_size(probe, osize)))));
         if (!tb[t].wfiles.back()) { fprintf(stderr, "allocation failed\n"); return 1; }
@@ -188,7 +194,7 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
-  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove && !bmixed) {
+  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove && !bmixed && !bverify) {
     for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, whole ? walgo : MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
   }
   if (mode == "bget" || mode == "bheal") {  // coalesced GETs / heals: part files through a temporary handle, then everything goes through the batcher
@@ -218,6 +224,22 @@ int main(int argc, char** argv) {
     mec_codec_free(cs);
     mec_codec_free(cw);
     if (bmixed) {
+      int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
+                                  getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
+      if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
+    }
+  }
+  if (verify) {  // every drive's shard file in the format of ALGO through temporary handles; the batcher of bverify
+    mec_codec* c0 = nullptr;
+    mec_codec_new(k, m, bs, walgo, device, &c0);
+    for (int t = 0; t < T; t++) {
+      std::vector<uint8_t*> f(vwhole ? tb[t].wfiles : tb[t].files);
+      tb[t].wsums.assign(static_cast<size_t>(n) * 64, 0);
+      const int64_t rc = vwhole ? mec_encode_whole(c0, tb[t].obj, osize, f.data(), tb[t].wsums.data(), k) : mec_encode(c0, tb[t].obj, osize, f.data(), k);
+      if (rc != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
+    }
+    mec_codec_free(c0);
+    if (bverify) {
       int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
                                   getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
       if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
@@ -296,6 +318,17 @@ int main(int argc, char** argv) {
       const int rc = bmixed ? mec_batcher_heal_mixed(bat, al, f, b.wsums.data(), nullptr, osize, o, bad)
                             : mec_heal_mixed(pool[t % P], al, f, b.wsums.data(), nullptr, osize, o, bad);
       return rc == MEC_OK ? osize : rc;
+    }
+    if (verify) {  // one part: drive t % n's shard file as stored, its length, ShardFileSize(part.Size) and the whole-file sum
+      const int i = t % n;
+      const int algo = walgo;
+      const uint8_t* f = vwhole ? b.wfiles[i] : b.files[i];
+      const int64_t sfs = mec_shard_file_size(probe, osize);
+      const int64_t flen = vwhole ? sfs : fsz;
+      int res = -1;
+      const int rc = bverify ? mec_batcher_verify(bat, 1, &algo, &f, &flen, &sfs, b.wsums.data() + i * 64, &res)
+                             : mec_bitrot_verify_parts(pool[t % P], 1, &algo, &f, &flen, &sfs, b.wsums.data() + i * 64, &res);
+      return rc == MEC_OK && res == MEC_OK ? osize : rc ? rc : res;
     }
     if (move) {  // drive 0 offline in the _rot modes
       const uint8_t* f[64];
@@ -380,7 +413,10 @@ int main(int argc, char** argv) {
            (long long)mec_batcher_stat(bat, "us_scatter"));
   if (move) printf(", \"dst\": \"%d,%d\", \"src_block_size\": %lld, \"dst_block_size\": %lld", k2, m2, static_cast<long long>(bs),
                   static_cast<long long>(bs2));
-  if (whole || mixed) printf(", \"algo\": %d", walgo);
+  if (whole || mixed || verify) printf(", \"algo\": %d", walgo);
+  if (bverify)
+    printf(", \"verifies\": %lld, \"verifies_serial\": %lld, \"whole_hash_launches\": %lld", static_cast<long long>(mec_batcher_stat(bat, "verifies")),
+           static_cast<long long>(mec_batcher_stat(bat, "verifies_serial")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
   if (mixed) printf(", \"healed\": %d", healed);
   if (bmixed)
     printf(", \"reads_whole\": %lld, \"reads_whole_serial\": %lld, \"redone\": %lld, \"whole_hash_launches\": %lld",
@@ -394,7 +430,7 @@ int main(int argc, char** argv) {
            static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole")), static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole_serial")),
            static_cast<long long>(mec_batcher_stat(bat, "redone")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
   if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode" || mode == "transcode_whole" || mode == "get_mixed" ||
-      mode == "heal_mixed")
+      mode == "heal_mixed" || mode == "verify")
     printf(", \"pool\": %d", P);
   printf("}\n");
   if (bat) mec_batcher_free(bat);
