@@ -32,6 +32,7 @@ enum {
   MEC_ERR_READ_QUORUM = -10,      /* errErasureReadQuorum  cmd/erasure-errors.go:23 */
   MEC_ERR_WRITE_QUORUM = -11,     /* errErasureWriteQuorum cmd/erasure-errors.go:26 */
   MEC_ERR_INVALID_ARGUMENT = -12, /* errInvalidArgument */
+  MEC_ERR_NOT_AUTHENTIC = -13,    /* sio.NotAuthentic -> errObjectTampered  cmd/encryption-v1.go:57 */
   MEC_ERR_CUDA = -100,            /* CUDA runtime / driver failure (see mec_last_error) */
   MEC_ERR_NO_DEVICE = -101,       /* no CUDA device: the library never falls back to the CPU */
   MEC_ERR_UNSUPPORTED = -102      /* geometry or algorithm outside the GPU path (see DESIGN.md) */
@@ -568,6 +569,43 @@ int mec_bitrot_verify_batch(mec_codec* c, int64_t nfiles, const uint8_t* const* 
  * with every part MEC_HIGHWAYHASH256S on a HighwayHash256S codec, except that it refuses a NULL file with part_lens[f] > 0 per file. */
 int mec_bitrot_verify_parts(mec_codec* c, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
                             const int64_t* part_lens, const uint8_t* sums, int* results);
+
+/* ---- server-side encryption: DARE 2.0 packages (minio/sio v0.4.1, AES-256-GCM) ------------------------------------------------
+ * sio.EncryptReader with Version20 (newEncryptReader, cmd/encryption-v1.go:417-428) and DecryptBlocksRequestR (:572).  A package is
+ * header[16] = 0x20 | cipher | uint16 LE (payload_len - 1) | nonce[12], the ciphertext and a 16-byte tag; every package but the last
+ * carries 65536 bytes, bit 7 of header[4] marks the final one, the AEAD nonce is header[4:16] with bytes 8..11 (uint32 LE) XORed with
+ * the sequence number, the additional data header[0:4].  Keys come from the caller (KMS, sealing and DerivePartKey stay in Go); the
+ * key schedule and H powers of a call are zeroed on the device and the host before it returns.  ChaCha20-Poly1305 (cipher 1) and
+ * DARE 1.0 (version 0x10) are MEC_ERR_UNSUPPORTED.  Counters: "dare_sealed", "dare_opened" (package rows run by the kernel). */
+/* sio.EncryptedSize / DecryptedSize; a negative size, more than 2^32 packages or a remainder of 1..32 bytes is
+ * MEC_ERR_INVALID_ARGUMENT. */
+int64_t mec_dare_encrypted_size(int64_t n);
+int64_t mec_dare_decrypted_size(int64_t enc);
+/* Seal or open many streams in device memory in ONE launch (shaped like mec_sums_device).  Stream s: key keys + 32s, first package
+ * at sequence number seq0[s].  SEAL: plaintext d_in[in_off[s], + lens[s]) -> packages at d_out + out_off[s], nonce nonces + 12s, the
+ * last package final.  OPEN: packages d_in[in_off[s], + lens[s]) -> plaintext at d_out + out_off[s]; enc_totals[s] is the stored size
+ * of the part, which fixes each package's length and which one is final.  Each package is checked for version, length, final bit,
+ * nonce (the first package's, final bit masked) and tag, and only one that passes gets plaintext written.  status[s] (host): 0, 13
+ * (-MEC_ERR_NOT_AUTHENTIC: a package failed, the stored size is no DARE size, or bytes are cut short or run past the part) or 102
+ * (-MEC_ERR_UNSUPPORTED).  Returns MEC_ERR_UNSUPPORTED if any stream is, else MEC_ERR_NOT_AUTHENTIC if any failed, else MEC_OK; waits
+ * for its work on cuda_stream.  NULL arrays, negative offsets or lengths, an unknown op or a seal past sequence number 2^32 - 1 are
+ * MEC_ERR_INVALID_ARGUMENT before any device work. */
+#define MEC_DARE_SEAL 1
+#define MEC_DARE_OPEN 2
+int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uint8_t* keys, const uint8_t* nonces, const uint32_t* seq0,
+                    const int64_t* enc_totals, const uint8_t* d_in, const int64_t* in_off, const int64_t* lens, uint8_t* d_out,
+                    const int64_t* out_off, uint8_t* status, void* cuda_stream);
+/* EncryptRequest + Erasure.Encode (cmd/object-handlers.go:2070): seals `len` bytes with `key` and the caller's 12 random nonce bytes
+ * and writes mec_encode's part files of the sealed stream (sized for mec_dare_encrypted_size(len)).  Returns the plaintext bytes
+ * consumed.  "checksums" covers the plaintext. */
+int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint8_t key[32], const uint8_t nonce[12],
+                       uint8_t* const* files, int write_quorum);
+/* Erasure.Decode + DecryptBlocksRequestR of one part (multipart callers pass the part key, one call per part): plaintext
+ * [offset, offset + length) of a part stored as enc_total bytes; files / prefer / heal_hint as mec_decode_prefer.  Returns length,
+ * MEC_ERR_NOT_AUTHENTIC or MEC_ERR_UNSUPPORTED (dst[0, length) zeroed), or mec_decode_prefer's errors.  Each package is opened once;
+ * the ciphertext range and its plaintext are held in device buffers of the codec. */
+int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
+                       int64_t enc_total, const uint8_t key[32], uint8_t* dst, int* heal_hint);
 
 /* ---- shard-shaped low-level calls (keep Erasure.EncodeData / reedsolomon.Encoder shapes) ---- */
 /* reedsolomon.Encoder.Encode: shards[0..k) in, shards[k..k+m) out, each shard_len bytes (host). */

@@ -8,11 +8,13 @@ import numpy as np
 SHA256, HIGHWAYHASH256, HIGHWAYHASH256S, BLAKE2B512 = 1, 2, 3, 4
 ERRORS = {-1: "ErrInvShardNum", -2: "ErrMaxShardNum", -3: "ErrTooFewShards", -4: "ErrShardNoData", -5: "ErrShardSize",
           -6: "ErrShortData", -7: "errFileCorrupt", -8: "errLessData", -9: "errUnexpected", -10: "errErasureReadQuorum",
-          -11: "errErasureWriteQuorum", -12: "errInvalidArgument", -100: "CUDA error", -101: "no CUDA device",
+          -11: "errErasureWriteQuorum", -12: "errInvalidArgument", -13: "sio.NotAuthentic (errObjectTampered)", -100: "CUDA error", -101: "no CUDA device",
           -102: "unsupported on the GPU path"}
 MIX_PATTERNS = 1  # MEC_BATCHER_MIX_PATTERNS
 CRC32, CRC32C, CRC64NVME = 1, 2, 4  # MEC_CRC*
 SUM_MD5, SUM_SHA1, SUM_SHA256 = 8, 16, 32  # MEC_SUM_*
+DARE_SEAL, DARE_OPEN = 1, 2  # MEC_DARE_*
+NOT_AUTHENTIC = -13  # MEC_ERR_NOT_AUTHENTIC
 SUM_BYTES = 96  # MEC_SUM_BYTES: one record of mec_sums_device / mec_batcher_encode_sums
 SUM_SLOTS = {"md5": (SUM_MD5, 0, 16), "sha1": (SUM_SHA1, 32, 20), "sha256": (SUM_SHA256, 64, 32)}  # name -> (bit, offset, length)
 
@@ -145,6 +147,14 @@ def lib():
     L.mec_hh256_batch.argtypes = [vp, vp, i64, i64, vp]
     L.mec_selftest.argtypes = [i32]
     L.mec_set_option.argtypes = [vp, C.c_char_p, i64]
+    for f in ("mec_dare_encrypted_size", "mec_dare_decrypted_size"):
+        getattr(L, f).restype = i64
+        getattr(L, f).argtypes = [i64]
+    L.mec_dare_device.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mec_encode_sse.restype = i64
+    L.mec_encode_sse.argtypes = [vp, vp, i64, vp, vp, vp, i32]
+    L.mec_decode_sse.restype = i64
+    L.mec_decode_sse.argtypes = [vp, vp, vp, i64, i64, i64, vp, vp, C.POINTER(i32)]
     _LIB = L
     return L
 
@@ -317,6 +327,54 @@ class Codec:
 
     def stat(self, name):
         return lib().mec_get_stat(self.h, name.encode())
+
+    # -- server-side encryption (DARE 2.0, AES-256-GCM)
+    def encode_sse(self, src, key, nonce, online=None, write_quorum=0):
+        """mec_encode_sse -> part files"""
+        src, key, nonce = _u8(src), _u8(key), _u8(nonce)
+        if key.size != 32 or nonce.size != 12:
+            raise ValueError("key is 32 bytes, nonce 12")
+        enc = dare_encrypted_size(src.size)
+        fsz = self.bitrot_file_size(enc)
+        online = [True] * self.n if online is None else online
+        files = [np.zeros(fsz, dtype=np.uint8) if online[i] else None for i in range(self.n)]
+        rc = lib().mec_encode_sse(self.h, src.ctypes.data if src.size else None, src.size, key.ctypes.data, nonce.ctypes.data,
+                                  _ptrs(files), write_quorum)
+        if rc < 0:
+            raise MecError(rc, "mec_encode_sse")
+        return files
+
+    def decode_sse(self, files, offset, length, enc_total, key, prefer=None):
+        """mec_decode_sse -> (plaintext [offset, offset + length), heal_hint)"""
+        files = [None if f is None else _u8(f) for f in files]
+        key = _u8(key)
+        if key.size != 32:
+            raise ValueError("key is 32 bytes")
+        dst = np.zeros(max(length, 1), dtype=np.uint8)
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        rc = lib().mec_decode_sse(self.h, _ptrs(files), None if pf is None else pf.ctypes.data, offset, length, enc_total,
+                                  key.ctypes.data, dst.ctypes.data, C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_decode_sse")
+        return dst[:length], hint.value
+
+    def dare_device(self, op, keys, d_in, in_off, lens, d_out, out_off, seq0=None, nonces=None, enc_totals=None, stream=0,
+                    check=True):
+        """mec_dare_device over len(lens) streams -> (rc, per-stream status); check=True raises MecError on rc != 0"""
+        ns = len(lens)
+        keys = np.ascontiguousarray(keys, dtype=np.uint8).reshape(ns, 32)
+        seq = np.zeros(ns, dtype=np.uint32) if seq0 is None else np.ascontiguousarray(seq0, dtype=np.uint32)
+        arr = {name: np.ascontiguousarray(v, dtype=np.int64) for name, v in (("in", in_off), ("lens", lens), ("out", out_off))}
+        nn = None if nonces is None else np.ascontiguousarray(nonces, dtype=np.uint8).reshape(ns, 12)
+        et = None if enc_totals is None else np.ascontiguousarray(enc_totals, dtype=np.int64)
+        status = np.zeros(max(ns, 1), dtype=np.uint8)
+        rc = lib().mec_dare_device(self.h, op, ns, keys.ctypes.data, None if nn is None else nn.ctypes.data, seq.ctypes.data,
+                                   None if et is None else et.ctypes.data, d_in, arr["in"].ctypes.data, arr["lens"].ctypes.data,
+                                   d_out, arr["out"].ctypes.data, status.ctypes.data, stream)
+        if check and rc:
+            raise MecError(rc, "mec_dare_device")
+        return rc, status[:ns]
 
     def decode(self, files, offset, length, total, prefer=None):
         files = [None if f is None else _u8(f) for f in files]
@@ -792,6 +850,22 @@ class Batcher:
                 self._dst_sizes.close()
 
     __del__ = close
+
+
+def dare_encrypted_size(n):
+    """sio.EncryptedSize; MecError on an invalid size"""
+    v = lib().mec_dare_encrypted_size(n)
+    if v < 0:
+        raise MecError(v, "mec_dare_encrypted_size")
+    return v
+
+
+def dare_decrypted_size(n):
+    """sio.DecryptedSize; MecError on an invalid size"""
+    v = lib().mec_dare_decrypted_size(n)
+    if v < 0:
+        raise MecError(v, "mec_dare_decrypted_size")
+    return v
 
 
 def pinned_array(nbytes, device=None):

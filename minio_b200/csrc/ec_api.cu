@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <thread>
 #include <vector>
@@ -17,6 +18,7 @@
 #include "crc.cuh"
 #include "obj_hash.cuh"
 #include "batch_copy.cuh"
+#include "dare.cuh"
 #include <nvtx3/nvToolsExt.h>
 
 struct NvtxRange {
@@ -71,7 +73,18 @@ struct Slot {
   // each request's first stream behind them; one 64-byte digest per staged file
   DevBuf wtab, wdig;
   PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum, hwtab, hwdig;
+  DevBuf dpk;                        // mec_encode_sse: the DarePkg rows of the chunk's packages
+  PinBuf hdpk;
   cudaStream_t st = nullptr;
+};
+
+// DARE 2.0 state of a codec (dare.cuh): the AES round tables (built once), the key schedules and H powers of the streams of the
+// call in flight (zeroed before the call returns), a package table and its verdicts; mec_decode_sse's ciphertext and plaintext
+// of the range.
+struct DareState {
+  bool tabs_ok = false;
+  DevBuf tabs, keys, pk, st, ct, pt;
+  PinBuf hkeys, hpk, hst;
 };
 
 struct mec_codec {
@@ -99,6 +112,8 @@ struct mec_codec {
   // and their digests; they stay on the device for the whole call while the slot arenas cycle through the chunks
   DevBuf whole, whole_dig;
   PinBuf hwhole_dig;
+  DareState dare;
+  int64_t st_dare_sealed = 0, st_dare_opened = 0;  // DARE packages sealed / opened (rows launched)
   int64_t S() const { return ceil_frac(block_size, k); }
 };
 
@@ -220,7 +235,10 @@ extern "C" void mec_codec_free(mec_codec* c) {
     s.hdig.release(); s.hflags.release(); s.hcrc.release(); s.crc_part.release(); s.crc_out.release(); s.dreq.release(); s.hreq.release(); s.blk.release(); s.hblk.release();
     s.crc_tab.release(); s.hcrc_tab.release(); s.sum_tab.release(); s.sum_out.release(); s.hsum_tab.release(); s.hsum.release();
     s.wtab.release(); s.hwtab.release(); s.wdig.release(); s.hwdig.release();
+    s.dpk.release(); s.hdpk.release();
   }
+  for (DevBuf* b : {&c->dare.tabs, &c->dare.keys, &c->dare.pk, &c->dare.st, &c->dare.ct, &c->dare.pt}) b->release();
+  for (PinBuf* b : {&c->dare.hkeys, &c->dare.hpk, &c->dare.hst}) b->release();
   c->flags.release();
   c->crc_tables.release();
   c->whole.release(); c->whole_dig.release(); c->hwhole_dig.release();
@@ -258,6 +276,8 @@ extern "C" int64_t mec_get_stat(const mec_codec* c, const char* name) {
   if (!strcmp(name, "bytes_h2d")) return c->st_h2d;
   if (!strcmp(name, "bytes_d2h")) return c->st_d2h;
   if (!strcmp(name, "whole_hash_launches")) return c->st_whole_hash;
+  if (!strcmp(name, "dare_sealed")) return c->st_dare_sealed;
+  if (!strcmp(name, "dare_opened")) return c->st_dare_opened;
   if (!strcmp(name, "jit_compiles")) return c->eng ? c->eng->jit_compiles() : 0;
   if (!strcmp(name, "jit_launches")) return c->eng ? c->eng->jit_launches() : 0;
   if (!strcmp(name, "small_launches")) return c->eng ? c->eng->small_launches() : 0;
@@ -589,11 +609,32 @@ struct EncChunk {
   cudaStream_t st = nullptr;
 };
 
-// The six-slot H2D -> fused kernel -> D2H pipeline behind every host-buffer encode entry point.  `enqueue(ch)` adds the
+// What a chunk's staging step leaves on the device: the chunk's object bytes (16-byte aligned) and the bytes the option
+// "checksums" covers for it.
+struct Staged {
+  const uint8_t* obj = nullptr;
+  const uint8_t* ck = nullptr;
+  int64_t ck_len = 0;
+};
+// the plain staging step: the chunk's object bytes [off, off + bytes) of `src` copied into the slot
+static auto plain_stage(mec_codec* c, const uint8_t* src) {
+  return [c, src](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
+    int rc;
+    if ((rc = s.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
+    MEC_CUDA_OK(cudaMemcpyAsync(s.src.p, src + off, static_cast<size_t>(bytes), cudaMemcpyHostToDevice, s.st));
+    c->st_h2d += bytes;
+    o->obj = o->ck = static_cast<const uint8_t*>(s.src.p);
+    o->ck_len = bytes;
+    return MEC_OK;
+  };
+}
+
+// The six-slot H2D -> fused kernel -> D2H pipeline behind every host-buffer encode entry point, over `len` object bytes.
+// `stage(s, off, bytes, &staged)` puts the chunk's object bytes [off, off + bytes) on the device on s.st; `enqueue(ch)` adds the
 // chunk's device->host copies to ch.s->st right behind the kernel; `retire(ch)` runs on the host once that stream has
 // drained (digest scatter into frames).  On any error every slot stream is drained before returning (SlotDrain).
-template <class Enqueue, class Retire>
-static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueue&& enqueue, Retire&& retire) {
+template <class Stage, class Enqueue, class Retire>
+static int encode_pipeline(mec_codec* c, int64_t len, Stage&& stage, Enqueue&& enqueue, Retire&& retire) {
   const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
   const int64_t nall = ceil_frac(len, bs);
   int64_t chunk = pick_chunk_blocks(c);
@@ -633,24 +674,23 @@ static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueu
     ch.b0 = b0; ch.nb = std::min(chunk, nall - b0); ch.s = &s; ch.pitch = pitch;
     const int64_t off = b0 * bs, bytes = std::min(len - off, ch.nb * bs);
     ch.nfull = bytes / bs; ch.tail = bytes % bs;
-    if ((rc = s.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
     if ((rc = s.out.ensure(static_cast<size_t>(ch.nb * std::max(c->m, 1) * pitch)))) return rc;
     if ((rc = s.dig.ensure(static_cast<size_t>(ch.nb * c->n * 32)))) return rc;
-    MEC_CUDA_OK(cudaMemcpyAsync(s.src.p, src + off, static_cast<size_t>(bytes), cudaMemcpyHostToDevice, s.st));
+    Staged sg;
+    if ((rc = stage(s, off, bytes, &sg))) return rc;
     if ((rc = s.hdig.ensure(static_cast<size_t>(ch.nb * c->n * 32)))) return rc;
     ch.st = s.st;
-    ch.d_src = static_cast<const uint8_t*>(s.src.p); ch.d_src_tail = ch.d_src + ch.nfull * bs;
+    ch.d_src = sg.obj; ch.d_src_tail = ch.d_src + ch.nfull * bs;
     ch.d_out = static_cast<uint8_t*>(s.out.p); ch.d_out_tail = ch.d_out + ch.nfull * c->m * pitch;
     ch.h_dig = static_cast<const uint8_t*>(s.hdig.p); ch.h_dig_tail = ch.h_dig + ch.nfull * c->n * 32;
-    if ((rc = encode_device_locked(c, static_cast<const uint8_t*>(s.src.p), bytes, static_cast<uint8_t*>(s.out.p), pitch,
-                                   static_cast<uint8_t*>(s.dig.p), s.st)))
+    if ((rc = encode_device_locked(c, sg.obj, bytes, static_cast<uint8_t*>(s.out.p), pitch, static_cast<uint8_t*>(s.dig.p), s.st)))
       return rc;
     if (ck) {
       if ((rc = s.crc_out.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
       if ((rc = s.hcrc.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
-      if ((rc = checksums_enqueue(c, static_cast<const uint8_t*>(s.src.p), bytes, ck, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), s.st))) return rc;
+      if ((rc = checksums_enqueue(c, sg.ck, sg.ck_len, ck, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), s.st))) return rc;
       MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
-      ck_len[si] = bytes;
+      ck_len[si] = sg.ck_len;
     }
     if ((rc = enqueue(ch))) return rc;
     inflight[si] = ch;
@@ -658,7 +698,6 @@ static int encode_pipeline(mec_codec* c, const uint8_t* src, int64_t len, Enqueu
   }
   if ((rc = ring.finish())) return rc;
   c->st_blocks_encoded += nall;
-  c->st_h2d += len;
   return MEC_OK;
 }
 
@@ -676,7 +715,7 @@ extern "C" int mec_encode_blocks(mec_codec* c, const uint8_t* src, int64_t len, 
   MEC_CUDA_OK(cudaSetDevice(c->device));
   const int64_t S = c->S();
   rc = encode_pipeline(
-      c, src, len,
+      c, len, plain_stage(c, src),
       [&](const EncChunk& ch) -> int {
         Slot& s = *ch.s;
         if (c->m > 0 && ch.nfull > 0)
@@ -851,7 +890,7 @@ static int64_t encode_frames(mec_codec* c, const uint8_t* src, int64_t len, uint
   std::lock_guard<std::mutex> lk(c->mu);
   MEC_CUDA_OK(cudaSetDevice(c->device));
   rc = encode_pipeline(
-      c, src, len,
+      c, len, plain_stage(c, src),
       [&](const EncChunk& ch) { return frames_enqueue_chunk(c, ch, files, with_data, data_digests); },
       [&](const EncChunk& ch) { frames_retire(c, ch, files, with_data, data_digests); });
   return rc ? rc : len;
@@ -899,9 +938,13 @@ static int stage_frames(const uint8_t* host, void* dev, const FrameGeom& g, cuda
 //                writeDataBlocks (cmd/erasure-utils.go:42) done by the copy engines: one 2-D copy per data shard and chunk
 //   transcode sink (data movement between pools, mec_transcode): the data shards of every block re-split on the device into the
 //                object bytes of the whole part, encoded by the codec `enc` and written as complete frames of its geometry to enc_files
+//   sealed-object sink (mec_decode_sse): the object sink into a DEVICE buffer (dst_dev), and `accepted(si, blocks)` called on the
+//                host each time the range's first `blocks` blocks are final, with slot si the one that carried the last of them
 struct RangeSink {
   uint8_t* const* out = nullptr;
   uint8_t* dst = nullptr;
+  bool dst_dev = false;
+  std::function<int(int, int64_t)> accepted;
   mec_codec* enc = nullptr;
   uint8_t* const* enc_files = nullptr;
   int64_t first_block = 0;   // index (within the part) of the range's first block
@@ -1006,6 +1049,8 @@ static int emit_object(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
                        CopyList* list = nullptr) {
   const int k = c->k, r = ch.r;
   const int64_t bs = sk.bs, S = g.S, P = g.dpitch();
+  const cudaMemcpyKind kind = sk.dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  const int64_t d2h = sk.dst_dev ? 0 : 1;  // device-to-device moves are no copy-back
   for (int i = 0; i < k; i++) {
     // device source of data shard i: a staged survivor frame or a rebuilt row
     const uint8_t* base = nullptr;
@@ -1027,9 +1072,9 @@ static int emit_object(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
             list->add(sk.dst + ((B + q) * bs + static_cast<int64_t>(i) * S - sk.lo), base + (run0 + q) * spitch, w);
         } else {
           MEC_CUDA_OK(cudaMemcpy2DAsync(sk.dst + (B * bs + static_cast<int64_t>(i) * S - sk.lo), static_cast<size_t>(bs), base + run0 * spitch,
-                                        static_cast<size_t>(spitch), static_cast<size_t>(w), static_cast<size_t>(run1 - run0), cudaMemcpyDeviceToHost, s.st));
+                                        static_cast<size_t>(spitch), static_cast<size_t>(w), static_cast<size_t>(run1 - run0), kind, s.st));
         }
-        c->st_d2h += w * (run1 - run0);
+        c->st_d2h += d2h * w * (run1 - run0);
       }
       run0 = -1;
       return MEC_OK;
@@ -1045,8 +1090,8 @@ static int emit_object(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
       const DataSlice sl = data_slice(B, i, cur, bs, sk.total, sk.lo, sk.hi);
       if (sl.e > sl.a) {
         if (list) list->add(sk.dst + (sl.a - sk.lo), base + b * spitch + sl.off, sl.e - sl.a);
-        else MEC_CUDA_OK(cudaMemcpyAsync(sk.dst + (sl.a - sk.lo), base + b * spitch + sl.off, static_cast<size_t>(sl.e - sl.a), cudaMemcpyDeviceToHost, s.st));
-        c->st_d2h += sl.e - sl.a;
+        else MEC_CUDA_OK(cudaMemcpyAsync(sk.dst + (sl.a - sk.lo), base + b * spitch + sl.off, static_cast<size_t>(sl.e - sl.a), kind, s.st));
+        c->st_d2h += d2h * (sl.e - sl.a);
       }
     }
     if ((rc = flush(ch.nb))) return rc;
@@ -1349,6 +1394,7 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     c->st_blocks_read += good;
     c->st_shards_rebuilt += good * ch.r;
     done = ch.b0 + good;
+    if (good > 0 && sk.accepted && (rc = sk.accepted(si, done))) return rc;
     if (bad < ch.nb) {  // drop every chosen reader that failed at block `bad`, resume there with the next readers
       for (int t = 0; t < k; t++)
         if (fl[bad * k + t]) {
@@ -1549,6 +1595,304 @@ extern "C" int64_t mec_transcode(mec_codec* src, const uint8_t* const* files, co
     for (int i = 0; i < n; i++)
       if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
   return total;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Server-side encryption: DARE 2.0 packages (minio/sio, AES-256-GCM, dare.cuh).  A call's key schedule and H powers live on the
+// device only until it returns.
+constexpr int64_t kPkg = kDarePkg, kEPkg = kDareEPkg;
+constexpr int64_t kDareMaxPackages = int64_t{1} << 32;  // sequence numbers are uint32 (sio's maxPackageCount)
+
+extern "C" int64_t mec_dare_encrypted_size(int64_t n) {
+  if (n < 0 || n > kDareMaxPackages * kPkg) return MEC_ERR_INVALID_ARGUMENT;
+  return (n / kPkg) * kEPkg + (n % kPkg ? n % kPkg + kDareOverhead : 0);
+}
+extern "C" int64_t mec_dare_decrypted_size(int64_t e) {
+  if (e < 0 || e > kDareMaxPackages * kEPkg) return MEC_ERR_INVALID_ARGUMENT;
+  const int64_t r = e % kEPkg;
+  if (r > 0 && r <= kDareOverhead) return MEC_ERR_INVALID_ARGUMENT;
+  return (e / kEPkg) * kPkg + (r ? r - kDareOverhead : 0);
+}
+
+// Key schedules (host) and H powers (dare_setup_kernel) of `ns` streams into c->dare.keys, enqueued on `st`; nonces: seal only.
+static int dare_keys(mec_codec* c, int64_t ns, const uint8_t* keys, const uint8_t* nonces, cudaStream_t st) {
+  DareState& d = c->dare;
+  int rc;
+  if (!d.tabs_ok) {
+    if ((rc = d.tabs.ensure(sizeof(DareTables)))) return rc;
+    dare_tables_kernel<<<1, 256, 0, st>>>(static_cast<DareTables*>(d.tabs.p));
+    MEC_CUDA_OK(cudaGetLastError());
+    c->eng->count_launch();
+    d.tabs_ok = true;
+  }
+  const size_t bytes = static_cast<size_t>(ns) * sizeof(DareStreamKeys), head = offsetof(DareStreamKeys, hpow);
+  if ((rc = d.keys.ensure(bytes)) || (rc = d.hkeys.ensure(bytes))) return rc;
+  DareStreamKeys* h = static_cast<DareStreamKeys*>(d.hkeys.p);
+  for (int64_t s = 0; s < ns; s++) {
+    memset(&h[s], 0, head);
+    dare_expand_key(keys + 32 * s, h[s].rk);
+    if (nonces) memcpy(h[s].nonce, nonces + 12 * s, 12);
+  }
+  MEC_CUDA_OK(cudaMemcpy2DAsync(d.keys.p, sizeof(DareStreamKeys), h, sizeof(DareStreamKeys), head, static_cast<size_t>(ns),
+                                cudaMemcpyHostToDevice, st));
+  dare_setup_kernel<<<static_cast<unsigned>(ns), kDareThreads, 0, st>>>(static_cast<const DareTables*>(d.tabs.p),
+                                                                         static_cast<DareStreamKeys*>(d.keys.p));
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  return MEC_OK;
+}
+
+// Zeroes the key material of the call, device and host, once everything on `st` (and before it) is done with it.
+struct DareScrub {
+  mec_codec* c;
+  int64_t ns;
+  cudaStream_t st;
+  ~DareScrub() {
+    const size_t bytes = static_cast<size_t>(ns) * sizeof(DareStreamKeys);
+    cudaMemsetAsync(c->dare.keys.p, 0, bytes, st);
+    cudaStreamSynchronize(st);
+    explicit_bzero(c->dare.hkeys.p, bytes);
+  }
+};
+
+// ONE launch over n package rows (device table pk); open writes status[row]
+static int dare_launch(mec_codec* c, bool seal, const DarePkg* pk, int64_t n, const uint8_t* in, uint8_t* out, uint8_t* status,
+                       cudaStream_t st) {
+  if (n <= 0) return MEC_OK;
+  const DareTables* t = static_cast<const DareTables*>(c->dare.tabs.p);
+  const DareStreamKeys* k = static_cast<const DareStreamKeys*>(c->dare.keys.p);
+  if (seal) dare_kernel<true><<<static_cast<unsigned>(n), kDareThreads, 0, st>>>(t, k, pk, in, out, status);
+  else dare_kernel<false><<<static_cast<unsigned>(n), kDareThreads, 0, st>>>(t, k, pk, in, out, status);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  (seal ? c->st_dare_sealed : c->st_dare_opened) += n;
+  return MEC_OK;
+}
+
+static inline DarePkg dare_row(int64_t in_off, int64_t out_off, int64_t ref_off, int64_t len, int64_t seq, int stream, bool final) {
+  DarePkg r;
+  r.in_off = in_off; r.out_off = out_off; r.ref_off = ref_off;
+  r.len = static_cast<int32_t>(len); r.seq = static_cast<uint32_t>(seq); r.stream = stream; r.final = final ? 1 : 0;
+  return r;
+}
+
+extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uint8_t* keys, const uint8_t* nonces, const uint32_t* seq0,
+                               const int64_t* enc_totals, const uint8_t* d_in, const int64_t* in_off, const int64_t* lens, uint8_t* d_out,
+                               const int64_t* out_off, uint8_t* status, void* stream) {
+  NvtxRange nvtx("mec_dare_device");
+  if (!c || (op != MEC_DARE_SEAL && op != MEC_DARE_OPEN) || nstreams < 0 || nstreams > (int64_t{1} << 31) - 1)
+    return MEC_ERR_INVALID_ARGUMENT;
+  if (nstreams == 0) return MEC_OK;
+  const bool seal = op == MEC_DARE_SEAL;
+  if (!keys || !seq0 || !in_off || !lens || !out_off || !status || (seal ? !nonces : !enc_totals)) return MEC_ERR_INVALID_ARGUMENT;
+  int64_t rows = 0;
+  for (int64_t s = 0; s < nstreams; s++) {
+    if (in_off[s] < 0 || out_off[s] < 0 || lens[s] < 0 || (lens[s] > 0 && (!d_in || !d_out))) return MEC_ERR_INVALID_ARGUMENT;
+    const int64_t np = seal ? ceil_frac(lens[s], kPkg) : ceil_frac(lens[s], kEPkg);
+    if (seal && static_cast<int64_t>(seq0[s]) + np > kDareMaxPackages) return MEC_ERR_INVALID_ARGUMENT;
+    rows += np;
+  }
+  std::lock_guard<std::mutex> lk(c->mu);
+  int rc;
+  if ((rc = ensure_engine(c))) return rc;
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  DareState& d = c->dare;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t tab = static_cast<size_t>(std::max<int64_t>(rows, 1)) * sizeof(DarePkg);
+  if ((rc = d.hpk.ensure(tab)) || (rc = d.pk.ensure(tab)) || (rc = d.st.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))) ||
+      (rc = d.hst.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))))
+    return rc;
+  if ((rc = dare_keys(c, nstreams, keys, seal ? nonces : nullptr, st))) return rc;
+  DareScrub scrub{c, nstreams, st};
+  DarePkg* t = static_cast<DarePkg*>(d.hpk.p);
+  int64_t w = 0;
+  for (int64_t s = 0; s < nstreams; s++) {
+    status[s] = 0;
+    const int si = static_cast<int>(s);
+    if (seal) {  // a stream of lens[s] bytes from sequence number seq0[s]: its last package is final
+      const int64_t np = ceil_frac(lens[s], kPkg);
+      for (int64_t j = 0; j < np; j++)
+        t[w++] = dare_row(in_off[s] + j * kPkg, out_off[s] + j * kEPkg, 0, std::min(kPkg, lens[s] - j * kPkg), seq0[s] + j, si, j == np - 1);
+      continue;
+    }
+    // open: packages from seq0[s] as the stored part size lays them out; a size that is no DARE size, bytes past the part or a
+    // package cut short fail the stream (the whole packages before that point are still opened)
+    const int64_t D = mec_dare_decrypted_size(enc_totals[s]);
+    if (D < 0) { status[s] = static_cast<uint8_t>(-MEC_ERR_NOT_AUTHENTIC); continue; }
+    const int64_t npart = ceil_frac(D, kPkg);
+    for (int64_t pos = 0, p = seq0[s]; pos < lens[s]; p++) {
+      const int64_t plen = p == npart - 1 ? D - p * kPkg : kPkg;
+      if (p >= npart || pos + plen + kDareOverhead > lens[s]) { status[s] = static_cast<uint8_t>(-MEC_ERR_NOT_AUTHENTIC); break; }
+      t[w++] = dare_row(in_off[s] + pos, out_off[s] + (p - seq0[s]) * kPkg, in_off[s], plen, p, si, p == npart - 1);
+      pos += plen + kDareOverhead;
+    }
+  }
+  if (w > 0) {
+    MEC_CUDA_OK(cudaMemcpyAsync(d.pk.p, t, static_cast<size_t>(w) * sizeof(DarePkg), cudaMemcpyHostToDevice, st));
+    if ((rc = dare_launch(c, seal, static_cast<const DarePkg*>(d.pk.p), w, d_in, d_out, static_cast<uint8_t*>(d.st.p), st))) return rc;
+    if (!seal) MEC_CUDA_OK(cudaMemcpyAsync(d.hst.p, d.st.p, static_cast<size_t>(w), cudaMemcpyDeviceToHost, st));
+  }
+  MEC_CUDA_OK(cudaStreamSynchronize(st));
+  if (!seal) {
+    const uint8_t* v = static_cast<const uint8_t*>(d.hst.p);
+    for (int64_t r = 0; r < w; r++) {
+      uint8_t& o = status[t[r].stream];
+      if (v[r] == kDareUnsupported) o = static_cast<uint8_t>(-MEC_ERR_UNSUPPORTED);
+      else if (v[r] == kDareNotAuthentic && o == 0) o = static_cast<uint8_t>(-MEC_ERR_NOT_AUTHENTIC);
+    }
+  }
+  int worst = MEC_OK;
+  for (int64_t s = 0; s < nstreams; s++) {
+    if (status[s] == static_cast<uint8_t>(-MEC_ERR_UNSUPPORTED)) worst = MEC_ERR_UNSUPPORTED;
+    else if (status[s] && worst == MEC_OK) worst = MEC_ERR_NOT_AUTHENTIC;
+  }
+  return worst;
+}
+
+// EncryptRequest + Erasure.Encode: chunks are whole erasure blocks of the ciphertext.  A chunk stages and seals every package that
+// overlaps it (one across a chunk boundary is sealed in both: sealing is deterministic) and encodes its ciphertext unchanged.
+// "checksums" covers the plaintext, as hash.Reader sees it: each chunk the packages that start in it.
+extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint8_t* key, const uint8_t* nonce,
+                                  uint8_t* const* files, int write_quorum) {
+  NvtxRange nvtx("mec_encode_sse");
+  if (!c || len < 0 || !files || !key || !nonce || (len > 0 && !src)) return MEC_ERR_INVALID_ARGUMENT;
+  const int64_t E = mec_dare_encrypted_size(len);
+  if (E < 0) return E;
+  int online = 0;
+  for (int i = 0; i < c->n; i++) online += files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  if (len == 0) {
+    reset_last_checksums(c);
+    return 0;
+  }
+  int rc = require_streaming(c);
+  if (rc) return rc;
+  if (c->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
+  std::lock_guard<std::mutex> lk(c->mu);
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  Slot& s0 = c->slots[0];
+  if ((rc = dare_keys(c, 1, key, nonce, s0.st))) return rc;
+  DareScrub scrub{c, 1, s0.st};
+  MEC_CUDA_OK(cudaStreamSynchronize(s0.st));  // every slot stream reads the keys
+  const int64_t npk = ceil_frac(len, kPkg);
+  auto stage = [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
+    const int64_t p0 = off / kEPkg, p1 = (off + bytes - 1) / kEPkg, np = p1 - p0 + 1;
+    const int64_t pt0 = p0 * kPkg, pt1 = std::min(len, (p1 + 1) * kPkg);
+    // package p0 is sealed `pad` bytes into the slot so that ciphertext byte `off` lands 16-byte aligned for the encode
+    const int64_t delta = off - p0 * kEPkg, pad = (16 - delta % 16) % 16;
+    int e;
+    if ((e = s.aux.ensure(static_cast<size_t>(round_up(pt1 - pt0, 16) + 256))) || (e = s.src.ensure(static_cast<size_t>(pad + np * kEPkg + 256))) ||
+        (e = s.hdpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))) || (e = s.dpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))))
+      return e;
+    MEC_CUDA_OK(cudaMemcpyAsync(s.aux.p, src + pt0, static_cast<size_t>(pt1 - pt0), cudaMemcpyHostToDevice, s.st));
+    DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+    for (int64_t j = 0; j < np; j++) {
+      const int64_t p = p0 + j;
+      t[j] = dare_row(j * kPkg, pad + j * kEPkg, 0, std::min(kPkg, len - p * kPkg), p, 0, p == npk - 1);
+    }
+    MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, t, static_cast<size_t>(np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
+    uint8_t* ct = static_cast<uint8_t*>(s.src.p);
+    if ((e = dare_launch(c, true, static_cast<const DarePkg*>(s.dpk.p), np, static_cast<const uint8_t*>(s.aux.p), ct, nullptr, s.st))) return e;
+    c->st_h2d += pt1 - pt0;
+    o->obj = ct + pad + delta;
+    const int64_t ps = ceil_frac(off, kEPkg);  // the first package that starts in the chunk
+    o->ck = static_cast<const uint8_t*>(s.aux.p) + (ps - p0) * kPkg;
+    o->ck_len = ps <= p1 ? pt1 - ps * kPkg : 0;
+    return MEC_OK;
+  };
+  rc = encode_pipeline(
+      c, E, stage,
+      [&](const EncChunk& ch) { return frames_enqueue_chunk(c, ch, files, true, nullptr); },
+      [&](const EncChunk& ch) { frames_retire(c, ch, files, true, nullptr); });
+  return rc ? rc : len;
+}
+
+// Erasure.Decode of the ciphertext range GetDecryptedRange maps the plaintext range to, then DecryptBlocksRequestR, for one part.
+// Chunks move their data slices device-to-device into a ciphertext buffer of the range; whenever a prefix of the range is final
+// the packages it completes are opened, each once, and their asked-for plaintext is copied back.
+extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
+                                  int64_t enc_total, const uint8_t* key, uint8_t* dst, int* heal_hint) {
+  NvtxRange nvtx("mec_decode_sse");
+  if (heal_hint) *heal_hint = 0;
+  if (!c || !files || !key || offset < 0 || length < 0 || enc_total < 0) return MEC_ERR_INVALID_ARGUMENT;
+  const int64_t D = mec_dare_decrypted_size(enc_total);
+  if (D < 0) return MEC_ERR_NOT_AUTHENTIC;  // ObjectInfo.DecryptedSize: errObjectTampered
+  if (offset + length > D) return MEC_ERR_INVALID_ARGUMENT;
+  if (length == 0) return 0;
+  if (!dst) return MEC_ERR_INVALID_ARGUMENT;
+  int rc = require_streaming(c);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  const int k = c->k, n = c->n;
+  const int64_t bs = c->block_size, S = c->S();
+  const int64_t npk = ceil_frac(D, kPkg);
+  const int64_t p_first = offset / kPkg, p_last = (offset + length - 1) / kPkg, np = p_last - p_first + 1;
+  const int64_t eoff = p_first * kEPkg, eend = std::min(enc_total, (p_last + 1) * kEPkg), elen = eend - eoff;
+  const ReadRange rr = read_range(c, eoff, elen, enc_total);
+  const FrameGeom g{rr.nblocks, S, rr.last_len};
+  if (static_cast<int64_t>(k) * g.last_len < eend - rr.last_block * bs) return MEC_ERR_SHORT_DATA;  // as mec_decode_prefer
+  DareState& d = c->dare;
+  if ((rc = d.ct.ensure(static_cast<size_t>(round_up(elen, 16) + 256))) || (rc = d.pt.ensure(static_cast<size_t>(np * kPkg))) ||
+      (rc = d.st.ensure(static_cast<size_t>(np))) || (rc = d.hst.ensure(static_cast<size_t>(np))) ||
+      (rc = d.pk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))) || (rc = d.hpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))))
+    return rc;
+  Slot& s0 = c->slots[0];
+  if ((rc = dare_keys(c, 1, key, nullptr, s0.st))) return rc;
+  DareScrub scrub{c, 1, s0.st};
+  DarePkg* t = static_cast<DarePkg*>(d.hpk.p);
+  for (int64_t j = 0; j < np; j++) {
+    const int64_t p = p_first + j;
+    t[j] = dare_row(j * kEPkg, j * kPkg, 0, p == npk - 1 ? D - p * kPkg : kPkg, p, 0, p == npk - 1);
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(d.pk.p, t, static_cast<size_t>(np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s0.st));
+  MEC_CUDA_OK(cudaMemsetAsync(d.st.p, 0, static_cast<size_t>(np), s0.st));
+  MEC_CUDA_OK(cudaStreamSynchronize(s0.st));
+  uint8_t* ct = static_cast<uint8_t*>(d.ct.p);
+  const uint8_t* pt = static_cast<const uint8_t*>(d.pt.p);
+  int64_t opened = 0;
+  RangeSink sk;
+  sk.dst = ct; sk.dst_dev = true; sk.first_block = rr.start_block; sk.lo = eoff; sk.hi = eend; sk.bs = bs; sk.total = enc_total;
+  sk.accepted = [&](int si, int64_t blocks) -> int {
+    const int64_t acc = std::min(eend, (rr.start_block + blocks) * bs) - eoff;  // final ciphertext bytes of the range
+    const int64_t upto = acc == elen ? np : acc / kEPkg;                        // packages they complete
+    if (upto <= opened) return MEC_OK;
+    Slot& s = c->slots[si];
+    int e;
+    if ((e = dare_launch(c, false, static_cast<const DarePkg*>(d.pk.p) + opened, upto - opened, ct, static_cast<uint8_t*>(d.pt.p),
+                         static_cast<uint8_t*>(d.st.p) + opened, s.st)))
+      return e;
+    const int64_t a = std::max(offset, (p_first + opened) * kPkg), z = std::min(offset + length, (p_first + upto) * kPkg);
+    if (z > a) {
+      MEC_CUDA_OK(cudaMemcpyAsync(dst + (a - offset), pt + (a - p_first * kPkg), static_cast<size_t>(z - a), cudaMemcpyDeviceToHost, s.st));
+      c->st_d2h += z - a;
+    }
+    opened = upto;
+    return MEC_OK;
+  };
+  const int64_t fstride = 32 + S, foff = rr.start_block * fstride;
+  std::vector<const uint8_t*> in(n);
+  std::vector<uint8_t> alive(n), want(n, 0), corrupt(n, 0);
+  for (int i = 0; i < n; i++) { in[i] = files[i] ? files[i] + foff : nullptr; alive[i] = files[i] != nullptr; }
+  for (int i = 0; i < k; i++) want[i] = 1;
+  rc = reconstruct_range(c, in.data(), g, want.data(), 1, sk, corrupt.data(), alive.data(), prefer, false);
+  if (rc) return rc;  // every slot stream has drained
+  if (opened != np) return MEC_ERR_UNEXPECTED;
+  MEC_CUDA_OK(cudaMemcpy(d.hst.p, d.st.p, static_cast<size_t>(np), cudaMemcpyDeviceToHost));
+  const uint8_t* v = static_cast<const uint8_t*>(d.hst.p);
+  int bad = MEC_OK;
+  for (int64_t j = 0; j < np; j++) {
+    if (v[j] == kDareUnsupported) bad = MEC_ERR_UNSUPPORTED;
+    else if (v[j] != kDareOk && bad == MEC_OK) bad = MEC_ERR_NOT_AUTHENTIC;
+  }
+  if (bad) {  // failed packages wrote no plaintext: hand out nothing of the range
+    memset(dst, 0, static_cast<size_t>(length));
+    return bad;
+  }
+  if (heal_hint)
+    for (int i = 0; i < n; i++)
+      if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
+  return length;
 }
 
 // Batched heal (SURVEY §8f rank 2, BASELINE config 4): objects are independent, so a pool of codec handles — each with
