@@ -411,6 +411,34 @@ int mec_batcher_heal_mixed(mec_batcher* b, const int* algos, const uint8_t* cons
  * largest batch; nothing more is allocated when the batcher is created. */
 int mec_batcher_verify(mec_batcher* b, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
                        const int64_t* part_lens, const uint8_t* sums, int* results);
+/* mec_encode_sse / mec_decode_sse (below) through the coalescer: arguments, results, part files and refusals are theirs, with the
+ * batcher in place of the codec, and every refusal is made on the caller's thread before anything is queued.
+ * mec_batcher_encode_sse joins merged PUT batches (encrypted and plain PUTs share them) as its ciphertext of
+ * mec_dare_encrypted_size(len) bytes, which max_batch_blocks and the wake rule count.  A batch stages the plain requests and the
+ * encrypted requests' plaintext in ONE batched copy (the plaintext into a per-slot arena), runs ONE key-setup launch and ONE seal
+ * launch over every package of every encrypted request (each package sealed once, into a per-request ciphertext arena), moves each
+ * ciphertext into its place in the batch layout in one batched device-to-device copy, and encodes and scatters as for plain PUTs.
+ * Returns len.
+ * mec_batcher_decode_sse maps [offset, offset + length) to the ciphertext range of its whole packages and reads that range as an
+ * ordinary merged GET of the part (reader sets as mec_batcher_decode_prefer; any with MEC_BATCHER_MIX_PATTERNS); the batch assembles
+ * every encrypted request's ciphertext on the device, runs ONE key-setup and ONE open launch over every package, and copies each
+ * request's plaintext range back in one batched copy.  A request that met a frame failing its digest is redone alone through
+ * mec_decode_sse on the private handle (counted in "redone"); otherwise a package of ChaCha20-Poly1305 or DARE 1.0 returns
+ * MEC_ERR_UNSUPPORTED and any other failing package MEC_ERR_NOT_AUTHENTIC, with dst[0, length) zeroed.  One request's failure never
+ * affects its batch neighbours.
+ * Calls whose buffers are not page-locked, and MEC_BATCHER_MEMCPY, run through mec_encode_sse / mec_decode_sse on the private handle.
+ * Each slot holds its own key table: the device copy is zeroed on the slot's stream behind the batch's cipher launch, the host copy
+ * before any caller of the batch is woken, and no pointer to a caller's key outlives the call.  Device memory: each slot's plaintext
+ * arena is sized on its first encrypted batch for a full batch, B x block_size bytes (B = max_batch_blocks + min(64,
+ * max_batch_blocks / 8 + 4); with six slots, 6 x B x block_size in all), and grows past that only for a batch led by a request of
+ * more than B blocks; a PUT batch's ciphertext arena is the slot's survivor arena, which mec_batcher_new* sizes and PUT batches do
+ * not otherwise use.  The codec's AES tables are built, to completion, by the first encrypted batch.
+ * Counters (mec_batcher_stat): "sse_puts" and "sse_gets" (calls completed by merged batches), "sse_serial" (calls of the private
+ * path, redos included); "dare_sealed", "dare_opened" and "launches" are the batcher codec's. */
+int64_t mec_batcher_encode_sse(mec_batcher* b, const uint8_t* src, int64_t len, const uint8_t key[32], const uint8_t nonce[12],
+                               uint8_t* const* files, int write_quorum);
+int64_t mec_batcher_decode_sse(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
+                               int64_t enc_total, const uint8_t key[32], uint8_t* dst, int* heal_hint);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------
@@ -574,8 +602,8 @@ int mec_bitrot_verify_parts(mec_codec* c, int64_t nparts, const int* algos, cons
  * sio.EncryptReader with Version20 (newEncryptReader, cmd/encryption-v1.go:417-428) and DecryptBlocksRequestR (:572).  A package is
  * header[16] = 0x20 | cipher | uint16 LE (payload_len - 1) | nonce[12], the ciphertext and a 16-byte tag; every package but the last
  * carries 65536 bytes, bit 7 of header[4] marks the final one, the AEAD nonce is header[4:16] with bytes 8..11 (uint32 LE) XORed with
- * the sequence number, the additional data header[0:4].  Keys come from the caller (KMS, sealing and DerivePartKey stay in Go); the
- * key schedule and H powers of a call are zeroed on the device and the host before it returns.  ChaCha20-Poly1305 (cipher 1) and
+ * the sequence number, the additional data header[0:4].  Keys come from the caller (KMS, sealing and DerivePartKey stay in Go) and
+ * only the raw key goes to the device, whose setup launch expands it; the key schedule and H powers of a call are zeroed on the device and the host before it returns.  ChaCha20-Poly1305 (cipher 1) and
  * DARE 1.0 (version 0x10) are MEC_ERR_UNSUPPORTED.  Counters: "dare_sealed", "dare_opened" (package rows run by the kernel). */
 /* sio.EncryptedSize / DecryptedSize; a negative size, more than 2^32 packages or a remainder of 1..32 bytes is
  * MEC_ERR_INVALID_ARGUMENT. */

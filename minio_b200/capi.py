@@ -155,6 +155,10 @@ def lib():
     L.mec_encode_sse.argtypes = [vp, vp, i64, vp, vp, vp, i32]
     L.mec_decode_sse.restype = i64
     L.mec_decode_sse.argtypes = [vp, vp, vp, i64, i64, i64, vp, vp, C.POINTER(i32)]
+    L.mec_batcher_encode_sse.restype = i64
+    L.mec_batcher_encode_sse.argtypes = [vp, vp, i64, vp, vp, vp, i32]
+    L.mec_batcher_decode_sse.restype = i64
+    L.mec_batcher_decode_sse.argtypes = [vp, vp, vp, i64, i64, i64, vp, vp, C.POINTER(i32)]
     _LIB = L
     return L
 
@@ -837,6 +841,40 @@ class Batcher:
         """mec_batcher_verify: Codec.bitrot_verify_parts through the coalescer on this batcher's geometry (arguments and results as
         there).  Page-locked files (pinned_array) let the call ride in merged batches."""
         return _verify_parts(lib().mec_batcher_verify, self.h, "mec_batcher_verify", files, algos, part_lens, sums)
+
+    def encode_sse(self, src, key, nonce, online=None, write_quorum=0, pinned=False):
+        """mec_batcher_encode_sse: Codec.encode_sse through the coalescer -> part files.  A page-locked `src` (pinned_array) and
+        pinned=True (the part files are allocated page-locked; the caller owns and should free them) let the call ride in merged
+        batches."""
+        src, key, nonce = _u8(src), _u8(key), _u8(nonce)
+        if key.size != 32 or nonce.size != 12:
+            raise ValueError("key is 32 bytes, nonce 12")
+        fsz = self._sizes.bitrot_file_size(dare_encrypted_size(src.size))
+        online = [True] * self.n if online is None else online
+        mk = (lambda nb: pinned_array(max(nb, 1))[:nb]) if pinned else (lambda nb: np.zeros(nb, dtype=np.uint8))
+        files = [mk(fsz) if online[i] else None for i in range(self.n)]
+        rc = lib().mec_batcher_encode_sse(self.h, src.ctypes.data if src.size else None, src.size, key.ctypes.data, nonce.ctypes.data,
+                                          _ptrs(files), write_quorum)
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_encode_sse")
+        return files
+
+    def decode_sse(self, files, offset, length, enc_total, key, prefer=None, dst=None):
+        """mec_batcher_decode_sse: Codec.decode_sse through the coalescer; page-locked part files and a page-locked dst let the
+        call ride in merged batches.  -> (plaintext [offset, offset + length), heal_hint)"""
+        files = [None if f is None else _u8(f) for f in files]
+        key = _u8(key)
+        if key.size != 32:
+            raise ValueError("key is 32 bytes")
+        if dst is None:
+            dst = np.zeros(max(length, 1), dtype=np.uint8)
+        hint = C.c_int(0)
+        pf = None if prefer is None else np.asarray(prefer, dtype=np.uint8)
+        rc = lib().mec_batcher_decode_sse(self.h, _ptrs(files), None if pf is None else pf.ctypes.data, offset, length, enc_total,
+                                          key.ctypes.data, dst.ctypes.data, C.byref(hint))
+        if rc < 0:
+            raise MecError(rc, "mec_batcher_decode_sse")
+        return dst[:length], hint.value
 
     def stat(self, name):
         return lib().mec_batcher_stat(self.h, name.encode())

@@ -3,8 +3,9 @@
 // Package layout in include/minio_ec.h.  GCM: CTR from counter 2 (J0 = nonce | 1 masks the tag), GHASH over the additional-data
 // block, the ciphertext blocks and the length block.  One CTA per package, driven by a table of DarePkg rows (any number of streams
 // and keys per launch).  Thread t runs AES on GHASH blocks t, t + 256, ... and a Horner run over them with H^256, aligned by one
-// multiplication with H^e (1 <= e <= 256); the runs are XORed together.  dare_setup_kernel computes H = E_K(0) and H^1..H^256 per
-// stream, dare_tables_kernel the AES tables once per codec.  Open checks header, final bit, nonce and tag before any plaintext.
+// multiplication with H^e (1 <= e <= 256); the runs are XORed together.  dare_setup_kernel expands the key schedule and computes
+// H = E_K(0) and H^1..H^256 per stream from the raw key, dare_tables_kernel the AES tables once per codec.  Open checks header,
+// final bit, nonce and tag before any plaintext.
 #pragma once
 #include <cstdint>
 
@@ -27,11 +28,13 @@ struct DarePkg {
   int32_t final;    // the part's last package
 };
 
+// The host writes the first kDareKeyHead bytes of a stream (nonce and the raw key as rk[0..7]); dare_setup_kernel the rest.
 struct DareStreamKeys {
-  uint32_t rk[60];       // AES-256 key schedule, big-endian words
   uint8_t nonce[16];     // seal: the stream's 12 nonce bytes
-  uint64_t hpow[256][2]; // H^(e+1) as (hi, lo) big-endian halves (dare_setup_kernel)
+  uint32_t rk[60];       // AES-256 key schedule, big-endian words
+  uint64_t hpow[256][2]; // H^(e+1) as (hi, lo) big-endian halves
 };
+constexpr size_t kDareKeyHead = 16 + 32;
 
 struct DareTables {
   uint32_t te[4][256];
@@ -63,28 +66,6 @@ __host__ __device__ inline uint8_t dare_sbox(uint8_t x) {
   uint8_t s = inv;
   for (int i = 1; i <= 4; i++) s ^= static_cast<uint8_t>((inv << i) | (inv >> (8 - i)));
   return s ^ 0x63;
-}
-
-// AES-256 key expansion (FIPS-197 §5.2), on the host
-inline void dare_expand_key(const uint8_t key[32], uint32_t rk[60]) {
-  static uint8_t sb[256];
-  static bool init = [] { for (int i = 0; i < 256; i++) sb[i] = dare_sbox(static_cast<uint8_t>(i)); return true; }();
-  (void)init;
-  for (int i = 0; i < 8; i++)
-    rk[i] = (uint32_t(key[4 * i]) << 24) | (uint32_t(key[4 * i + 1]) << 16) | (uint32_t(key[4 * i + 2]) << 8) | key[4 * i + 3];
-  uint32_t rcon = 1;
-  for (int i = 8; i < 60; i++) {
-    uint32_t t = rk[i - 1];
-    if (i % 8 == 0) {
-      t = (t << 8) | (t >> 24);
-      t = (uint32_t(sb[t >> 24]) << 24) | (uint32_t(sb[(t >> 16) & 0xff]) << 16) | (uint32_t(sb[(t >> 8) & 0xff]) << 8) | sb[t & 0xff];
-      t ^= rcon << 24;
-      rcon = dare_gmul8(static_cast<uint8_t>(rcon), 2);
-    } else if (i % 8 == 4) {
-      t = (uint32_t(sb[t >> 24]) << 24) | (uint32_t(sb[(t >> 16) & 0xff]) << 16) | (uint32_t(sb[(t >> 8) & 0xff]) << 8) | sb[t & 0xff];
-    }
-    rk[i] = rk[i - 8] ^ t;
-  }
 }
 
 // Te0[x] = (2s, s, s, 3s) big-endian; Te1..Te3 are its byte rotations
@@ -210,34 +191,54 @@ __device__ __forceinline__ void dare_store(uint8_t* p, int n, const uint32_t w[4
   for (int j = 0; j < n; j++) p[j] = static_cast<uint8_t>(w[j >> 2] >> (24 - 8 * (j & 3)));
 }
 
-// Per stream: H = E_K(0^128) and its powers H^1..H^256 (thread t: H^(t+1) from the squares H^(2^j)).
+// Per stream (one CTA): the AES-256 key schedule from rk[0..7] (FIPS-197 §5.2), H = E_K(0^128) and H^1..H^256 by a doubling
+// ladder: at step j one thread builds the 4-bit table of H^(2^j), then threads t < 2^j make H^(2^j+t+1) = H^(t+1) * H^(2^j).
 __global__ void __launch_bounds__(kDareThreads) dare_setup_kernel(const DareTables* __restrict__ tabs, DareStreamKeys* keys) {
   __shared__ DareSmem sm;
-  __shared__ uint64_t sq[9][2];
+  __shared__ uint64_t hp[256][2];
   DareStreamKeys& K = keys[blockIdx.x];
   const int t = threadIdx.x;
   for (int i = t; i < 1024; i += kDareThreads) (&sm.te[0][0])[i] = (&tabs->te[0][0])[i];
   sm.sbox[t] = tabs->sbox[t];
-  if (t < 60) sm.rk[t] = K.rk[t];
+  if (t < 8) sm.rk[t] = K.rk[t];
+  if (t < 16) sm.r4[t] = dare_last4(t);
   __syncthreads();
   if (t == 0) {
+    const uint32_t* S = sm.sbox;
+    uint32_t rcon = 1;
+    for (int i = 8; i < 60; i++) {
+      uint32_t w = sm.rk[i - 1];
+      if (i % 8 == 0) {
+        w = (w << 8) | (w >> 24);
+        w = (S[w >> 24] << 24) | (S[(w >> 16) & 0xff] << 16) | (S[(w >> 8) & 0xff] << 8) | S[w & 0xff];
+        w ^= rcon << 24;
+        rcon = dare_gmul8(static_cast<uint8_t>(rcon), 2);
+      } else if (i % 8 == 4) {
+        w = (S[w >> 24] << 24) | (S[(w >> 16) & 0xff] << 16) | (S[(w >> 8) & 0xff] << 8) | S[w & 0xff];
+      }
+      sm.rk[i] = sm.rk[i - 8] ^ w;
+    }
     uint32_t h[4];
     dare_aes(sm, 0, 0, 0, 0, h);
-    sq[0][0] = (uint64_t(h[0]) << 32) | h[1];
-    sq[0][1] = (uint64_t(h[2]) << 32) | h[3];
-    for (int j = 1; j < 9; j++) dare_gfmul(sq[j - 1][0], sq[j - 1][1], sq[j - 1][0], sq[j - 1][1], sq[j][0], sq[j][1]);
+    hp[0][0] = (uint64_t(h[0]) << 32) | h[1];
+    hp[0][1] = (uint64_t(h[2]) << 32) | h[3];
   }
   __syncthreads();
-  const int e = t + 1;
-  uint64_t ah = 0, al = 0;
-  bool first = true;
-  for (int j = 0; j < 9; j++) {
-    if (!((e >> j) & 1)) continue;
-    if (first) { ah = sq[j][0]; al = sq[j][1]; first = false; }
-    else dare_gfmul(ah, al, sq[j][0], sq[j][1], ah, al);
+  if (t >= 8 && t < 60) K.rk[t] = sm.rk[t];
+#pragma unroll 1
+  for (int j = 0; j < 8; j++) {
+    const int p = 1 << j;  // hp[p - 1] = H^p
+    if (t == 0) dare_table4(hp[p - 1][0], hp[p - 1][1], sm.mh, sm.ml);
+    __syncthreads();
+    if (t < p) {
+      uint64_t xh = hp[t][0], xl = hp[t][1];
+      dare_mul_table(sm.mh, sm.ml, sm.r4, xh, xl);
+      hp[p + t][0] = xh; hp[p + t][1] = xl;
+    }
+    __syncthreads();
   }
-  K.hpow[t][0] = ah;
-  K.hpow[t][1] = al;
+  K.hpow[t][0] = hp[t][0];
+  K.hpow[t][1] = hp[t][1];
 }
 
 // kSeal: in = plaintext, out = the package.  Open: in = the package, out = plaintext; status[row] = kDare*.

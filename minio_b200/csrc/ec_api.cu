@@ -73,8 +73,13 @@ struct Slot {
   // each request's first stream behind them; one 64-byte digest per staged file
   DevBuf wtab, wdig;
   PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum, hwtab, hwdig;
-  DevBuf dpk;                        // mec_encode_sse: the DarePkg rows of the chunk's packages
+  DevBuf dpk;                        // mec_encode_sse: the DarePkg rows of the chunk's packages; a merged batch: of all its packages
   PinBuf hdpk;
+  // merged batches with encrypted requests (mec_batcher_encode_sse / _decode_sse): the streams' DareStreamKeys and their host-written
+  // heads, the plaintext arena, and the package verdicts of an open
+  DevBuf sse_keys, sse_pt, sse_st;
+  PinBuf hsse_keys, hsse_st;
+  int64_t sse_heads = 0;             // key heads written to hsse_keys by the slot's batch in flight (zeroed by batcher_finish)
   cudaStream_t st = nullptr;
 };
 
@@ -236,6 +241,7 @@ extern "C" void mec_codec_free(mec_codec* c) {
     s.crc_tab.release(); s.hcrc_tab.release(); s.sum_tab.release(); s.sum_out.release(); s.hsum_tab.release(); s.hsum.release();
     s.wtab.release(); s.hwtab.release(); s.wdig.release(); s.hwdig.release();
     s.dpk.release(); s.hdpk.release();
+    s.sse_keys.release(); s.sse_pt.release(); s.sse_st.release(); s.hsse_keys.release(); s.hsse_st.release();
   }
   for (DevBuf* b : {&c->dare.tabs, &c->dare.keys, &c->dare.pk, &c->dare.st, &c->dare.ct, &c->dare.pt}) b->release();
   for (PinBuf* b : {&c->dare.hkeys, &c->dare.hpk, &c->dare.hst}) b->release();
@@ -1614,32 +1620,52 @@ extern "C" int64_t mec_dare_decrypted_size(int64_t e) {
   return (e / kEPkg) * kPkg + (r ? r - kDareOverhead : 0);
 }
 
-// Key schedules (host) and H powers (dare_setup_kernel) of `ns` streams into c->dare.keys, enqueued on `st`; nonces: seal only.
-static int dare_keys(mec_codec* c, int64_t ns, const uint8_t* keys, const uint8_t* nonces, cudaStream_t st) {
+// The AES round tables of the codec, built by its first DARE call.  Built to completion before any use: later calls and merged batches
+// read them from other (non-blocking) slot streams, with nothing else ordering them after this launch.
+static int dare_tables(mec_codec* c, cudaStream_t st) {
   DareState& d = c->dare;
+  if (d.tabs_ok) return MEC_OK;
   int rc;
-  if (!d.tabs_ok) {
-    if ((rc = d.tabs.ensure(sizeof(DareTables)))) return rc;
-    dare_tables_kernel<<<1, 256, 0, st>>>(static_cast<DareTables*>(d.tabs.p));
-    MEC_CUDA_OK(cudaGetLastError());
-    c->eng->count_launch();
-    d.tabs_ok = true;
-  }
-  const size_t bytes = static_cast<size_t>(ns) * sizeof(DareStreamKeys), head = offsetof(DareStreamKeys, hpow);
-  if ((rc = d.keys.ensure(bytes)) || (rc = d.hkeys.ensure(bytes))) return rc;
-  DareStreamKeys* h = static_cast<DareStreamKeys*>(d.hkeys.p);
-  for (int64_t s = 0; s < ns; s++) {
-    memset(&h[s], 0, head);
-    dare_expand_key(keys + 32 * s, h[s].rk);
-    if (nonces) memcpy(h[s].nonce, nonces + 12 * s, 12);
-  }
-  MEC_CUDA_OK(cudaMemcpy2DAsync(d.keys.p, sizeof(DareStreamKeys), h, sizeof(DareStreamKeys), head, static_cast<size_t>(ns),
+  if ((rc = d.tabs.ensure(sizeof(DareTables)))) return rc;
+  dare_tables_kernel<<<1, 256, 0, st>>>(static_cast<DareTables*>(d.tabs.p));
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  MEC_CUDA_OK(cudaStreamSynchronize(st));
+  d.tabs_ok = true;
+  return MEC_OK;
+}
+
+// The first kDareKeyHead bytes of a stream's DareStreamKeys: its nonce (seal; zero for open) and its raw key as big-endian words
+static void dare_key_head(uint8_t* h, const uint8_t* key, const uint8_t* nonce) {
+  memset(h, 0, kDareKeyHead);
+  if (nonce) memcpy(h, nonce, 12);
+  uint32_t* rk = reinterpret_cast<uint32_t*>(h + offsetof(DareStreamKeys, rk));
+  for (int i = 0; i < 8; i++)
+    rk[i] = (uint32_t(key[4 * i]) << 24) | (uint32_t(key[4 * i + 1]) << 16) | (uint32_t(key[4 * i + 2]) << 8) | key[4 * i + 3];
+}
+
+// ONE dare_setup_kernel launch over `ns` streams on `st`: the key heads in `heads` (pinned, kDareKeyHead bytes each) go to the
+// device table `dk`, which the kernel completes with the key schedules and H powers
+static int dare_setup(mec_codec* c, DareStreamKeys* dk, const uint8_t* heads, int64_t ns, cudaStream_t st) {
+  int rc;
+  if ((rc = dare_tables(c, st))) return rc;
+  MEC_CUDA_OK(cudaMemcpy2DAsync(dk, sizeof(DareStreamKeys), heads, kDareKeyHead, kDareKeyHead, static_cast<size_t>(ns),
                                 cudaMemcpyHostToDevice, st));
-  dare_setup_kernel<<<static_cast<unsigned>(ns), kDareThreads, 0, st>>>(static_cast<const DareTables*>(d.tabs.p),
-                                                                         static_cast<DareStreamKeys*>(d.keys.p));
+  dare_setup_kernel<<<static_cast<unsigned>(ns), kDareThreads, 0, st>>>(static_cast<const DareTables*>(c->dare.tabs.p), dk);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
   return MEC_OK;
+}
+
+// Key schedules and H powers of `ns` streams into c->dare.keys, enqueued on `st`; nonces: seal only.
+static int dare_keys(mec_codec* c, int64_t ns, const uint8_t* keys, const uint8_t* nonces, cudaStream_t st) {
+  DareState& d = c->dare;
+  int rc;
+  if ((rc = d.keys.ensure(static_cast<size_t>(ns) * sizeof(DareStreamKeys))) || (rc = d.hkeys.ensure(static_cast<size_t>(ns) * kDareKeyHead)))
+    return rc;
+  uint8_t* h = static_cast<uint8_t*>(d.hkeys.p);
+  for (int64_t s = 0; s < ns; s++) dare_key_head(h + s * kDareKeyHead, keys + 32 * s, nonces ? nonces + 12 * s : nullptr);
+  return dare_setup(c, static_cast<DareStreamKeys*>(d.keys.p), h, ns, st);
 }
 
 // Zeroes the key material of the call, device and host, once everything on `st` (and before it) is done with it.
@@ -1648,19 +1674,17 @@ struct DareScrub {
   int64_t ns;
   cudaStream_t st;
   ~DareScrub() {
-    const size_t bytes = static_cast<size_t>(ns) * sizeof(DareStreamKeys);
-    cudaMemsetAsync(c->dare.keys.p, 0, bytes, st);
+    cudaMemsetAsync(c->dare.keys.p, 0, static_cast<size_t>(ns) * sizeof(DareStreamKeys), st);
     cudaStreamSynchronize(st);
-    explicit_bzero(c->dare.hkeys.p, bytes);
+    explicit_bzero(c->dare.hkeys.p, static_cast<size_t>(ns) * kDareKeyHead);
   }
 };
 
-// ONE launch over n package rows (device table pk); open writes status[row]
-static int dare_launch(mec_codec* c, bool seal, const DarePkg* pk, int64_t n, const uint8_t* in, uint8_t* out, uint8_t* status,
-                       cudaStream_t st) {
+// ONE launch over n package rows (device table pk) with the streams' keys `k`; open writes status[row]
+static int dare_launch(mec_codec* c, bool seal, const DareStreamKeys* k, const DarePkg* pk, int64_t n, const uint8_t* in, uint8_t* out,
+                       uint8_t* status, cudaStream_t st) {
   if (n <= 0) return MEC_OK;
   const DareTables* t = static_cast<const DareTables*>(c->dare.tabs.p);
-  const DareStreamKeys* k = static_cast<const DareStreamKeys*>(c->dare.keys.p);
   if (seal) dare_kernel<true><<<static_cast<unsigned>(n), kDareThreads, 0, st>>>(t, k, pk, in, out, status);
   else dare_kernel<false><<<static_cast<unsigned>(n), kDareThreads, 0, st>>>(t, k, pk, in, out, status);
   MEC_CUDA_OK(cudaGetLastError());
@@ -1668,6 +1692,7 @@ static int dare_launch(mec_codec* c, bool seal, const DarePkg* pk, int64_t n, co
   (seal ? c->st_dare_sealed : c->st_dare_opened) += n;
   return MEC_OK;
 }
+static const DareStreamKeys* dare_call_keys(const mec_codec* c) { return static_cast<const DareStreamKeys*>(c->dare.keys.p); }
 
 static inline DarePkg dare_row(int64_t in_off, int64_t out_off, int64_t ref_off, int64_t len, int64_t seq, int stream, bool final) {
   DarePkg r;
@@ -1729,7 +1754,7 @@ extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uin
   }
   if (w > 0) {
     MEC_CUDA_OK(cudaMemcpyAsync(d.pk.p, t, static_cast<size_t>(w) * sizeof(DarePkg), cudaMemcpyHostToDevice, st));
-    if ((rc = dare_launch(c, seal, static_cast<const DarePkg*>(d.pk.p), w, d_in, d_out, static_cast<uint8_t*>(d.st.p), st))) return rc;
+    if ((rc = dare_launch(c, seal, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p), w, d_in, d_out, static_cast<uint8_t*>(d.st.p), st))) return rc;
     if (!seal) MEC_CUDA_OK(cudaMemcpyAsync(d.hst.p, d.st.p, static_cast<size_t>(w), cudaMemcpyDeviceToHost, st));
   }
   MEC_CUDA_OK(cudaStreamSynchronize(st));
@@ -1792,7 +1817,7 @@ extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len,
     }
     MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, t, static_cast<size_t>(np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
     uint8_t* ct = static_cast<uint8_t*>(s.src.p);
-    if ((e = dare_launch(c, true, static_cast<const DarePkg*>(s.dpk.p), np, static_cast<const uint8_t*>(s.aux.p), ct, nullptr, s.st))) return e;
+    if ((e = dare_launch(c, true, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.p), np, static_cast<const uint8_t*>(s.aux.p), ct, nullptr, s.st))) return e;
     c->st_h2d += pt1 - pt0;
     o->obj = ct + pad + delta;
     const int64_t ps = ceil_frac(off, kEPkg);  // the first package that starts in the chunk
@@ -1859,7 +1884,7 @@ extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, con
     if (upto <= opened) return MEC_OK;
     Slot& s = c->slots[si];
     int e;
-    if ((e = dare_launch(c, false, static_cast<const DarePkg*>(d.pk.p) + opened, upto - opened, ct, static_cast<uint8_t*>(d.pt.p),
+    if ((e = dare_launch(c, false, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p) + opened, upto - opened, ct, static_cast<uint8_t*>(d.pt.p),
                          static_cast<uint8_t*>(d.st.p) + opened, s.st)))
       return e;
     const int64_t a = std::max(offset, (p_first + opened) * kPkg), z = std::min(offset + length, (p_first + upto) * kPkg);
@@ -3029,6 +3054,13 @@ struct BatchReq {
   const int64_t* vpart_lens = nullptr;
   const uint8_t* vsums = nullptr;
   int* vresults = nullptr;
+  // mec_batcher_encode_sse / _decode_sse: the stream's key (and a PUT's nonce), read by the worker while the caller waits; the
+  // plaintext bytes of a PUT (len is its ciphertext), the plaintext range and size of a GET (offset / length / total are the
+  // ciphertext range of its whole packages); where the batch placed its ciphertext and its first package row
+  const uint8_t* sse_key = nullptr;
+  const uint8_t* sse_nonce = nullptr;
+  int64_t sse_offset = 0, sse_len = 0, sse_total = 0;
+  int64_t sse_ct = 0, sse_row0 = 0;
   int64_t result = 0;
   bool done = false;
   std::condition_variable cv;  // one per request: a finished batch wakes its own callers, not every thread parked in the batcher
@@ -3099,6 +3131,8 @@ struct mec_batcher {
   std::atomic<int64_t> st_reads_whole{0}, st_reads_whole_serial{0};
   // mec_batcher_verify: calls completed by merged batches / by the private handle
   std::atomic<int64_t> st_verifies{0}, st_verifies_serial{0};
+  // mec_batcher_encode_sse / _decode_sse: calls completed by merged batches, and calls of the private path (redos included)
+  std::atomic<int64_t> st_sse_puts{0}, st_sse_gets{0}, st_sse_serial{0};
 };
 
 namespace {
@@ -3127,6 +3161,13 @@ static inline int whole_index(int algo) { return algo == MEC_SHA256 ? 0 : algo =
 // write quorum already checked on the caller's thread; a whole-file move does the same through mec_transcode_whole, whose source
 // handle carries the part's algorithm)
 static int64_t batcher_run_alone(mec_batcher* b, const BatchReq& r) {
+  if (r.sse_key) {  // an encrypted PUT or GET: mec_encode_sse / mec_decode_sse, the write quorum already checked
+    b->st_sse_serial++;
+    mec_codec* sc = batcher_private(b, b->codec, b->serial);
+    if (!sc) return MEC_ERR_UNEXPECTED;
+    if (r.kind == ReqKind::Put) return mec_encode_sse(sc, r.src, r.sse_len, r.sse_key, r.sse_nonce, r.files, 0);
+    return mec_decode_sse(sc, r.gfiles, r.prefer, r.sse_offset, r.sse_len, r.total, r.sse_key, r.dst, r.heal_hint);
+  }
   if (r.kind == ReqKind::TranscodeWhole) {
     b->st_transcodes_whole_serial++;
     mec_codec* sc = batcher_private(b, b->codec, b->serial_whole[whole_index(r.whole_algo)], r.whole_algo);
@@ -3162,7 +3203,7 @@ static void verify_whole_firsts(const std::vector<BatchReq*>& reqs, int64_t (&fi
 }
 
 // Completes the batch that ran on slot `s` (rc: how its stream ended) and wakes its callers.
-static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int rc) {
+static void batcher_finish(mec_batcher* b, InflightBatch& fb, Slot& s, int rc) {
   mec_codec* c = b->codec;
   if (fb.kind == ReqKind::Verify) {
     // the frame verdicts in s.hflags and the whole-file digests in s.hwdig, both in batcher_submit_verify's order
@@ -3200,7 +3241,7 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
     int64_t stream = 0;
     for (size_t q = 0; q < fb.reqs.size(); q++) {
       BatchReq* r = fb.reqs[q];
-      int64_t res = rc != MEC_OK ? rc : r->kind == ReqKind::Heal ? MEC_OK : is_move(r->kind) ? r->total : r->length;
+      int64_t res = rc != MEC_OK ? rc : r->kind == ReqKind::Heal ? MEC_OK : is_move(r->kind) ? r->total : r->sse_key ? r->sse_len : r->length;
       if (rc == MEC_OK) {
         bool bad = false;
         const uint32_t wpos = r->whole_algo ? tab[q].whole_pos : 0;
@@ -3218,6 +3259,21 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
           res = batcher_run_alone(b, *r);
         } else {
           if (r->heal_hint) *r->heal_hint = 0;
+          if (r->sse_key) {  // the verdicts of its packages (sse_get_open): a package that fails hands out nothing of the range
+            const uint8_t* v = static_cast<const uint8_t*>(s.hsse_st.p) + r->sse_row0;
+            const int64_t nrows = (r->sse_offset + r->sse_len - 1) / kPkg - r->sse_offset / kPkg + 1;
+            int64_t e = MEC_OK;
+            for (int64_t j = 0; j < nrows; j++) {
+              if (v[j] == kDareUnsupported) e = MEC_ERR_UNSUPPORTED;
+              else if (v[j] != kDareOk && e == MEC_OK) e = MEC_ERR_NOT_AUTHENTIC;
+            }
+            if (e != MEC_OK) {
+              memset(r->dst, 0, static_cast<size_t>(r->sse_len));
+              res = e;
+            } else {
+              b->st_sse_gets++;
+            }
+          }
           if (r->kind == ReqKind::Transcode) b->st_transcodes++;
           if (r->kind == ReqKind::TranscodeWhole) b->st_transcodes_whole++;
           if (r->algos && r->whole_algo) b->st_reads_whole++;
@@ -3240,8 +3296,13 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, const Slot& s, int
           if (r->sum_which & (MEC_SUM_MD5 << a)) memcpy(r->sums + 32 * a, h + 32 * a, static_cast<size_t>(sum_digest_len(a)));
         b->st_sum_requests++;
       }
-      r->result = rc == MEC_OK ? r->len : rc;
+      if (rc == MEC_OK && r->sse_key) b->st_sse_puts++;
+      r->result = rc != MEC_OK ? rc : r->sse_key ? r->sse_len : r->len;
     }
+  }
+  if (s.sse_heads) {  // the key heads this batch wrote (the device copy was zeroed behind the cipher)
+    explicit_bzero(s.hsse_keys.p, static_cast<size_t>(s.sse_heads) * kDareKeyHead);
+    s.sse_heads = 0;
   }
   {
     std::lock_guard<std::mutex> lk(b->mu);
@@ -3371,6 +3432,136 @@ static int batcher_sums_join(mec_batcher* b, Slot& s, size_t nreq, int64_t nwork
   return MEC_OK;
 }
 
+// Server-side encryption in merged batches (mec_batcher_encode_sse / _decode_sse).  The encrypted requests of a batch are the streams
+// of ONE dare_setup_kernel launch (stream z = the z-th such request in batch order) and their packages the rows of ONE dare_kernel
+// launch.  Each slot has its own key table, package table (s.dpk) and verdicts: six batches in flight never share key material.
+// The device keys are zeroed on the slot's stream behind the cipher launch, the host-written heads by batcher_finish.
+static int sse_batch_setup(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, bool seal, int64_t* nsse) {
+  *nsse = 0;
+  for (const BatchReq* r : reqs) *nsse += r->sse_key != nullptr;
+  if (*nsse == 0) return MEC_OK;
+  int rc;
+  if ((rc = s.sse_keys.ensure(static_cast<size_t>(*nsse) * sizeof(DareStreamKeys))) ||
+      (rc = s.hsse_keys.ensure(static_cast<size_t>(*nsse) * kDareKeyHead)))
+    return rc;
+  uint8_t* h = static_cast<uint8_t*>(s.hsse_keys.p);
+  for (const BatchReq* r : reqs)
+    if (r->sse_key) { dare_key_head(h, r->sse_key, seal ? r->sse_nonce : nullptr); h += kDareKeyHead; }
+  s.sse_heads = *nsse;
+  return dare_setup(b->codec, static_cast<DareStreamKeys*>(s.sse_keys.p), static_cast<const uint8_t*>(s.hsse_keys.p), *nsse, s.st);
+}
+// The plaintext arena: sized for a full batch (batcher_slot_blocks x block_size) on the slot's first encrypted batch; it only grows
+// past that for a batch led by a request larger than max_batch_blocks.  A batch's plaintext is at most its ciphertext, which batch
+// formation bounds.
+static int64_t batcher_slot_blocks(const mec_batcher* b);
+static int size_sse_arena(mec_batcher* b, Slot& s, int64_t bytes) {
+  return s.sse_pt.ensure(static_cast<size_t>(std::max(bytes, batcher_slot_blocks(b) * b->codec->block_size)));
+}
+// ONE cipher launch over the batch's package rows s.hdpk[0, rows) (an open writes its verdicts to s.sse_st), then the keys are zeroed
+static int sse_batch_cipher(mec_batcher* b, Slot& s, bool seal, int64_t nsse, int64_t rows, const uint8_t* in, uint8_t* out) {
+  MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, s.hdpk.p, static_cast<size_t>(rows) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
+  const int rc = dare_launch(b->codec, seal, static_cast<const DareStreamKeys*>(s.sse_keys.p), static_cast<const DarePkg*>(s.dpk.p), rows,
+                             in, out, seal ? nullptr : static_cast<uint8_t*>(s.sse_st.p), s.st);
+  if (rc) return rc;
+  MEC_CUDA_OK(cudaMemsetAsync(s.sse_keys.p, 0, static_cast<size_t>(nsse) * sizeof(DareStreamKeys), s.st));
+  return MEC_OK;
+}
+
+// The encrypted PUTs of a batch, before its staging copy: their plaintext goes to the arena s.sse_pt by pieces added to `h2d` (the
+// batch's one batched copy), their packages are laid out contiguously per request in the ciphertext arena s.aux (unused by PUT
+// batches; r->sse_ct), and the key setup is enqueued.  *rows = 0: the batch has no encrypted request.
+static int sse_put_plan(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, CopyList& h2d, int64_t* nsse, int64_t* rows) {
+  *rows = 0;
+  int64_t pt_total = 0, ct_total = 0;
+  for (const BatchReq* r : reqs)
+    if (r->sse_key) {
+      *rows += ceil_frac(r->sse_len, kPkg);
+      pt_total += round_up(r->sse_len, 256);
+      ct_total += round_up(r->len, 256);
+    }
+  if (*rows == 0) return MEC_OK;
+  int rc;
+  if ((rc = size_sse_arena(b, s, pt_total)) || (rc = s.aux.ensure(static_cast<size_t>(ct_total))) ||
+      (rc = s.dpk.ensure(static_cast<size_t>(*rows) * sizeof(DarePkg))) || (rc = s.hdpk.ensure(static_cast<size_t>(*rows) * sizeof(DarePkg))))
+    return rc;
+  DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+  uint8_t* pt = static_cast<uint8_t*>(s.sse_pt.p);
+  int64_t w = 0, po = 0, co = 0;
+  int z = 0;
+  for (BatchReq* r : reqs) {
+    if (!r->sse_key) continue;
+    const int64_t np = ceil_frac(r->sse_len, kPkg);
+    for (int64_t j = 0; j < np; j++) t[w++] = dare_row(po + j * kPkg, co + j * kEPkg, 0, std::min(kPkg, r->sse_len - j * kPkg), j, z, j == np - 1);
+    h2d.add(pt + po, r->src, r->sse_len);
+    r->sse_ct = co;
+    po += round_up(r->sse_len, 256);
+    co += round_up(r->len, 256);
+    z++;
+  }
+  return sse_batch_setup(b, s, reqs, true, nsse);
+}
+// Once the batch is staged: ONE seal launch over every package (each sealed once), then ONE batched device-to-device copy of each
+// request's ciphertext into its places in the PUT layout (full blocks at ch.d_src, the short last block at ch.d_src_tail)
+static int sse_put_seal(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t nsse, int64_t rows) {
+  if (rows == 0) return MEC_OK;
+  const uint8_t* ct = static_cast<const uint8_t*>(s.aux.p);
+  int rc = sse_batch_cipher(b, s, true, nsse, rows, static_cast<const uint8_t*>(s.sse_pt.p), static_cast<uint8_t*>(s.aux.p));
+  if (rc) return rc;
+  const int64_t bs = b->codec->block_size;
+  CopyList cl;
+  for (const BatchReq* r : reqs) {
+    if (!r->sse_key) continue;
+    cl.add(const_cast<uint8_t*>(r->ch.d_src), ct + r->sse_ct, r->ch.nfull * bs);
+    cl.add(const_cast<uint8_t*>(r->ch.d_src_tail), ct + r->sse_ct + r->ch.nfull * bs, r->ch.tail);
+  }
+  return cl.flush(s.st);
+}
+
+// The encrypted GETs of a batch, once the scatter has put each one's ciphertext range (whole packages) at s.src + asm_off[q]: ONE
+// setup and ONE open launch over every package into the arena s.sse_pt, the verdicts back to s.hsse_st (r->sse_row0 on), and ONE
+// batched copy of each request's plaintext range to its caller.  The arena is cleared first, so a package that fails leaves zeros.
+static int sse_get_open(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const std::vector<int64_t>& asm_off) {
+  int64_t rows = 0, pt_total = 0;
+  for (const BatchReq* r : reqs)
+    if (r->sse_key) {
+      const int64_t np = (r->sse_offset + r->sse_len - 1) / kPkg - r->sse_offset / kPkg + 1;
+      rows += np;
+      pt_total += np * kPkg;
+    }
+  if (rows == 0) return MEC_OK;
+  int rc;
+  if ((rc = size_sse_arena(b, s, pt_total)) || (rc = s.dpk.ensure(static_cast<size_t>(rows) * sizeof(DarePkg))) ||
+      (rc = s.hdpk.ensure(static_cast<size_t>(rows) * sizeof(DarePkg))) || (rc = s.sse_st.ensure(static_cast<size_t>(rows))) ||
+      (rc = s.hsse_st.ensure(static_cast<size_t>(rows))))
+    return rc;
+  int64_t nsse;
+  if ((rc = sse_batch_setup(b, s, reqs, false, &nsse))) return rc;
+  DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+  uint8_t* pt = static_cast<uint8_t*>(s.sse_pt.p);
+  CopyList d2h;
+  int64_t w = 0, po = 0;
+  int z = 0;
+  for (size_t q = 0; q < reqs.size(); q++) {
+    BatchReq* r = reqs[q];
+    if (!r->sse_key) continue;
+    const int64_t D = r->sse_total, npk = ceil_frac(D, kPkg);
+    const int64_t p0 = r->sse_offset / kPkg, np = (r->sse_offset + r->sse_len - 1) / kPkg - p0 + 1;
+    r->sse_row0 = w;
+    for (int64_t j = 0; j < np; j++) {
+      const int64_t p = p0 + j;
+      t[w++] = dare_row(asm_off[q] + j * kEPkg, po + j * kPkg, asm_off[q], p == npk - 1 ? D - p * kPkg : kPkg, p, z, p == npk - 1);
+    }
+    d2h.add(r->dst, pt + po + (r->sse_offset - p0 * kPkg), r->sse_len);
+    b->codec->st_d2h += r->sse_len;
+    po += np * kPkg;
+    z++;
+  }
+  MEC_CUDA_OK(cudaMemsetAsync(pt, 0, static_cast<size_t>(pt_total), s.st));
+  if ((rc = sse_batch_cipher(b, s, false, nsse, rows, static_cast<const uint8_t*>(s.src.p), pt))) return rc;
+  MEC_CUDA_OK(cudaMemcpyAsync(s.hsse_st.p, s.sse_st.p, static_cast<size_t>(rows), cudaMemcpyDeviceToHost, s.st));
+  return d2h.flush(s.st);
+}
+
 // The PUT layout of a merged batch on slot `s` of codec `c`, in request order: every request's full blocks contiguous from s.src
 // (from block full0 on), the short last blocks behind all of them at 256-byte-rounded offsets (block tail_slot, byte tail_src_off);
 // parity rows [block][m][pitch] in s.out, digests [block][n][32] in s.dig.  A request is r->len object bytes for the frames in
@@ -3483,8 +3674,9 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   const int k = c->k, m = c->m, n = c->n;
   const int64_t bs = c->block_size, S = c->S(), pitch = round_up(S, 16);
   *needs_retire = true;
-  bool all_mapped = n <= kBatchMaxFiles && !b->sw.memcpy;
-  for (BatchReq* r : reqs) all_mapped &= r->mapped;
+  bool all_mapped = n <= kBatchMaxFiles && !b->sw.memcpy, sse = false;
+  for (BatchReq* r : reqs) { all_mapped &= r->mapped; sse |= r->sse_key != nullptr; }
+  int64_t nsse = 0, sse_rows = 0;
   PutLayout lay;
   int rc;
   if ((rc = put_layout(c, s, reqs, all_mapped, true, lay))) return rc;
@@ -3499,7 +3691,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     const BatchReqDesc* tab = static_cast<const BatchReqDesc*>(s.hreq.p);
     for (const BatchReq* r : reqs) {
       const int64_t nf = r->len / bs, tl = r->len % bs;
-      c->st_h2d += r->len;
+      c->st_h2d += r->sse_key ? r->sse_len : r->len;
       c->st_d2h += (nf * S + (tl ? ceil_frac(tl, k) : 0)) * (r->with_data ? n : m);
     }
     const int si = static_cast<int>(&s - c->slots);
@@ -3516,8 +3708,9 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     // staging: the copy engines are the faster reader of host memory (one call per request); the gather kernel (SM loads over
     // PCIe, no per-request call at all) is kept for hosts where the worker thread is the bottleneck
     // requests [0, ndma) go through the copy engine, [ndma, nreq) through the gather kernel on the aux stream, concurrently
-    size_t ndma = b->sw.gather ? 0 : reqs.size();
-    if (!b->sw.gather && b->sw.gather_pct > 0 && b->aux && reqs.size() >= 8)
+    // (a batch with encrypted requests stages all of them by the copy engine: their plaintext goes to the arena, not the layout)
+    size_t ndma = b->sw.gather && !sse ? 0 : reqs.size();
+    if (!b->sw.gather && !sse && b->sw.gather_pct > 0 && b->aux && reqs.size() >= 8)
       ndma = reqs.size() - reqs.size() * static_cast<size_t>(b->sw.gather_pct) / 100;
     if (ndma < reqs.size()) {
       cudaStream_t gs = s.st;
@@ -3540,17 +3733,19 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     {
       // ONE cudaMemcpyBatchAsync for the whole batch: the copy engine runs a train of 1 MiB pieces at the link rate, faster than the
       // same pieces as separate cudaMemcpyAsync calls (tools/copy_probe.cu compares the two)
-      std::vector<void*> dsts, srcs;
-      std::vector<size_t> sizes;
+      CopyList cl;
       for (size_t q = 0; q < ndma; q++) {
+        if (reqs[q]->sse_key) continue;
         const BatchReqDesc& d = tab[q];
         const int64_t fbytes = d.len / bs * bs, tl = d.len - fbytes;
-        if (fbytes > 0) { dsts.push_back(dsrc + d.full0 * bs); srcs.push_back(const_cast<uint8_t*>(d.src)); sizes.push_back(static_cast<size_t>(fbytes)); }
-        if (tl > 0) { dsts.push_back(dsrc + d.tail_src_off); srcs.push_back(const_cast<uint8_t*>(d.src) + fbytes); sizes.push_back(static_cast<size_t>(tl)); }
+        cl.add(dsrc + d.full0 * bs, d.src, fbytes);
+        cl.add(dsrc + d.tail_src_off, d.src + fbytes, tl);
       }
-      if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
+      if ((rc = sse_put_plan(b, s, reqs, cl, &nsse, &sse_rows))) return rc;
+      if ((rc = cl.flush(s.st))) return rc;
     }
     if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[si], 0));
+    if ((rc = sse_put_seal(b, s, reqs, nsse, sse_rows))) return rc;
     mark_phase(b, s, 1);
     if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
     if ((rc = batcher_crc_launch(b, s, crc))) return rc;
@@ -3566,12 +3761,18 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   int64_t nsum;
   if ((rc = batcher_sums_table(b, s, reqs, &nsum))) return rc;
   for (BatchReq* r : reqs) {
+    if (r->sse_key) continue;
     const EncChunk& ch = r->ch;
     if (ch.nfull > 0)
       MEC_CUDA_OK(cudaMemcpyAsync(const_cast<uint8_t*>(ch.d_src), r->src, static_cast<size_t>(ch.nfull * bs), cudaMemcpyHostToDevice, s.st));
     if (ch.tail > 0)
       MEC_CUDA_OK(cudaMemcpyAsync(const_cast<uint8_t*>(ch.d_src_tail), r->src + ch.nfull * bs, static_cast<size_t>(ch.tail), cudaMemcpyHostToDevice, s.st));
     c->st_h2d += r->len;
+  }
+  if (sse) {  // encrypted requests beside a pageable one: their plaintext in one batched copy, then the seal into the layout
+    CopyList cl;
+    if ((rc = sse_put_plan(b, s, reqs, cl, &nsse, &sse_rows)) || (rc = cl.flush(s.st)) || (rc = sse_put_seal(b, s, reqs, nsse, sse_rows))) return rc;
+    for (const BatchReq* r : reqs) c->st_h2d += r->sse_key ? r->sse_len : 0;
   }
   if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
   if ((rc = batcher_crc_launch(b, s, crc))) return rc;
@@ -3869,12 +4070,17 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   // buffers instead of assembling there.
   const bool whole = reqs.front()->whole_algo != 0;
   const int out_mode = whole && b->sw.get_out == 0 ? 1 : b->sw.get_out;
-  std::vector<int64_t> asm_off(reqs.size(), 0);
-  if (out_mode == 0) {
+  // An encrypted GET's ciphertext range is assembled there in every mode, for sse_get_open (such a batch has no whole-file reader).
+  std::vector<int64_t> asm_off(reqs.size(), -1);
+  bool sse = false;
+  for (const BatchReq* r : reqs) sse |= r->sse_key != nullptr;
+  if (out_mode == 0 || sse) {
     int64_t total = 0;
-    for (size_t q = 0; q < reqs.size(); q++) { asm_off[q] = total; total += round_up(tab[q].length, 256); }
+    for (size_t q = 0; q < reqs.size(); q++)
+      if (out_mode == 0 || reqs[q]->sse_key) { asm_off[q] = total; total += round_up(tab[q].length, 256); }
     if ((rc = s.src.ensure(static_cast<size_t>(total + 256)))) return rc;
-    for (size_t q = 0; q < reqs.size(); q++) tab[q].dst = static_cast<uint8_t*>(s.src.p) + asm_off[q];
+    for (size_t q = 0; q < reqs.size(); q++)
+      if (asm_off[q] >= 0) tab[q].dst = static_cast<uint8_t*>(s.src.p) + asm_off[q];
   }
   WholeFiles wf;
   if (whole && (rc = batch_whole_stage(b, s, reqs, tab, &wf))) return rc;
@@ -3911,12 +4117,13 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
       std::vector<void*> dsts, srcs;
       std::vector<size_t> sizes;
       for (size_t q = 0; q < reqs.size(); q++) {
-        if (tab[q].length <= 0) continue;
+        if (tab[q].length <= 0 || reqs[q]->sse_key) continue;
         dsts.push_back(reqs[q]->dst); srcs.push_back(static_cast<uint8_t*>(s.src.p) + asm_off[q]); sizes.push_back(static_cast<size_t>(tab[q].length));
       }
       if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
     }
   }
+  if (sse && (rc = sse_get_open(b, s, reqs, asm_off))) return rc;
   mark_phase(b, s, 3);
   *nblocks = nslots;
   return MEC_OK;
@@ -4271,6 +4478,7 @@ static void batcher_main(mec_batcher* b) {
       const bool kernel_batch = fb.kind != ReqKind::Put || !fb.needs_retire;
       fb.traced = b->sw.trace && rc == MEC_OK && kernel_batch;
       if (rc != MEC_OK) {  // drain what was enqueued before the failure, then fail the whole batch
+        if (s.sse_keys.p) cudaMemsetAsync(s.sse_keys.p, 0, s.sse_keys.cap, s.st);  // a failure between key setup and cipher
         cudaStreamSynchronize(s.st);
         if (b->sum_st[head]) cudaStreamSynchronize(b->sum_st[head]);
         batcher_finish(b, fb, s, rc);
@@ -4592,22 +4800,13 @@ static int batch_readers(const mec_codec* c, BatchReq& r, bool* mapped) {
   return MEC_OK;
 }
 
-// Erasure.Decode through the coalescer: GETs that are queued together and read the same drives are merged into one launch — without
-// `prefer` the same drives online, with it the same k readers parallelReader picks; with MEC_BATCHER_MIX_PATTERNS any reads.
-// Calls whose buffers are not page-locked, and calls that meet bitrot, run on their own through a private handle.
-extern "C" int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset,
-                                             int64_t length, int64_t total, uint8_t* dst, int* heal_hint) {
-  if (heal_hint) *heal_hint = 0;
-  if (!b || !files) return MEC_ERR_INVALID_ARGUMENT;
-  if (offset < 0 || length < 0 || offset + length > total) return MEC_ERR_INVALID_ARGUMENT;  // cmd/erasure-decode.go:240-245
-  if (length == 0) return 0;
-  if (!dst) return MEC_ERR_INVALID_ARGUMENT;
+// A GET request `r` (files, range, dst and prefer set) into a merged batch, or on its own through the private handle when its buffers
+// are not page-locked: the reader set it merges on is chosen here, on the caller's thread.
+static int64_t batcher_get(mec_batcher* b, BatchReq& r) {
   const int n = b->codec->n, k = b->codec->k;
-  BatchReq r;
-  r.kind = ReqKind::Get; r.gfiles = files; r.offset = offset; r.length = length; r.total = total; r.dst = dst; r.heal_hint = heal_hint;
-  r.prefer = prefer;
-  bool mapped = !b->sw.memcpy && n <= kBatchMaxFiles && n <= 64 && k <= 32 && mec_is_pinned(dst) != 0;
-  if (prefer && n <= kBatchMaxFiles) {
+  const uint8_t* const* files = r.gfiles;
+  bool mapped = !b->sw.memcpy && n <= kBatchMaxFiles && n <= 64 && k <= 32 && mec_is_pinned(r.dst) != 0;
+  if (r.prefer && n <= kBatchMaxFiles) {
     // with preferReaders (cmd/erasure-decode.go:92-123): a k-bit mask equals an alive mask only when exactly those k drives are online
     const int rc = batch_readers(b->codec, r, &mapped);
     if (rc) return rc;
@@ -4624,6 +4823,22 @@ extern "C" int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* cons
       if (files[i]) { mapped = mec_is_pinned(files[i]) != 0; cnt++; }
   }
   return mapped ? batcher_enqueue_wait(b, r) : batcher_run_alone(b, r);
+}
+
+// Erasure.Decode through the coalescer: GETs that are queued together and read the same drives are merged into one launch — without
+// `prefer` the same drives online, with it the same k readers parallelReader picks; with MEC_BATCHER_MIX_PATTERNS any reads.
+// Calls whose buffers are not page-locked, and calls that meet bitrot, run on their own through a private handle.
+extern "C" int64_t mec_batcher_decode_prefer(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset,
+                                             int64_t length, int64_t total, uint8_t* dst, int* heal_hint) {
+  if (heal_hint) *heal_hint = 0;
+  if (!b || !files) return MEC_ERR_INVALID_ARGUMENT;
+  if (offset < 0 || length < 0 || offset + length > total) return MEC_ERR_INVALID_ARGUMENT;  // cmd/erasure-decode.go:240-245
+  if (length == 0) return 0;
+  if (!dst) return MEC_ERR_INVALID_ARGUMENT;
+  BatchReq r;
+  r.kind = ReqKind::Get; r.gfiles = files; r.offset = offset; r.length = length; r.total = total; r.dst = dst; r.heal_hint = heal_hint;
+  r.prefer = prefer;
+  return batcher_get(b, r);
 }
 extern "C" int64_t mec_batcher_decode(mec_batcher* b, const uint8_t* const* files, int64_t offset, int64_t length, int64_t total,
                                       uint8_t* dst, int* heal_hint) {
@@ -4850,6 +5065,56 @@ extern "C" int mec_batcher_verify(mec_batcher* b, int64_t nparts, const int* alg
   return static_cast<int>(batcher_enqueue_wait(b, r));
 }
 
+// EncryptRequest + Erasure.Encode through the coalescer: mec_encode_sse's refusals on the caller's thread, then the request joins a
+// merged PUT batch as its ciphertext of mec_dare_encrypted_size(len) bytes; the batch seals it (sse_put_plan, sse_put_seal).  Calls
+// whose buffers are not page-locked, and MEC_BATCHER_MEMCPY, go through mec_encode_sse on the private handle.
+extern "C" int64_t mec_batcher_encode_sse(mec_batcher* b, const uint8_t* src, int64_t len, const uint8_t* key, const uint8_t* nonce,
+                                          uint8_t* const* files, int write_quorum) {
+  NvtxRange nvtx("mec_batcher_encode_sse");
+  if (!b || len < 0 || !files || !key || !nonce || (len > 0 && !src)) return MEC_ERR_INVALID_ARGUMENT;
+  const int64_t E = mec_dare_encrypted_size(len);
+  if (E < 0) return E;
+  const int n = b->codec->n;
+  int online = 0;
+  for (int i = 0; i < n; i++) online += files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  if (len == 0) return 0;
+  BatchReq r;
+  r.src = src; r.len = E; r.files = files; r.with_data = true;
+  r.sse_key = key; r.sse_nonce = nonce; r.sse_len = len;
+  bool mapped = !b->sw.memcpy && mec_is_pinned(src) != 0;
+  for (int i = 0; i < n && mapped; i++)
+    if (files[i]) mapped = mec_is_pinned(files[i]) != 0;
+  r.mapped = mapped;
+  return mapped ? batcher_enqueue_wait(b, r) : batcher_run_alone(b, r);
+}
+
+// Erasure.Decode + DecryptBlocksRequestR through the coalescer, one part per call: mec_decode_sse's refusals on the caller's thread,
+// then the ciphertext range of the whole packages that hold [offset, offset + length) is read as an ordinary merged GET (the reader
+// rules of mec_batcher_decode_prefer) and opened by the batch (sse_get_open).  A request that meets bitrot is redone alone through
+// mec_decode_sse on the private handle, as are calls whose buffers are not page-locked.
+extern "C" int64_t mec_batcher_decode_sse(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset,
+                                          int64_t length, int64_t enc_total, const uint8_t* key, uint8_t* dst, int* heal_hint) {
+  NvtxRange nvtx("mec_batcher_decode_sse");
+  if (heal_hint) *heal_hint = 0;
+  if (!b || !files || !key || offset < 0 || length < 0 || enc_total < 0) return MEC_ERR_INVALID_ARGUMENT;
+  const int64_t D = mec_dare_decrypted_size(enc_total);
+  if (D < 0) return MEC_ERR_NOT_AUTHENTIC;  // ObjectInfo.DecryptedSize: errObjectTampered
+  if (offset + length > D) return MEC_ERR_INVALID_ARGUMENT;
+  if (length == 0) return 0;
+  if (!dst) return MEC_ERR_INVALID_ARGUMENT;
+  const mec_codec* c = b->codec;
+  const int64_t p_first = offset / kPkg, p_last = (offset + length - 1) / kPkg;
+  const int64_t eoff = p_first * kEPkg, eend = std::min(enc_total, (p_last + 1) * kEPkg);
+  const ReadRange rr = read_range(c, eoff, eend - eoff, enc_total);
+  if (static_cast<int64_t>(c->k) * rr.last_len < eend - rr.last_block * c->block_size) return MEC_ERR_SHORT_DATA;  // as mec_decode_sse
+  BatchReq r;
+  r.kind = ReqKind::Get; r.gfiles = files; r.offset = eoff; r.length = eend - eoff; r.total = enc_total; r.dst = dst;
+  r.heal_hint = heal_hint; r.prefer = prefer;
+  r.sse_key = key; r.sse_offset = offset; r.sse_len = length; r.sse_total = D;
+  return batcher_get(b, r);
+}
+
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!b || !name) return -1;
   if (!strcmp(name, "batches")) return b->st_batches.load();
@@ -4877,6 +5142,9 @@ extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
   if (!strcmp(name, "reads_whole_serial")) return b->st_reads_whole_serial.load();
   if (!strcmp(name, "verifies")) return b->st_verifies.load();
   if (!strcmp(name, "verifies_serial")) return b->st_verifies_serial.load();
+  if (!strcmp(name, "sse_puts")) return b->st_sse_puts.load();
+  if (!strcmp(name, "sse_gets")) return b->st_sse_gets.load();
+  if (!strcmp(name, "sse_serial")) return b->st_sse_serial.load();
   if (!strncmp(name, "dst_", 4)) return b->dst ? mec_get_stat(b->dst, name + 4) : -1;  // the destination codec of merged moves
   return mec_get_stat(b->codec, name);  // the batcher's codec: which kernel forms its merged launches ran ("form_*", "last_*", ...)
 }

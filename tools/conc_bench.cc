@@ -33,6 +33,13 @@
 //                  t % n's shard file of the thread's object, written with ALGO (3 = HighwayHash256S frames; 1, 2, 4 = a raw shard file
 //                  with its whole-file sum made once by mec_encode_whole), through ONE mec_batcher (mec_batcher_verify) or each a
 //                  mec_bitrot_verify_parts call on a handle from the pool.  Every call must return MEC_OK with a clean result.
+//   mode bsse_put / sse_put : encrypted PUTs (DARE 2.0, a key and nonce per thread) through ONE mec_batcher (mec_batcher_encode_sse)
+//                  or each a mec_encode_sse call on a handle from the pool; after the timed window every thread's part files are
+//                  compared with a mec_encode_sse of its object here
+//   mode bsse_get / sse_get : degraded GETs (4 data drives offline) of whole encrypted objects through ONE mec_batcher
+//                  (mec_batcher_decode_sse) or each a mec_decode_sse call on a handle from the pool
+//   mode bsse_mixget : even threads GET encrypted objects, odd threads plain ones, through ONE mec_batcher (the two kinds share batches)
+//                  (after the timed window every GET's bytes are compared with the object)
 //   MIX=1        : the batcher of the b* modes is created with MEC_BATCHER_MIX_PATTERNS (reads of different patterns share batches)
 //   mode cpu     : the C oracle's SIMD encode + HighwayHash on the calling thread (the reference's per-request CPU path)
 // Prints one JSON line: aggregate GiB/s, calls/s, p50/p99 latency.  Buffers are pinned (mec_alloc_pinned_on) for the GPU modes.
@@ -144,10 +151,21 @@ int main(int argc, char** argv) {
   const int64_t bs = move && getenv("SRC_BS") ? atoll(getenv("SRC_BS")) : 1 << 20;
   const int64_t bs2 = move && getenv("DST_BS") ? atoll(getenv("DST_BS")) : 1 << 20;
   const bool gpu = mode != "cpu";
+  const bool bsse = mode == "bsse_put" || mode == "bsse_get" || mode == "bsse_mixget";  // through the batcher
+  const bool sse = bsse || mode == "sse_put" || mode == "sse_get";
+  const bool sse_put = mode == "bsse_put" || mode == "sse_put";
   mec_codec* probe = nullptr;
   mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &probe);
-  const int64_t S = mec_shard_size(probe), fsz = mec_bitrot_shard_file_size(mec_shard_file_size(probe, osize), S, MEC_HIGHWAYHASH256S);
-  const int64_t nb = (osize + bs - 1) / bs;
+  // an encrypted object is stored as its DARE 2.0 stream: part files are sized for that
+  const int64_t esize = sse ? mec_dare_encrypted_size(osize) : osize;
+  const int64_t S = mec_shard_size(probe), fsz = mec_bitrot_shard_file_size(mec_shard_file_size(probe, esize), S, MEC_HIGHWAYHASH256S);
+  const int64_t nb = (esize + bs - 1) / bs;
+  // thread t's key and nonce (encrypted modes; bsse_mixget: even threads)
+  auto sse_key = [](int t, uint8_t* key, uint8_t* nonce) {
+    for (int i = 0; i < 32; i++) key[i] = static_cast<uint8_t>(t * 131 + i * 7 + 1);
+    for (int i = 0; i < 12; i++) nonce[i] = static_cast<uint8_t>(t * 17 + i * 29 + 3);
+  };
+  auto encrypted = [&](int t) { return sse && (mode != "bsse_mixget" || t % 2 == 0); };
   int k2 = 6, m2 = 2;
   if (const char* e = getenv("DST")) sscanf(e, "%d,%d", &k2, &m2);
   const int n2 = k2 + m2;
@@ -162,7 +180,8 @@ int main(int argc, char** argv) {
               uint8_t sums[MEC_SUM_BYTES];
               std::vector<uint8_t> wsums;  // whole-file and mixed modes: the expected digest of every source shard file, n x 64
               std::vector<uint8_t*> wfiles;  // mixed modes: every drive's raw shard file of the whole-file algorithm
-              std::vector<uint8_t*> outs; };  // outs: the destination part files of the transcode modes
+              std::vector<uint8_t*> outs;  // outs: the destination part files of the transcode modes
+              uint8_t key[32], nonce[12]; };  // outs: the destination part files of the transcode modes
   std::vector<TB> tb(T);
   uint8_t* arena = alloc(static_cast<size_t>(T) * (osize * 2 + (n + 1) * fsz + nb * n * 32 + nb * m * S + 4096 * 25));
   if (!arena) { fprintf(stderr, "allocation failed\n"); return 1; }
@@ -194,7 +213,7 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d %s\n", rc, mec_last_error()); return 1; }
-  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove && !bmixed && !bverify) {
+  } else if (gpu && mode != "bget" && mode != "bheal" && !bmove && !bmixed && !bverify && !bsse) {
     for (int i = 0; i < P; i++) { mec_codec* c = nullptr; mec_codec_new(k, m, bs, whole ? walgo : MEC_HIGHWAYHASH256S, device, &c); if (getenv("POOL_JIT")) mec_set_option(c, "jit", 1); pool.push_back(c); }
   }
   if (mode == "bget" || mode == "bheal") {  // coalesced GETs / heals: part files through a temporary handle, then everything goes through the batcher
@@ -207,6 +226,23 @@ int main(int argc, char** argv) {
     int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512, getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100,
                                 bflags, &bat);
     if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
+  }
+  if (sse) {  // keys; the stored parts of the GET modes through a temporary handle; the batcher of the bsse_* modes
+    mec_codec* c0 = nullptr; mec_codec_new(k, m, bs, MEC_HIGHWAYHASH256S, device, &c0);
+    for (int t = 0; t < T; t++) {
+      sse_key(t, tb[t].key, tb[t].nonce);
+      if (sse_put) continue;
+      std::vector<uint8_t*> f(tb[t].files);
+      const int64_t rc = encrypted(t) ? mec_encode_sse(c0, tb[t].obj, osize, tb[t].key, tb[t].nonce, f.data(), k)
+                                      : mec_encode(c0, tb[t].obj, osize, f.data(), k);
+      if (rc != osize) { fprintf(stderr, "prep encode failed\n"); return 1; }
+    }
+    mec_codec_free(c0);
+    if (bsse) {
+      int rc = mec_batcher_new_ex(k, m, bs, device, getenv("MAX_BATCH") ? atoll(getenv("MAX_BATCH")) : 512,
+                                  getenv("MAX_WAIT_US") ? atoi(getenv("MAX_WAIT_US")) : 100, bflags, &bat);
+      if (rc) { fprintf(stderr, "batcher: %d\n", rc); return 1; }
+    }
   }
   if (mixed) {  // both formats of every part through temporary handles; the batcher of the b*_mixed modes
     mec_codec* cs = nullptr;
@@ -301,6 +337,18 @@ int main(int argc, char** argv) {
       const int rc = mode == "bheal" ? mec_batcher_heal(bat, f, nullptr, osize, o, bad) : mec_heal_prefer(pool[t % P], f, nullptr, osize, o, bad);
       return rc == MEC_OK ? osize : rc;
     }
+    if (sse_put) {
+      if (mode == "bsse_put") return mec_batcher_encode_sse(bat, b.obj, osize, b.key, b.nonce, b.files.data(), k + 1);
+      return mec_encode_sse(pool[t % P], b.obj, osize, b.key, b.nonce, b.files.data(), k + 1);
+    }
+    if (sse) {  // 4 data drives offline
+      const uint8_t* f[64];
+      for (int i = 0; i < n; i++) f[i] = i < 4 ? nullptr : b.files[i];
+      int hint = 0;
+      if (!encrypted(t)) return mec_batcher_decode(bat, f, 0, osize, osize, b.dst, &hint);
+      if (bsse) return mec_batcher_decode_sse(bat, f, nullptr, 0, osize, esize, b.key, b.dst, &hint);
+      return mec_decode_sse(pool[t % P], f, nullptr, 0, osize, esize, b.key, b.dst, &hint);
+    }
     if (mixed) {  // drives [0, healed) stream, the others are raw shard files; a heal rebuilds drive mixed_stale
       const uint8_t* f[64];
       uint8_t* o[64] = {};
@@ -369,6 +417,19 @@ int main(int argc, char** argv) {
       if (mixed_get ? memcmp(tb[t].dst, tb[t].obj, static_cast<size_t>(osize)) != 0
                     : memcmp(tb[t].healed, tb[t].files[mixed_stale], static_cast<size_t>(fsz)) != 0)
         errors++;
+  if (sse_put) {  // every thread's part files equal a mec_encode_sse of its object with its key and nonce
+    std::vector<uint8_t*> want(n);
+    for (int i = 0; i < n; i++) want[i] = static_cast<uint8_t*>(malloc(static_cast<size_t>(fsz)));
+    for (int t = 0; t < T; t++) {
+      if (mec_encode_sse(probe, tb[t].obj, osize, tb[t].key, tb[t].nonce, want.data(), k) != osize) { errors++; continue; }
+      for (int i = 0; i < n; i++)
+        if (memcmp(tb[t].files[i], want[i], static_cast<size_t>(fsz)) != 0) errors++;
+    }
+    for (auto w : want) free(w);
+  } else if (sse) {  // every GET's bytes equal the object
+    for (int t = 0; t < T; t++)
+      if (memcmp(tb[t].dst, tb[t].obj, static_cast<size_t>(osize)) != 0) errors++;
+  }
   if (move) {  // every destination part file equals what a plain mec_encode of the destination geometry writes
     std::vector<uint8_t*> want(n2);
     for (int i = 0; i < n2; i++) want[i] = static_cast<uint8_t*>(malloc(static_cast<size_t>(fsz2)));
@@ -418,6 +479,10 @@ int main(int argc, char** argv) {
     printf(", \"verifies\": %lld, \"verifies_serial\": %lld, \"whole_hash_launches\": %lld", static_cast<long long>(mec_batcher_stat(bat, "verifies")),
            static_cast<long long>(mec_batcher_stat(bat, "verifies_serial")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
   if (mixed) printf(", \"healed\": %d", healed);
+  if (bsse)
+    printf(", \"sse_puts\": %lld, \"sse_gets\": %lld, \"sse_serial\": %lld, \"redone\": %lld", static_cast<long long>(mec_batcher_stat(bat, "sse_puts")),
+           static_cast<long long>(mec_batcher_stat(bat, "sse_gets")), static_cast<long long>(mec_batcher_stat(bat, "sse_serial")),
+           static_cast<long long>(mec_batcher_stat(bat, "redone")));
   if (bmixed)
     printf(", \"reads_whole\": %lld, \"reads_whole_serial\": %lld, \"redone\": %lld, \"whole_hash_launches\": %lld",
            static_cast<long long>(mec_batcher_stat(bat, "reads_whole")), static_cast<long long>(mec_batcher_stat(bat, "reads_whole_serial")),
@@ -430,7 +495,7 @@ int main(int argc, char** argv) {
            static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole")), static_cast<long long>(mec_batcher_stat(bat, "transcodes_whole_serial")),
            static_cast<long long>(mec_batcher_stat(bat, "redone")), static_cast<long long>(mec_batcher_stat(bat, "whole_hash_launches")));
   if (mode == "pool" || mode == "get" || mode == "heal" || mode == "transcode" || mode == "transcode_whole" || mode == "get_mixed" ||
-      mode == "heal_mixed" || mode == "verify")
+      mode == "heal_mixed" || mode == "verify" || mode == "sse_put" || mode == "sse_get")
     printf(", \"pool\": %d", P);
   printf("}\n");
   if (bat) mec_batcher_free(bat);
