@@ -33,6 +33,11 @@ enum {
   MEC_ERR_WRITE_QUORUM = -11,     /* errErasureWriteQuorum cmd/erasure-errors.go:26 */
   MEC_ERR_INVALID_ARGUMENT = -12, /* errInvalidArgument */
   MEC_ERR_NOT_AUTHENTIC = -13,    /* sio.NotAuthentic -> errObjectTampered  cmd/encryption-v1.go:57 */
+  MEC_ERR_SIGNATURE_MISMATCH = -14, /* errSignatureMismatch  cmd/typed-errors.go:31 */
+  MEC_ERR_MALFORMED_ENCODING = -15, /* errMalformedEncoding  cmd/streaming-signature-v4.go:184 */
+  MEC_ERR_CHUNK_TOO_BIG = -16,      /* errChunkTooBig        cmd/streaming-signature-v4.go:187 */
+  MEC_ERR_INCOMPLETE_BODY = -17,    /* io.ErrUnexpectedEOF / IncompleteBody  cmd/erasure-object.go:1450-1453 */
+  MEC_ERR_OVERREAD = -18,           /* ioutil.ErrOverread    internal/ioutil/hardlimitreader.go:27 */
   MEC_ERR_CUDA = -100,            /* CUDA runtime / driver failure (see mec_last_error) */
   MEC_ERR_NO_DEVICE = -101,       /* no CUDA device: the library never falls back to the CPU */
   MEC_ERR_UNSUPPORTED = -102      /* geometry or algorithm outside the GPU path (see DESIGN.md) */
@@ -634,6 +639,43 @@ int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint
  * the ciphertext range and its plaintext are held in device buffers of the codec. */
 int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
                        int64_t enc_total, const uint8_t key[32], uint8_t* dst, int* heal_hint);
+
+/* ---- Signature V4 streaming payloads (x-amz-content-sha256: STREAMING-AWS4-HMAC-SHA256-PAYLOAD[-TRAILER]) ------------------
+ * Each aws-chunk's signature is HMAC-SHA256(signing key, string to sign) over SHA-256 of its payload and the previous chunk's
+ * signature (getChunkSignature / getTrailerChunkSignature, cmd/streaming-signature-v4.go:54-94).  `key` is getSigningKey's 32 bytes
+ * (cmd/signature-v4.go:141), `date` the request time as "20060102T150405Z" and `scope` "yyyymmdd/region/s3/aws4_request" (NUL-
+ * terminated; strlen(date) + strlen(scope) <= 254).  Both calls derive the HMAC chaining states of the key on the host and zero
+ * them, device and host copies, before they return.  Counters (mec_get_stat): "sigv4_chunks", rows verified; "sigv4_key_bytes",
+ * the non-zero bytes of key material left in the codec (its host copy and a read-back of its device copy), 0 after every call.
+ *
+ * mec_chunk_signatures_device verifies `count` rows whose messages are already in device memory in ONE launch (shaped like
+ * mec_sums_device): row i hashes d_base[offsets[i], + lens[i]) (any alignment), with prev + 64i the previous signature and
+ * claimed + 64i the claimed one; kinds[i] is MEC_SIGV4_PAYLOAD (a chunk payload) or MEC_SIGV4_TRAILER (a trailer value, with
+ * the '\n' readTrailers appends already in place).  verdicts[i] (host) is 1 when the claim equals the lowercase hex signature
+ * byte for byte, else 0.  Returns MEC_OK once the verdicts are written (it waits for its work on cuda_stream); NULL arrays with
+ * count > 0, negative offsets or lengths, an unknown kind or a head that does not fit are MEC_ERR_INVALID_ARGUMENT before any
+ * device work.
+ *
+ * mec_encode_chunked is newSignV4ChunkedReader + Erasure.Encode of PutObject / PutObjectPart / PutObjectExtract: it de-frames the
+ * aws-chunked `body` as s3ChunkedReader.Read does (cmd/streaming-signature-v4.go:264-442; only header bytes are read on the host),
+ * checks every chunk's signature on the device, starting from the seed signature `seed` (64 lowercase hex bytes), and writes
+ * mec_encode's part files of the decoded_len (x-amz-decoded-content-length) decoded bytes.  trailer != 0 reads the signed trailer
+ * behind the final chunk as readTrailers does (:445-512) and returns its value as signed (with the '\n' readTrailers appends) in
+ * trailer_out[0, min(trailer_cap, *trailer_len)); parsing its key:value lines and checking them against X-Amz-Trailer stay with
+ * the caller.  Returns decoded_len, or the first error in stream order, per chunk: MEC_ERR_MALFORMED_ENCODING /
+ * MEC_ERR_CHUNK_TOO_BIG (its header), MEC_ERR_INCOMPLETE_BODY (the body ends), MEC_ERR_SIGNATURE_MISMATCH, MEC_ERR_MALFORMED_ENCODING
+ * (the CRLF behind the payload), MEC_ERR_OVERREAD (more payload than decoded_len); then MEC_ERR_INCOMPLETE_BODY for fewer payload
+ * bytes than decoded_len.  After an error the part files are unspecified.  NULL or negative arguments, a seed that is not 64
+ * lowercase hex bytes or a head that does not fit are MEC_ERR_INVALID_ARGUMENT, then MEC_ERR_WRITE_QUORUM, both before any device
+ * work; so is an error in the first chunk's header.  "checksums" covers the decoded bytes. */
+#define MEC_SIGV4_PAYLOAD 0
+#define MEC_SIGV4_TRAILER 1
+int mec_chunk_signatures_device(mec_codec* c, const uint8_t key[32], const char* date, const char* scope, const uint8_t* d_base,
+                                const int64_t* offsets, const int64_t* lens, const uint8_t* prev, const uint8_t* claimed,
+                                const int32_t* kinds, int64_t count, uint8_t* verdicts, void* cuda_stream);
+int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t key[32],
+                           const uint8_t seed[64], const char* date, const char* scope, int trailer, uint8_t* const* files,
+                           int write_quorum, uint8_t* trailer_out, int64_t trailer_cap, int64_t* trailer_len);
 
 /* ---- shard-shaped low-level calls (keep Erasure.EncodeData / reedsolomon.Encoder shapes) ---- */
 /* reedsolomon.Encoder.Encode: shards[0..k) in, shards[k..k+m) out, each shard_len bytes (host). */

@@ -8,13 +8,17 @@ import numpy as np
 SHA256, HIGHWAYHASH256, HIGHWAYHASH256S, BLAKE2B512 = 1, 2, 3, 4
 ERRORS = {-1: "ErrInvShardNum", -2: "ErrMaxShardNum", -3: "ErrTooFewShards", -4: "ErrShardNoData", -5: "ErrShardSize",
           -6: "ErrShortData", -7: "errFileCorrupt", -8: "errLessData", -9: "errUnexpected", -10: "errErasureReadQuorum",
-          -11: "errErasureWriteQuorum", -12: "errInvalidArgument", -13: "sio.NotAuthentic (errObjectTampered)", -100: "CUDA error", -101: "no CUDA device",
+          -11: "errErasureWriteQuorum", -12: "errInvalidArgument", -13: "sio.NotAuthentic (errObjectTampered)", -14: "errSignatureMismatch",
+          -15: "errMalformedEncoding", -16: "errChunkTooBig", -17: "io.ErrUnexpectedEOF (IncompleteBody)", -18: "ioutil.ErrOverread", -100: "CUDA error", -101: "no CUDA device",
           -102: "unsupported on the GPU path"}
 MIX_PATTERNS = 1  # MEC_BATCHER_MIX_PATTERNS
 CRC32, CRC32C, CRC64NVME = 1, 2, 4  # MEC_CRC*
 SUM_MD5, SUM_SHA1, SUM_SHA256 = 8, 16, 32  # MEC_SUM_*
 DARE_SEAL, DARE_OPEN = 1, 2  # MEC_DARE_*
 NOT_AUTHENTIC = -13  # MEC_ERR_NOT_AUTHENTIC
+# MEC_ERR_* of Signature V4 streaming bodies (mec_encode_chunked)
+SIGNATURE_MISMATCH, MALFORMED_ENCODING, CHUNK_TOO_BIG, INCOMPLETE_BODY, OVERREAD = -14, -15, -16, -17, -18
+SIGV4_PAYLOAD, SIGV4_TRAILER = 0, 1  # MEC_SIGV4_*
 SUM_BYTES = 96  # MEC_SUM_BYTES: one record of mec_sums_device / mec_batcher_encode_sums
 SUM_SLOTS = {"md5": (SUM_MD5, 0, 16), "sha1": (SUM_SHA1, 32, 20), "sha256": (SUM_SHA256, 64, 32)}  # name -> (bit, offset, length)
 
@@ -159,6 +163,9 @@ def lib():
     L.mec_batcher_encode_sse.argtypes = [vp, vp, i64, vp, vp, vp, i32]
     L.mec_batcher_decode_sse.restype = i64
     L.mec_batcher_decode_sse.argtypes = [vp, vp, vp, i64, i64, i64, vp, vp, C.POINTER(i32)]
+    L.mec_chunk_signatures_device.argtypes = [vp, vp, C.c_char_p, C.c_char_p, vp, vp, vp, vp, vp, vp, i64, vp, vp]
+    L.mec_encode_chunked.restype = i64
+    L.mec_encode_chunked.argtypes = [vp, vp, i64, i64, vp, vp, C.c_char_p, C.c_char_p, i32, vp, i32, vp, i64, C.POINTER(i64)]
     _LIB = L
     return L
 
@@ -379,6 +386,52 @@ class Codec:
         if check and rc:
             raise MecError(rc, "mec_dare_device")
         return rc, status[:ns]
+
+    # -- Signature V4 streaming payloads (aws-chunked bodies)
+    def chunk_signatures_device(self, key, date, scope, d_base, offsets, lens, prev, claimed, kinds, stream=0):
+        """mec_chunk_signatures_device over len(lens) rows in ONE launch -> verdicts (1 = the claimed signature matches).
+        prev / claimed: 64 bytes per row (bytes objects or an (n, 64) uint8 array); kinds: SIGV4_PAYLOAD / SIGV4_TRAILER."""
+        n = len(lens)
+        key = _u8(key)
+        if key.size != 32:
+            raise ValueError("the signing key is 32 bytes")
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        ln = np.ascontiguousarray(lens, dtype=np.int64)
+        pv = np.frombuffer(b"".join(prev), dtype=np.uint8) if isinstance(prev, (list, tuple)) else _u8(prev)
+        cl = np.frombuffer(b"".join(claimed), dtype=np.uint8) if isinstance(claimed, (list, tuple)) else _u8(claimed)
+        kd = np.ascontiguousarray(kinds, dtype=np.int32)
+        if not (off.size == ln.size == kd.size == n and pv.size == cl.size == 64 * n):
+            raise ValueError("one offset, length, kind and 64-byte previous and claimed signature per row")
+        out = np.zeros(max(n, 1), dtype=np.uint8)
+        rc = lib().mec_chunk_signatures_device(self.h, key.ctypes.data, date.encode(), scope.encode(), d_base, off.ctypes.data,
+                                               ln.ctypes.data, pv.ctypes.data, cl.ctypes.data, kd.ctypes.data, n, out.ctypes.data,
+                                               stream)
+        if rc:
+            raise MecError(rc, "mec_chunk_signatures_device")
+        return out[:n]
+
+    def encode_chunked(self, body, decoded_len, key, seed, date, scope, trailer=False, online=None, write_quorum=0,
+                       trailer_cap=4096):
+        """mec_encode_chunked: an aws-chunked body -> part files of its decoded_len decoded bytes; with trailer=True
+        (part files, trailer value as signed)"""
+        body, key = _u8(body), _u8(key)
+        seed = seed if isinstance(seed, bytes) else bytes(_u8(seed))
+        if key.size != 32 or len(seed) != 64:
+            raise ValueError("the signing key is 32 bytes, the seed signature 64")
+        fsz = self.bitrot_file_size(decoded_len) if decoded_len > 0 else 0
+        online = [True] * self.n if online is None else online
+        files = [np.zeros(fsz, dtype=np.uint8) if online[i] else None for i in range(self.n)]
+        sd = np.frombuffer(seed, dtype=np.uint8)
+        tout = np.zeros(max(trailer_cap, 1), dtype=np.uint8)
+        tlen = C.c_int64(0)
+        rc = lib().mec_encode_chunked(self.h, body.ctypes.data if body.size else None, body.size, decoded_len, key.ctypes.data,
+                                      sd.ctypes.data, date.encode(), scope.encode(), int(trailer), _ptrs(files), write_quorum,
+                                      tout.ctypes.data, trailer_cap, C.byref(tlen))
+        if rc < 0:
+            raise MecError(rc, "mec_encode_chunked")
+        if trailer:
+            return files, bytes(tout[:min(tlen.value, trailer_cap)])
+        return files
 
     def decode(self, files, offset, length, total, prefer=None):
         files = [None if f is None else _u8(f) for f in files]

@@ -19,6 +19,7 @@
 #include "obj_hash.cuh"
 #include "batch_copy.cuh"
 #include "dare.cuh"
+#include "sigv4.cuh"
 #include <nvtx3/nvToolsExt.h>
 
 struct NvtxRange {
@@ -80,7 +81,12 @@ struct Slot {
   DevBuf sse_keys, sse_pt, sse_st;
   PinBuf hsse_keys, hsse_st;
   int64_t sse_heads = 0;             // key heads written to hsse_keys by the slot's batch in flight (zeroed by batcher_finish)
-  cudaStream_t st = nullptr;
+  // mec_encode_chunked: the signature rows of the chunk and their verdicts behind them; the second stream that verifies them while
+  // s.st encodes, with the events that order it after the staging and s.st after it
+  DevBuf sig_tab;
+  PinBuf hsig_tab;
+  cudaStream_t st = nullptr, st2 = nullptr;
+  cudaEvent_t ev_staged = nullptr, ev_verified = nullptr;
 };
 
 // DARE 2.0 state of a codec (dare.cuh): the AES round tables (built once), the key schedules and H powers of the streams of the
@@ -90,6 +96,13 @@ struct DareState {
   bool tabs_ok = false;
   DevBuf tabs, keys, pk, st, ct, pt;
   PinBuf hkeys, hpk, hst;
+};
+
+// Signature V4 streaming state of a codec (sigv4.cuh): the SigCall of the call in flight (key states zeroed before it returns) and
+// mec_chunk_signatures_device's row table with the verdicts behind the rows.
+struct SigState {
+  DevBuf call, rows;
+  PinBuf hcall, hrows;
 };
 
 struct mec_codec {
@@ -119,6 +132,8 @@ struct mec_codec {
   PinBuf hwhole_dig;
   DareState dare;
   int64_t st_dare_sealed = 0, st_dare_opened = 0;  // DARE packages sealed / opened (rows launched)
+  SigState sig;
+  int64_t st_sigv4_chunks = 0;  // signature rows verified
   int64_t S() const { return ceil_frac(block_size, k); }
 };
 
@@ -242,7 +257,13 @@ extern "C" void mec_codec_free(mec_codec* c) {
     s.wtab.release(); s.hwtab.release(); s.wdig.release(); s.hwdig.release();
     s.dpk.release(); s.hdpk.release();
     s.sse_keys.release(); s.sse_pt.release(); s.sse_st.release(); s.hsse_keys.release(); s.hsse_st.release();
+    s.sig_tab.release(); s.hsig_tab.release();
+    if (s.st2) { cudaStreamSynchronize(s.st2); cudaStreamDestroy(s.st2); }
+    if (s.ev_staged) cudaEventDestroy(s.ev_staged);
+    if (s.ev_verified) cudaEventDestroy(s.ev_verified);
   }
+  for (DevBuf* b : {&c->sig.call, &c->sig.rows}) b->release();
+  for (PinBuf* b : {&c->sig.hcall, &c->sig.hrows}) b->release();
   for (DevBuf* b : {&c->dare.tabs, &c->dare.keys, &c->dare.pk, &c->dare.st, &c->dare.ct, &c->dare.pt}) b->release();
   for (PinBuf* b : {&c->dare.hkeys, &c->dare.hpk, &c->dare.hst}) b->release();
   c->flags.release();
@@ -272,6 +293,24 @@ extern "C" int mec_set_option(mec_codec* c, const char* name, int64_t v) {
   else return MEC_ERR_INVALID_ARGUMENT;
   return MEC_OK;
 }
+// non-zero bytes of signing-key material left in the codec: the host copy of the key states and a read-back of the device copy
+static int64_t sig_key_bytes(const mec_codec* c) {
+  const size_t kb = offsetof(SigCall, head_len);
+  int64_t nz = 0;
+  for (int dev = 0; dev < 2; dev++) {
+    const void* p = dev ? c->sig.call.p : c->sig.hcall.p;
+    if (!p) continue;
+    uint8_t buf[offsetof(SigCall, head_len)];
+    if (dev) {
+      if (cudaSetDevice(c->device) != cudaSuccess || cudaMemcpy(buf, p, kb, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+    } else {
+      memcpy(buf, p, kb);
+    }
+    for (size_t i = 0; i < kb; i++) nz += buf[i] != 0;
+  }
+  return nz;
+}
+
 extern "C" int64_t mec_get_stat(const mec_codec* c, const char* name) {
   if (!c || !name) return -1;
   if (!strcmp(name, "launches")) return c->eng ? c->eng->launches() : 0;
@@ -284,6 +323,8 @@ extern "C" int64_t mec_get_stat(const mec_codec* c, const char* name) {
   if (!strcmp(name, "whole_hash_launches")) return c->st_whole_hash;
   if (!strcmp(name, "dare_sealed")) return c->st_dare_sealed;
   if (!strcmp(name, "dare_opened")) return c->st_dare_opened;
+  if (!strcmp(name, "sigv4_chunks")) return c->st_sigv4_chunks;
+  if (!strcmp(name, "sigv4_key_bytes")) return sig_key_bytes(c);
   if (!strcmp(name, "jit_compiles")) return c->eng ? c->eng->jit_compiles() : 0;
   if (!strcmp(name, "jit_launches")) return c->eng ? c->eng->jit_launches() : 0;
   if (!strcmp(name, "small_launches")) return c->eng ? c->eng->small_launches() : 0;
@@ -1918,6 +1959,359 @@ extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, con
     for (int i = 0; i < n; i++)
       if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
   return length;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Signature V4 streaming payloads (sigv4.cuh): the aws-chunked body of a PutObject is de-framed on the host, header bytes only,
+// and every chunk's signature is checked on the device, one thread per chunk.
+constexpr int64_t kMaxAwsChunk = 16 << 20;  // maxChunkSize, cmd/streaming-signature-v4.go:260
+static_assert(MEC_SIGV4_PAYLOAD == kSigPayload && MEC_SIGV4_TRAILER == kSigTrailer, "sigv4.cuh");
+
+static bool lower_hex64(const uint8_t* s) {
+  for (int i = 0; i < 64; i++)
+    if (!((s[i] >= '0' && s[i] <= '9') || (s[i] >= 'a' && s[i] <= 'f'))) return false;
+  return true;
+}
+
+// The call's SigCall into the codec's pinned copy: key states and "date\nscope\n".  False when the head does not fit.
+static bool sig_call_host(mec_codec* c, const uint8_t* key, const char* date, const char* scope) {
+  const size_t dl = strlen(date), sl = strlen(scope);
+  if (dl + sl + 2 > static_cast<size_t>(kSigMaxHead)) return false;
+  SigCall* k = static_cast<SigCall*>(c->sig.hcall.p);
+  memset(k, 0, sizeof(SigCall));
+  sig_key_states(key, k);
+  memcpy(k->head, date, dl);
+  k->head[dl] = '\n';
+  memcpy(k->head + dl + 1, scope, sl);
+  k->head[dl + sl + 1] = '\n';
+  k->head_len = static_cast<int32_t>(dl + sl + 2);
+  return true;
+}
+
+// Zeroes the call's key states, device and host, once `st` and the slots' verify streams are done with them.
+struct SigScrub {
+  mec_codec* c;
+  cudaStream_t st;
+  ~SigScrub() {
+    for (auto& s : c->slots)
+      if (s.st2) cudaStreamSynchronize(s.st2);
+    cudaMemsetAsync(c->sig.call.p, 0, sizeof(SigCall), st);
+    cudaStreamSynchronize(st);
+    explicit_bzero(c->sig.hcall.p, sizeof(SigCall));
+  }
+};
+
+// Uploads the call's SigCall on `st` and waits for it: every slot stream reads it
+static int sig_call_upload(mec_codec* c, cudaStream_t st) {
+  MEC_CUDA_OK(cudaMemcpyAsync(c->sig.call.p, c->sig.hcall.p, sizeof(SigCall), cudaMemcpyHostToDevice, st));
+  MEC_CUDA_OK(cudaStreamSynchronize(st));
+  return MEC_OK;
+}
+
+// enqueue: the n rows of the host table `h` (sorted here) to the device table `d` on st, then ONE sigv4_chunk_kernel launch whose
+// verdicts follow the n rows in `d`
+static int sig_launch(mec_codec* c, SigRow* h, SigRow* d, int64_t n, cudaStream_t st) {
+  std::sort(h, h + n, [](const SigRow& x, const SigRow& y) { return x.len > y.len; });
+  MEC_CUDA_OK(cudaMemcpyAsync(d, h, static_cast<size_t>(n) * sizeof(SigRow), cudaMemcpyHostToDevice, st));
+  SigParams p;
+  p.rows = d; p.nrows = n; p.call = static_cast<const SigCall*>(c->sig.call.p);
+  p.verdict = reinterpret_cast<uint8_t*>(d + n);
+  sigv4_chunk_kernel<<<static_cast<unsigned>(ceil_frac(n, kSigThreads)), kSigThreads, 0, st>>>(p);
+  MEC_CUDA_OK(cudaGetLastError());
+  c->eng->count_launch();
+  c->st_sigv4_chunks += n;
+  return MEC_OK;
+}
+static inline SigRow sig_row(const uint8_t* msg, int64_t len, int64_t out, int32_t kind, const uint8_t* prev, const uint8_t* claim) {
+  SigRow r;
+  r.msg = msg; r.len = len; r.out = out; r.kind = kind; r.pad = 0;
+  memcpy(r.prev, prev, 64);
+  memcpy(r.claim, claim, 64);
+  return r;
+}
+
+static int sig_ensure(mec_codec* c) {
+  int rc;
+  if ((rc = c->sig.call.ensure(sizeof(SigCall))) || (rc = c->sig.hcall.ensure(sizeof(SigCall)))) return rc;
+  return MEC_OK;
+}
+
+extern "C" int mec_chunk_signatures_device(mec_codec* c, const uint8_t* key, const char* date, const char* scope, const uint8_t* d_base,
+                                           const int64_t* offsets, const int64_t* lens, const uint8_t* prev, const uint8_t* claimed,
+                                           const int32_t* kinds, int64_t count, uint8_t* verdicts, void* stream) {
+  NvtxRange nvtx("mec_chunk_signatures_device");
+  if (!c || !key || !date || !scope || count < 0 || strlen(date) + strlen(scope) + 2 > static_cast<size_t>(kSigMaxHead))
+    return MEC_ERR_INVALID_ARGUMENT;
+  if (count == 0) return MEC_OK;
+  if (!offsets || !lens || !prev || !claimed || !kinds || !verdicts) return MEC_ERR_INVALID_ARGUMENT;
+  for (int64_t i = 0; i < count; i++)
+    if (offsets[i] < 0 || lens[i] < 0 || (lens[i] > 0 && !d_base) || (kinds[i] != kSigPayload && kinds[i] != kSigTrailer))
+      return MEC_ERR_INVALID_ARGUMENT;
+  if (count > (int64_t{1} << 36)) return MEC_ERR_UNSUPPORTED;  // the grid's x dimension
+  std::lock_guard<std::mutex> lk(c->mu);
+  int rc;
+  if ((rc = ensure_engine(c))) return rc;
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t tab = static_cast<size_t>(count) * (sizeof(SigRow) + 1);
+  if ((rc = sig_ensure(c)) || (rc = c->sig.rows.ensure(tab)) || (rc = c->sig.hrows.ensure(tab))) return rc;
+  sig_call_host(c, key, date, scope);
+  SigScrub scrub{c, st};
+  if ((rc = sig_call_upload(c, st))) return rc;
+  SigRow* h = static_cast<SigRow*>(c->sig.hrows.p);
+  for (int64_t i = 0; i < count; i++)
+    h[i] = sig_row(d_base + offsets[i], lens[i], i, kinds[i], prev + 64 * i, claimed + 64 * i);
+  SigRow* d = static_cast<SigRow*>(c->sig.rows.p);
+  if ((rc = sig_launch(c, h, d, count, st))) return rc;
+  MEC_CUDA_OK(cudaMemcpyAsync(h + count, d + count, static_cast<size_t>(count), cudaMemcpyDeviceToHost, st));
+  MEC_CUDA_OK(cudaStreamSynchronize(st));
+  memcpy(verdicts, h + count, static_cast<size_t>(count));
+  return MEC_OK;
+}
+
+// One aws-chunk whose header framed and whose payload is in the body: one signature row
+struct AwsChunk {
+  int64_t pay, size;  // body offset and length of the payload
+  int64_t doff;       // decoded offset of its first payload byte
+  const uint8_t* prev;
+  const uint8_t* claim;
+};
+struct ChunkedBody {
+  std::vector<AwsChunk> ch;
+  std::vector<uint8_t> tmsg;        // trailer mode: the trailer value as signed (with the '\n' readTrailers adds)
+  const uint8_t* tclaim = nullptr;  // its claimed signature (NULL: no trailer row)
+  int64_t decoded = 0;
+};
+
+// bytes.TrimSpace: ASCII white space and the UTF-8 forms of Unicode White_Space
+static int space_prefix(const uint8_t* p, int64_t n) {
+  if (n >= 1 && (p[0] == ' ' || (p[0] >= '\t' && p[0] <= '\r'))) return 1;
+  if (n >= 2 && p[0] == 0xc2 && (p[1] == 0x85 || p[1] == 0xa0)) return 2;
+  if (n >= 3 && ((p[0] == 0xe1 && p[1] == 0x9a && p[2] == 0x80) || (p[0] == 0xe3 && p[1] == 0x80 && p[2] == 0x80) ||
+                 (p[0] == 0xe2 && p[1] == 0x80 && ((p[2] >= 0x80 && p[2] <= 0x8a) || p[2] == 0xa8 || p[2] == 0xa9 || p[2] == 0xaf)) ||
+                 (p[0] == 0xe2 && p[1] == 0x81 && p[2] == 0x9f)))
+    return 3;
+  return 0;
+}
+static void trim_space(const uint8_t*& p, int64_t& n) {
+  for (int k; n > 0 && (k = space_prefix(p, n)) > 0;) { p += k; n -= k; }
+  for (bool more = true; more && n > 0;) {
+    more = false;
+    for (int k = 1; k <= 3 && k <= n; k++)
+      if (space_prefix(p + n - k, k) == k) { n -= k; more = true; break; }
+  }
+}
+
+// s3ChunkedReader.Read (cmd/streaming-signature-v4.go:264-442) and readTrailers (:445-512) over the body, byte for byte, reading
+// header bytes only.  Returns what the serial reader reports once every row recorded in `o` has passed its signature check: MEC_OK,
+// a framing error, MEC_ERR_OVERREAD (HardLimitReader, internal/ioutil/hardlimitreader.go:46-56), MEC_ERR_INCOMPLETE_BODY (an
+// unexpected EOF, or fewer payload bytes than D: cmd/erasure-object.go:1450-1453) or MEC_ERR_SIGNATURE_MISMATCH (a trailer
+// signature that is not 64 bytes long).
+static int parse_chunked(const uint8_t* b, int64_t blen, int64_t D, const uint8_t* seed, bool trailer, ChunkedBody* o) {
+  int64_t pos = 0;
+  const uint8_t* prev = seed;
+  for (;;) {
+    int64_t size = 0;
+    for (;;) {  // hex size digits of either case up to ';' (none: a zero-size chunk)
+      if (pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+      const uint8_t x = b[pos++];
+      if (x == ';') break;
+      int v;
+      if (x >= '0' && x <= '9') v = x - '0';
+      else if (x >= 'a' && x <= 'f') v = x - 'a' + 10;
+      else if (x >= 'A' && x <= 'F') v = x - 'A' + 10;
+      else return MEC_ERR_MALFORMED_ENCODING;
+      size = size << 4 | v;
+      if (size > kMaxAwsChunk) return MEC_ERR_CHUNK_TOO_BIG;
+    }
+    if (blen - pos < 80) return MEC_ERR_INCOMPLETE_BODY;
+    if (memcmp(b + pos, "chunk-signature=", 16)) return MEC_ERR_MALFORMED_ENCODING;
+    const uint8_t* claim = b + pos + 16;
+    pos += 80;
+    for (const uint8_t want : {'\r', '\n'}) {
+      if (pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+      if (b[pos++] != want) return MEC_ERR_MALFORMED_ENCODING;
+    }
+    if (blen - pos < size) return MEC_ERR_INCOMPLETE_BODY;
+    o->ch.push_back(AwsChunk{pos, size, o->decoded, prev, claim});
+    prev = claim;
+    pos += size;
+    o->decoded += size;
+    if (size == 0) break;
+    // the CRLF behind the payload: a missing or cut-off '\r' is malformed, a cut-off '\n' an unexpected EOF
+    if (pos >= blen || b[pos] != '\r') return MEC_ERR_MALFORMED_ENCODING;
+    if (++pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+    if (b[pos++] != '\n') return MEC_ERR_MALFORMED_ENCODING;
+    if (o->decoded > D) return MEC_ERR_OVERREAD;  // the reader yields a chunk only after its signature and CRLF passed
+  }
+  if (trailer) {
+    const int64_t v0 = pos;
+    for (;; pos++) {  // the value: every byte up to '\r', which must be followed by '\n'
+      if (pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+      if (b[pos] == '\r') break;
+    }
+    o->tmsg.assign(b + v0, b + pos);
+    if (++pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+    if (b[pos++] != '\n') return MEC_ERR_MALFORMED_ENCODING;
+    const int64_t s0 = pos;
+    for (;; pos++) {  // the signature line up to '\r', then exactly "\n\r\n" (a cut-off part of it is malformed)
+      if (pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+      if (b[pos] == '\r') break;
+    }
+    const int64_t s1 = pos++;
+    if (pos >= blen) return MEC_ERR_INCOMPLETE_BODY;
+    if (blen - pos < 3 || memcmp(b + pos, "\n\r\n", 3)) return MEC_ERR_MALFORMED_ENCODING;
+    static const char kPrefix[] = "x-amz-trailer-signature:";
+    const int64_t np = sizeof(kPrefix) - 1;
+    if (s1 - s0 < np || memcmp(b + s0, kPrefix, np)) return MEC_ERR_MALFORMED_ENCODING;
+    if (!o->tmsg.empty() && o->tmsg.back() != '\n') o->tmsg.push_back('\n');
+    const uint8_t* sig = b + s0 + np;
+    int64_t sl = s1 - s0 - np;
+    trim_space(sig, sl);
+    if (sl != 64) return MEC_ERR_SIGNATURE_MISMATCH;
+    o->tclaim = sig;
+  }
+  return o->decoded < D ? MEC_ERR_INCOMPLETE_BODY : MEC_OK;
+}
+
+// Per-slot second stream and events of the chunked encode's verify launches, created on first use
+static int sig_streams(mec_codec* c) {
+  for (auto& s : c->slots) {
+    if (s.st2) continue;
+    MEC_CUDA_OK(cudaStreamCreateWithFlags(&s.st2, cudaStreamNonBlocking));
+    MEC_CUDA_OK(cudaEventCreateWithFlags(&s.ev_staged, cudaEventDisableTiming));
+    MEC_CUDA_OK(cudaEventCreateWithFlags(&s.ev_verified, cudaEventDisableTiming));
+  }
+  return MEC_OK;
+}
+
+// The staging step of mec_encode_chunked for the object bytes [off, off + bytes), `last` for the pipeline's last chunk (or the one
+// step of an empty object).  ONE batched copy stages, back to back, the payload of every aws-chunk that overlaps the range or whose
+// row this step verifies, placed so that object byte `off` lands 16-byte aligned; the trailer message follows in the last step.  The
+// rows of the aws-chunks that start in the range (the last step: from `off` on, and the trailer row) are then verified by ONE launch
+// on the slot's second stream, behind the staging, so that the encode on s.st does not queue behind the hash.  *r0 / *nrow: the
+// first row and the number of rows of the step, whose verdicts land behind its rows in s.hsig_tab once s.st2 has drained.
+static int chunked_stage(mec_codec* c, Slot& s, const uint8_t* body, const ChunkedBody& P, int64_t off, int64_t bytes, bool last,
+                         Staged* o, int64_t* r0, int64_t* nrow) {
+  const std::vector<AwsChunk>& ch = P.ch;
+  const int64_t nch = static_cast<int64_t>(ch.size()), end = off + bytes;
+  auto first = [&](auto pred) { return std::partition_point(ch.begin(), ch.end(), pred) - ch.begin(); };
+  const int64_t a1 = first([&](const AwsChunk& x) { return x.doff + x.size <= off; });  // first chunk that overlaps or follows
+  const int64_t h0 = first([&](const AwsChunk& x) { return x.doff < off; });           // first chunk that starts in the range
+  const int64_t h1 = last ? nch : first([&](const AwsChunk& x) { return x.doff < end; });
+  const int64_t a = std::min(a1, h0), e = h1;  // the overlapping chunks end where the rows do
+  const int64_t lo = a < e ? ch[a].doff : off, hi = a < e ? ch[e - 1].doff + ch[e - 1].size : off;
+  const int64_t pad = (16 - (off - lo) % 16) % 16;
+  const bool trow = last && P.tclaim;
+  const int64_t tpos = round_up(pad + std::max(hi, end) - lo, 16);
+  int rc;
+  if ((rc = s.src.ensure(static_cast<size_t>(tpos + (trow ? static_cast<int64_t>(P.tmsg.size()) : 0) + 256)))) return rc;
+  uint8_t* base = static_cast<uint8_t*>(s.src.p) + pad - lo;  // object byte x at base + x
+  CopyList list;
+  int64_t staged = 0;
+  for (int64_t j = a; j < e; j++) {
+    list.add(base + ch[j].doff, body + ch[j].pay, ch[j].size);
+    staged += ch[j].size;
+  }
+  if (trow) {
+    list.add(static_cast<uint8_t*>(s.src.p) + tpos, P.tmsg.data(), static_cast<int64_t>(P.tmsg.size()));
+    staged += static_cast<int64_t>(P.tmsg.size());
+  }
+  if ((rc = list.flush(s.st))) return rc;
+  c->st_h2d += staged;
+  o->obj = o->ck = base + off;
+  o->ck_len = bytes;
+  *r0 = h0;
+  *nrow = h1 - h0 + (trow ? 1 : 0);
+  if (*nrow == 0) return MEC_OK;
+  const size_t tab = static_cast<size_t>(*nrow) * (sizeof(SigRow) + 1);
+  if ((rc = s.sig_tab.ensure(tab)) || (rc = s.hsig_tab.ensure(tab))) return rc;
+  SigRow* h = static_cast<SigRow*>(s.hsig_tab.p);
+  for (int64_t j = h0; j < h1; j++) h[j - h0] = sig_row(base + ch[j].doff, ch[j].size, j - h0, kSigPayload, ch[j].prev, ch[j].claim);
+  if (trow)
+    h[h1 - h0] = sig_row(static_cast<uint8_t*>(s.src.p) + tpos, static_cast<int64_t>(P.tmsg.size()), h1 - h0, kSigTrailer,
+                         ch.back().claim, P.tclaim);
+  MEC_CUDA_OK(cudaEventRecord(s.ev_staged, s.st));
+  MEC_CUDA_OK(cudaStreamWaitEvent(s.st2, s.ev_staged, 0));
+  SigRow* d = static_cast<SigRow*>(s.sig_tab.p);
+  if ((rc = sig_launch(c, h, d, *nrow, s.st2))) return rc;
+  MEC_CUDA_OK(cudaMemcpyAsync(h + *nrow, d + *nrow, static_cast<size_t>(*nrow), cudaMemcpyDeviceToHost, s.st2));
+  MEC_CUDA_OK(cudaEventRecord(s.ev_verified, s.st2));
+  return MEC_OK;
+}
+
+// newSignV4ChunkedReader + Erasure.Encode (cmd/object-handlers.go:1890, cmd/object-multipart-handlers.go:682,
+// cmd/object-handlers.go:2294): the body is de-framed on the host, its payloads go to the device through chunked_stage, and the
+// encode runs over the D decoded bytes as mec_encode does.
+extern "C" int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t* key,
+                                      const uint8_t* seed, const char* date, const char* scope, int trailer, uint8_t* const* files,
+                                      int write_quorum, uint8_t* trailer_out, int64_t trailer_cap, int64_t* trailer_len) {
+  NvtxRange nvtx("mec_encode_chunked");
+  if (!c || body_len < 0 || (body_len > 0 && !body) || decoded_len < 0 || !key || !seed || !date || !scope || !files)
+    return MEC_ERR_INVALID_ARGUMENT;
+  if (trailer && (!trailer_len || trailer_cap < 0 || (trailer_cap > 0 && !trailer_out))) return MEC_ERR_INVALID_ARGUMENT;
+  if (!lower_hex64(seed) || strlen(date) + strlen(scope) + 2 > static_cast<size_t>(kSigMaxHead)) return MEC_ERR_INVALID_ARGUMENT;
+  if (trailer_len) *trailer_len = 0;
+  int online = 0;
+  for (int i = 0; i < c->n; i++) online += files[i] != nullptr;
+  if (online < write_quorum) return MEC_ERR_WRITE_QUORUM;  // cmd/erasure-encode.go:59-65
+  ChunkedBody P;
+  const int perr = parse_chunked(body, body_len, decoded_len, seed, trailer != 0, &P);
+  const int64_t nrows = static_cast<int64_t>(P.ch.size()) + (P.tclaim ? 1 : 0);
+  if (nrows == 0) return perr;  // the first header already fails: no signature to check before it
+  int rc = require_streaming(c);
+  if (rc) return rc;
+  if (c->S() >= (1ll << 31)) return MEC_ERR_UNSUPPORTED;
+  std::lock_guard<std::mutex> lk(c->mu);
+  MEC_CUDA_OK(cudaSetDevice(c->device));
+  if ((rc = sig_ensure(c)) || (rc = sig_streams(c))) return rc;
+  Slot& s0 = c->slots[0];
+  sig_call_host(c, key, date, scope);
+  SigScrub scrub{c, s0.st};
+  if ((rc = sig_call_upload(c, s0.st))) return rc;
+  std::vector<uint8_t> verdict(static_cast<size_t>(nrows), 0);
+  int64_t r0[kSlots] = {}, nr[kSlots] = {};
+  auto collect = [&](int si) {
+    const uint8_t* v = reinterpret_cast<const uint8_t*>(static_cast<const SigRow*>(c->slots[si].hsig_tab.p) + nr[si]);
+    memcpy(verdict.data() + r0[si], v, static_cast<size_t>(nr[si]));
+  };
+  const int64_t D = decoded_len;
+  if (D == 0) {  // no encode: the rows of the empty object in one step
+    Staged sg;
+    if ((rc = chunked_stage(c, s0, body, P, 0, 0, true, &sg, &r0[0], &nr[0]))) return rc;
+    MEC_CUDA_OK(cudaStreamSynchronize(s0.st2));
+    collect(0);
+  } else {
+    rc = encode_pipeline(
+        c, D,
+        [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
+          const int si = static_cast<int>(&s - c->slots);
+          return chunked_stage(c, s, body, P, off, bytes, off + bytes == D, o, &r0[si], &nr[si]);
+        },
+        [&](const EncChunk& ch) -> int {
+          const int e = frames_enqueue_chunk(c, ch, files, true, nullptr);
+          if (e) return e;
+          if (nr[ch.s - c->slots]) MEC_CUDA_OK(cudaStreamWaitEvent(ch.st, ch.s->ev_verified, 0));  // the slot drains its verify too
+          return MEC_OK;
+        },
+        [&](const EncChunk& ch) {
+          frames_retire(c, ch, files, true, nullptr);
+          collect(static_cast<int>(ch.s - c->slots));
+        });
+    if (rc) return rc;
+  }
+  for (uint8_t v : verdict)
+    if (!v) return MEC_ERR_SIGNATURE_MISMATCH;  // every row precedes the point where the serial reader stopped
+  if (perr) return perr;
+  if (D == 0 && c->checksums) {  // the empty stream's checksums, as reset_last_checksums leaves them
+    for (auto& v : c->last_crc) v = 0;
+    c->last_crc_len = 0;
+  }
+  if (trailer) {
+    *trailer_len = static_cast<int64_t>(P.tmsg.size());
+    if (trailer_cap > 0) memcpy(trailer_out, P.tmsg.data(), static_cast<size_t>(std::min<int64_t>(trailer_cap, *trailer_len)));
+  }
+  return D;
 }
 
 // Batched heal (SURVEY §8f rank 2, BASELINE config 4): objects are independent, so a pool of codec handles — each with

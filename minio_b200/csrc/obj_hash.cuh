@@ -165,13 +165,10 @@ __device__ __forceinline__ void sum_bytes(uint32_t (&w)[16], const uint8_t* s0, 
   }
 }
 
+// The whole two-segment message s0[0, l0) ++ s1[0, l1), padding and length included, into the freshly initialised `st`
 template <int A>
-__device__ __forceinline__ void sum_item(const SumParams& p, const SumWork& wk) {
-  SumState<A> st;
-  st.init();
-  const uint8_t* s0 = p.base + wk.off0;
-  const uint8_t* s1 = p.base + wk.off1;
-  const int64_t l0 = wk.len0, total = l0 + wk.len1;
+__device__ __forceinline__ void sum_message(SumState<A>& st, const uint8_t* s0, int64_t l0, const uint8_t* s1, int64_t l1) {
+  const int64_t total = l0 + l1;
   uint32_t w[16];
   sum_run(st, s0, l0 >> 6);
   int64_t o = l0 & ~static_cast<int64_t>(63);
@@ -197,6 +194,13 @@ __device__ __forceinline__ void sum_item(const SumParams& p, const SumWork& wk) 
   if (A == 0) { w[14] = static_cast<uint32_t>(bits); w[15] = static_cast<uint32_t>(bits >> 32); }
   else { w[14] = bswap32(static_cast<uint32_t>(bits >> 32)); w[15] = bswap32(static_cast<uint32_t>(bits)); }
   st.block(w);
+}
+
+template <int A>
+__device__ __forceinline__ void sum_item(const SumParams& p, const SumWork& wk) {
+  SumState<A> st;
+  st.init();
+  sum_message(st, p.base + wk.off0, wk.len0, p.base + wk.off1, wk.len1);
   uint8_t* o8 = p.out + wk.out;  // any alignment: bytewise
 #pragma unroll
   for (int i = 0; i < SumState<A>::kWords; i++)
