@@ -676,6 +676,20 @@ int mec_chunk_signatures_device(mec_codec* c, const uint8_t key[32], const char*
 int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t key[32],
                            const uint8_t seed[64], const char* date, const char* scope, int trailer, uint8_t* const* files,
                            int write_quorum, uint8_t* trailer_out, int64_t trailer_cap, int64_t* trailer_len);
+/* mec_encode_chunked_sse is newSignV4ChunkedReader + EncryptRequest + Erasure.Encode, the PutObject / PutObjectPart of an encrypted
+ * bucket (SSE-S3, SSE-KMS) with a streaming-signed body: mec_encode_chunked's de-framing and verdicts (sig_key as its `key`), then
+ * mec_encode_sse of the decoded bytes with sse_key (the object key, or the part key) and nonce, in one pass of the encode pipeline.
+ * On success the part files are byte-identical to mec_encode_sse's of the decoded bytes (sized for
+ * mec_dare_encrypted_size(decoded_len)) and it returns decoded_len.  For any body it returns what mec_encode_chunked returns for that
+ * body, in the same stream order; trailer mode returns the signed trailer value as mec_encode_chunked does.  Refusals:
+ * mec_encode_chunked's, a NULL sse_key or nonce (MEC_ERR_INVALID_ARGUMENT) and a decoded_len no DARE stream holds, then
+ * MEC_ERR_WRITE_QUORUM, all before any device work; so is an error in the first chunk's header.  After an error the part files are
+ * unspecified.  An empty object verifies its final chunk (and trailer) rows and writes nothing.  "checksums" covers the decoded
+ * plaintext, each byte once.  Both keys are zeroed on the device and the host before it returns. */
+int64_t mec_encode_chunked_sse(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t sig_key[32],
+                               const uint8_t seed[64], const char* date, const char* scope, int trailer, const uint8_t sse_key[32],
+                               const uint8_t nonce[12], uint8_t* const* files, int write_quorum, uint8_t* trailer_out,
+                               int64_t trailer_cap, int64_t* trailer_len);
 
 /* ---- shard-shaped low-level calls (keep Erasure.EncodeData / reedsolomon.Encoder shapes) ---- */
 /* reedsolomon.Encoder.Encode: shards[0..k) in, shards[k..k+m) out, each shard_len bytes (host). */

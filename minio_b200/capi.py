@@ -166,6 +166,9 @@ def lib():
     L.mec_chunk_signatures_device.argtypes = [vp, vp, C.c_char_p, C.c_char_p, vp, vp, vp, vp, vp, vp, i64, vp, vp]
     L.mec_encode_chunked.restype = i64
     L.mec_encode_chunked.argtypes = [vp, vp, i64, i64, vp, vp, C.c_char_p, C.c_char_p, i32, vp, i32, vp, i64, C.POINTER(i64)]
+    L.mec_encode_chunked_sse.restype = i64
+    L.mec_encode_chunked_sse.argtypes = [vp, vp, i64, i64, vp, vp, C.c_char_p, C.c_char_p, i32, vp, vp, vp, i32, vp, i64,
+                                         C.POINTER(i64)]
     _LIB = L
     return L
 
@@ -429,6 +432,31 @@ class Codec:
                                       tout.ctypes.data, trailer_cap, C.byref(tlen))
         if rc < 0:
             raise MecError(rc, "mec_encode_chunked")
+        if trailer:
+            return files, bytes(tout[:min(tlen.value, trailer_cap)])
+        return files
+
+    def encode_chunked_sse(self, body, decoded_len, key, seed, date, scope, sse_key, nonce, trailer=False, online=None,
+                           write_quorum=0, trailer_cap=4096):
+        """mec_encode_chunked_sse: an aws-chunked body of an encrypted bucket -> the part files encode_sse writes for its decoded_len
+        decoded bytes; with trailer=True (part files, trailer value as signed)"""
+        body, key, sse_key, nonce = _u8(body), _u8(key), _u8(sse_key), _u8(nonce)
+        seed = seed if isinstance(seed, bytes) else bytes(_u8(seed))
+        if key.size != 32 or len(seed) != 64:
+            raise ValueError("the signing key is 32 bytes, the seed signature 64")
+        if sse_key.size != 32 or nonce.size != 12:
+            raise ValueError("the SSE key is 32 bytes, the nonce 12")
+        fsz = self.bitrot_file_size(dare_encrypted_size(decoded_len)) if decoded_len > 0 else 0
+        online = [True] * self.n if online is None else online
+        files = [np.zeros(fsz, dtype=np.uint8) if online[i] else None for i in range(self.n)]
+        sd = np.frombuffer(seed, dtype=np.uint8)
+        tout = np.zeros(max(trailer_cap, 1), dtype=np.uint8)
+        tlen = C.c_int64(0)
+        rc = lib().mec_encode_chunked_sse(self.h, body.ctypes.data if body.size else None, body.size, decoded_len, key.ctypes.data,
+                                          sd.ctypes.data, date.encode(), scope.encode(), int(trailer), sse_key.ctypes.data,
+                                          nonce.ctypes.data, _ptrs(files), write_quorum, tout.ctypes.data, trailer_cap, C.byref(tlen))
+        if rc < 0:
+            raise MecError(rc, "mec_encode_chunked_sse")
         if trailer:
             return files, bytes(tout[:min(tlen.value, trailer_cap)])
         return files

@@ -1815,6 +1815,46 @@ extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uin
   return worst;
 }
 
+// The packages of a sealed stream of `len` plaintext bytes that overlap the ciphertext bytes [off, off + bytes) of an encode chunk
+struct DareSpan {
+  int64_t p0, p1, np;  // packages [p0, p1], np of them
+  int64_t pt0, pt1;    // their plaintext [pt0, pt1)
+  int64_t ps;          // the first package that starts in the chunk (p1 + 1: none does)
+  int64_t delta, pad;  // ciphertext byte off is delta bytes into package p0, which is sealed pad bytes into the slot so that off
+                       // lands 16-byte aligned for the encode
+};
+static DareSpan dare_span(int64_t len, int64_t off, int64_t bytes) {
+  DareSpan d;
+  d.p0 = off / kEPkg; d.p1 = (off + bytes - 1) / kEPkg; d.np = d.p1 - d.p0 + 1;
+  d.pt0 = d.p0 * kPkg; d.pt1 = std::min(len, (d.p1 + 1) * kPkg);
+  d.ps = ceil_frac(off, kEPkg);
+  d.delta = off - d.p0 * kEPkg; d.pad = (16 - d.delta % 16) % 16;
+  return d;
+}
+
+// Seals the packages of `d` on s.st from their plaintext at `pt` (device, plaintext byte d.pt0; 16-byte aligned for the fast
+// loads) into s.src, and points the chunk's staged object bytes at the ciphertext and its checksum bytes at the plaintext of the
+// packages that start in the chunk, as hash.Reader sees each byte once.
+static int dare_seal_chunk(mec_codec* c, Slot& s, const DareSpan& d, int64_t len, const uint8_t* pt, Staged* o) {
+  const int64_t npk = ceil_frac(len, kPkg);
+  int e;
+  if ((e = s.src.ensure(static_cast<size_t>(d.pad + d.np * kEPkg + 256))) || (e = s.hdpk.ensure(static_cast<size_t>(d.np) * sizeof(DarePkg))) ||
+      (e = s.dpk.ensure(static_cast<size_t>(d.np) * sizeof(DarePkg))))
+    return e;
+  DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+  for (int64_t j = 0; j < d.np; j++) {
+    const int64_t p = d.p0 + j;
+    t[j] = dare_row(j * kPkg, d.pad + j * kEPkg, 0, std::min(kPkg, len - p * kPkg), p, 0, p == npk - 1);
+  }
+  MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, t, static_cast<size_t>(d.np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
+  uint8_t* ct = static_cast<uint8_t*>(s.src.p);
+  if ((e = dare_launch(c, true, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.p), d.np, pt, ct, nullptr, s.st))) return e;
+  o->obj = ct + d.pad + d.delta;
+  o->ck = pt + (d.ps - d.p0) * kPkg;
+  o->ck_len = d.ps <= d.p1 ? d.pt1 - d.ps * kPkg : 0;
+  return MEC_OK;
+}
+
 // EncryptRequest + Erasure.Encode: chunks are whole erasure blocks of the ciphertext.  A chunk stages and seals every package that
 // overlaps it (one across a chunk boundary is sealed in both: sealing is deterministic) and encodes its ciphertext unchanged.
 // "checksums" covers the plaintext, as hash.Reader sees it: each chunk the packages that start in it.
@@ -1840,31 +1880,13 @@ extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len,
   if ((rc = dare_keys(c, 1, key, nonce, s0.st))) return rc;
   DareScrub scrub{c, 1, s0.st};
   MEC_CUDA_OK(cudaStreamSynchronize(s0.st));  // every slot stream reads the keys
-  const int64_t npk = ceil_frac(len, kPkg);
   auto stage = [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
-    const int64_t p0 = off / kEPkg, p1 = (off + bytes - 1) / kEPkg, np = p1 - p0 + 1;
-    const int64_t pt0 = p0 * kPkg, pt1 = std::min(len, (p1 + 1) * kPkg);
-    // package p0 is sealed `pad` bytes into the slot so that ciphertext byte `off` lands 16-byte aligned for the encode
-    const int64_t delta = off - p0 * kEPkg, pad = (16 - delta % 16) % 16;
+    const DareSpan d = dare_span(len, off, bytes);
     int e;
-    if ((e = s.aux.ensure(static_cast<size_t>(round_up(pt1 - pt0, 16) + 256))) || (e = s.src.ensure(static_cast<size_t>(pad + np * kEPkg + 256))) ||
-        (e = s.hdpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))) || (e = s.dpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))))
-      return e;
-    MEC_CUDA_OK(cudaMemcpyAsync(s.aux.p, src + pt0, static_cast<size_t>(pt1 - pt0), cudaMemcpyHostToDevice, s.st));
-    DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
-    for (int64_t j = 0; j < np; j++) {
-      const int64_t p = p0 + j;
-      t[j] = dare_row(j * kPkg, pad + j * kEPkg, 0, std::min(kPkg, len - p * kPkg), p, 0, p == npk - 1);
-    }
-    MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, t, static_cast<size_t>(np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
-    uint8_t* ct = static_cast<uint8_t*>(s.src.p);
-    if ((e = dare_launch(c, true, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.p), np, static_cast<const uint8_t*>(s.aux.p), ct, nullptr, s.st))) return e;
-    c->st_h2d += pt1 - pt0;
-    o->obj = ct + pad + delta;
-    const int64_t ps = ceil_frac(off, kEPkg);  // the first package that starts in the chunk
-    o->ck = static_cast<const uint8_t*>(s.aux.p) + (ps - p0) * kPkg;
-    o->ck_len = ps <= p1 ? pt1 - ps * kPkg : 0;
-    return MEC_OK;
+    if ((e = s.aux.ensure(static_cast<size_t>(round_up(d.pt1 - d.pt0, 16) + 256)))) return e;
+    MEC_CUDA_OK(cudaMemcpyAsync(s.aux.p, src + d.pt0, static_cast<size_t>(d.pt1 - d.pt0), cudaMemcpyHostToDevice, s.st));
+    c->st_h2d += d.pt1 - d.pt0;
+    return dare_seal_chunk(c, s, d, len, static_cast<const uint8_t*>(s.aux.p), o);
   };
   rc = encode_pipeline(
       c, E, stage,
@@ -2185,51 +2207,65 @@ static int sig_streams(mec_codec* c) {
   return MEC_OK;
 }
 
-// The staging step of mec_encode_chunked for the object bytes [off, off + bytes), `last` for the pipeline's last chunk (or the one
-// step of an empty object).  ONE batched copy stages, back to back, the payload of every aws-chunk that overlaps the range or whose
-// row this step verifies, placed so that object byte `off` lands 16-byte aligned; the trailer message follows in the last step.  The
-// rows of the aws-chunks that start in the range (the last step: from `off` on, and the trailer row) are then verified by ONE launch
-// on the slot's second stream, behind the staging, so that the encode on s.st does not queue behind the hash.  *r0 / *nrow: the
-// first row and the number of rows of the step, whose verdicts land behind its rows in s.hsig_tab once s.st2 has drained.
-static int chunked_stage(mec_codec* c, Slot& s, const uint8_t* body, const ChunkedBody& P, int64_t off, int64_t bytes, bool last,
-                         Staged* o, int64_t* r0, int64_t* nrow) {
+// The aws-chunks of one staging step: [h0, h1) are the rows it verifies, those whose decoded start falls in [own0, own1) (the last
+// step: from own0 on, and the trailer row); [a, e) are the chunks it stages, every chunk that overlaps the decoded bytes from `lo`
+// on that the step needs, and its rows' chunks.  The steps' [own0, own1) tile the decoded bytes, so every row is verified once;
+// the bytes a step needs end at or before own1, so the overlapping chunks end where the rows do.
+struct AwsSpan {
+  int64_t a, e;    // staged chunks
+  int64_t h0, h1;  // verified rows
+  bool trow;       // and the trailer row
+};
+static AwsSpan aws_span(const ChunkedBody& P, int64_t lo, int64_t own0, int64_t own1, bool last) {
   const std::vector<AwsChunk>& ch = P.ch;
-  const int64_t nch = static_cast<int64_t>(ch.size()), end = off + bytes;
   auto first = [&](auto pred) { return std::partition_point(ch.begin(), ch.end(), pred) - ch.begin(); };
-  const int64_t a1 = first([&](const AwsChunk& x) { return x.doff + x.size <= off; });  // first chunk that overlaps or follows
-  const int64_t h0 = first([&](const AwsChunk& x) { return x.doff < off; });           // first chunk that starts in the range
-  const int64_t h1 = last ? nch : first([&](const AwsChunk& x) { return x.doff < end; });
-  const int64_t a = std::min(a1, h0), e = h1;  // the overlapping chunks end where the rows do
-  const int64_t lo = a < e ? ch[a].doff : off, hi = a < e ? ch[e - 1].doff + ch[e - 1].size : off;
-  const int64_t pad = (16 - (off - lo) % 16) % 16;
-  const bool trow = last && P.tclaim;
-  const int64_t tpos = round_up(pad + std::max(hi, end) - lo, 16);
+  AwsSpan sp;
+  const int64_t a1 = first([&](const AwsChunk& x) { return x.doff + x.size <= lo; });  // first chunk that overlaps or follows
+  sp.h0 = first([&](const AwsChunk& x) { return x.doff < own0; });
+  sp.h1 = last ? static_cast<int64_t>(ch.size()) : first([&](const AwsChunk& x) { return x.doff < own1; });
+  sp.a = std::min(a1, sp.h0);
+  sp.e = sp.h1;
+  sp.trow = last && P.tclaim;
+  return sp;
+}
+
+// ONE batched copy stages into `buf`, back to back, the payloads of the chunks [sp.a, sp.e), placed so that decoded byte `lo` lands
+// 16-byte aligned and the buffer reaches at least decoded byte `hi`; the trailer message follows when the step has the trailer
+// row.  *base: decoded byte x is at *base + x.  The step's rows are then verified by ONE launch on the slot's second stream, behind
+// the staging, so that the work queued on s.st next does not wait for the hash.  *r0 / *nrow: the first row and the number of rows
+// of the step, whose verdicts land behind its rows in s.hsig_tab once s.st2 has drained.
+static int aws_stage(mec_codec* c, Slot& s, DevBuf& buf, const uint8_t* body, const ChunkedBody& P, const AwsSpan& sp, int64_t lo,
+                     int64_t hi, uint8_t** base, int64_t* r0, int64_t* nrow) {
+  const std::vector<AwsChunk>& ch = P.ch;
+  const int64_t a = sp.a, e = sp.e, h0 = sp.h0, h1 = sp.h1;
+  const int64_t lo_s = a < e ? ch[a].doff : lo, hi_s = a < e ? ch[e - 1].doff + ch[e - 1].size : lo;
+  const int64_t pad = (16 - (lo - lo_s) % 16) % 16;
+  const int64_t tpos = round_up(pad + std::max(hi_s, hi) - lo_s, 16);
   int rc;
-  if ((rc = s.src.ensure(static_cast<size_t>(tpos + (trow ? static_cast<int64_t>(P.tmsg.size()) : 0) + 256)))) return rc;
-  uint8_t* base = static_cast<uint8_t*>(s.src.p) + pad - lo;  // object byte x at base + x
+  if ((rc = buf.ensure(static_cast<size_t>(tpos + (sp.trow ? static_cast<int64_t>(P.tmsg.size()) : 0) + 256)))) return rc;
+  uint8_t* b = static_cast<uint8_t*>(buf.p) + pad - lo_s;
+  *base = b;
   CopyList list;
   int64_t staged = 0;
   for (int64_t j = a; j < e; j++) {
-    list.add(base + ch[j].doff, body + ch[j].pay, ch[j].size);
+    list.add(b + ch[j].doff, body + ch[j].pay, ch[j].size);
     staged += ch[j].size;
   }
-  if (trow) {
-    list.add(static_cast<uint8_t*>(s.src.p) + tpos, P.tmsg.data(), static_cast<int64_t>(P.tmsg.size()));
+  if (sp.trow) {
+    list.add(static_cast<uint8_t*>(buf.p) + tpos, P.tmsg.data(), static_cast<int64_t>(P.tmsg.size()));
     staged += static_cast<int64_t>(P.tmsg.size());
   }
   if ((rc = list.flush(s.st))) return rc;
   c->st_h2d += staged;
-  o->obj = o->ck = base + off;
-  o->ck_len = bytes;
   *r0 = h0;
-  *nrow = h1 - h0 + (trow ? 1 : 0);
+  *nrow = h1 - h0 + (sp.trow ? 1 : 0);
   if (*nrow == 0) return MEC_OK;
   const size_t tab = static_cast<size_t>(*nrow) * (sizeof(SigRow) + 1);
   if ((rc = s.sig_tab.ensure(tab)) || (rc = s.hsig_tab.ensure(tab))) return rc;
   SigRow* h = static_cast<SigRow*>(s.hsig_tab.p);
-  for (int64_t j = h0; j < h1; j++) h[j - h0] = sig_row(base + ch[j].doff, ch[j].size, j - h0, kSigPayload, ch[j].prev, ch[j].claim);
-  if (trow)
-    h[h1 - h0] = sig_row(static_cast<uint8_t*>(s.src.p) + tpos, static_cast<int64_t>(P.tmsg.size()), h1 - h0, kSigTrailer,
+  for (int64_t j = h0; j < h1; j++) h[j - h0] = sig_row(b + ch[j].doff, ch[j].size, j - h0, kSigPayload, ch[j].prev, ch[j].claim);
+  if (sp.trow)
+    h[h1 - h0] = sig_row(static_cast<uint8_t*>(buf.p) + tpos, static_cast<int64_t>(P.tmsg.size()), h1 - h0, kSigTrailer,
                          ch.back().claim, P.tclaim);
   MEC_CUDA_OK(cudaEventRecord(s.ev_staged, s.st));
   MEC_CUDA_OK(cudaStreamWaitEvent(s.st2, s.ev_staged, 0));
@@ -2240,17 +2276,42 @@ static int chunked_stage(mec_codec* c, Slot& s, const uint8_t* body, const Chunk
   return MEC_OK;
 }
 
+// The staging step of mec_encode_chunked for the object bytes [off, off + bytes), `last` for the pipeline's last chunk (or the one
+// step of an empty object): the aws-chunks that overlap the range or start in it go to s.src with object byte `off` 16-byte
+// aligned for the encode, and the rows of those that start in it are verified.
+static int chunked_stage(mec_codec* c, Slot& s, const uint8_t* body, const ChunkedBody& P, int64_t off, int64_t bytes, bool last,
+                         Staged* o, int64_t* r0, int64_t* nrow) {
+  uint8_t* base;
+  const int rc = aws_stage(c, s, s.src, body, P, aws_span(P, off, off, off + bytes, last), off, off + bytes, &base, r0, nrow);
+  if (rc) return rc;
+  o->obj = o->ck = base + off;
+  o->ck_len = bytes;
+  return MEC_OK;
+}
+
+// The staging step of mec_encode_chunked_sse for the ciphertext bytes [off, off + bytes) of a stream of D plaintext bytes.  The
+// packages that overlap the range need the plaintext [pt0, pt1): the aws-chunks that overlap it go to s.aux with pt0 16-byte
+// aligned, and the rows whose decoded start falls among the packages that start in the range are verified (the steps' package
+// starts tile the plaintext).  The packages are then sealed into s.src as mec_encode_sse seals them.
+static int chunked_sse_stage(mec_codec* c, Slot& s, const uint8_t* body, const ChunkedBody& P, int64_t D, int64_t off, int64_t bytes,
+                             bool last, Staged* o, int64_t* r0, int64_t* nrow) {
+  const DareSpan d = dare_span(D, off, bytes);
+  const AwsSpan sp = aws_span(P, d.pt0, d.ps * kPkg, (d.p1 + 1) * kPkg, last);
+  uint8_t* base;
+  const int rc = aws_stage(c, s, s.aux, body, P, sp, d.pt0, d.pt1, &base, r0, nrow);
+  if (rc) return rc;
+  return dare_seal_chunk(c, s, d, D, base + d.pt0, o);
+}
+
 // newSignV4ChunkedReader + Erasure.Encode (cmd/object-handlers.go:1890, cmd/object-multipart-handlers.go:682,
 // cmd/object-handlers.go:2294): the body is de-framed on the host, its payloads go to the device through chunked_stage, and the
-// encode runs over the D decoded bytes as mec_encode does.
-extern "C" int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t* key,
-                                      const uint8_t* seed, const char* date, const char* scope, int trailer, uint8_t* const* files,
-                                      int write_quorum, uint8_t* trailer_out, int64_t trailer_cap, int64_t* trailer_len) {
-  NvtxRange nvtx("mec_encode_chunked");
-  if (!c || body_len < 0 || (body_len > 0 && !body) || decoded_len < 0 || !key || !seed || !date || !scope || !files)
-    return MEC_ERR_INVALID_ARGUMENT;
-  if (trailer && (!trailer_len || trailer_cap < 0 || (trailer_cap > 0 && !trailer_out))) return MEC_ERR_INVALID_ARGUMENT;
-  if (!lower_hex64(seed) || strlen(date) + strlen(scope) + 2 > static_cast<size_t>(kSigMaxHead)) return MEC_ERR_INVALID_ARGUMENT;
+// encode runs over the D decoded bytes as mec_encode does.  With an SSE key (mec_encode_chunked_sse: newSignV4ChunkedReader +
+// EncryptRequest + Erasure.Encode) the payloads go through chunked_sse_stage instead and the encode runs over their DARE stream as
+// mec_encode_sse does.  The caller has checked the arguments.
+static int64_t encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t* key,
+                              const uint8_t* seed, const char* date, const char* scope, int trailer, const uint8_t* sse_key,
+                              const uint8_t* nonce, uint8_t* const* files, int write_quorum, uint8_t* trailer_out, int64_t trailer_cap,
+                              int64_t* trailer_len) {
   if (trailer_len) *trailer_len = 0;
   int online = 0;
   for (int i = 0; i < c->n; i++) online += files[i] != nullptr;
@@ -2276,28 +2337,41 @@ extern "C" int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t
     memcpy(verdict.data() + r0[si], v, static_cast<size_t>(nr[si]));
   };
   const int64_t D = decoded_len;
+  const int64_t len = sse_key ? mec_dare_encrypted_size(D) : D;  // the bytes the encode covers
   if (D == 0) {  // no encode: the rows of the empty object in one step
     Staged sg;
     if ((rc = chunked_stage(c, s0, body, P, 0, 0, true, &sg, &r0[0], &nr[0]))) return rc;
     MEC_CUDA_OK(cudaStreamSynchronize(s0.st2));
     collect(0);
   } else {
-    rc = encode_pipeline(
-        c, D,
-        [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
-          const int si = static_cast<int>(&s - c->slots);
-          return chunked_stage(c, s, body, P, off, bytes, off + bytes == D, o, &r0[si], &nr[si]);
-        },
-        [&](const EncChunk& ch) -> int {
-          const int e = frames_enqueue_chunk(c, ch, files, true, nullptr);
-          if (e) return e;
-          if (nr[ch.s - c->slots]) MEC_CUDA_OK(cudaStreamWaitEvent(ch.st, ch.s->ev_verified, 0));  // the slot drains its verify too
-          return MEC_OK;
-        },
-        [&](const EncChunk& ch) {
-          frames_retire(c, ch, files, true, nullptr);
-          collect(static_cast<int>(ch.s - c->slots));
-        });
+    auto run = [&]() -> int {
+      return encode_pipeline(
+          c, len,
+          [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
+            const int si = static_cast<int>(&s - c->slots);
+            const bool last = off + bytes == len;
+            if (sse_key) return chunked_sse_stage(c, s, body, P, D, off, bytes, last, o, &r0[si], &nr[si]);
+            return chunked_stage(c, s, body, P, off, bytes, last, o, &r0[si], &nr[si]);
+          },
+          [&](const EncChunk& ch) -> int {
+            const int e = frames_enqueue_chunk(c, ch, files, true, nullptr);
+            if (e) return e;
+            if (nr[ch.s - c->slots]) MEC_CUDA_OK(cudaStreamWaitEvent(ch.st, ch.s->ev_verified, 0));  // the slot drains its verify too
+            return MEC_OK;
+          },
+          [&](const EncChunk& ch) {
+            frames_retire(c, ch, files, true, nullptr);
+            collect(static_cast<int>(ch.s - c->slots));
+          });
+    };
+    if (sse_key) {
+      if ((rc = dare_keys(c, 1, sse_key, nonce, s0.st))) return rc;
+      DareScrub dscrub{c, 1, s0.st};
+      MEC_CUDA_OK(cudaStreamSynchronize(s0.st));  // every slot stream reads the keys
+      rc = run();
+    } else {
+      rc = run();
+    }
     if (rc) return rc;
   }
   for (uint8_t v : verdict)
@@ -2312,6 +2386,41 @@ extern "C" int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t
     if (trailer_cap > 0) memcpy(trailer_out, P.tmsg.data(), static_cast<size_t>(std::min<int64_t>(trailer_cap, *trailer_len)));
   }
   return D;
+}
+
+// mec_encode_chunked's argument checks
+static bool chunked_args_ok(const mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t* key,
+                            const uint8_t* seed, const char* date, const char* scope, int trailer, uint8_t* const* files,
+                            const uint8_t* trailer_out, int64_t trailer_cap, const int64_t* trailer_len) {
+  if (!c || body_len < 0 || (body_len > 0 && !body) || decoded_len < 0 || !key || !seed || !date || !scope || !files) return false;
+  if (trailer && (!trailer_len || trailer_cap < 0 || (trailer_cap > 0 && !trailer_out))) return false;
+  return lower_hex64(seed) && strlen(date) + strlen(scope) + 2 <= static_cast<size_t>(kSigMaxHead);
+}
+
+extern "C" int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t* key,
+                                      const uint8_t* seed, const char* date, const char* scope, int trailer, uint8_t* const* files,
+                                      int write_quorum, uint8_t* trailer_out, int64_t trailer_cap, int64_t* trailer_len) {
+  NvtxRange nvtx("mec_encode_chunked");
+  if (!chunked_args_ok(c, body, body_len, decoded_len, key, seed, date, scope, trailer, files, trailer_out, trailer_cap, trailer_len))
+    return MEC_ERR_INVALID_ARGUMENT;
+  return encode_chunked(c, body, body_len, decoded_len, key, seed, date, scope, trailer, nullptr, nullptr, files, write_quorum,
+                        trailer_out, trailer_cap, trailer_len);
+}
+
+// newSignV4ChunkedReader + EncryptRequest + Erasure.Encode (cmd/object-handlers.go:1892, :2070): mec_encode_chunked's de-framing and
+// verdicts, and mec_encode_sse's part files of the decoded bytes, in one pass of the encode pipeline.
+extern "C" int64_t mec_encode_chunked_sse(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len,
+                                          const uint8_t* sig_key, const uint8_t* seed, const char* date, const char* scope, int trailer,
+                                          const uint8_t* sse_key, const uint8_t* nonce, uint8_t* const* files, int write_quorum,
+                                          uint8_t* trailer_out, int64_t trailer_cap, int64_t* trailer_len) {
+  NvtxRange nvtx("mec_encode_chunked_sse");
+  if (!chunked_args_ok(c, body, body_len, decoded_len, sig_key, seed, date, scope, trailer, files, trailer_out, trailer_cap, trailer_len) ||
+      !sse_key || !nonce)
+    return MEC_ERR_INVALID_ARGUMENT;
+  const int64_t E = mec_dare_encrypted_size(decoded_len);
+  if (E < 0) return E;
+  return encode_chunked(c, body, body_len, decoded_len, sig_key, seed, date, scope, trailer, sse_key, nonce, files, write_quorum,
+                        trailer_out, trailer_cap, trailer_len);
 }
 
 // Batched heal (SURVEY §8f rank 2, BASELINE config 4): objects are independent, so a pool of codec handles — each with
