@@ -428,9 +428,14 @@ int mec_batcher_verify(mec_batcher* b, int64_t nparts, const int* algos, const u
  * ordinary merged GET of the part (reader sets as mec_batcher_decode_prefer; any with MEC_BATCHER_MIX_PATTERNS); the batch assembles
  * every encrypted request's ciphertext on the device, runs ONE key-setup and ONE open launch over every package, and copies each
  * request's plaintext range back in one batched copy.  A request that met a frame failing its digest is redone alone through
- * mec_decode_sse on the private handle (counted in "redone"); otherwise a package of ChaCha20-Poly1305 or DARE 1.0 returns
- * MEC_ERR_UNSUPPORTED and any other failing package MEC_ERR_NOT_AUTHENTIC, with dst[0, length) zeroed.  One request's failure never
- * affects its batch neighbours.
+ * mec_decode_sse on the private handle (counted in "redone"); otherwise a package the request may not open (DARE 1.0; ChaCha20-
+ * Poly1305 at option "dare_chacha20" 0) returns MEC_ERR_UNSUPPORTED and any other failing package MEC_ERR_NOT_AUTHENTIC, with
+ * dst[0, length) zeroed.  One request's failure never affects its batch neighbours.
+ * Option "dare_chacha20" (mec_batcher_set_option): each encrypted request records the batcher's value when it is admitted and runs
+ * under it, in whichever batch it merges and when it is redone alone; one batch may hold requests admitted under different values.
+ * A GET batch with a request at 1 or 2 adds ONE ChaCha20-Poly1305 open launch behind the AES one, which opens the cipher-1 packages
+ * of exactly those requests.  A PUT batch seals the packages of its requests at 2 with ONE ChaCha20-Poly1305 launch, and those of the
+ * others with the AES one; a batch whose encrypted requests are all at 2 has no setup and no AES launch.
  * Calls whose buffers are not page-locked, and MEC_BATCHER_MEMCPY, run through mec_encode_sse / mec_decode_sse on the private handle.
  * Each slot holds its own key table: the device copy is zeroed on the slot's stream behind the batch's cipher launch, the host copy
  * before any caller of the batch is woken, and no pointer to a caller's key outlives the call.  Device memory: each slot's plaintext
@@ -439,12 +444,16 @@ int mec_batcher_verify(mec_batcher* b, int64_t nparts, const int* algos, const u
  * more than B blocks; a PUT batch's ciphertext arena is the slot's survivor arena, which mec_batcher_new* sizes and PUT batches do
  * not otherwise use.  The codec's AES tables are built, to completion, by the first encrypted batch.
  * Counters (mec_batcher_stat): "sse_puts" and "sse_gets" (calls completed by merged batches), "sse_serial" (calls of the private
- * path, redos included); "dare_sealed", "dare_opened" and "launches" are the batcher codec's. */
+ * path, redos included); "dare_sealed", "dare_opened", "dare_chacha20" and "launches" are the batcher codec's. */
 int64_t mec_batcher_encode_sse(mec_batcher* b, const uint8_t* src, int64_t len, const uint8_t key[32], const uint8_t nonce[12],
                                uint8_t* const* files, int write_quorum);
 int64_t mec_batcher_decode_sse(mec_batcher* b, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
                                int64_t enc_total, const uint8_t key[32], uint8_t* dst, int* heal_hint);
 int64_t mec_batcher_stat(const mec_batcher* b, const char* name);
+/* Options of a batcher: only "dare_chacha20" (0, 1 or 2, as mec_set_option), applied to the batcher's codec and its private handle;
+ * requests admitted afterwards run under the new value.  A NULL batcher or name, another name or another value is
+ * MEC_ERR_INVALID_ARGUMENT and changes nothing. */
+int mec_batcher_set_option(mec_batcher* b, const char* name, int64_t value);
 
 /* ---- object checksums of the PutObject stream (internal/hash/checksum.go:64-73, internal/hash/crc.go) ---------------------
  * CRC32 (IEEE), CRC32C (Castagnoli) and CRC64NVME — the checksum types hash.Reader can merge (ChecksumType.CanMerge) — of a
@@ -603,13 +612,20 @@ int mec_bitrot_verify_batch(mec_codec* c, int64_t nfiles, const uint8_t* const* 
 int mec_bitrot_verify_parts(mec_codec* c, int64_t nparts, const int* algos, const uint8_t* const* files, const int64_t* file_lens,
                             const int64_t* part_lens, const uint8_t* sums, int* results);
 
-/* ---- server-side encryption: DARE 2.0 packages (minio/sio v0.4.1, AES-256-GCM) ------------------------------------------------
+/* ---- server-side encryption: DARE 2.0 packages (minio/sio v0.4.1, AES-256-GCM and ChaCha20-Poly1305) ---------------------------
  * sio.EncryptReader with Version20 (newEncryptReader, cmd/encryption-v1.go:417-428) and DecryptBlocksRequestR (:572).  A package is
  * header[16] = 0x20 | cipher | uint16 LE (payload_len - 1) | nonce[12], the ciphertext and a 16-byte tag; every package but the last
  * carries 65536 bytes, bit 7 of header[4] marks the final one, the AEAD nonce is header[4:16] with bytes 8..11 (uint32 LE) XORed with
  * the sequence number, the additional data header[0:4].  Keys come from the caller (KMS, sealing and DerivePartKey stay in Go) and
- * only the raw key goes to the device, whose setup launch expands it; the key schedule and H powers of a call are zeroed on the device and the host before it returns.  ChaCha20-Poly1305 (cipher 1) and
- * DARE 1.0 (version 0x10) are MEC_ERR_UNSUPPORTED.  Counters: "dare_sealed", "dare_opened" (package rows run by the kernel). */
+ * only the raw key goes to the device, whose setup launch expands it; the key schedule and H powers of a call are zeroed on the device and the host before it returns.
+ * Option "dare_chacha20" (mec_set_option) picks the AEAD of header[1]:
+ *   0 (default) seals AES-256-GCM (cipher 0); a ChaCha20-Poly1305 package (cipher 1) is MEC_ERR_UNSUPPORTED and gets no plaintext.
+ *   1 seals AES-256-GCM and opens every package with the AEAD its own header names (0 or 1; RFC 8439 §2.8 for cipher 1, with the
+ *     same nonce and additional data).  An open runs ONE more launch, behind the AES one over the same rows.
+ *   2 as 1, and every seal (mec_dare_device, mec_encode_sse, mec_encode_chunked_sse) writes ChaCha20-Poly1305 packages (cipher 1)
+ *     with no key-setup launch.
+ * At 1 and 2, MEC_ERR_UNSUPPORTED means a DARE 1.0 stream (version 0x10) only; other cipher bytes are MEC_ERR_NOT_AUTHENTIC.
+ * Counters: "dare_sealed", "dare_opened" (package rows, each counted once whichever kernels ran it), "dare_chacha20" (the option). */
 /* sio.EncryptedSize / DecryptedSize; a negative size, more than 2^32 packages or a remainder of 1..32 bytes is
  * MEC_ERR_INVALID_ARGUMENT. */
 int64_t mec_dare_encrypted_size(int64_t n);
@@ -620,7 +636,8 @@ int64_t mec_dare_decrypted_size(int64_t enc);
  * of the part, which fixes each package's length and which one is final.  Each package is checked for version, length, final bit,
  * nonce (the first package's, final bit masked) and tag, and only one that passes gets plaintext written.  status[s] (host): 0, 13
  * (-MEC_ERR_NOT_AUTHENTIC: a package failed, the stored size is no DARE size, or bytes are cut short or run past the part) or 102
- * (-MEC_ERR_UNSUPPORTED).  Returns MEC_ERR_UNSUPPORTED if any stream is, else MEC_ERR_NOT_AUTHENTIC if any failed, else MEC_OK; waits
+ * (-MEC_ERR_UNSUPPORTED: a package of a cipher or version the option does not open).  Returns MEC_ERR_UNSUPPORTED if any stream
+ * is, else MEC_ERR_NOT_AUTHENTIC if any failed, else MEC_OK; waits
  * for its work on cuda_stream.  NULL arrays, negative offsets or lengths, an unknown op or a seal past sequence number 2^32 - 1 are
  * MEC_ERR_INVALID_ARGUMENT before any device work. */
 #define MEC_DARE_SEAL 1
@@ -630,13 +647,14 @@ int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uint8_t* keys,
                     const int64_t* out_off, uint8_t* status, void* cuda_stream);
 /* EncryptRequest + Erasure.Encode (cmd/object-handlers.go:2070): seals `len` bytes with `key` and the caller's 12 random nonce bytes
  * and writes mec_encode's part files of the sealed stream (sized for mec_dare_encrypted_size(len)).  Returns the plaintext bytes
- * consumed.  "checksums" covers the plaintext. */
+ * consumed.  "checksums" covers the plaintext.  At option "dare_chacha20" 2 the packages are ChaCha20-Poly1305. */
 int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint8_t key[32], const uint8_t nonce[12],
                        uint8_t* const* files, int write_quorum);
 /* Erasure.Decode + DecryptBlocksRequestR of one part (multipart callers pass the part key, one call per part): plaintext
  * [offset, offset + length) of a part stored as enc_total bytes; files / prefer / heal_hint as mec_decode_prefer.  Returns length,
- * MEC_ERR_NOT_AUTHENTIC or MEC_ERR_UNSUPPORTED (dst[0, length) zeroed), or mec_decode_prefer's errors.  Each package is opened once;
- * the ciphertext range and its plaintext are held in device buffers of the codec. */
+ * MEC_ERR_NOT_AUTHENTIC or MEC_ERR_UNSUPPORTED (dst[0, length) zeroed; ChaCha20-Poly1305 packages are UNSUPPORTED at option
+ * "dare_chacha20" 0 only, DARE 1.0 always), or mec_decode_prefer's errors.  Each package is opened once; the ciphertext range and its
+ * plaintext are held in device buffers of the codec. */
 int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
                        int64_t enc_total, const uint8_t key[32], uint8_t* dst, int* heal_hint);
 
@@ -685,7 +703,8 @@ int64_t mec_encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_len, 
  * mec_encode_chunked's, a NULL sse_key or nonce (MEC_ERR_INVALID_ARGUMENT) and a decoded_len no DARE stream holds, then
  * MEC_ERR_WRITE_QUORUM, all before any device work; so is an error in the first chunk's header.  After an error the part files are
  * unspecified.  An empty object verifies its final chunk (and trailer) rows and writes nothing.  "checksums" covers the decoded
- * plaintext, each byte once.  Both keys are zeroed on the device and the host before it returns. */
+ * plaintext, each byte once.  Both keys are zeroed on the device and the host before it returns.  At option "dare_chacha20" 2 the
+ * packages are ChaCha20-Poly1305, as mec_encode_sse's. */
 int64_t mec_encode_chunked_sse(mec_codec* c, const uint8_t* body, int64_t body_len, int64_t decoded_len, const uint8_t sig_key[32],
                                const uint8_t seed[64], const char* date, const char* scope, int trailer, const uint8_t sse_key[32],
                                const uint8_t nonce[12], uint8_t* const* files, int write_quorum, uint8_t* trailer_out,
@@ -705,7 +724,8 @@ int mec_hh256_batch(mec_codec* c, const uint8_t* msgs, int64_t msg_len, int64_t 
 /* erasureSelfTest + bitrotSelfTest (cmd/erasure-coding.go:149, cmd/bitrot.go:224) on the GPU. */
 int mec_selftest(int device);
 
-/* tuning knobs for benchmarks/tests (erasure blocks per CTA, loader, GF specialisation).
+/* tuning knobs for benchmarks/tests (erasure blocks per CTA, loader, GF specialisation), and "dare_chacha20" (0, 1 or 2: which
+ * DARE 2.0 AEADs the SSE calls open and seal, see above; any other value is MEC_ERR_INVALID_ARGUMENT and keeps the old one).
  * "jit": run-time specialisation of decode matrices / uncompiled (k, m) geometries with NVRTC, cached per process:
  *   -1 (default) a pattern that has been seen with 32 MiB of input is compiled on a background thread; calls that
  *      arrive before it is ready run the generic runtime-matrix kernel — no request ever waits for the compiler;

@@ -99,6 +99,7 @@ def lib():
     L.mec_batcher_heal_mixed.argtypes = [vp, vp, vp, vp, vp, i64, vp, vp]
     L.mec_batcher_stat.restype = i64
     L.mec_batcher_stat.argtypes = [vp, C.c_char_p]
+    L.mec_batcher_set_option.argtypes = [vp, C.c_char_p, i64]
     L.mec_checksums.argtypes = [vp, vp, i64, i32, vp]
     L.mec_checksums_device.argtypes = [vp, vp, i64, i32, vp, vp]
     L.mec_checksum_combine.restype = C.c_uint64
@@ -956,6 +957,12 @@ class Batcher:
         if rc < 0:
             raise MecError(rc, "mec_batcher_decode_sse")
         return dst[:length], hint.value
+
+    def set_option(self, name, value):
+        """mec_batcher_set_option: "dare_chacha20" (0, 1, 2) for requests admitted from now on"""
+        rc = lib().mec_batcher_set_option(self.h, name.encode(), int(value))
+        if rc:
+            raise MecError(rc, "mec_batcher_set_option")
 
     def stat(self, name):
         return lib().mec_batcher_stat(self.h, name.encode())

@@ -5,7 +5,7 @@
 // and keys per launch).  Thread t runs AES on GHASH blocks t, t + 256, ... and a Horner run over them with H^256, aligned by one
 // multiplication with H^e (1 <= e <= 256); the runs are XORed together.  dare_setup_kernel expands the key schedule and computes
 // H = E_K(0) and H^1..H^256 per stream from the raw key, dare_tables_kernel the AES tables once per codec.  Open checks header,
-// final bit, nonce and tag before any plaintext.
+// final bit, nonce and tag before any plaintext.  Packages that name ChaCha20-Poly1305 (cipher 1) are chacha.cuh's.
 #pragma once
 #include <cstdint>
 
@@ -28,13 +28,30 @@ struct DarePkg {
   int32_t final;    // the part's last package
 };
 
-// The host writes the first kDareKeyHead bytes of a stream (nonce and the raw key as rk[0..7]); dare_setup_kernel the rest.
+// The host writes the first kDareKeyHead bytes of a stream (nonce, policy byte and the raw key as rk[0..7]); dare_setup_kernel the rest.
 struct DareStreamKeys {
-  uint8_t nonce[16];     // seal: the stream's 12 nonce bytes
+  uint8_t nonce[16];     // seal: the stream's 12 nonce bytes; nonce[kDarePolicy]: the stream opens ChaCha20-Poly1305 packages
   uint32_t rk[60];       // AES-256 key schedule, big-endian words
   uint64_t hpow[256][2]; // H^(e+1) as (hi, lo) big-endian halves
 };
 constexpr size_t kDareKeyHead = 16 + 32;
+constexpr int kDarePolicy = 12;
+
+// The header checks of an open, in order: version, cipher, length against the position, final bit, the stream's nonce (ref: the
+// header of the stream's first package in the call).  `cipher` is the AEAD the caller opens (0 AES-256-GCM, 1 ChaCha20-Poly1305); a
+// package that names the other one is kDareUnsupported, as is DARE 1.0.
+__device__ __forceinline__ uint32_t dare_check_header(const uint8_t* hdr, const uint8_t* ref, int len, bool final, uint8_t cipher) {
+  uint32_t st = kDareOk;
+  if (hdr[0] != 0x20) st = hdr[0] == 0x10 ? kDareUnsupported : kDareNotAuthentic;
+  else if (hdr[1] != cipher) st = hdr[1] <= 1 ? kDareUnsupported : kDareNotAuthentic;
+  else if ((hdr[2] | (hdr[3] << 8)) + 1 != len) st = kDareNotAuthentic;
+  else if (((hdr[4] & 0x80) != 0) != final) st = kDareNotAuthentic;
+  else {
+    if (((hdr[4] ^ ref[4]) & 0x7f) != 0) st = kDareNotAuthentic;
+    for (int j = 5; j < 16; j++) if (hdr[j] != ref[j]) st = kDareNotAuthentic;
+  }
+  return st;
+}
 
 struct DareTables {
   uint32_t te[4][256];
@@ -267,16 +284,7 @@ __global__ void __launch_bounds__(kDareThreads, 4) dare_kernel(const DareTables*
       for (int j = 0; j < 16; j++) dst[j] = sm.hdr[j];
     } else {
       for (int j = 0; j < 16; j++) sm.hdr[j] = src[j];
-      const uint8_t* ref = in + row.ref_off;
-      // the checks in order: version, cipher, length against the position, final bit, the stream's nonce
-      if (sm.hdr[0] != 0x20) st = sm.hdr[0] == 0x10 ? kDareUnsupported : kDareNotAuthentic;
-      else if (sm.hdr[1] != 0) st = sm.hdr[1] == 1 ? kDareUnsupported : kDareNotAuthentic;
-      else if ((sm.hdr[2] | (sm.hdr[3] << 8)) + 1 != len) st = kDareNotAuthentic;
-      else if (((sm.hdr[4] & 0x80) != 0) != (row.final != 0)) st = kDareNotAuthentic;
-      else {
-        if (((sm.hdr[4] ^ ref[4]) & 0x7f) != 0) st = kDareNotAuthentic;
-        for (int j = 5; j < 16; j++) if (sm.hdr[j] != ref[j]) st = kDareNotAuthentic;
-      }
+      st = dare_check_header(sm.hdr, in + row.ref_off, len, row.final != 0, 0);
     }
     sm.nonce[0] = (uint32_t(sm.hdr[4]) << 24) | (uint32_t(sm.hdr[5]) << 16) | (uint32_t(sm.hdr[6]) << 8) | sm.hdr[7];
     sm.nonce[1] = (uint32_t(sm.hdr[8]) << 24) | (uint32_t(sm.hdr[9]) << 16) | (uint32_t(sm.hdr[10]) << 8) | sm.hdr[11];

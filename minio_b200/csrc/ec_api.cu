@@ -18,6 +18,7 @@
 #include "crc.cuh"
 #include "obj_hash.cuh"
 #include "batch_copy.cuh"
+#include "chacha.cuh"
 #include "dare.cuh"
 #include "sigv4.cuh"
 #include <nvtx3/nvToolsExt.h>
@@ -131,7 +132,8 @@ struct mec_codec {
   DevBuf whole, whole_dig;
   PinBuf hwhole_dig;
   DareState dare;
-  int64_t st_dare_sealed = 0, st_dare_opened = 0;  // DARE packages sealed / opened (rows launched)
+  int64_t st_dare_sealed = 0, st_dare_opened = 0;  // DARE packages sealed / opened (rows launched, each once whatever its cipher)
+  std::atomic<int> dare_chacha20{0};  // option "dare_chacha20": 0 AES-256-GCM only; 1 also open ChaCha20-Poly1305; 2 also seal with it
   SigState sig;
   int64_t st_sigv4_chunks = 0;  // signature rows verified
   int64_t S() const { return ceil_frac(block_size, k); }
@@ -290,6 +292,10 @@ extern "C" int mec_set_option(mec_codec* c, const char* name, int64_t v) {
   else if (!strcmp(name, "static_groups")) c->opt.static_groups = static_cast<int>(v);
   else if (!strcmp(name, "small_blocks")) c->opt.small_blocks = v;
   else if (!strcmp(name, "checksums")) c->checksums = static_cast<int>(v) & 7;
+  else if (!strcmp(name, "dare_chacha20")) {
+    if (v < 0 || v > 2) return MEC_ERR_INVALID_ARGUMENT;
+    c->dare_chacha20 = static_cast<int>(v);
+  }
   else return MEC_ERR_INVALID_ARGUMENT;
   return MEC_OK;
 }
@@ -323,6 +329,7 @@ extern "C" int64_t mec_get_stat(const mec_codec* c, const char* name) {
   if (!strcmp(name, "whole_hash_launches")) return c->st_whole_hash;
   if (!strcmp(name, "dare_sealed")) return c->st_dare_sealed;
   if (!strcmp(name, "dare_opened")) return c->st_dare_opened;
+  if (!strcmp(name, "dare_chacha20")) return c->dare_chacha20.load();
   if (!strcmp(name, "sigv4_chunks")) return c->st_sigv4_chunks;
   if (!strcmp(name, "sigv4_key_bytes")) return sig_key_bytes(c);
   if (!strcmp(name, "jit_compiles")) return c->eng ? c->eng->jit_compiles() : 0;
@@ -1676,37 +1683,41 @@ static int dare_tables(mec_codec* c, cudaStream_t st) {
   return MEC_OK;
 }
 
-// The first kDareKeyHead bytes of a stream's DareStreamKeys: its nonce (seal; zero for open) and its raw key as big-endian words
-static void dare_key_head(uint8_t* h, const uint8_t* key, const uint8_t* nonce) {
+// The first kDareKeyHead bytes of a stream's DareStreamKeys: its nonce (seal; zero for open), whether it opens ChaCha20-Poly1305
+// packages (option "dare_chacha20" >= 1), and its raw key as big-endian words
+static void dare_key_head(uint8_t* h, const uint8_t* key, const uint8_t* nonce, int chacha) {
   memset(h, 0, kDareKeyHead);
   if (nonce) memcpy(h, nonce, 12);
+  h[kDarePolicy] = chacha >= 1;
   uint32_t* rk = reinterpret_cast<uint32_t*>(h + offsetof(DareStreamKeys, rk));
   for (int i = 0; i < 8; i++)
     rk[i] = (uint32_t(key[4 * i]) << 24) | (uint32_t(key[4 * i + 1]) << 16) | (uint32_t(key[4 * i + 2]) << 8) | key[4 * i + 3];
 }
 
-// ONE dare_setup_kernel launch over `ns` streams on `st`: the key heads in `heads` (pinned, kDareKeyHead bytes each) go to the
-// device table `dk`, which the kernel completes with the key schedules and H powers
-static int dare_setup(mec_codec* c, DareStreamKeys* dk, const uint8_t* heads, int64_t ns, cudaStream_t st) {
+// The key heads in `heads` (pinned, kDareKeyHead bytes each) of `ns` streams go to the device table `dk` on `st`; with `aes`, ONE
+// dare_setup_kernel launch completes it with the key schedules and H powers (a ChaCha20 seal needs neither)
+static int dare_setup(mec_codec* c, DareStreamKeys* dk, const uint8_t* heads, int64_t ns, cudaStream_t st, bool aes = true) {
   int rc;
-  if ((rc = dare_tables(c, st))) return rc;
+  if (aes && (rc = dare_tables(c, st))) return rc;
   MEC_CUDA_OK(cudaMemcpy2DAsync(dk, sizeof(DareStreamKeys), heads, kDareKeyHead, kDareKeyHead, static_cast<size_t>(ns),
                                 cudaMemcpyHostToDevice, st));
+  if (!aes) return MEC_OK;
   dare_setup_kernel<<<static_cast<unsigned>(ns), kDareThreads, 0, st>>>(static_cast<const DareTables*>(c->dare.tabs.p), dk);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
   return MEC_OK;
 }
 
-// Key schedules and H powers of `ns` streams into c->dare.keys, enqueued on `st`; nonces: seal only.
-static int dare_keys(mec_codec* c, int64_t ns, const uint8_t* keys, const uint8_t* nonces, cudaStream_t st) {
+// Key schedules and H powers of `ns` streams into c->dare.keys, enqueued on `st`; nonces: seal only.  chacha: the call's value of
+// option "dare_chacha20" (a seal at 2 writes the raw keys only).
+static int dare_keys(mec_codec* c, int64_t ns, const uint8_t* keys, const uint8_t* nonces, cudaStream_t st, int chacha) {
   DareState& d = c->dare;
   int rc;
   if ((rc = d.keys.ensure(static_cast<size_t>(ns) * sizeof(DareStreamKeys))) || (rc = d.hkeys.ensure(static_cast<size_t>(ns) * kDareKeyHead)))
     return rc;
   uint8_t* h = static_cast<uint8_t*>(d.hkeys.p);
-  for (int64_t s = 0; s < ns; s++) dare_key_head(h + s * kDareKeyHead, keys + 32 * s, nonces ? nonces + 12 * s : nullptr);
-  return dare_setup(c, static_cast<DareStreamKeys*>(d.keys.p), h, ns, st);
+  for (int64_t s = 0; s < ns; s++) dare_key_head(h + s * kDareKeyHead, keys + 32 * s, nonces ? nonces + 12 * s : nullptr, chacha);
+  return dare_setup(c, static_cast<DareStreamKeys*>(d.keys.p), h, ns, st, !(nonces && chacha == 2));
 }
 
 // Zeroes the key material of the call, device and host, once everything on `st` (and before it) is done with it.
@@ -1721,15 +1732,24 @@ struct DareScrub {
   }
 };
 
-// ONE launch over n package rows (device table pk) with the streams' keys `k`; open writes status[row]
-static int dare_launch(mec_codec* c, bool seal, const DareStreamKeys* k, const DarePkg* pk, int64_t n, const uint8_t* in, uint8_t* out,
-                       uint8_t* status, cudaStream_t st) {
+// ONE launch over n package rows (device table pk) with the streams' keys `k`; open writes status[row].  chacha: a seal is
+// ChaCha20-Poly1305 instead of AES-256-GCM; an open is followed by ONE dare_chacha_kernel launch over the same rows, which opens the
+// cipher-1 packages of the streams that allow it.
+static int dare_launch(mec_codec* c, bool seal, bool chacha, const DareStreamKeys* k, const DarePkg* pk, int64_t n, const uint8_t* in,
+                       uint8_t* out, uint8_t* status, cudaStream_t st) {
   if (n <= 0) return MEC_OK;
   const DareTables* t = static_cast<const DareTables*>(c->dare.tabs.p);
-  if (seal) dare_kernel<true><<<static_cast<unsigned>(n), kDareThreads, 0, st>>>(t, k, pk, in, out, status);
-  else dare_kernel<false><<<static_cast<unsigned>(n), kDareThreads, 0, st>>>(t, k, pk, in, out, status);
+  const unsigned g = static_cast<unsigned>(n);
+  if (seal && chacha) dare_chacha_kernel<true><<<g, kDareThreads, 0, st>>>(k, pk, in, out, status);
+  else if (seal) dare_kernel<true><<<g, kDareThreads, 0, st>>>(t, k, pk, in, out, status);
+  else dare_kernel<false><<<g, kDareThreads, 0, st>>>(t, k, pk, in, out, status);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
+  if (!seal && chacha) {
+    dare_chacha_kernel<false><<<g, kDareThreads, 0, st>>>(k, pk, in, out, status);
+    MEC_CUDA_OK(cudaGetLastError());
+    c->eng->count_launch();
+  }
   (seal ? c->st_dare_sealed : c->st_dare_opened) += n;
   return MEC_OK;
 }
@@ -1764,11 +1784,12 @@ extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uin
   MEC_CUDA_OK(cudaSetDevice(c->device));
   DareState& d = c->dare;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int chacha = c->dare_chacha20.load();
   const size_t tab = static_cast<size_t>(std::max<int64_t>(rows, 1)) * sizeof(DarePkg);
   if ((rc = d.hpk.ensure(tab)) || (rc = d.pk.ensure(tab)) || (rc = d.st.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))) ||
       (rc = d.hst.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))))
     return rc;
-  if ((rc = dare_keys(c, nstreams, keys, seal ? nonces : nullptr, st))) return rc;
+  if ((rc = dare_keys(c, nstreams, keys, seal ? nonces : nullptr, st, chacha))) return rc;
   DareScrub scrub{c, nstreams, st};
   DarePkg* t = static_cast<DarePkg*>(d.hpk.p);
   int64_t w = 0;
@@ -1795,7 +1816,9 @@ extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uin
   }
   if (w > 0) {
     MEC_CUDA_OK(cudaMemcpyAsync(d.pk.p, t, static_cast<size_t>(w) * sizeof(DarePkg), cudaMemcpyHostToDevice, st));
-    if ((rc = dare_launch(c, seal, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p), w, d_in, d_out, static_cast<uint8_t*>(d.st.p), st))) return rc;
+    if ((rc = dare_launch(c, seal, seal ? chacha == 2 : chacha >= 1, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p), w, d_in, d_out,
+                          static_cast<uint8_t*>(d.st.p), st)))
+      return rc;
     if (!seal) MEC_CUDA_OK(cudaMemcpyAsync(d.hst.p, d.st.p, static_cast<size_t>(w), cudaMemcpyDeviceToHost, st));
   }
   MEC_CUDA_OK(cudaStreamSynchronize(st));
@@ -1834,8 +1857,8 @@ static DareSpan dare_span(int64_t len, int64_t off, int64_t bytes) {
 
 // Seals the packages of `d` on s.st from their plaintext at `pt` (device, plaintext byte d.pt0; 16-byte aligned for the fast
 // loads) into s.src, and points the chunk's staged object bytes at the ciphertext and its checksum bytes at the plaintext of the
-// packages that start in the chunk, as hash.Reader sees each byte once.
-static int dare_seal_chunk(mec_codec* c, Slot& s, const DareSpan& d, int64_t len, const uint8_t* pt, Staged* o) {
+// packages that start in the chunk, as hash.Reader sees each byte once.  chacha: ChaCha20-Poly1305 packages (option 2).
+static int dare_seal_chunk(mec_codec* c, Slot& s, const DareSpan& d, int64_t len, const uint8_t* pt, Staged* o, bool chacha) {
   const int64_t npk = ceil_frac(len, kPkg);
   int e;
   if ((e = s.src.ensure(static_cast<size_t>(d.pad + d.np * kEPkg + 256))) || (e = s.hdpk.ensure(static_cast<size_t>(d.np) * sizeof(DarePkg))) ||
@@ -1848,7 +1871,7 @@ static int dare_seal_chunk(mec_codec* c, Slot& s, const DareSpan& d, int64_t len
   }
   MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, t, static_cast<size_t>(d.np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
   uint8_t* ct = static_cast<uint8_t*>(s.src.p);
-  if ((e = dare_launch(c, true, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.p), d.np, pt, ct, nullptr, s.st))) return e;
+  if ((e = dare_launch(c, true, chacha, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.p), d.np, pt, ct, nullptr, s.st))) return e;
   o->obj = ct + d.pad + d.delta;
   o->ck = pt + (d.ps - d.p0) * kPkg;
   o->ck_len = d.ps <= d.p1 ? d.pt1 - d.ps * kPkg : 0;
@@ -1857,10 +1880,10 @@ static int dare_seal_chunk(mec_codec* c, Slot& s, const DareSpan& d, int64_t len
 
 // EncryptRequest + Erasure.Encode: chunks are whole erasure blocks of the ciphertext.  A chunk stages and seals every package that
 // overlaps it (one across a chunk boundary is sealed in both: sealing is deterministic) and encodes its ciphertext unchanged.
-// "checksums" covers the plaintext, as hash.Reader sees it: each chunk the packages that start in it.
-extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint8_t* key, const uint8_t* nonce,
-                                  uint8_t* const* files, int write_quorum) {
-  NvtxRange nvtx("mec_encode_sse");
+// "checksums" covers the plaintext, as hash.Reader sees it: each chunk the packages that start in it.  chacha: the value of option
+// "dare_chacha20" the call runs under (2 seals ChaCha20-Poly1305 packages).
+static int64_t encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint8_t* key, const uint8_t* nonce, uint8_t* const* files,
+                          int write_quorum, int chacha) {
   if (!c || len < 0 || !files || !key || !nonce || (len > 0 && !src)) return MEC_ERR_INVALID_ARGUMENT;
   const int64_t E = mec_dare_encrypted_size(len);
   if (E < 0) return E;
@@ -1877,7 +1900,7 @@ extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len,
   std::lock_guard<std::mutex> lk(c->mu);
   MEC_CUDA_OK(cudaSetDevice(c->device));
   Slot& s0 = c->slots[0];
-  if ((rc = dare_keys(c, 1, key, nonce, s0.st))) return rc;
+  if ((rc = dare_keys(c, 1, key, nonce, s0.st, chacha))) return rc;
   DareScrub scrub{c, 1, s0.st};
   MEC_CUDA_OK(cudaStreamSynchronize(s0.st));  // every slot stream reads the keys
   auto stage = [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
@@ -1886,7 +1909,7 @@ extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len,
     if ((e = s.aux.ensure(static_cast<size_t>(round_up(d.pt1 - d.pt0, 16) + 256)))) return e;
     MEC_CUDA_OK(cudaMemcpyAsync(s.aux.p, src + d.pt0, static_cast<size_t>(d.pt1 - d.pt0), cudaMemcpyHostToDevice, s.st));
     c->st_h2d += d.pt1 - d.pt0;
-    return dare_seal_chunk(c, s, d, len, static_cast<const uint8_t*>(s.aux.p), o);
+    return dare_seal_chunk(c, s, d, len, static_cast<const uint8_t*>(s.aux.p), o, chacha == 2);
   };
   rc = encode_pipeline(
       c, E, stage,
@@ -1894,13 +1917,18 @@ extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len,
       [&](const EncChunk& ch) { frames_retire(c, ch, files, true, nullptr); });
   return rc ? rc : len;
 }
+extern "C" int64_t mec_encode_sse(mec_codec* c, const uint8_t* src, int64_t len, const uint8_t* key, const uint8_t* nonce,
+                                  uint8_t* const* files, int write_quorum) {
+  NvtxRange nvtx("mec_encode_sse");
+  return encode_sse(c, src, len, key, nonce, files, write_quorum, c ? c->dare_chacha20.load() : 0);
+}
 
 // Erasure.Decode of the ciphertext range GetDecryptedRange maps the plaintext range to, then DecryptBlocksRequestR, for one part.
 // Chunks move their data slices device-to-device into a ciphertext buffer of the range; whenever a prefix of the range is final
-// the packages it completes are opened, each once, and their asked-for plaintext is copied back.
-extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
-                                  int64_t enc_total, const uint8_t* key, uint8_t* dst, int* heal_hint) {
-  NvtxRange nvtx("mec_decode_sse");
+// the packages it completes are opened, each once, and their asked-for plaintext is copied back.  chacha: the value of option
+// "dare_chacha20" the call runs under (>= 1 opens ChaCha20-Poly1305 packages too).
+static int64_t decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
+                          int64_t enc_total, const uint8_t* key, uint8_t* dst, int* heal_hint, int chacha) {
   if (heal_hint) *heal_hint = 0;
   if (!c || !files || !key || offset < 0 || length < 0 || enc_total < 0) return MEC_ERR_INVALID_ARGUMENT;
   const int64_t D = mec_dare_decrypted_size(enc_total);
@@ -1926,7 +1954,7 @@ extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, con
       (rc = d.pk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))) || (rc = d.hpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))))
     return rc;
   Slot& s0 = c->slots[0];
-  if ((rc = dare_keys(c, 1, key, nullptr, s0.st))) return rc;
+  if ((rc = dare_keys(c, 1, key, nullptr, s0.st, chacha))) return rc;
   DareScrub scrub{c, 1, s0.st};
   DarePkg* t = static_cast<DarePkg*>(d.hpk.p);
   for (int64_t j = 0; j < np; j++) {
@@ -1947,8 +1975,8 @@ extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, con
     if (upto <= opened) return MEC_OK;
     Slot& s = c->slots[si];
     int e;
-    if ((e = dare_launch(c, false, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p) + opened, upto - opened, ct, static_cast<uint8_t*>(d.pt.p),
-                         static_cast<uint8_t*>(d.st.p) + opened, s.st)))
+    if ((e = dare_launch(c, false, chacha >= 1, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p) + opened, upto - opened, ct,
+                         static_cast<uint8_t*>(d.pt.p), static_cast<uint8_t*>(d.st.p) + opened, s.st)))
       return e;
     const int64_t a = std::max(offset, (p_first + opened) * kPkg), z = std::min(offset + length, (p_first + upto) * kPkg);
     if (z > a) {
@@ -1981,6 +2009,11 @@ extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, con
     for (int i = 0; i < n; i++)
       if (corrupt[i]) *heal_hint = MEC_ERR_FILE_CORRUPT;
   return length;
+}
+extern "C" int64_t mec_decode_sse(mec_codec* c, const uint8_t* const* files, const uint8_t* prefer, int64_t offset, int64_t length,
+                                  int64_t enc_total, const uint8_t* key, uint8_t* dst, int* heal_hint) {
+  NvtxRange nvtx("mec_decode_sse");
+  return decode_sse(c, files, prefer, offset, length, enc_total, key, dst, heal_hint, c ? c->dare_chacha20.load() : 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2294,13 +2327,13 @@ static int chunked_stage(mec_codec* c, Slot& s, const uint8_t* body, const Chunk
 // aligned, and the rows whose decoded start falls among the packages that start in the range are verified (the steps' package
 // starts tile the plaintext).  The packages are then sealed into s.src as mec_encode_sse seals them.
 static int chunked_sse_stage(mec_codec* c, Slot& s, const uint8_t* body, const ChunkedBody& P, int64_t D, int64_t off, int64_t bytes,
-                             bool last, Staged* o, int64_t* r0, int64_t* nrow) {
+                             bool last, Staged* o, int64_t* r0, int64_t* nrow, int chacha) {
   const DareSpan d = dare_span(D, off, bytes);
   const AwsSpan sp = aws_span(P, d.pt0, d.ps * kPkg, (d.p1 + 1) * kPkg, last);
   uint8_t* base;
   const int rc = aws_stage(c, s, s.aux, body, P, sp, d.pt0, d.pt1, &base, r0, nrow);
   if (rc) return rc;
-  return dare_seal_chunk(c, s, d, D, base + d.pt0, o);
+  return dare_seal_chunk(c, s, d, D, base + d.pt0, o, chacha == 2);
 }
 
 // newSignV4ChunkedReader + Erasure.Encode (cmd/object-handlers.go:1890, cmd/object-multipart-handlers.go:682,
@@ -2338,6 +2371,7 @@ static int64_t encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_le
   };
   const int64_t D = decoded_len;
   const int64_t len = sse_key ? mec_dare_encrypted_size(D) : D;  // the bytes the encode covers
+  const int chacha = c->dare_chacha20.load();
   if (D == 0) {  // no encode: the rows of the empty object in one step
     Staged sg;
     if ((rc = chunked_stage(c, s0, body, P, 0, 0, true, &sg, &r0[0], &nr[0]))) return rc;
@@ -2350,7 +2384,7 @@ static int64_t encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_le
           [&](Slot& s, int64_t off, int64_t bytes, Staged* o) -> int {
             const int si = static_cast<int>(&s - c->slots);
             const bool last = off + bytes == len;
-            if (sse_key) return chunked_sse_stage(c, s, body, P, D, off, bytes, last, o, &r0[si], &nr[si]);
+            if (sse_key) return chunked_sse_stage(c, s, body, P, D, off, bytes, last, o, &r0[si], &nr[si], chacha);
             return chunked_stage(c, s, body, P, off, bytes, last, o, &r0[si], &nr[si]);
           },
           [&](const EncChunk& ch) -> int {
@@ -2365,7 +2399,7 @@ static int64_t encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_le
           });
     };
     if (sse_key) {
-      if ((rc = dare_keys(c, 1, sse_key, nonce, s0.st))) return rc;
+      if ((rc = dare_keys(c, 1, sse_key, nonce, s0.st, chacha))) return rc;
       DareScrub dscrub{c, 1, s0.st};
       MEC_CUDA_OK(cudaStreamSynchronize(s0.st));  // every slot stream reads the keys
       rc = run();
@@ -3564,6 +3598,7 @@ struct BatchReq {
   const uint8_t* sse_nonce = nullptr;
   int64_t sse_offset = 0, sse_len = 0, sse_total = 0;
   int64_t sse_ct = 0, sse_row0 = 0;
+  int sse_chacha = 0;  // the batcher's option "dare_chacha20" when the request was admitted (mec_batcher_set_option)
   int64_t result = 0;
   bool done = false;
   std::condition_variable cv;  // one per request: a finished batch wakes its own callers, not every thread parked in the batcher
@@ -3636,6 +3671,7 @@ struct mec_batcher {
   std::atomic<int64_t> st_verifies{0}, st_verifies_serial{0};
   // mec_batcher_encode_sse / _decode_sse: calls completed by merged batches, and calls of the private path (redos included)
   std::atomic<int64_t> st_sse_puts{0}, st_sse_gets{0}, st_sse_serial{0};
+  std::atomic<int> dare_chacha20{0};  // mec_batcher_set_option: recorded by every encrypted request as it is admitted
 };
 
 namespace {
@@ -3652,6 +3688,7 @@ static mec_codec* batcher_private(mec_batcher* b, const mec_codec* g, mec_codec*
   if (!h) {
     mec_codec* p = nullptr;
     if (mec_codec_new(g->k, g->m, g->block_size, algo, g->device, &p) == MEC_OK) h = p;
+    if (p && &h == &b->serial) p->dare_chacha20 = b->dare_chacha20.load();
   }
   return h;
 }
@@ -3664,12 +3701,13 @@ static inline int whole_index(int algo) { return algo == MEC_SHA256 ? 0 : algo =
 // write quorum already checked on the caller's thread; a whole-file move does the same through mec_transcode_whole, whose source
 // handle carries the part's algorithm)
 static int64_t batcher_run_alone(mec_batcher* b, const BatchReq& r) {
-  if (r.sse_key) {  // an encrypted PUT or GET: mec_encode_sse / mec_decode_sse, the write quorum already checked
+  if (r.sse_key) {  // an encrypted PUT or GET: mec_encode_sse / mec_decode_sse under the option it was admitted with, the write
+                    // quorum already checked
     b->st_sse_serial++;
     mec_codec* sc = batcher_private(b, b->codec, b->serial);
     if (!sc) return MEC_ERR_UNEXPECTED;
-    if (r.kind == ReqKind::Put) return mec_encode_sse(sc, r.src, r.sse_len, r.sse_key, r.sse_nonce, r.files, 0);
-    return mec_decode_sse(sc, r.gfiles, r.prefer, r.sse_offset, r.sse_len, r.total, r.sse_key, r.dst, r.heal_hint);
+    if (r.kind == ReqKind::Put) return encode_sse(sc, r.src, r.sse_len, r.sse_key, r.sse_nonce, r.files, 0, r.sse_chacha);
+    return decode_sse(sc, r.gfiles, r.prefer, r.sse_offset, r.sse_len, r.total, r.sse_key, r.dst, r.heal_hint, r.sse_chacha);
   }
   if (r.kind == ReqKind::TranscodeWhole) {
     b->st_transcodes_whole_serial++;
@@ -3937,11 +3975,16 @@ static int batcher_sums_join(mec_batcher* b, Slot& s, size_t nreq, int64_t nwork
 
 // Server-side encryption in merged batches (mec_batcher_encode_sse / _decode_sse).  The encrypted requests of a batch are the streams
 // of ONE dare_setup_kernel launch (stream z = the z-th such request in batch order) and their packages the rows of ONE dare_kernel
-// launch.  Each slot has its own key table, package table (s.dpk) and verdicts: six batches in flight never share key material.
-// The device keys are zeroed on the slot's stream behind the cipher launch, the host-written heads by batcher_finish.
+// launch.  Each request carries the option "dare_chacha20" it was admitted with: an open batch with a request at 1 or 2 adds ONE
+// dare_chacha_kernel launch behind the AES one (each stream's key head says whether it opens ChaCha20); a seal batch seals the
+// packages of its requests at 2 with ONE dare_chacha_kernel launch instead, and needs the setup only for the others.  Each slot
+// has its own key table, package table (s.dpk) and verdicts: six batches in flight never share key material.  The device keys are
+// zeroed on the slot's stream behind the cipher launches, the host-written heads by batcher_finish.
 static int sse_batch_setup(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, bool seal, int64_t* nsse) {
   *nsse = 0;
-  for (const BatchReq* r : reqs) *nsse += r->sse_key != nullptr;
+  bool aes = !seal;
+  for (const BatchReq* r : reqs)
+    if (r->sse_key) { ++*nsse; aes |= r->sse_chacha != 2; }
   if (*nsse == 0) return MEC_OK;
   int rc;
   if ((rc = s.sse_keys.ensure(static_cast<size_t>(*nsse) * sizeof(DareStreamKeys))) ||
@@ -3949,9 +3992,9 @@ static int sse_batch_setup(mec_batcher* b, Slot& s, const std::vector<BatchReq*>
     return rc;
   uint8_t* h = static_cast<uint8_t*>(s.hsse_keys.p);
   for (const BatchReq* r : reqs)
-    if (r->sse_key) { dare_key_head(h, r->sse_key, seal ? r->sse_nonce : nullptr); h += kDareKeyHead; }
+    if (r->sse_key) { dare_key_head(h, r->sse_key, seal ? r->sse_nonce : nullptr, r->sse_chacha); h += kDareKeyHead; }
   s.sse_heads = *nsse;
-  return dare_setup(b->codec, static_cast<DareStreamKeys*>(s.sse_keys.p), static_cast<const uint8_t*>(s.hsse_keys.p), *nsse, s.st);
+  return dare_setup(b->codec, static_cast<DareStreamKeys*>(s.sse_keys.p), static_cast<const uint8_t*>(s.hsse_keys.p), *nsse, s.st, aes);
 }
 // The plaintext arena: sized for a full batch (batcher_slot_blocks x block_size) on the slot's first encrypted batch; it only grows
 // past that for a batch led by a request larger than max_batch_blocks.  A batch's plaintext is at most its ciphertext, which batch
@@ -3960,20 +4003,32 @@ static int64_t batcher_slot_blocks(const mec_batcher* b);
 static int size_sse_arena(mec_batcher* b, Slot& s, int64_t bytes) {
   return s.sse_pt.ensure(static_cast<size_t>(std::max(bytes, batcher_slot_blocks(b) * b->codec->block_size)));
 }
-// ONE cipher launch over the batch's package rows s.hdpk[0, rows) (an open writes its verdicts to s.sse_st), then the keys are zeroed
-static int sse_batch_cipher(mec_batcher* b, Slot& s, bool seal, int64_t nsse, int64_t rows, const uint8_t* in, uint8_t* out) {
+// The cipher launches over the batch's package rows s.hdpk[0, rows) (an open writes its verdicts to s.sse_st), then the keys are
+// zeroed.  A seal seals rows [0, chacha_from) with AES-256-GCM and the rest with ChaCha20-Poly1305; an open with chacha_from < rows
+// adds the ChaCha20 open behind the AES one.
+static int sse_batch_cipher(mec_batcher* b, Slot& s, bool seal, int64_t nsse, int64_t rows, int64_t chacha_from, const uint8_t* in,
+                            uint8_t* out) {
   MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, s.hdpk.p, static_cast<size_t>(rows) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
-  const int rc = dare_launch(b->codec, seal, static_cast<const DareStreamKeys*>(s.sse_keys.p), static_cast<const DarePkg*>(s.dpk.p), rows,
-                             in, out, seal ? nullptr : static_cast<uint8_t*>(s.sse_st.p), s.st);
-  if (rc) return rc;
+  const DareStreamKeys* k = static_cast<const DareStreamKeys*>(s.sse_keys.p);
+  const DarePkg* pk = static_cast<const DarePkg*>(s.dpk.p);
+  int rc;
+  if (seal) {
+    if ((rc = dare_launch(b->codec, true, false, k, pk, chacha_from, in, out, nullptr, s.st)) ||
+        (rc = dare_launch(b->codec, true, true, k, pk + chacha_from, rows - chacha_from, in, out, nullptr, s.st)))
+      return rc;
+  } else if ((rc = dare_launch(b->codec, false, chacha_from < rows, k, pk, rows, in, out, static_cast<uint8_t*>(s.sse_st.p), s.st))) {
+    return rc;
+  }
   MEC_CUDA_OK(cudaMemsetAsync(s.sse_keys.p, 0, static_cast<size_t>(nsse) * sizeof(DareStreamKeys), s.st));
   return MEC_OK;
 }
 
 // The encrypted PUTs of a batch, before its staging copy: their plaintext goes to the arena s.sse_pt by pieces added to `h2d` (the
 // batch's one batched copy), their packages are laid out contiguously per request in the ciphertext arena s.aux (unused by PUT
-// batches; r->sse_ct), and the key setup is enqueued.  *rows = 0: the batch has no encrypted request.
-static int sse_put_plan(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, CopyList& h2d, int64_t* nsse, int64_t* rows) {
+// batches; r->sse_ct), and the key setup is enqueued.  *rows = 0: the batch has no encrypted request.  The rows of the requests
+// admitted at option 2 (ChaCha20-Poly1305) come last, from *chacha_from on.
+static int sse_put_plan(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, CopyList& h2d, int64_t* nsse, int64_t* rows,
+                        int64_t* chacha_from) {
   *rows = 0;
   int64_t pt_total = 0, ct_total = 0;
   for (const BatchReq* r : reqs)
@@ -3990,25 +4045,29 @@ static int sse_put_plan(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
   DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
   uint8_t* pt = static_cast<uint8_t*>(s.sse_pt.p);
   int64_t w = 0, po = 0, co = 0;
-  int z = 0;
-  for (BatchReq* r : reqs) {
-    if (!r->sse_key) continue;
-    const int64_t np = ceil_frac(r->sse_len, kPkg);
-    for (int64_t j = 0; j < np; j++) t[w++] = dare_row(po + j * kPkg, co + j * kEPkg, 0, std::min(kPkg, r->sse_len - j * kPkg), j, z, j == np - 1);
-    h2d.add(pt + po, r->src, r->sse_len);
-    r->sse_ct = co;
-    po += round_up(r->sse_len, 256);
-    co += round_up(r->len, 256);
-    z++;
+  for (int pass = 0; pass < 2; pass++) {  // the AES-256-GCM requests, then the ChaCha20-Poly1305 ones
+    if (pass == 1) *chacha_from = w;
+    int z = 0;  // the request's stream: its place among the batch's encrypted requests
+    for (BatchReq* r : reqs) {
+      if (!r->sse_key) continue;
+      if ((r->sse_chacha == 2) != (pass == 1)) { z++; continue; }
+      const int64_t np = ceil_frac(r->sse_len, kPkg);
+      for (int64_t j = 0; j < np; j++) t[w++] = dare_row(po + j * kPkg, co + j * kEPkg, 0, std::min(kPkg, r->sse_len - j * kPkg), j, z, j == np - 1);
+      h2d.add(pt + po, r->src, r->sse_len);
+      r->sse_ct = co;
+      po += round_up(r->sse_len, 256);
+      co += round_up(r->len, 256);
+      z++;
+    }
   }
   return sse_batch_setup(b, s, reqs, true, nsse);
 }
 // Once the batch is staged: ONE seal launch over every package (each sealed once), then ONE batched device-to-device copy of each
 // request's ciphertext into its places in the PUT layout (full blocks at ch.d_src, the short last block at ch.d_src_tail)
-static int sse_put_seal(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t nsse, int64_t rows) {
+static int sse_put_seal(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t nsse, int64_t rows, int64_t chacha_from) {
   if (rows == 0) return MEC_OK;
   const uint8_t* ct = static_cast<const uint8_t*>(s.aux.p);
-  int rc = sse_batch_cipher(b, s, true, nsse, rows, static_cast<const uint8_t*>(s.sse_pt.p), static_cast<uint8_t*>(s.aux.p));
+  int rc = sse_batch_cipher(b, s, true, nsse, rows, chacha_from, static_cast<const uint8_t*>(s.sse_pt.p), static_cast<uint8_t*>(s.aux.p));
   if (rc) return rc;
   const int64_t bs = b->codec->block_size;
   CopyList cl;
@@ -4025,11 +4084,13 @@ static int sse_put_seal(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
 // batched copy of each request's plaintext range to its caller.  The arena is cleared first, so a package that fails leaves zeros.
 static int sse_get_open(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const std::vector<int64_t>& asm_off) {
   int64_t rows = 0, pt_total = 0;
+  bool chacha = false;
   for (const BatchReq* r : reqs)
     if (r->sse_key) {
       const int64_t np = (r->sse_offset + r->sse_len - 1) / kPkg - r->sse_offset / kPkg + 1;
       rows += np;
       pt_total += np * kPkg;
+      chacha |= r->sse_chacha >= 1;
     }
   if (rows == 0) return MEC_OK;
   int rc;
@@ -4060,7 +4121,7 @@ static int sse_get_open(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
     z++;
   }
   MEC_CUDA_OK(cudaMemsetAsync(pt, 0, static_cast<size_t>(pt_total), s.st));
-  if ((rc = sse_batch_cipher(b, s, false, nsse, rows, static_cast<const uint8_t*>(s.src.p), pt))) return rc;
+  if ((rc = sse_batch_cipher(b, s, false, nsse, rows, chacha ? 0 : rows, static_cast<const uint8_t*>(s.src.p), pt))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(s.hsse_st.p, s.sse_st.p, static_cast<size_t>(rows), cudaMemcpyDeviceToHost, s.st));
   return d2h.flush(s.st);
 }
@@ -4179,7 +4240,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   *needs_retire = true;
   bool all_mapped = n <= kBatchMaxFiles && !b->sw.memcpy, sse = false;
   for (BatchReq* r : reqs) { all_mapped &= r->mapped; sse |= r->sse_key != nullptr; }
-  int64_t nsse = 0, sse_rows = 0;
+  int64_t nsse = 0, sse_rows = 0, sse_chacha_from = 0;
   PutLayout lay;
   int rc;
   if ((rc = put_layout(c, s, reqs, all_mapped, true, lay))) return rc;
@@ -4244,11 +4305,11 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
         cl.add(dsrc + d.full0 * bs, d.src, fbytes);
         cl.add(dsrc + d.tail_src_off, d.src + fbytes, tl);
       }
-      if ((rc = sse_put_plan(b, s, reqs, cl, &nsse, &sse_rows))) return rc;
+      if ((rc = sse_put_plan(b, s, reqs, cl, &nsse, &sse_rows, &sse_chacha_from))) return rc;
       if ((rc = cl.flush(s.st))) return rc;
     }
     if (ndma > 0 && ndma < reqs.size()) MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_gather[si], 0));
-    if ((rc = sse_put_seal(b, s, reqs, nsse, sse_rows))) return rc;
+    if ((rc = sse_put_seal(b, s, reqs, nsse, sse_rows, sse_chacha_from))) return rc;
     mark_phase(b, s, 1);
     if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
     if ((rc = batcher_crc_launch(b, s, crc))) return rc;
@@ -4274,7 +4335,9 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   }
   if (sse) {  // encrypted requests beside a pageable one: their plaintext in one batched copy, then the seal into the layout
     CopyList cl;
-    if ((rc = sse_put_plan(b, s, reqs, cl, &nsse, &sse_rows)) || (rc = cl.flush(s.st)) || (rc = sse_put_seal(b, s, reqs, nsse, sse_rows))) return rc;
+    if ((rc = sse_put_plan(b, s, reqs, cl, &nsse, &sse_rows, &sse_chacha_from)) || (rc = cl.flush(s.st)) ||
+        (rc = sse_put_seal(b, s, reqs, nsse, sse_rows, sse_chacha_from)))
+      return rc;
     for (const BatchReq* r : reqs) c->st_h2d += r->sse_key ? r->sse_len : 0;
   }
   if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
@@ -5584,7 +5647,7 @@ extern "C" int64_t mec_batcher_encode_sse(mec_batcher* b, const uint8_t* src, in
   if (len == 0) return 0;
   BatchReq r;
   r.src = src; r.len = E; r.files = files; r.with_data = true;
-  r.sse_key = key; r.sse_nonce = nonce; r.sse_len = len;
+  r.sse_key = key; r.sse_nonce = nonce; r.sse_len = len; r.sse_chacha = b->dare_chacha20.load();
   bool mapped = !b->sw.memcpy && mec_is_pinned(src) != 0;
   for (int i = 0; i < n && mapped; i++)
     if (files[i]) mapped = mec_is_pinned(files[i]) != 0;
@@ -5614,8 +5677,19 @@ extern "C" int64_t mec_batcher_decode_sse(mec_batcher* b, const uint8_t* const* 
   BatchReq r;
   r.kind = ReqKind::Get; r.gfiles = files; r.offset = eoff; r.length = eend - eoff; r.total = enc_total; r.dst = dst;
   r.heal_hint = heal_hint; r.prefer = prefer;
-  r.sse_key = key; r.sse_offset = offset; r.sse_len = length; r.sse_total = D;
+  r.sse_key = key; r.sse_offset = offset; r.sse_len = length; r.sse_total = D; r.sse_chacha = b->dare_chacha20.load();
   return batcher_get(b, r);
+}
+
+// Options of a batcher: "dare_chacha20" (0, 1, 2; see mec_set_option) for its codec and private handle.  Each encrypted request
+// records the value when it is admitted and runs under it, whichever batch it merges into and if it is redone alone.
+extern "C" int mec_batcher_set_option(mec_batcher* b, const char* name, int64_t value) {
+  if (!b || !name || strcmp(name, "dare_chacha20") != 0 || value < 0 || value > 2) return MEC_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(b->serial_mu);  // a private handle created meanwhile takes the new value
+  b->dare_chacha20 = static_cast<int>(value);
+  int rc = mec_set_option(b->codec, name, value);
+  if (rc == MEC_OK && b->serial) rc = mec_set_option(b->serial, name, value);
+  return rc;
 }
 
 extern "C" int64_t mec_batcher_stat(const mec_batcher* b, const char* name) {
