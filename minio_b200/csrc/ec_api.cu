@@ -45,49 +45,31 @@ static inline int64_t round_up(int64_t v, int64_t a) { return (v + a - 1) / a * 
 
 constexpr int kSlots = 6;
 
-// grow-only page-locked host staging (digests and digest verdicts: small, read by the host right after a stream drains)
-struct PinBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t n) {
-    if (n <= cap) return MEC_OK;
-    release();
-    const size_t want = n + (n >> 2) + 4096;
-    MEC_CUDA_OK(cudaHostAlloc(&p, want, cudaHostAllocPortable));
-    cap = want;
-    return MEC_OK;
-  }
-  void release() {
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
-  }
-};
-
 struct Slot {
-  DevBuf src, out, dig, aux, flags;  // aux: survivor arena of a reconstruct chunk / shard files of the whole-file path
-  DevBuf crc_part, crc_out;          // object checksums of an encode chunk (crc.cuh); of a merged batch: per-item partials, per-request results
-  DevBuf crc_tab;                    // checksum work table of a merged batch ([CrcReq nreq][CrcWork nwork], crc.cuh)
-  DevBuf dreq;                       // request table of a merged batch (batch_copy.cuh)
-  DevBuf blk;                        // per-block geometry of a merged launch (SmallBlock / per-frame lengths)
-  DevBuf sum_tab, sum_out;           // object hashes of a merged batch: SumWork table, one kSumRecord record per request (obj_hash.cuh)
+  DevBuf src, out, aux;              // aux: survivor arena of a reconstruct chunk / shard files of the whole-file path
+  Mirror dig, flags;                 // digests and digest verdicts: small, read by the host right after the stream drains
+  // object checksums of an encode chunk (crc.cuh); of a merged batch: per-item partials (crc_part), per-request results (crc_out)
+  DevBuf crc_part;
+  Mirror crc_out;
+  Mirror crc_tab;                    // checksum work table of a merged batch ([CrcReq nreq][CrcWork nwork], crc.cuh)
+  Mirror dreq;                       // request table of a merged batch (batch_copy.cuh)
+  Mirror blk;                        // per-block geometry of a merged launch (SmallBlock / per-frame lengths)
+  Mirror sum_tab, sum_out;           // object hashes of a merged batch: SumWork table, one kSumRecord record per request (obj_hash.cuh)
   // merged batches with whole-file readers (batch_whole_stage): the WholeStream of every staged shard file (whole_hash.cuh) and
   // each request's first stream behind them; one 64-byte digest per staged file
-  DevBuf wtab, wdig;
-  PinBuf hdig, hflags, hcrc, hreq, hblk, hcrc_tab, hsum_tab, hsum, hwtab, hwdig;
-  DevBuf dpk;                        // mec_encode_sse: the DarePkg rows of the chunk's packages; a merged batch: of all its packages
-  PinBuf hdpk;
+  Mirror wtab, wdig;
+  Mirror dpk;                        // mec_encode_sse: the DarePkg rows of the chunk's packages; a merged batch: of all its packages
   // merged batches with encrypted requests (mec_batcher_encode_sse / _decode_sse): the streams' DareStreamKeys and their host-written
   // heads, the plaintext arena, and the package verdicts of an open
-  DevBuf sse_keys, sse_pt, sse_st;
-  PinBuf hsse_keys, hsse_st;
+  DevBuf sse_keys, sse_pt;
+  PinBuf hsse_keys;
+  Mirror sse_st;
   int64_t sse_heads = 0;             // key heads written to hsse_keys by the slot's batch in flight (zeroed by batcher_finish)
   // mec_encode_chunked: the signature rows of the chunk and their verdicts behind them; the second stream that verifies them while
   // s.st encodes, with the events that order it after the staging and s.st after it
-  DevBuf sig_tab;
-  PinBuf hsig_tab;
-  cudaStream_t st = nullptr, st2 = nullptr;
-  cudaEvent_t ev_staged = nullptr, ev_verified = nullptr;
+  Mirror sig_tab;
+  Stream st, st2;
+  Event ev_staged, ev_verified;
 };
 
 // DARE 2.0 state of a codec (dare.cuh): the AES round tables (built once), the key schedules and H powers of the streams of the
@@ -95,15 +77,15 @@ struct Slot {
 // of the range.
 struct DareState {
   bool tabs_ok = false;
-  DevBuf tabs, keys, pk, st, ct, pt;
-  PinBuf hkeys, hpk, hst;
+  DevBuf tabs, keys, ct, pt;
+  PinBuf hkeys;
+  Mirror pk, st;
 };
 
 // Signature V4 streaming state of a codec (sigv4.cuh): the SigCall of the call in flight (key states zeroed before it returns) and
 // mec_chunk_signatures_device's row table with the verdicts behind the rows.
 struct SigState {
-  DevBuf call, rows;
-  PinBuf hcall, hrows;
+  Mirror call, rows;
 };
 
 struct mec_codec {
@@ -121,16 +103,15 @@ struct mec_codec {
   uint64_t last_crc[kCrcTypes] = {0, 0, 0};
   int64_t last_crc_len = 0;
   // mec_sums_device: the work table of the last call, and an event behind its kernel (the next call refills the table after it)
-  DevBuf sum_tab;
-  PinBuf hsum_tab;
-  cudaEvent_t sum_ev = nullptr;
+  Mirror sum_tab;
+  Event sum_ev;
   // boundary counters (mec_get_stat)
   int64_t st_blocks_encoded = 0, st_blocks_read = 0, st_shards_rebuilt = 0, st_corrupt = 0, st_h2d = 0, st_d2h = 0;
   int64_t st_whole_hash = 0;  // whole_hash_kernel launches
   // mec_decode_mixed / mec_heal_mixed: the verified whole-file readers of the call (k files at a pitch of round_up(sfs, 16) + 256)
   // and their digests; they stay on the device for the whole call while the slot arenas cycle through the chunks
-  DevBuf whole, whole_dig;
-  PinBuf hwhole_dig;
+  DevBuf whole;
+  Mirror whole_dig;
   DareState dare;
   int64_t st_dare_sealed = 0, st_dare_opened = 0;  // DARE packages sealed / opened (rows launched, each once whatever its cipher)
   std::atomic<int> dare_chacha20{0};  // option "dare_chacha20": 0 AES-256-GCM only; 1 also open ChaCha20-Poly1305; 2 also seal with it
@@ -236,44 +217,24 @@ static int ensure_engine(mec_codec* c) {
   int rc = e->init();
   if (rc) return rc;
   for (auto& s : c->slots)
-    if (cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking) != cudaSuccess) {
+    if (s.st.create(cudaStreamNonBlocking) != cudaSuccess) {
       set_last_error(std::string("cudaStreamCreate: ") + cudaGetErrorString(cudaGetLastError()));
-      for (auto& q : c->slots)
-        if (q.st) { cudaStreamDestroy(q.st); q.st = nullptr; }
       return MEC_ERR_CUDA;
     }
-
   c->eng = std::move(e);
   return MEC_OK;
 }
 
 extern "C" void mec_codec_free(mec_codec* c) {
   if (!c) return;
-  if (!c->eng) { delete c; return; }
-  cudaSetDevice(c->device);
-  for (auto& s : c->slots) {
-    if (s.st) { cudaStreamSynchronize(s.st); cudaStreamDestroy(s.st); }
-    s.src.release(); s.out.release(); s.dig.release(); s.aux.release(); s.flags.release();
-    s.hdig.release(); s.hflags.release(); s.hcrc.release(); s.crc_part.release(); s.crc_out.release(); s.dreq.release(); s.hreq.release(); s.blk.release(); s.hblk.release();
-    s.crc_tab.release(); s.hcrc_tab.release(); s.sum_tab.release(); s.sum_out.release(); s.hsum_tab.release(); s.hsum.release();
-    s.wtab.release(); s.hwtab.release(); s.wdig.release(); s.hwdig.release();
-    s.dpk.release(); s.hdpk.release();
-    s.sse_keys.release(); s.sse_pt.release(); s.sse_st.release(); s.hsse_keys.release(); s.hsse_st.release();
-    s.sig_tab.release(); s.hsig_tab.release();
-    if (s.st2) { cudaStreamSynchronize(s.st2); cudaStreamDestroy(s.st2); }
-    if (s.ev_staged) cudaEventDestroy(s.ev_staged);
-    if (s.ev_verified) cudaEventDestroy(s.ev_verified);
+  if (c->eng) {
+    // every slot's streams drain before any stream, event or buffer of the codec is destroyed
+    cudaSetDevice(c->device);
+    for (auto& s : c->slots) {
+      if (s.st) cudaStreamSynchronize(s.st);
+      if (s.st2) cudaStreamSynchronize(s.st2);
+    }
   }
-  for (DevBuf* b : {&c->sig.call, &c->sig.rows}) b->release();
-  for (PinBuf* b : {&c->sig.hcall, &c->sig.hrows}) b->release();
-  for (DevBuf* b : {&c->dare.tabs, &c->dare.keys, &c->dare.pk, &c->dare.st, &c->dare.ct, &c->dare.pt}) b->release();
-  for (PinBuf* b : {&c->dare.hkeys, &c->dare.hpk, &c->dare.hst}) b->release();
-  c->flags.release();
-  c->crc_tables.release();
-  c->whole.release(); c->whole_dig.release(); c->hwhole_dig.release();
-  if (c->sum_ev) cudaEventDestroy(c->sum_ev);
-  c->sum_tab.release();
-  c->hsum_tab.release();
   delete c;
 }
 
@@ -304,7 +265,7 @@ static int64_t sig_key_bytes(const mec_codec* c) {
   const size_t kb = offsetof(SigCall, head_len);
   int64_t nz = 0;
   for (int dev = 0; dev < 2; dev++) {
-    const void* p = dev ? c->sig.call.p : c->sig.hcall.p;
+    const void* p = dev ? c->sig.call.d.p : c->sig.call.h.p;
     if (!p) continue;
     uint8_t buf[offsetof(SigCall, head_len)];
     if (dev) {
@@ -465,9 +426,9 @@ extern "C" int mec_checksums_device(mec_codec* c, const uint8_t* d_src, int64_t 
   MEC_CUDA_OK(cudaSetDevice(c->device));
   Slot& s = c->slots[0];
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if ((rc = s.crc_out.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
-  if ((rc = checksums_enqueue(c, d_src, len, which, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), st))) return rc;
-  MEC_CUDA_OK(cudaMemcpyAsync(out3, s.crc_out.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  if ((rc = s.crc_out.d.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
+  if ((rc = checksums_enqueue(c, d_src, len, which, s.crc_part, static_cast<uint64_t*>(s.crc_out.d.p), st))) return rc;
+  MEC_CUDA_OK(cudaMemcpyAsync(out3, s.crc_out.d.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   MEC_CUDA_OK(cudaStreamSynchronize(st));
   return MEC_OK;
 }
@@ -513,19 +474,18 @@ extern "C" int mec_sums_device(mec_codec* c, int which, const uint8_t* d_base, c
   int rc;
   if ((rc = ensure_engine(c))) return rc;
   MEC_CUDA_OK(cudaSetDevice(c->device));
-  if (!c->sum_ev) MEC_CUDA_OK(cudaEventCreateWithFlags(&c->sum_ev, cudaEventDisableTiming));
+  MEC_CUDA_OK(c->sum_ev.create(cudaEventDisableTiming));
   MEC_CUDA_OK(cudaEventSynchronize(c->sum_ev));  // the previous call's kernel has read its table
   const int64_t nwork = count * per;
   const size_t bytes = static_cast<size_t>(nwork) * sizeof(SumWork);
-  if ((rc = c->hsum_tab.ensure(bytes))) return rc;
   if ((rc = c->sum_tab.ensure(bytes))) return rc;
-  SumWork* t = static_cast<SumWork*>(c->hsum_tab.p);
+  SumWork* t = static_cast<SumWork*>(c->sum_tab.h.p);
   int64_t w = 0;
   for (int64_t i = 0; i < count; i++) w = sum_items(t, w, which, i * kSumRecord, offsets[i], lens[i], 0, 0);
   sum_sort(t, nwork);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  MEC_CUDA_OK(cudaMemcpyAsync(c->sum_tab.p, t, bytes, cudaMemcpyHostToDevice, st));
-  if ((rc = sum_launch(c, d_base, static_cast<const SumWork*>(c->sum_tab.p), nwork, d_sums, st))) return rc;
+  MEC_CUDA_OK(c->sum_tab.upload(bytes, st));
+  if ((rc = sum_launch(c, d_base, static_cast<const SumWork*>(c->sum_tab.d.p), nwork, d_sums, st))) return rc;
   MEC_CUDA_OK(cudaEventRecord(c->sum_ev, st));
   return MEC_OK;
 }
@@ -543,7 +503,7 @@ extern "C" int mec_checksums(mec_codec* c, const uint8_t* src, int64_t len, int 
   int64_t done = 0;
   int64_t clen[kSlots] = {};
   SlotRing ring(c, [&](int si) {
-    const uint64_t* h = static_cast<const uint64_t*>(c->slots[si].hcrc.p);
+    const uint64_t* h = static_cast<const uint64_t*>(c->slots[si].crc_out.h.p);
     for (int ty = 0; ty < kCrcTypes; ty++) {
       const CrcSpec sp = crc_spec(ty);
       acc[ty] = done == 0 ? h[ty] : crc_combine(c->crc_host->xp8[ty], acc[ty], h[ty], clen[si], sp.poly, sp.bits);
@@ -557,10 +517,9 @@ extern "C" int mec_checksums(mec_codec* c, const uint8_t* src, int64_t len, int 
     const int64_t n = std::min(chunk, len - off);
     if ((rc = s.src.ensure(static_cast<size_t>(round_up(n, 16) + 256)))) return rc;
     if ((rc = s.crc_out.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
-    if ((rc = s.hcrc.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
     MEC_CUDA_OK(cudaMemcpyAsync(s.src.p, src + off, static_cast<size_t>(n), cudaMemcpyHostToDevice, s.st));
-    if ((rc = checksums_enqueue(c, static_cast<const uint8_t*>(s.src.p), n, which, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), s.st))) return rc;
-    MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
+    if ((rc = checksums_enqueue(c, static_cast<const uint8_t*>(s.src.p), n, which, s.crc_part, static_cast<uint64_t*>(s.crc_out.d.p), s.st))) return rc;
+    MEC_CUDA_OK(s.crc_out.download(kCrcTypes * sizeof(uint64_t), s.st));
     clen[si] = n;
     c->st_h2d += n;
     ring.submitted();
@@ -709,7 +668,7 @@ static int encode_pipeline(mec_codec* c, int64_t len, Stage&& stage, Enqueue&& e
   }
   SlotRing ring(c, [&](int q) {
     if (ck) {
-      const uint64_t* h = static_cast<const uint64_t*>(c->slots[q].hcrc.p);
+      const uint64_t* h = static_cast<const uint64_t*>(c->slots[q].crc_out.h.p);
       for (int ty = 0; ty < kCrcTypes; ty++) {
         if (!(ck & (1 << ty))) continue;
         const CrcSpec sp = crc_spec(ty);
@@ -729,21 +688,20 @@ static int encode_pipeline(mec_codec* c, int64_t len, Stage&& stage, Enqueue&& e
     const int64_t off = b0 * bs, bytes = std::min(len - off, ch.nb * bs);
     ch.nfull = bytes / bs; ch.tail = bytes % bs;
     if ((rc = s.out.ensure(static_cast<size_t>(ch.nb * std::max(c->m, 1) * pitch)))) return rc;
-    if ((rc = s.dig.ensure(static_cast<size_t>(ch.nb * c->n * 32)))) return rc;
+    if ((rc = s.dig.d.ensure(static_cast<size_t>(ch.nb * c->n * 32)))) return rc;
     Staged sg;
     if ((rc = stage(s, off, bytes, &sg))) return rc;
-    if ((rc = s.hdig.ensure(static_cast<size_t>(ch.nb * c->n * 32)))) return rc;
+    if ((rc = s.dig.h.ensure(static_cast<size_t>(ch.nb * c->n * 32)))) return rc;
     ch.st = s.st;
     ch.d_src = sg.obj; ch.d_src_tail = ch.d_src + ch.nfull * bs;
     ch.d_out = static_cast<uint8_t*>(s.out.p); ch.d_out_tail = ch.d_out + ch.nfull * c->m * pitch;
-    ch.h_dig = static_cast<const uint8_t*>(s.hdig.p); ch.h_dig_tail = ch.h_dig + ch.nfull * c->n * 32;
-    if ((rc = encode_device_locked(c, sg.obj, bytes, static_cast<uint8_t*>(s.out.p), pitch, static_cast<uint8_t*>(s.dig.p), s.st)))
+    ch.h_dig = static_cast<const uint8_t*>(s.dig.h.p); ch.h_dig_tail = ch.h_dig + ch.nfull * c->n * 32;
+    if ((rc = encode_device_locked(c, sg.obj, bytes, static_cast<uint8_t*>(s.out.p), pitch, static_cast<uint8_t*>(s.dig.d.p), s.st)))
       return rc;
     if (ck) {
       if ((rc = s.crc_out.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
-      if ((rc = s.hcrc.ensure(kCrcTypes * sizeof(uint64_t)))) return rc;
-      if ((rc = checksums_enqueue(c, sg.ck, sg.ck_len, ck, s.crc_part, static_cast<uint64_t*>(s.crc_out.p), s.st))) return rc;
-      MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
+      if ((rc = checksums_enqueue(c, sg.ck, sg.ck_len, ck, s.crc_part, static_cast<uint64_t*>(s.crc_out.d.p), s.st))) return rc;
+      MEC_CUDA_OK(s.crc_out.download(kCrcTypes * sizeof(uint64_t), s.st));
       ck_len[si] = sg.ck_len;
     }
     if ((rc = enqueue(ch))) return rc;
@@ -781,7 +739,7 @@ extern "C" int mec_encode_blocks(mec_codec* c, const uint8_t* src, int64_t len, 
                                         static_cast<uint8_t*>(s.out.p) + ch.nfull * c->m * ch.pitch, static_cast<size_t>(ch.pitch),
                                         static_cast<size_t>(St), static_cast<size_t>(c->m), cudaMemcpyDeviceToHost, s.st));
         }
-        MEC_CUDA_OK(cudaMemcpyAsync(digests + ch.b0 * c->n * 32, s.dig.p, static_cast<size_t>(ch.nb * c->n * 32),
+        MEC_CUDA_OK(cudaMemcpyAsync(digests + ch.b0 * c->n * 32, s.dig.d.p, static_cast<size_t>(ch.nb * c->n * 32),
                                     cudaMemcpyDeviceToHost, s.st));
         return MEC_OK;
       },
@@ -919,11 +877,11 @@ static void frames_retire(mec_codec* c, const EncChunk& ch, uint8_t* const* file
 static int frames_enqueue_chunk(mec_codec* c, const EncChunk& ch, uint8_t* const* files, bool with_data, uint8_t* data_digests) {
   if (ch.nb <= kBatchedCopyBlocks) {  // a small object: digests and every frame piece in ONE batched copy call
     CopyList list;
-    list.add(ch.s->hdig.p, ch.s->dig.p, ch.nb * c->n * 32);
+    list.add(ch.s->dig.h.p, ch.s->dig.d.p, ch.nb * c->n * 32);
     const int e = frames_enqueue(c, ch, files, with_data, data_digests, &list);
     return e ? e : list.flush(ch.st);
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(ch.s->hdig.p, ch.s->dig.p, static_cast<size_t>(ch.nb * c->n * 32), cudaMemcpyDeviceToHost, ch.st));
+  MEC_CUDA_OK(ch.s->dig.download(static_cast<size_t>(ch.nb * c->n * 32), ch.st));
   return frames_enqueue(c, ch, files, with_data, data_digests);
 }
 
@@ -1037,8 +995,8 @@ static int launch_reconstruct(mec_codec* c, const FrameGeom& g, const RChunk& ch
       d.map_base[t] = base; d.map_len[t] = stride; d.expect_ptr[t] = (raw && raw[t]) ? nullptr : base; d.in_ptr[t] = base + 32;
     }
     d.out = static_cast<uint8_t*>(s.out.p);
-    d.digests = static_cast<uint8_t*>(s.dig.p);
-    d.corrupt = static_cast<uint8_t*>(s.flags.p);
+    d.digests = static_cast<uint8_t*>(s.dig.d.p);
+    d.corrupt = static_cast<uint8_t*>(s.flags.d.p);
     return c->eng->launch_fused(d, c->opt, s.st);
   }
   for (int pass = 0; pass < 2; pass++) {
@@ -1055,8 +1013,8 @@ static int launch_reconstruct(mec_codec* c, const FrameGeom& g, const RChunk& ch
       d.in_ptr[t] = base + 32;
     }
     d.out = static_cast<uint8_t*>(s.out.p) + first * r * pitch;
-    d.digests = static_cast<uint8_t*>(s.dig.p) + first * (k + r) * 32;
-    d.corrupt = static_cast<uint8_t*>(s.flags.p) + first * k;
+    d.digests = static_cast<uint8_t*>(s.dig.d.p) + first * (k + r) * 32;
+    d.corrupt = static_cast<uint8_t*>(s.flags.d.p) + first * k;
     int rc = c->eng->launch_fused(d, c->opt, s.st);
     if (rc) return rc;
   }
@@ -1165,21 +1123,21 @@ static int emit_frames(mec_codec* c, const FrameGeom& g, const RangeSink& sk, co
     dst += ch.b0 * fstride;
     if (list) {
       for (int64_t b = 0; b < ch.nb; b++) {
-        list->add(dst + b * fstride, static_cast<uint8_t*>(s.dig.p) + (b * (k + r) + k + q) * 32, 32);
+        list->add(dst + b * fstride, static_cast<uint8_t*>(s.dig.d.p) + (b * (k + r) + k + q) * 32, 32);
         list->add(dst + b * fstride + 32, static_cast<uint8_t*>(s.out.p) + (b * r + q) * pitch, (has_short && b == nfull) ? g.last_len : g.S);
       }
       c->st_d2h += nfull * (32 + g.S) + (has_short ? 32 + g.last_len : 0);
       continue;
     }
     if (nfull > 0) {
-      MEC_CUDA_OK(cudaMemcpy2DAsync(dst, static_cast<size_t>(fstride), static_cast<uint8_t*>(s.dig.p) + (k + q) * 32,
+      MEC_CUDA_OK(cudaMemcpy2DAsync(dst, static_cast<size_t>(fstride), static_cast<uint8_t*>(s.dig.d.p) + (k + q) * 32,
                                     static_cast<size_t>((k + r) * 32), 32, static_cast<size_t>(nfull), cudaMemcpyDeviceToHost, s.st));
       MEC_CUDA_OK(cudaMemcpy2DAsync(dst + 32, static_cast<size_t>(fstride), static_cast<uint8_t*>(s.out.p) + q * pitch,
                                     static_cast<size_t>(r * pitch), static_cast<size_t>(g.S), static_cast<size_t>(nfull), cudaMemcpyDeviceToHost, s.st));
     }
     if (has_short) {
       const int64_t b = nfull;
-      MEC_CUDA_OK(cudaMemcpyAsync(dst + b * fstride, static_cast<uint8_t*>(s.dig.p) + (b * (k + r) + k + q) * 32, 32, cudaMemcpyDeviceToHost, s.st));
+      MEC_CUDA_OK(cudaMemcpyAsync(dst + b * fstride, static_cast<uint8_t*>(s.dig.d.p) + (b * (k + r) + k + q) * 32, 32, cudaMemcpyDeviceToHost, s.st));
       MEC_CUDA_OK(cudaMemcpyAsync(dst + b * fstride + 32, static_cast<uint8_t*>(s.out.p) + (b * r + q) * pitch, static_cast<size_t>(g.last_len),
                                   cudaMemcpyDeviceToHost, s.st));
     }
@@ -1206,7 +1164,6 @@ static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk,
   if ((rc = d.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
   if ((rc = d.out.ensure(static_cast<size_t>(enb * std::max(e->m, 1) * epitch)))) return rc;
   if ((rc = d.dig.ensure(static_cast<size_t>(enb * e->n * 32)))) return rc;
-  if ((rc = d.hdig.ensure(static_cast<size_t>(enb * e->n * 32)))) return rc;
   ResplitParams p;
   p.obj = static_cast<uint8_t*>(d.src.p);
   p.arena = static_cast<const uint8_t*>(s.aux.p); p.arena_stride = stride; p.P = g.dpitch();
@@ -1219,13 +1176,13 @@ static int emit_transcode(mec_codec* c, const FrameGeom& g, const RangeSink& sk,
   transcode_resplit_kernel<<<dim3(static_cast<unsigned>(ch.nb), static_cast<unsigned>(k)), 128, 0, s.st>>>(p);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
-  if ((rc = encode_device_locked(e, p.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.p), s.st))) return rc;
+  if ((rc = encode_device_locked(e, p.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.d.p), s.st))) return rc;
   EncChunk& ec = *out;
   ec = EncChunk{};
   ec.b0 = ch.b0 * (bs / ebs); ec.nb = enb; ec.nfull = bytes / ebs; ec.tail = bytes % ebs; ec.s = &d; ec.pitch = epitch; ec.st = s.st;
   ec.d_src = p.obj; ec.d_src_tail = p.obj + ec.nfull * ebs;
   ec.d_out = static_cast<uint8_t*>(d.out.p); ec.d_out_tail = ec.d_out + ec.nfull * e->m * epitch;
-  ec.h_dig = static_cast<const uint8_t*>(d.hdig.p); ec.h_dig_tail = ec.h_dig + ec.nfull * e->n * 32;
+  ec.h_dig = static_cast<const uint8_t*>(d.dig.h.p); ec.h_dig_tail = ec.h_dig + ec.nfull * e->n * 32;
   return frames_enqueue_chunk(e, ec, sk.enc_files, true, nullptr);
 }
 
@@ -1371,9 +1328,8 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
         }
     if ((e = s.aux.ensure(static_cast<size_t>(k * stride)))) return e;
     if ((e = s.out.ensure(static_cast<size_t>(ch.nb * std::max(ch.r, 1) * pitch)))) return e;
-    if ((e = s.dig.ensure(static_cast<size_t>(ch.nb * (k + ch.r) * 32)))) return e;
+    if ((e = s.dig.d.ensure(static_cast<size_t>(ch.nb * (k + ch.r) * 32)))) return e;
     if ((e = s.flags.ensure(static_cast<size_t>(ch.nb * k)))) return e;
-    if ((e = s.hflags.ensure(static_cast<size_t>(ch.nb * k)))) return e;
     FrameGeom sub = g;  // geometry of the chunk: its last block is short only if it is the range's last block
     sub.nblocks = ch.nb;
     sub.last_len = (b0 + ch.nb == g.nblocks) ? g.last_len : g.S;
@@ -1399,9 +1355,9 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
       MEC_CUDA_OK(cudaGetLastError());
       c->eng->count_launch();
     }
-    MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(ch.nb * k), s.st));
+    MEC_CUDA_OK(cudaMemsetAsync(s.flags.d.p, 0, static_cast<size_t>(ch.nb * k), s.st));
     if ((e = launch_reconstruct(c, g, ch, s, stride, ch.rows.data(), pitch, hash_outputs, whole ? raw : nullptr))) return e;
-    MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(ch.nb * k), cudaMemcpyDeviceToHost, s.st));
+    MEC_CUDA_OK(s.flags.download(static_cast<size_t>(ch.nb * k), s.st));
     if (sk.enc) { if ((e = emit_transcode(c, g, sk, ch, si, stride, pitch, &enc_inflight[si]))) return e; }
     else if (sk.dst) { if ((e = emit_object(c, g, sk, ch, s, stride, pitch, batched ? &list : nullptr))) return e; }
     else if (sk.out) { if ((e = emit_frames(c, g, sk, ch, s, pitch, batched ? &list : nullptr))) return e; }
@@ -1424,7 +1380,7 @@ static int reconstruct_range(mec_codec* c, const uint8_t* const* frames, const F
     busy[si] = false;
     tail = (tail + 1) % kSlots;
     nbusy--;
-    const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
+    const uint8_t* fl = static_cast<const uint8_t*>(s.flags.h.p);
     int64_t bad = ch.nb;
     for (int64_t b = 0; b < ch.nb && bad == ch.nb; b++)
       for (int t = 0; t < k; t++)
@@ -1786,12 +1742,11 @@ extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uin
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int chacha = c->dare_chacha20.load();
   const size_t tab = static_cast<size_t>(std::max<int64_t>(rows, 1)) * sizeof(DarePkg);
-  if ((rc = d.hpk.ensure(tab)) || (rc = d.pk.ensure(tab)) || (rc = d.st.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))) ||
-      (rc = d.hst.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))))
+  if ((rc = d.pk.ensure(tab)) || (rc = d.st.ensure(static_cast<size_t>(std::max<int64_t>(rows, 1)))))
     return rc;
   if ((rc = dare_keys(c, nstreams, keys, seal ? nonces : nullptr, st, chacha))) return rc;
   DareScrub scrub{c, nstreams, st};
-  DarePkg* t = static_cast<DarePkg*>(d.hpk.p);
+  DarePkg* t = static_cast<DarePkg*>(d.pk.h.p);
   int64_t w = 0;
   for (int64_t s = 0; s < nstreams; s++) {
     status[s] = 0;
@@ -1815,15 +1770,15 @@ extern "C" int mec_dare_device(mec_codec* c, int op, int64_t nstreams, const uin
     }
   }
   if (w > 0) {
-    MEC_CUDA_OK(cudaMemcpyAsync(d.pk.p, t, static_cast<size_t>(w) * sizeof(DarePkg), cudaMemcpyHostToDevice, st));
-    if ((rc = dare_launch(c, seal, seal ? chacha == 2 : chacha >= 1, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p), w, d_in, d_out,
-                          static_cast<uint8_t*>(d.st.p), st)))
+    MEC_CUDA_OK(d.pk.upload(static_cast<size_t>(w) * sizeof(DarePkg), st));
+    if ((rc = dare_launch(c, seal, seal ? chacha == 2 : chacha >= 1, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.d.p), w, d_in, d_out,
+                          static_cast<uint8_t*>(d.st.d.p), st)))
       return rc;
-    if (!seal) MEC_CUDA_OK(cudaMemcpyAsync(d.hst.p, d.st.p, static_cast<size_t>(w), cudaMemcpyDeviceToHost, st));
+    if (!seal) MEC_CUDA_OK(d.st.download(static_cast<size_t>(w), st));
   }
   MEC_CUDA_OK(cudaStreamSynchronize(st));
   if (!seal) {
-    const uint8_t* v = static_cast<const uint8_t*>(d.hst.p);
+    const uint8_t* v = static_cast<const uint8_t*>(d.st.h.p);
     for (int64_t r = 0; r < w; r++) {
       uint8_t& o = status[t[r].stream];
       if (v[r] == kDareUnsupported) o = static_cast<uint8_t>(-MEC_ERR_UNSUPPORTED);
@@ -1861,17 +1816,16 @@ static DareSpan dare_span(int64_t len, int64_t off, int64_t bytes) {
 static int dare_seal_chunk(mec_codec* c, Slot& s, const DareSpan& d, int64_t len, const uint8_t* pt, Staged* o, bool chacha) {
   const int64_t npk = ceil_frac(len, kPkg);
   int e;
-  if ((e = s.src.ensure(static_cast<size_t>(d.pad + d.np * kEPkg + 256))) || (e = s.hdpk.ensure(static_cast<size_t>(d.np) * sizeof(DarePkg))) ||
-      (e = s.dpk.ensure(static_cast<size_t>(d.np) * sizeof(DarePkg))))
+  if ((e = s.src.ensure(static_cast<size_t>(d.pad + d.np * kEPkg + 256))) || (e = s.dpk.ensure(static_cast<size_t>(d.np) * sizeof(DarePkg))))
     return e;
-  DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+  DarePkg* t = static_cast<DarePkg*>(s.dpk.h.p);
   for (int64_t j = 0; j < d.np; j++) {
     const int64_t p = d.p0 + j;
     t[j] = dare_row(j * kPkg, d.pad + j * kEPkg, 0, std::min(kPkg, len - p * kPkg), p, 0, p == npk - 1);
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, t, static_cast<size_t>(d.np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(s.dpk.upload(static_cast<size_t>(d.np) * sizeof(DarePkg), s.st));
   uint8_t* ct = static_cast<uint8_t*>(s.src.p);
-  if ((e = dare_launch(c, true, chacha, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.p), d.np, pt, ct, nullptr, s.st))) return e;
+  if ((e = dare_launch(c, true, chacha, dare_call_keys(c), static_cast<const DarePkg*>(s.dpk.d.p), d.np, pt, ct, nullptr, s.st))) return e;
   o->obj = ct + d.pad + d.delta;
   o->ck = pt + (d.ps - d.p0) * kPkg;
   o->ck_len = d.ps <= d.p1 ? d.pt1 - d.ps * kPkg : 0;
@@ -1950,19 +1904,19 @@ static int64_t decode_sse(mec_codec* c, const uint8_t* const* files, const uint8
   if (static_cast<int64_t>(k) * g.last_len < eend - rr.last_block * bs) return MEC_ERR_SHORT_DATA;  // as mec_decode_prefer
   DareState& d = c->dare;
   if ((rc = d.ct.ensure(static_cast<size_t>(round_up(elen, 16) + 256))) || (rc = d.pt.ensure(static_cast<size_t>(np * kPkg))) ||
-      (rc = d.st.ensure(static_cast<size_t>(np))) || (rc = d.hst.ensure(static_cast<size_t>(np))) ||
-      (rc = d.pk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))) || (rc = d.hpk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))))
+      (rc = d.st.ensure(static_cast<size_t>(np))) ||
+      (rc = d.pk.ensure(static_cast<size_t>(np) * sizeof(DarePkg))))
     return rc;
   Slot& s0 = c->slots[0];
   if ((rc = dare_keys(c, 1, key, nullptr, s0.st, chacha))) return rc;
   DareScrub scrub{c, 1, s0.st};
-  DarePkg* t = static_cast<DarePkg*>(d.hpk.p);
+  DarePkg* t = static_cast<DarePkg*>(d.pk.h.p);
   for (int64_t j = 0; j < np; j++) {
     const int64_t p = p_first + j;
     t[j] = dare_row(j * kEPkg, j * kPkg, 0, p == npk - 1 ? D - p * kPkg : kPkg, p, 0, p == npk - 1);
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(d.pk.p, t, static_cast<size_t>(np) * sizeof(DarePkg), cudaMemcpyHostToDevice, s0.st));
-  MEC_CUDA_OK(cudaMemsetAsync(d.st.p, 0, static_cast<size_t>(np), s0.st));
+  MEC_CUDA_OK(d.pk.upload(static_cast<size_t>(np) * sizeof(DarePkg), s0.st));
+  MEC_CUDA_OK(cudaMemsetAsync(d.st.d.p, 0, static_cast<size_t>(np), s0.st));
   MEC_CUDA_OK(cudaStreamSynchronize(s0.st));
   uint8_t* ct = static_cast<uint8_t*>(d.ct.p);
   const uint8_t* pt = static_cast<const uint8_t*>(d.pt.p);
@@ -1975,8 +1929,8 @@ static int64_t decode_sse(mec_codec* c, const uint8_t* const* files, const uint8
     if (upto <= opened) return MEC_OK;
     Slot& s = c->slots[si];
     int e;
-    if ((e = dare_launch(c, false, chacha >= 1, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.p) + opened, upto - opened, ct,
-                         static_cast<uint8_t*>(d.pt.p), static_cast<uint8_t*>(d.st.p) + opened, s.st)))
+    if ((e = dare_launch(c, false, chacha >= 1, dare_call_keys(c), static_cast<const DarePkg*>(d.pk.d.p) + opened, upto - opened, ct,
+                         static_cast<uint8_t*>(d.pt.p), static_cast<uint8_t*>(d.st.d.p) + opened, s.st)))
       return e;
     const int64_t a = std::max(offset, (p_first + opened) * kPkg), z = std::min(offset + length, (p_first + upto) * kPkg);
     if (z > a) {
@@ -1994,8 +1948,8 @@ static int64_t decode_sse(mec_codec* c, const uint8_t* const* files, const uint8
   rc = reconstruct_range(c, in.data(), g, want.data(), 1, sk, corrupt.data(), alive.data(), prefer, false);
   if (rc) return rc;  // every slot stream has drained
   if (opened != np) return MEC_ERR_UNEXPECTED;
-  MEC_CUDA_OK(cudaMemcpy(d.hst.p, d.st.p, static_cast<size_t>(np), cudaMemcpyDeviceToHost));
-  const uint8_t* v = static_cast<const uint8_t*>(d.hst.p);
+  MEC_CUDA_OK(cudaMemcpy(d.st.h.p, d.st.d.p, static_cast<size_t>(np), cudaMemcpyDeviceToHost));
+  const uint8_t* v = static_cast<const uint8_t*>(d.st.h.p);
   int bad = MEC_OK;
   for (int64_t j = 0; j < np; j++) {
     if (v[j] == kDareUnsupported) bad = MEC_ERR_UNSUPPORTED;
@@ -2032,7 +1986,7 @@ static bool lower_hex64(const uint8_t* s) {
 static bool sig_call_host(mec_codec* c, const uint8_t* key, const char* date, const char* scope) {
   const size_t dl = strlen(date), sl = strlen(scope);
   if (dl + sl + 2 > static_cast<size_t>(kSigMaxHead)) return false;
-  SigCall* k = static_cast<SigCall*>(c->sig.hcall.p);
+  SigCall* k = static_cast<SigCall*>(c->sig.call.h.p);
   memset(k, 0, sizeof(SigCall));
   sig_key_states(key, k);
   memcpy(k->head, date, dl);
@@ -2050,15 +2004,15 @@ struct SigScrub {
   ~SigScrub() {
     for (auto& s : c->slots)
       if (s.st2) cudaStreamSynchronize(s.st2);
-    cudaMemsetAsync(c->sig.call.p, 0, sizeof(SigCall), st);
+    cudaMemsetAsync(c->sig.call.d.p, 0, sizeof(SigCall), st);
     cudaStreamSynchronize(st);
-    explicit_bzero(c->sig.hcall.p, sizeof(SigCall));
+    explicit_bzero(c->sig.call.h.p, sizeof(SigCall));
   }
 };
 
 // Uploads the call's SigCall on `st` and waits for it: every slot stream reads it
 static int sig_call_upload(mec_codec* c, cudaStream_t st) {
-  MEC_CUDA_OK(cudaMemcpyAsync(c->sig.call.p, c->sig.hcall.p, sizeof(SigCall), cudaMemcpyHostToDevice, st));
+  MEC_CUDA_OK(c->sig.call.upload(sizeof(SigCall), st));
   MEC_CUDA_OK(cudaStreamSynchronize(st));
   return MEC_OK;
 }
@@ -2069,7 +2023,7 @@ static int sig_launch(mec_codec* c, SigRow* h, SigRow* d, int64_t n, cudaStream_
   std::sort(h, h + n, [](const SigRow& x, const SigRow& y) { return x.len > y.len; });
   MEC_CUDA_OK(cudaMemcpyAsync(d, h, static_cast<size_t>(n) * sizeof(SigRow), cudaMemcpyHostToDevice, st));
   SigParams p;
-  p.rows = d; p.nrows = n; p.call = static_cast<const SigCall*>(c->sig.call.p);
+  p.rows = d; p.nrows = n; p.call = static_cast<const SigCall*>(c->sig.call.d.p);
   p.verdict = reinterpret_cast<uint8_t*>(d + n);
   sigv4_chunk_kernel<<<static_cast<unsigned>(ceil_frac(n, kSigThreads)), kSigThreads, 0, st>>>(p);
   MEC_CUDA_OK(cudaGetLastError());
@@ -2087,7 +2041,7 @@ static inline SigRow sig_row(const uint8_t* msg, int64_t len, int64_t out, int32
 
 static int sig_ensure(mec_codec* c) {
   int rc;
-  if ((rc = c->sig.call.ensure(sizeof(SigCall))) || (rc = c->sig.hcall.ensure(sizeof(SigCall)))) return rc;
+  if ((rc = c->sig.call.ensure(sizeof(SigCall)))) return rc;
   return MEC_OK;
 }
 
@@ -2109,14 +2063,14 @@ extern "C" int mec_chunk_signatures_device(mec_codec* c, const uint8_t* key, con
   MEC_CUDA_OK(cudaSetDevice(c->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t tab = static_cast<size_t>(count) * (sizeof(SigRow) + 1);
-  if ((rc = sig_ensure(c)) || (rc = c->sig.rows.ensure(tab)) || (rc = c->sig.hrows.ensure(tab))) return rc;
+  if ((rc = sig_ensure(c)) || (rc = c->sig.rows.ensure(tab))) return rc;
   sig_call_host(c, key, date, scope);
   SigScrub scrub{c, st};
   if ((rc = sig_call_upload(c, st))) return rc;
-  SigRow* h = static_cast<SigRow*>(c->sig.hrows.p);
+  SigRow* h = static_cast<SigRow*>(c->sig.rows.h.p);
   for (int64_t i = 0; i < count; i++)
     h[i] = sig_row(d_base + offsets[i], lens[i], i, kinds[i], prev + 64 * i, claimed + 64 * i);
-  SigRow* d = static_cast<SigRow*>(c->sig.rows.p);
+  SigRow* d = static_cast<SigRow*>(c->sig.rows.d.p);
   if ((rc = sig_launch(c, h, d, count, st))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(h + count, d + count, static_cast<size_t>(count), cudaMemcpyDeviceToHost, st));
   MEC_CUDA_OK(cudaStreamSynchronize(st));
@@ -2232,10 +2186,9 @@ static int parse_chunked(const uint8_t* b, int64_t blen, int64_t D, const uint8_
 // Per-slot second stream and events of the chunked encode's verify launches, created on first use
 static int sig_streams(mec_codec* c) {
   for (auto& s : c->slots) {
-    if (s.st2) continue;
-    MEC_CUDA_OK(cudaStreamCreateWithFlags(&s.st2, cudaStreamNonBlocking));
-    MEC_CUDA_OK(cudaEventCreateWithFlags(&s.ev_staged, cudaEventDisableTiming));
-    MEC_CUDA_OK(cudaEventCreateWithFlags(&s.ev_verified, cudaEventDisableTiming));
+    MEC_CUDA_OK(s.st2.create(cudaStreamNonBlocking));
+    MEC_CUDA_OK(s.ev_staged.create(cudaEventDisableTiming));
+    MEC_CUDA_OK(s.ev_verified.create(cudaEventDisableTiming));
   }
   return MEC_OK;
 }
@@ -2266,7 +2219,7 @@ static AwsSpan aws_span(const ChunkedBody& P, int64_t lo, int64_t own0, int64_t 
 // 16-byte aligned and the buffer reaches at least decoded byte `hi`; the trailer message follows when the step has the trailer
 // row.  *base: decoded byte x is at *base + x.  The step's rows are then verified by ONE launch on the slot's second stream, behind
 // the staging, so that the work queued on s.st next does not wait for the hash.  *r0 / *nrow: the first row and the number of rows
-// of the step, whose verdicts land behind its rows in s.hsig_tab once s.st2 has drained.
+// of the step, whose verdicts land behind its rows in s.sig_tab.h once s.st2 has drained.
 static int aws_stage(mec_codec* c, Slot& s, DevBuf& buf, const uint8_t* body, const ChunkedBody& P, const AwsSpan& sp, int64_t lo,
                      int64_t hi, uint8_t** base, int64_t* r0, int64_t* nrow) {
   const std::vector<AwsChunk>& ch = P.ch;
@@ -2294,15 +2247,15 @@ static int aws_stage(mec_codec* c, Slot& s, DevBuf& buf, const uint8_t* body, co
   *nrow = h1 - h0 + (sp.trow ? 1 : 0);
   if (*nrow == 0) return MEC_OK;
   const size_t tab = static_cast<size_t>(*nrow) * (sizeof(SigRow) + 1);
-  if ((rc = s.sig_tab.ensure(tab)) || (rc = s.hsig_tab.ensure(tab))) return rc;
-  SigRow* h = static_cast<SigRow*>(s.hsig_tab.p);
+  if ((rc = s.sig_tab.ensure(tab))) return rc;
+  SigRow* h = static_cast<SigRow*>(s.sig_tab.h.p);
   for (int64_t j = h0; j < h1; j++) h[j - h0] = sig_row(b + ch[j].doff, ch[j].size, j - h0, kSigPayload, ch[j].prev, ch[j].claim);
   if (sp.trow)
     h[h1 - h0] = sig_row(static_cast<uint8_t*>(buf.p) + tpos, static_cast<int64_t>(P.tmsg.size()), h1 - h0, kSigTrailer,
                          ch.back().claim, P.tclaim);
   MEC_CUDA_OK(cudaEventRecord(s.ev_staged, s.st));
   MEC_CUDA_OK(cudaStreamWaitEvent(s.st2, s.ev_staged, 0));
-  SigRow* d = static_cast<SigRow*>(s.sig_tab.p);
+  SigRow* d = static_cast<SigRow*>(s.sig_tab.d.p);
   if ((rc = sig_launch(c, h, d, *nrow, s.st2))) return rc;
   MEC_CUDA_OK(cudaMemcpyAsync(h + *nrow, d + *nrow, static_cast<size_t>(*nrow), cudaMemcpyDeviceToHost, s.st2));
   MEC_CUDA_OK(cudaEventRecord(s.ev_verified, s.st2));
@@ -2366,7 +2319,7 @@ static int64_t encode_chunked(mec_codec* c, const uint8_t* body, int64_t body_le
   std::vector<uint8_t> verdict(static_cast<size_t>(nrows), 0);
   int64_t r0[kSlots] = {}, nr[kSlots] = {};
   auto collect = [&](int si) {
-    const uint8_t* v = reinterpret_cast<const uint8_t*>(static_cast<const SigRow*>(c->slots[si].hsig_tab.p) + nr[si]);
+    const uint8_t* v = reinterpret_cast<const uint8_t*>(static_cast<const SigRow*>(c->slots[si].sig_tab.h.p) + nr[si]);
     memcpy(verdict.data() + r0[si], v, static_cast<size_t>(nr[si]));
   };
   const int64_t D = decoded_len;
@@ -2493,15 +2446,14 @@ extern "C" int mec_heal_batch(mec_codec* const* pool, int npool, int64_t nobject
 // lens[j] shard bytes; (arena_frames - j) * P + 512 readable bytes from frame j on), enqueued on the slot's stream.  `lens` is
 // page-locked host memory.  one_launch (the codec's options allow the latency kernel at this size): every frame, full or short,
 // hashes in ONE launch with a per-frame length table.  Otherwise one launch over each run of full frames and one per short frame
-// (a short frame's digest covers fewer bytes).  Verdicts come back to s.hflags[0, nframes).  Shared by bitrotVerify on a codec
+// (a short frame's digest covers fewer bytes).  Verdicts come back to s.flags.h[0, nframes).  Shared by bitrotVerify on a codec
 // (verify_files_locked) and merged verify batches (batcher_submit_verify).
 static int verify_frames(mec_codec* c, Slot& s, const uint8_t* base, int64_t arena_frames, int64_t nframes, const int32_t* lens, bool one_launch) {
   const int64_t S = c->S(), P = round_up(32 + S, 16);
   int rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(nframes * 32)))) return rc;
+  if ((rc = s.dig.d.ensure(static_cast<size_t>(nframes * 32)))) return rc;
   if ((rc = s.flags.ensure(static_cast<size_t>(nframes)))) return rc;
-  if ((rc = s.hflags.ensure(static_cast<size_t>(nframes)))) return rc;
-  MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nframes), s.st));
+  MEC_CUDA_OK(cudaMemsetAsync(s.flags.d.p, 0, static_cast<size_t>(nframes), s.st));
   const int32_t* block_len = nullptr;
   auto launch = [&](int64_t slot0, int64_t cnt, int64_t len) -> int {
     FusedDesc d;
@@ -2512,14 +2464,14 @@ static int verify_frames(mec_codec* c, Slot& s, const uint8_t* base, int64_t are
     d.nblocks = cnt; d.S = static_cast<int32_t>(len);
     d.map_base[0] = at; d.map_len[0] = (arena_frames - slot0) * P + 512;
     d.expect_ptr[0] = at; d.in_ptr[0] = at + 32;
-    d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * 32;
-    d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0;
+    d.digests = static_cast<uint8_t*>(s.dig.d.p) + slot0 * 32;
+    d.corrupt = static_cast<uint8_t*>(s.flags.d.p) + slot0;
     return c->eng->launch_fused(d, c->opt, s.st);
   };
   if (one_launch) {
-    if ((rc = s.dreq.ensure(static_cast<size_t>(nframes) * sizeof(int32_t)))) return rc;
-    MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, lens, static_cast<size_t>(nframes) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
-    block_len = static_cast<const int32_t*>(s.dreq.p);
+    if ((rc = s.dreq.d.ensure(static_cast<size_t>(nframes) * sizeof(int32_t)))) return rc;
+    MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.d.p, lens, static_cast<size_t>(nframes) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
+    block_len = static_cast<const int32_t*>(s.dreq.d.p);
     if ((rc = launch(0, nframes, S))) return rc;
   } else {
     // runs of full frames between the short ones
@@ -2531,7 +2483,7 @@ static int verify_frames(mec_codec* c, Slot& s, const uint8_t* base, int64_t are
       at = j + 1;
     }
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nframes), cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(s.flags.download(static_cast<size_t>(nframes), s.st));
   c->st_blocks_read += nframes;
   return MEC_OK;
 }
@@ -2553,7 +2505,7 @@ static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* cons
   const int64_t chunk = std::max<int64_t>(1, (32ll << 20) / fstride);  // frames per chunk (~32 MiB)
   int rc;
   SlotRing ring(c, [&](int si) {
-    const uint8_t* fl = static_cast<const uint8_t*>(c->slots[si].hflags.p);
+    const uint8_t* fl = static_cast<const uint8_t*>(c->slots[si].flags.h.p);
     int64_t o = 0;
     for (const Piece& pc : inflight[si]) {
       for (int64_t b = 0; b < pc.nb; b++)
@@ -2568,14 +2520,14 @@ static int verify_files_locked(mec_codec* c, int64_t nfiles, const uint8_t* cons
     const int si = ring.si;
     Slot& s = c->slots[si];
     if ((rc = s.src.ensure(static_cast<size_t>(chunk * P + 512)))) return rc;
-    if ((rc = s.hreq.ensure(static_cast<size_t>(chunk) * sizeof(int32_t)))) return rc;
+    if ((rc = s.dreq.h.ensure(static_cast<size_t>(chunk) * sizeof(int32_t)))) return rc;
     int64_t used = 0;
     // fill the chunk with frames of consecutive files.  When the chunk is a launch the latency kernel takes (it is, unless options
     // say otherwise: ~380 frames of a 1 MiB-block part file), short runs of frames are staged by ONE batched copy call: a scan over
     // thousands of small part files costs two driver calls per 32 MiB, not two per file.
     const bool one_launch = c->eng->small_ok(c->opt, chunk);
     CopyList list;
-    int32_t* lens = static_cast<int32_t*>(s.hreq.p);
+    int32_t* lens = static_cast<int32_t*>(s.dreq.h.p);
     while (f < nfiles && used < chunk) {
       if (results[f] != MEC_OK || part_lens[f] == 0 || (algos && algos[f] != MEC_HIGHWAYHASH256S)) { f++; b0 = 0; continue; }
       const int64_t nblocks = ceil_frac(part_lens[f], S), last_len = part_lens[f] - (nblocks - 1) * S;
@@ -2631,9 +2583,9 @@ static int verify_whole_locked(mec_codec* c, int64_t nparts, const int* algos, c
     if (nfiles == 0) break;
     // the file arena as batch_whole_stage lays it out: each file 16-byte aligned with 256 readable bytes behind it
     const size_t tab_bytes = static_cast<size_t>(nfiles) * sizeof(WholeStream);
-    if ((rc = s.hwtab.ensure(tab_bytes)) || (rc = s.wtab.ensure(tab_bytes))) return rc;
-    if ((rc = s.wdig.ensure(static_cast<size_t>(nfiles) * 64)) || (rc = s.hwdig.ensure(static_cast<size_t>(nfiles) * 64))) return rc;
-    WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+    if ((rc = s.wtab.ensure(tab_bytes))) return rc;
+    if ((rc = s.wdig.ensure(static_cast<size_t>(nfiles) * 64))) return rc;
+    WholeStream* ws = static_cast<WholeStream*>(s.wtab.h.p);
     int64_t arena = 0, j = 0, counts[kWholeGroups];
     for (int g = 0; g < kWholeGroups; g++) {
       counts[g] = static_cast<int64_t>(group[g].size());
@@ -2644,20 +2596,20 @@ static int verify_whole_locked(mec_codec* c, int64_t nparts, const int* algos, c
     }
     if ((rc = s.src.ensure(static_cast<size_t>(arena)))) return rc;
     uint8_t* d = static_cast<uint8_t*>(s.src.p);
-    MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, tab_bytes, cudaMemcpyHostToDevice, s.st));
+    MEC_CUDA_OK(s.wtab.upload(tab_bytes, s.st));
     CopyList list;
     j = 0;
     for (int g = 0; g < kWholeGroups; g++)
       for (int64_t q : group[g]) list.add(d + ws[j++].off, files[q], file_lens[q]);
     if ((rc = list.flush(s.st))) return rc;
-    if ((rc = whole_hash_groups(c, kWholeGroups, kWholeAlgos, counts, d, 0, 0, static_cast<uint8_t*>(s.wdig.p), s.st,
-                                static_cast<const WholeStream*>(s.wtab.p))))
+    if ((rc = whole_hash_groups(c, kWholeGroups, kWholeAlgos, counts, d, 0, 0, static_cast<uint8_t*>(s.wdig.d.p), s.st,
+                                static_cast<const WholeStream*>(s.wtab.d.p))))
       return rc;
     c->eng->count_launch();
-    MEC_CUDA_OK(cudaMemcpyAsync(s.hwdig.p, s.wdig.p, static_cast<size_t>(nfiles) * 64, cudaMemcpyDeviceToHost, s.st));
+    MEC_CUDA_OK(s.wdig.download(static_cast<size_t>(nfiles) * 64, s.st));
     MEC_CUDA_OK(cudaStreamSynchronize(s.st));
     c->st_h2d += bytes;
-    const uint8_t* got = static_cast<const uint8_t*>(s.hwdig.p);
+    const uint8_t* got = static_cast<const uint8_t*>(s.wdig.h.p);
     j = 0;
     for (int g = 0; g < kWholeGroups; g++)
       for (int64_t q : group[g])
@@ -2800,13 +2752,13 @@ extern "C" int mec_whole_hash(mec_codec* c, int algo, const uint8_t* msgs, int64
   Slot& s = c->slots[0];
   const int64_t pitch = round_up(msg_len, 16) + 128;  // the kernel reads whole 16-byte vectors
   if ((rc = s.src.ensure(static_cast<size_t>(count * pitch + 256)))) return rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(count * 64)))) return rc;
+  if ((rc = s.dig.d.ensure(static_cast<size_t>(count * 64)))) return rc;
   if (msg_len > 0)
     MEC_CUDA_OK(cudaMemcpy2DAsync(s.src.p, static_cast<size_t>(pitch), msgs, static_cast<size_t>(msg_len), static_cast<size_t>(msg_len),
                                   static_cast<size_t>(count), cudaMemcpyHostToDevice, s.st));
-  if ((rc = whole_hash_device(c, algo, static_cast<const uint8_t*>(s.src.p), pitch, msg_len, count, static_cast<uint8_t*>(s.dig.p), s.st))) return rc;
+  if ((rc = whole_hash_device(c, algo, static_cast<const uint8_t*>(s.src.p), pitch, msg_len, count, static_cast<uint8_t*>(s.dig.d.p), s.st))) return rc;
   const int ds = mec_digest_size(algo);
-  MEC_CUDA_OK(cudaMemcpy2DAsync(digests, static_cast<size_t>(ds), s.dig.p, 64, static_cast<size_t>(ds), static_cast<size_t>(count),
+  MEC_CUDA_OK(cudaMemcpy2DAsync(digests, static_cast<size_t>(ds), s.dig.d.p, 64, static_cast<size_t>(ds), static_cast<size_t>(count),
                                 cudaMemcpyDeviceToHost, s.st));
   MEC_CUDA_OK(cudaStreamSynchronize(s.st));
   c->eng->count_launch();
@@ -2858,7 +2810,7 @@ extern "C" int64_t mec_encode_whole(mec_codec* c, const uint8_t* src, int64_t le
   if ((rc = s.src.ensure(static_cast<size_t>(round_up(len, 16) + 256)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(std::max<int64_t>(nall, 1) * std::max(m, 1) * pitch)))) return rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(n * fpitch + 256)))) return rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(n * 64)))) return rc;
+  if ((rc = s.dig.d.ensure(static_cast<size_t>(n * 64)))) return rc;
   if (len > 0) {
     MEC_CUDA_OK(cudaMemcpyAsync(s.src.p, src, static_cast<size_t>(len), cudaMemcpyHostToDevice, s.st));
     if (m > 0) {  // parity only: the hash is not per block for these algorithms
@@ -2886,12 +2838,12 @@ extern "C" int64_t mec_encode_whole(mec_codec* c, const uint8_t* src, int64_t le
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
   }
-  if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p), fpitch, flen, n, static_cast<uint8_t*>(s.dig.p), s.st))) return rc;
+  if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.aux.p), fpitch, flen, n, static_cast<uint8_t*>(s.dig.d.p), s.st))) return rc;
   c->eng->count_launch();
   for (int i = 0; i < n; i++)
     if (files[i] && flen > 0)
       MEC_CUDA_OK(cudaMemcpyAsync(files[i], static_cast<uint8_t*>(s.aux.p) + i * fpitch, static_cast<size_t>(flen), cudaMemcpyDeviceToHost, s.st));
-  if (sums) MEC_CUDA_OK(cudaMemcpyAsync(sums, s.dig.p, static_cast<size_t>(n * 64), cudaMemcpyDeviceToHost, s.st));
+  if (sums) MEC_CUDA_OK(cudaMemcpyAsync(sums, s.dig.d.p, static_cast<size_t>(n * 64), cudaMemcpyDeviceToHost, s.st));
   MEC_CUDA_OK(cudaStreamSynchronize(s.st));
   return len;
 }
@@ -2919,9 +2871,8 @@ static int stage_verified_whole(mec_codec* c, const uint8_t* const* files, const
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * fpitch + 256)))) return rc;
   if ((rc = s.dig.ensure(static_cast<size_t>(k * 64)))) return rc;
-  if ((rc = s.hdig.ensure(static_cast<size_t>(k * 64)))) return rc;
-  WholeSet w{files, sums, nullptr, c->algo, sfs, fpitch, static_cast<uint8_t*>(s.aux.p), static_cast<uint8_t*>(s.dig.p),
-             static_cast<uint8_t*>(s.hdig.p), {}};
+  WholeSet w{files, sums, nullptr, c->algo, sfs, fpitch, static_cast<uint8_t*>(s.aux.p), static_cast<uint8_t*>(s.dig.d.p),
+             static_cast<uint8_t*>(s.dig.h.p), {}};
   for (int i = 0; i < n; i++) w.slot_of[i] = -1;
   for (bool dropped = true; dropped;) {
     int want[kMaxShards];
@@ -3057,7 +3008,6 @@ extern "C" int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const u
     // rebuilt rows -> contiguous shard files on the device (for the whole-file hash), then files and sums go home
     if ((rc = s.src.ensure(static_cast<size_t>(r * fpitch + 256)))) return rc;
     if ((rc = s.dig.ensure(static_cast<size_t>((k + r) * 64)))) return rc;
-    if ((rc = s.hdig.ensure(static_cast<size_t>((k + r) * 64)))) return rc;
     for (int q = 0; q < r; q++) {
       uint8_t* f = static_cast<uint8_t*>(s.src.p) + q * fpitch;
       const int64_t nfull = last_len == S ? nblocks : nblocks - 1;
@@ -3069,12 +3019,12 @@ extern "C" int mec_heal_whole(mec_codec* c, const uint8_t* const* files, const u
                                     cudaMemcpyDeviceToDevice, s.st));
       MEC_CUDA_OK(cudaMemsetAsync(f + sfs, 0, 256, s.st));
     }
-    if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.src.p), fpitch, sfs, r, static_cast<uint8_t*>(s.dig.p) + k * 64, s.st))) return rc;
+    if ((rc = whole_hash_device(c, c->algo, static_cast<const uint8_t*>(s.src.p), fpitch, sfs, r, static_cast<uint8_t*>(s.dig.d.p) + k * 64, s.st))) return rc;
     c->eng->count_launch();
     for (int q = 0; q < r; q++) {
       MEC_CUDA_OK(cudaMemcpyAsync(out_files[targets[q]], static_cast<uint8_t*>(s.src.p) + q * fpitch, static_cast<size_t>(sfs), cudaMemcpyDeviceToHost, s.st));
       if (out_sums)
-        MEC_CUDA_OK(cudaMemcpyAsync(out_sums + static_cast<size_t>(targets[q]) * 64, static_cast<uint8_t*>(s.dig.p) + (k + q) * 64, 64, cudaMemcpyDeviceToHost, s.st));
+        MEC_CUDA_OK(cudaMemcpyAsync(out_sums + static_cast<size_t>(targets[q]) * 64, static_cast<uint8_t*>(s.dig.d.p) + (k + q) * 64, 64, cudaMemcpyDeviceToHost, s.st));
       c->st_d2h += sfs;
     }
   }
@@ -3164,21 +3114,20 @@ extern "C" int64_t mec_transcode_whole(mec_codec* src, const uint8_t* const* fil
     if ((rc = d.src.ensure(static_cast<size_t>(round_up(bytes, 16) + 256)))) return rc;
     if ((rc = d.out.ensure(static_cast<size_t>(enb * std::max(dst->m, 1) * epitch)))) return rc;
     if ((rc = d.dig.ensure(static_cast<size_t>(enb * dst->n * 32)))) return rc;
-    if ((rc = d.hdig.ensure(static_cast<size_t>(enb * dst->n * 32)))) return rc;
     rp.obj = static_cast<uint8_t*>(d.src.p);
     rp.rebuilt = static_cast<const uint8_t*>(s.out.p);
     rp.b0 = b0;
     whole_resplit_kernel<<<dim3(static_cast<unsigned>(nb), static_cast<unsigned>(k)), 128, 0, s.st>>>(rp);
     MEC_CUDA_OK(cudaGetLastError());
     src->eng->count_launch();
-    if ((rc = encode_device_locked(dst, rp.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.p), s.st)))
+    if ((rc = encode_device_locked(dst, rp.obj, bytes, static_cast<uint8_t*>(d.out.p), epitch, static_cast<uint8_t*>(d.dig.d.p), s.st)))
       return rc;
     EncChunk& ec = inflight[si];
     ec = EncChunk{};
     ec.b0 = b0 * (bs / ebs); ec.nb = enb; ec.nfull = bytes / ebs; ec.tail = bytes % ebs; ec.s = &d; ec.pitch = epitch; ec.st = s.st;
     ec.d_src = rp.obj; ec.d_src_tail = rp.obj + ec.nfull * ebs;
     ec.d_out = static_cast<uint8_t*>(d.out.p); ec.d_out_tail = ec.d_out + ec.nfull * dst->m * epitch;
-    ec.h_dig = static_cast<const uint8_t*>(d.hdig.p); ec.h_dig_tail = ec.h_dig + ec.nfull * dst->n * 32;
+    ec.h_dig = static_cast<const uint8_t*>(d.dig.h.p); ec.h_dig_tail = ec.h_dig + ec.nfull * dst->n * 32;
     if ((rc = frames_enqueue_chunk(dst, ec, out_files, true, nullptr))) return rc;
     ring.submitted();
   }
@@ -3232,11 +3181,10 @@ static int mixed_range(mec_codec* c, const int* algos, const uint8_t* const* fil
   int rc;
   if ((rc = c->whole.ensure(static_cast<size_t>(k * fpitch + 256)))) return rc;
   if ((rc = c->whole_dig.ensure(static_cast<size_t>(k * 64)))) return rc;
-  if ((rc = c->hwhole_dig.ensure(static_cast<size_t>(k * 64)))) return rc;
   uint8_t whole[kMaxShards] = {};
   for (int i = 0; i < n; i++) whole[i] = alive[i] && algos[i] != MEC_HIGHWAYHASH256S;
-  WholeSet w{files, sums, whole, walgo, sfs, fpitch, static_cast<uint8_t*>(c->whole.p), static_cast<uint8_t*>(c->whole_dig.p),
-             static_cast<uint8_t*>(c->hwhole_dig.p), {}};
+  WholeSet w{files, sums, whole, walgo, sfs, fpitch, static_cast<uint8_t*>(c->whole.p), static_cast<uint8_t*>(c->whole_dig.d.p),
+             static_cast<uint8_t*>(c->whole_dig.h.p), {}};
   for (int i = 0; i < n; i++) w.slot_of[i] = -1;
   return reconstruct_range(c, frames, g, want, data_only, sk, corrupt, alive, prefer, hash_outputs, &w);
 }
@@ -3387,7 +3335,7 @@ extern "C" int mec_hh256_batch(mec_codec* c, const uint8_t* msgs, int64_t msg_le
   if ((rc = ensure_engine(c))) return rc;
   MEC_CUDA_OK(cudaSetDevice(c->device));
   Slot& s = c->slots[0];
-  if ((rc = s.dig.ensure(static_cast<size_t>(count * 32)))) return rc;
+  if ((rc = s.dig.d.ensure(static_cast<size_t>(count * 32)))) return rc;
   const int64_t mp = std::max<int64_t>(round_up(msg_len, 16), 16);
   if ((rc = s.src.ensure(static_cast<size_t>(count * mp + 512)))) return rc;
   if (msg_len > 0)
@@ -3400,9 +3348,9 @@ extern "C" int mec_hh256_batch(mec_codec* c, const uint8_t* msgs, int64_t msg_le
   d.in_ptr[0] = static_cast<const uint8_t*>(s.src.p);
   d.map_base[0] = d.in_ptr[0];
   d.map_len[0] = count * mp + 256;
-  d.digests = static_cast<uint8_t*>(s.dig.p);
+  d.digests = static_cast<uint8_t*>(s.dig.d.p);
   if ((rc = c->eng->launch_fused(d, c->opt, s.st))) return rc;
-  MEC_CUDA_OK(cudaMemcpyAsync(digests, s.dig.p, static_cast<size_t>(count * 32), cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(cudaMemcpyAsync(digests, s.dig.d.p, static_cast<size_t>(count * 32), cudaMemcpyDeviceToHost, s.st));
   MEC_CUDA_OK(cudaStreamSynchronize(s.st));
   return MEC_OK;
 }
@@ -3640,8 +3588,8 @@ struct mec_batcher {
   std::atomic<int64_t> st_sum_requests{0};  // PUTs that got at least one object hash (mec_batcher_encode_sums)
   // object hashes of a PUT batch run on a second stream per slot, forked once the batch is staged (ev_staged) and joined before the
   // slot's stream ends (ev_summed), so the batch's encode is not queued behind them
-  cudaStream_t sum_st[kSlots] = {};
-  cudaEvent_t ev_staged[kSlots] = {}, ev_summed[kSlots] = {};
+  Stream sum_st[kSlots];
+  Event ev_staged[kSlots], ev_summed[kSlots];
   // MEC_BATCHER_MIX_PATTERNS (and a codec whose options allow the latency kernel): GETs merge with GETs and heals with heals
   // whatever their reader and stale sets, as long as a batch of several erasure patterns fits one latency launch
   bool mix = false;
@@ -3650,10 +3598,10 @@ struct mec_batcher {
   std::unordered_map<uint64_t, BatchPattern> patterns;
   BatcherSwitches sw;
   // hybrid staging (sw.gather_pct): part of a batch is read by the gather kernel on `aux` while the copy engine moves the rest
-  cudaStream_t aux = nullptr;
-  cudaEvent_t ev_table[kSlots] = {}, ev_gather[kSlots] = {};
+  Stream aux;
+  Event ev_table[kSlots], ev_gather[kSlots];
   // where the worker's time and each batch's stream time go (mec_batcher_stat "us_*"); device phases need sw.trace
-  cudaEvent_t ev_ph[kSlots][4] = {};
+  Event ev_ph[kSlots][4];
   std::atomic<int64_t> us_submit{0}, us_sync{0}, us_finish{0}, us_idle{0}, us_stage{0}, us_kernel{0}, us_scatter{0};
   // mec_batcher_new_transcode: the destination codec of merged moves (private; its slot i carries the destination side of the batch
   // on source slot i), and the destination half of the private pair for moves that cannot ride in a batch (with `serial`)
@@ -3672,6 +3620,11 @@ struct mec_batcher {
   // mec_batcher_encode_sse / _decode_sse: calls completed by merged batches, and calls of the private path (redos included)
   std::atomic<int64_t> st_sse_puts{0}, st_sse_gets{0}, st_sse_serial{0};
   std::atomic<int> dare_chacha20{0};  // mec_batcher_set_option: recorded by every encrypted request as it is admitted
+  // the batcher owns its codecs; each drains its slots before it is freed.  The worker has been joined (mec_batcher_free) or
+  // never started (batcher_create's failures).
+  ~mec_batcher() {
+    for (mec_codec* h : {serial, serial_dst, serial_whole[0], serial_whole[1], serial_whole[2], dst, codec}) mec_codec_free(h);
+  }
 };
 
 namespace {
@@ -3747,9 +3700,9 @@ static void verify_whole_firsts(const std::vector<BatchReq*>& reqs, int64_t (&fi
 static void batcher_finish(mec_batcher* b, InflightBatch& fb, Slot& s, int rc) {
   mec_codec* c = b->codec;
   if (fb.kind == ReqKind::Verify) {
-    // the frame verdicts in s.hflags and the whole-file digests in s.hwdig, both in batcher_submit_verify's order
-    const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
-    const uint8_t* wd = static_cast<const uint8_t*>(s.hwdig.p);
+    // the frame verdicts in s.flags.h and the whole-file digests in s.wdig.h, both in batcher_submit_verify's order
+    const uint8_t* fl = static_cast<const uint8_t*>(s.flags.h.p);
+    const uint8_t* wd = static_cast<const uint8_t*>(s.wdig.h.p);
     const int64_t S = c->S();
     int64_t frame = 0, next[kWholeGroups];
     verify_whole_firsts(fb.reqs, next);
@@ -3774,10 +3727,10 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, Slot& s, int rc) {
     // per-frame digest verdicts of the merged launch: a request that met a corrupt frame is redone on its own; the others are done
     // (their bytes are in place; a heal's `corrupt` was zeroed when it was queued).  A whole-file reader has no frames: the flags at
     // its arena position mean nothing, and the digest of its staged shard file (batch_whole_stage: streams in request order, a
-    // request's in ascending position order, digest j at s.hwdig + j*64) is compared with its expected sum instead.
-    const uint8_t* fl = static_cast<const uint8_t*>(s.hflags.p);
-    const uint8_t* wd = static_cast<const uint8_t*>(s.hwdig.p);
-    const BatchGetDesc* tab = static_cast<const BatchGetDesc*>(s.hreq.p);
+    // request's in ascending position order, digest j at s.wdig.h + j*64) is compared with its expected sum instead.
+    const uint8_t* fl = static_cast<const uint8_t*>(s.flags.h.p);
+    const uint8_t* wd = static_cast<const uint8_t*>(s.wdig.h.p);
+    const BatchGetDesc* tab = static_cast<const BatchGetDesc*>(s.dreq.h.p);
     const int k = c->k;
     int64_t stream = 0;
     for (size_t q = 0; q < fb.reqs.size(); q++) {
@@ -3801,7 +3754,7 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, Slot& s, int rc) {
         } else {
           if (r->heal_hint) *r->heal_hint = 0;
           if (r->sse_key) {  // the verdicts of its packages (sse_get_open): a package that fails hands out nothing of the range
-            const uint8_t* v = static_cast<const uint8_t*>(s.hsse_st.p) + r->sse_row0;
+            const uint8_t* v = static_cast<const uint8_t*>(s.sse_st.h.p) + r->sse_row0;
             const int64_t nrows = (r->sse_offset + r->sse_len - 1) / kPkg - r->sse_offset / kPkg + 1;
             int64_t e = MEC_OK;
             for (int64_t j = 0; j < nrows; j++) {
@@ -3827,12 +3780,12 @@ static void batcher_finish(mec_batcher* b, InflightBatch& fb, Slot& s, int rc) {
       BatchReq* r = fb.reqs[q];
       if (rc == MEC_OK && fb.needs_retire) frames_retire(c, r->ch, r->files, r->with_data, r->data_digests);
       if (rc == MEC_OK && r->crc_which) {  // batcher_crc_enqueue's results, row q of the slot's pinned mirror
-        const uint64_t* h = static_cast<const uint64_t*>(s.hcrc.p) + q * kCrcTypes;
+        const uint64_t* h = static_cast<const uint64_t*>(s.crc_out.h.p) + q * kCrcTypes;
         for (int ty = 0; ty < kCrcTypes; ty++) r->crc_out[ty] = h[ty];
         b->st_crc_requests++;
       }
       if (rc == MEC_OK && r->sum_which) {  // batcher_sums_fork's records, record q of the slot's pinned mirror
-        const uint8_t* h = static_cast<const uint8_t*>(s.hsum.p) + q * kSumRecord;
+        const uint8_t* h = static_cast<const uint8_t*>(s.sum_out.h.p) + q * kSumRecord;
         for (int a = 0; a < kSumAlgos; a++)
           if (r->sum_which & (MEC_SUM_MD5 << a)) memcpy(r->sums + 32 * a, h + 32 * a, static_cast<size_t>(sum_digest_len(a)));
         b->st_sum_requests++;
@@ -3862,7 +3815,7 @@ static void mark_phase(mec_batcher* b, Slot& s, int j) {
 // its full blocks at ch.d_src and its short last block at ch.d_src_tail; each is cut into kCrcRegion work items.  batcher_crc_table
 // writes the work table and enqueues its copy ahead of the staging (behind other slots' staging on the copy engine it would hold up
 // this batch's kernels); batcher_crc_launch, enqueued once the batch is staged, runs the region kernel over every item and the fold
-// kernel that merges each request's items into row q of s.crc_out, and copies the rows to s.hcrc, where batcher_finish reads them.
+// kernel that merges each request's items into row q of s.crc_out, and copies the rows to s.crc_out.h, where batcher_finish reads them.
 // Two launches and one small copy each way per batch, whatever the number of requests; a batch without such requests (p->nreq == 0)
 // enqueues nothing.  The buffers were sized by mec_batcher_new; they only grow here for a batch led by a request larger than
 // max_batch_blocks.
@@ -3880,12 +3833,10 @@ static int batcher_crc_table(mec_batcher* b, Slot& s, const std::vector<BatchReq
     if (r->crc_which) nwork += regions(r->ch.nfull * bs) + regions(r->ch.tail);
   const size_t nreq = reqs.size(), tab_bytes = nreq * sizeof(CrcReq) + static_cast<size_t>(nwork) * sizeof(CrcWork);
   int rc;
-  if ((rc = s.hcrc_tab.ensure(tab_bytes))) return rc;
   if ((rc = s.crc_tab.ensure(tab_bytes))) return rc;
   if ((rc = s.crc_part.ensure(static_cast<size_t>(nwork) * kCrcTypes * sizeof(uint64_t)))) return rc;
   if ((rc = s.crc_out.ensure(nreq * kCrcTypes * sizeof(uint64_t)))) return rc;
-  if ((rc = s.hcrc.ensure(nreq * kCrcTypes * sizeof(uint64_t)))) return rc;
-  CrcReq* rt = static_cast<CrcReq*>(s.hcrc_tab.p);
+  CrcReq* rt = static_cast<CrcReq*>(s.crc_tab.h.p);
   CrcWork* wt = reinterpret_cast<CrcWork*>(rt + nreq);
   int64_t w = 0;
   for (size_t q = 0; q < nreq; q++) {
@@ -3901,14 +3852,14 @@ static int batcher_crc_table(mec_batcher* b, Slot& s, const std::vector<BatchReq
     }
     rt[q].w1 = static_cast<int32_t>(w);
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(s.crc_tab.p, rt, tab_bytes, cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(s.crc_tab.upload(tab_bytes, s.st));
   p->base = base;
-  p->reqs = static_cast<const CrcReq*>(s.crc_tab.p);
+  p->reqs = static_cast<const CrcReq*>(s.crc_tab.d.p);
   p->work = reinterpret_cast<const CrcWork*>(p->reqs + nreq);
   p->nwork = nwork; p->nreq = static_cast<int>(nreq); p->which = which;
   p->tables = static_cast<const CrcTables*>(c->crc_tables.p);
   p->partial = static_cast<uint64_t*>(s.crc_part.p);
-  p->out = static_cast<uint64_t*>(s.crc_out.p);
+  p->out = static_cast<uint64_t*>(s.crc_out.d.p);
   return MEC_OK;
 }
 static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
@@ -3921,7 +3872,7 @@ static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
   crc_seg_fold_kernel<<<static_cast<unsigned>(ceil_frac(static_cast<int64_t>(p.nreq) * 32, kCrcFoldThreads)), kCrcFoldThreads, 0, s.st>>>(p);
   MEC_CUDA_OK(cudaGetLastError());
   c->eng->count_launch();
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hcrc.p, s.crc_out.p, static_cast<size_t>(p.nreq) * kCrcTypes * sizeof(uint64_t), cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(s.crc_out.download(static_cast<size_t>(p.nreq) * kCrcTypes * sizeof(uint64_t), s.st));
   return MEC_OK;
 }
 
@@ -3930,7 +3881,7 @@ static int batcher_crc_launch(mec_batcher* b, Slot& s, const CrcSegParams& p) {
 // request q.  batcher_sums_table writes the table and enqueues its copy ahead of the staging, as batcher_crc_table does, and
 // returns the number of items (0: the batch enqueues nothing for hashes).  batcher_sums_fork, enqueued once the batch is staged,
 // runs ONE stream_sums_kernel on the slot's second stream; batcher_sums_join makes the slot's stream wait for it and copies the
-// records to s.hsum, where batcher_finish reads them.  The buffers were sized by mec_batcher_new; they only grow here for a batch led
+// records to s.sum_out.h, where batcher_finish reads them.  The buffers were sized by mec_batcher_new; they only grow here for a batch led
 // by a request larger than max_batch_blocks.
 static int batcher_sums_table(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t* nwork) {
   *nwork = 0;
@@ -3939,12 +3890,10 @@ static int batcher_sums_table(mec_batcher* b, Slot& s, const std::vector<BatchRe
   const int64_t bs = b->codec->block_size;
   const size_t bytes = static_cast<size_t>(*nwork) * sizeof(SumWork);
   int rc;
-  if ((rc = s.hsum_tab.ensure(bytes))) return rc;
   if ((rc = s.sum_tab.ensure(bytes))) return rc;
   if ((rc = s.sum_out.ensure(reqs.size() * kSumRecord))) return rc;
-  if ((rc = s.hsum.ensure(reqs.size() * kSumRecord))) return rc;
   const uint8_t* base = static_cast<const uint8_t*>(s.src.p);
-  SumWork* t = static_cast<SumWork*>(s.hsum_tab.p);
+  SumWork* t = static_cast<SumWork*>(s.sum_tab.h.p);
   int64_t w = 0;
   for (size_t q = 0; q < reqs.size(); q++) {
     const EncChunk& ch = reqs[q]->ch;
@@ -3952,7 +3901,7 @@ static int batcher_sums_table(mec_batcher* b, Slot& s, const std::vector<BatchRe
                   ch.tail ? ch.d_src_tail - base : 0, ch.tail);
   }
   sum_sort(t, w);
-  MEC_CUDA_OK(cudaMemcpyAsync(s.sum_tab.p, t, bytes, cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(s.sum_tab.upload(bytes, s.st));
   return MEC_OK;
 }
 static int batcher_sums_fork(mec_batcher* b, Slot& s, int64_t nwork) {
@@ -3960,8 +3909,8 @@ static int batcher_sums_fork(mec_batcher* b, Slot& s, int64_t nwork) {
   const int si = static_cast<int>(&s - b->codec->slots);
   MEC_CUDA_OK(cudaEventRecord(b->ev_staged[si], s.st));
   MEC_CUDA_OK(cudaStreamWaitEvent(b->sum_st[si], b->ev_staged[si], 0));
-  int rc = sum_launch(b->codec, static_cast<const uint8_t*>(s.src.p), static_cast<const SumWork*>(s.sum_tab.p), nwork,
-                      static_cast<uint8_t*>(s.sum_out.p), b->sum_st[si]);
+  int rc = sum_launch(b->codec, static_cast<const uint8_t*>(s.src.p), static_cast<const SumWork*>(s.sum_tab.d.p), nwork,
+                      static_cast<uint8_t*>(s.sum_out.d.p), b->sum_st[si]);
   if (rc) return rc;
   MEC_CUDA_OK(cudaEventRecord(b->ev_summed[si], b->sum_st[si]));
   return MEC_OK;
@@ -3969,7 +3918,7 @@ static int batcher_sums_fork(mec_batcher* b, Slot& s, int64_t nwork) {
 static int batcher_sums_join(mec_batcher* b, Slot& s, size_t nreq, int64_t nwork) {
   if (nwork == 0) return MEC_OK;
   MEC_CUDA_OK(cudaStreamWaitEvent(s.st, b->ev_summed[&s - b->codec->slots], 0));
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hsum.p, s.sum_out.p, nreq * kSumRecord, cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(s.sum_out.download(nreq * kSumRecord, s.st));
   return MEC_OK;
 }
 
@@ -4003,20 +3952,20 @@ static int64_t batcher_slot_blocks(const mec_batcher* b);
 static int size_sse_arena(mec_batcher* b, Slot& s, int64_t bytes) {
   return s.sse_pt.ensure(static_cast<size_t>(std::max(bytes, batcher_slot_blocks(b) * b->codec->block_size)));
 }
-// The cipher launches over the batch's package rows s.hdpk[0, rows) (an open writes its verdicts to s.sse_st), then the keys are
+// The cipher launches over the batch's package rows s.dpk.h[0, rows) (an open writes its verdicts to s.sse_st), then the keys are
 // zeroed.  A seal seals rows [0, chacha_from) with AES-256-GCM and the rest with ChaCha20-Poly1305; an open with chacha_from < rows
 // adds the ChaCha20 open behind the AES one.
 static int sse_batch_cipher(mec_batcher* b, Slot& s, bool seal, int64_t nsse, int64_t rows, int64_t chacha_from, const uint8_t* in,
                             uint8_t* out) {
-  MEC_CUDA_OK(cudaMemcpyAsync(s.dpk.p, s.hdpk.p, static_cast<size_t>(rows) * sizeof(DarePkg), cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(s.dpk.upload(static_cast<size_t>(rows) * sizeof(DarePkg), s.st));
   const DareStreamKeys* k = static_cast<const DareStreamKeys*>(s.sse_keys.p);
-  const DarePkg* pk = static_cast<const DarePkg*>(s.dpk.p);
+  const DarePkg* pk = static_cast<const DarePkg*>(s.dpk.d.p);
   int rc;
   if (seal) {
     if ((rc = dare_launch(b->codec, true, false, k, pk, chacha_from, in, out, nullptr, s.st)) ||
         (rc = dare_launch(b->codec, true, true, k, pk + chacha_from, rows - chacha_from, in, out, nullptr, s.st)))
       return rc;
-  } else if ((rc = dare_launch(b->codec, false, chacha_from < rows, k, pk, rows, in, out, static_cast<uint8_t*>(s.sse_st.p), s.st))) {
+  } else if ((rc = dare_launch(b->codec, false, chacha_from < rows, k, pk, rows, in, out, static_cast<uint8_t*>(s.sse_st.d.p), s.st))) {
     return rc;
   }
   MEC_CUDA_OK(cudaMemsetAsync(s.sse_keys.p, 0, static_cast<size_t>(nsse) * sizeof(DareStreamKeys), s.st));
@@ -4040,9 +3989,9 @@ static int sse_put_plan(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
   if (*rows == 0) return MEC_OK;
   int rc;
   if ((rc = size_sse_arena(b, s, pt_total)) || (rc = s.aux.ensure(static_cast<size_t>(ct_total))) ||
-      (rc = s.dpk.ensure(static_cast<size_t>(*rows) * sizeof(DarePkg))) || (rc = s.hdpk.ensure(static_cast<size_t>(*rows) * sizeof(DarePkg))))
+      (rc = s.dpk.ensure(static_cast<size_t>(*rows) * sizeof(DarePkg))))
     return rc;
-  DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+  DarePkg* t = static_cast<DarePkg*>(s.dpk.h.p);
   uint8_t* pt = static_cast<uint8_t*>(s.sse_pt.p);
   int64_t w = 0, po = 0, co = 0;
   for (int pass = 0; pass < 2; pass++) {  // the AES-256-GCM requests, then the ChaCha20-Poly1305 ones
@@ -4080,7 +4029,7 @@ static int sse_put_seal(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
 }
 
 // The encrypted GETs of a batch, once the scatter has put each one's ciphertext range (whole packages) at s.src + asm_off[q]: ONE
-// setup and ONE open launch over every package into the arena s.sse_pt, the verdicts back to s.hsse_st (r->sse_row0 on), and ONE
+// setup and ONE open launch over every package into the arena s.sse_pt, the verdicts back to s.sse_st.h (r->sse_row0 on), and ONE
 // batched copy of each request's plaintext range to its caller.  The arena is cleared first, so a package that fails leaves zeros.
 static int sse_get_open(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const std::vector<int64_t>& asm_off) {
   int64_t rows = 0, pt_total = 0;
@@ -4094,13 +4043,11 @@ static int sse_get_open(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
     }
   if (rows == 0) return MEC_OK;
   int rc;
-  if ((rc = size_sse_arena(b, s, pt_total)) || (rc = s.dpk.ensure(static_cast<size_t>(rows) * sizeof(DarePkg))) ||
-      (rc = s.hdpk.ensure(static_cast<size_t>(rows) * sizeof(DarePkg))) || (rc = s.sse_st.ensure(static_cast<size_t>(rows))) ||
-      (rc = s.hsse_st.ensure(static_cast<size_t>(rows))))
+  if ((rc = size_sse_arena(b, s, pt_total)) || (rc = s.dpk.ensure(static_cast<size_t>(rows) * sizeof(DarePkg))) || (rc = s.sse_st.ensure(static_cast<size_t>(rows))))
     return rc;
   int64_t nsse;
   if ((rc = sse_batch_setup(b, s, reqs, false, &nsse))) return rc;
-  DarePkg* t = static_cast<DarePkg*>(s.hdpk.p);
+  DarePkg* t = static_cast<DarePkg*>(s.dpk.h.p);
   uint8_t* pt = static_cast<uint8_t*>(s.sse_pt.p);
   CopyList d2h;
   int64_t w = 0, po = 0;
@@ -4122,15 +4069,15 @@ static int sse_get_open(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& r
   }
   MEC_CUDA_OK(cudaMemsetAsync(pt, 0, static_cast<size_t>(pt_total), s.st));
   if ((rc = sse_batch_cipher(b, s, false, nsse, rows, chacha ? 0 : rows, static_cast<const uint8_t*>(s.src.p), pt))) return rc;
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hsse_st.p, s.sse_st.p, static_cast<size_t>(rows), cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(s.sse_st.download(static_cast<size_t>(rows), s.st));
   return d2h.flush(s.st);
 }
 
 // The PUT layout of a merged batch on slot `s` of codec `c`, in request order: every request's full blocks contiguous from s.src
 // (from block full0 on), the short last blocks behind all of them at 256-byte-rounded offsets (block tail_slot, byte tail_src_off);
 // parity rows [block][m][pitch] in s.out, digests [block][n][32] in s.dig.  A request is r->len object bytes for the frames in
-// r->files.  Sizes those buffers and fills request q's row of the BatchReqDesc table in s.hreq (`rows`) and / or its EncChunk
-// r->ch, whose digests come back to s.hdig (`chunks`).
+// r->files.  Sizes those buffers and fills request q's row of the BatchReqDesc table in s.dreq.h (`rows`) and / or its EncChunk
+// r->ch, whose digests come back to s.dig.h (`chunks`).
 struct PutLayout {
   int64_t total_full = 0, nslots = 0, max_nb = 0;  // full blocks, all blocks, the most blocks of one request
 };
@@ -4147,14 +4094,13 @@ static int put_layout(mec_codec* c, Slot& s, const std::vector<BatchReq*>& reqs,
   int rc;
   if ((rc = s.src.ensure(static_cast<size_t>(lay.total_full * bs + tail_bytes + 512)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(nb1 * std::max(m, 1) * pitch)))) return rc;
-  if ((rc = s.dig.ensure(static_cast<size_t>(nb1 * n * 32)))) return rc;
-  if (chunks && (rc = s.hdig.ensure(static_cast<size_t>(nb1 * n * 32)))) return rc;
-  if (rows && (rc = s.hreq.ensure(reqs.size() * sizeof(BatchReqDesc)))) return rc;
+  if ((rc = s.dig.d.ensure(static_cast<size_t>(nb1 * n * 32)))) return rc;
+  if (chunks && (rc = s.dig.h.ensure(static_cast<size_t>(nb1 * n * 32)))) return rc;
   if (rows && (rc = s.dreq.ensure(reqs.size() * sizeof(BatchReqDesc)))) return rc;
   uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
   uint8_t* dout = static_cast<uint8_t*>(s.out.p);
-  const uint8_t* hdig = static_cast<const uint8_t*>(s.hdig.p);
-  BatchReqDesc* tab = static_cast<BatchReqDesc*>(s.hreq.p);
+  const uint8_t* hdig = static_cast<const uint8_t*>(s.dig.h.p);
+  BatchReqDesc* tab = static_cast<BatchReqDesc*>(s.dreq.h.p);
   int64_t fb = 0, tb = lay.total_full, toff = lay.total_full * bs;
   for (size_t q = 0; q < reqs.size(); q++) {
     BatchReq* r = reqs[q];
@@ -4193,21 +4139,20 @@ static int batch_encode_scatter(mec_codec* c, Slot& s, cudaStream_t st, const Ba
   const int64_t total_full = lay.total_full, nslots = lay.nslots;
   uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
   uint8_t* dout = static_cast<uint8_t*>(s.out.p);
-  uint8_t* ddig = static_cast<uint8_t*>(s.dig.p);
+  uint8_t* ddig = static_cast<uint8_t*>(s.dig.d.p);
   int rc;
   if (c->eng->small_ok(c->opt, nslots)) {
     // ONE launch for every block of the batch, full or short (objects smaller than a block are nothing but a short block): the
     // latency kernel takes the geometry of each block from a table
-    if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(SmallBlock)))) return rc;
     if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(SmallBlock)))) return rc;
-    SmallBlock* bt = static_cast<SmallBlock*>(s.hblk.p);
+    SmallBlock* bt = static_cast<SmallBlock*>(s.blk.h.p);
     for (int64_t q = 0; q < total_full; q++) bt[q] = SmallBlock{q * bs, static_cast<int32_t>(S), static_cast<int32_t>(bs)};
     for (size_t q = 0; q < nreq; q++)
       if (tab[q].tail_slot >= 0) {
         const int64_t tl = tab[q].len % bs;
         bt[tab[q].tail_slot] = SmallBlock{tab[q].tail_src_off, static_cast<int32_t>(ceil_frac(tl, k)), static_cast<int32_t>(tl)};
       }
-    MEC_CUDA_OK(cudaMemcpyAsync(s.blk.p, bt, static_cast<size_t>(nslots) * sizeof(SmallBlock), cudaMemcpyHostToDevice, st));
+    MEC_CUDA_OK(s.blk.upload(static_cast<size_t>(nslots) * sizeof(SmallBlock), st));
     FusedDesc d;
     d.k = k; d.r = m;
     d.coef = c->matrix.data() + static_cast<size_t>(k) * k;
@@ -4215,7 +4160,7 @@ static int batch_encode_scatter(mec_codec* c, Slot& s, cudaStream_t st, const Ba
     d.nblocks = nslots; d.S = static_cast<int32_t>(S);
     d.in_base = dsrc; d.in_block_stride = bs; d.in_block_len = bs;
     d.out = dout; d.digests = ddig;
-    d.blocks = static_cast<const SmallBlock*>(s.blk.p);
+    d.blocks = static_cast<const SmallBlock*>(s.blk.d.p);
     if ((rc = c->eng->launch_fused(d, c->opt, st))) return rc;
   } else {
     if (total_full > 0 && (rc = encode_device_locked(c, dsrc, total_full * bs, dout, pitch, ddig, st))) return rc;
@@ -4248,11 +4193,11 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   *nblocks = nslots;
   uint8_t* dsrc = static_cast<uint8_t*>(s.src.p);
   uint8_t* dout = static_cast<uint8_t*>(s.out.p);
-  uint8_t* ddig = static_cast<uint8_t*>(s.dig.p);
+  uint8_t* ddig = static_cast<uint8_t*>(s.dig.d.p);
   if (all_mapped) {
     // gather kernel -> ONE fused launch over all full blocks (+ one per tail) -> scatter kernel: a handful of launches and one
     // small table copy per batch, whatever the number of requests
-    const BatchReqDesc* tab = static_cast<const BatchReqDesc*>(s.hreq.p);
+    const BatchReqDesc* tab = static_cast<const BatchReqDesc*>(s.dreq.h.p);
     for (const BatchReq* r : reqs) {
       const int64_t nf = r->len / bs, tl = r->len % bs;
       c->st_h2d += r->sse_key ? r->sse_len : r->len;
@@ -4260,13 +4205,13 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     }
     const int si = static_cast<int>(&s - c->slots);
     mark_phase(b, s, 0);
-    MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, reqs.size() * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
+    MEC_CUDA_OK(s.dreq.upload(reqs.size() * sizeof(BatchReqDesc), s.st));
     CrcSegParams crc;
     if ((rc = batcher_crc_table(b, s, reqs, &crc))) return rc;
     int64_t nsum;
     if ((rc = batcher_sums_table(b, s, reqs, &nsum))) return rc;
     BatchCopyParams cp;
-    cp.reqs = static_cast<const BatchReqDesc*>(s.dreq.p);
+    cp.reqs = static_cast<const BatchReqDesc*>(s.dreq.d.p);
     cp.nreq = static_cast<int>(reqs.size()); cp.k = k; cp.m = m; cp.bs = bs; cp.S = S; cp.pitch = pitch;
     cp.staged = dsrc; cp.parity = dout; cp.digests = ddig;
     // staging: the copy engines are the faster reader of host memory (one call per request); the gather kernel (SM loads over
@@ -4313,7 +4258,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
     mark_phase(b, s, 1);
     if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
     if ((rc = batcher_crc_launch(b, s, crc))) return rc;
-    if ((rc = batch_encode_scatter(c, s, s.st, tab, reqs.size(), lay, cp, b->sw.trace ? b->ev_ph[si][2] : nullptr))) return rc;
+    if ((rc = batch_encode_scatter(c, s, s.st, tab, reqs.size(), lay, cp, b->sw.trace ? cudaEvent_t{b->ev_ph[si][2]} : nullptr))) return rc;
     mark_phase(b, s, 3);
     if ((rc = batcher_sums_join(b, s, reqs.size(), nsum))) return rc;
     *needs_retire = false;
@@ -4343,14 +4288,14 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
   if ((rc = batcher_sums_fork(b, s, nsum))) return rc;
   if ((rc = batcher_crc_launch(b, s, crc))) return rc;
   if (lay.total_full > 0 && (rc = encode_device_locked(c, dsrc, lay.total_full * bs, dout, pitch, ddig, s.st))) return rc;  // ONE launch for every caller's full blocks
-  const uint8_t* hdig = static_cast<const uint8_t*>(s.hdig.p);
+  const uint8_t* hdig = static_cast<const uint8_t*>(s.dig.h.p);
   for (BatchReq* r : reqs) {
     const EncChunk& ch = r->ch;
     if (ch.tail > 0 && (rc = encode_device_locked(c, ch.d_src_tail, ch.tail, ch.d_out_tail, pitch,
                                                   ddig + (ch.h_dig_tail - hdig), s.st)))
       return rc;
   }
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hdig.p, s.dig.p, static_cast<size_t>(nslots * n * 32), cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(s.dig.download(static_cast<size_t>(nslots * n * 32), s.st));
   for (BatchReq* r : reqs)
     if ((rc = frames_enqueue(c, r->ch, r->files, r->with_data, r->data_digests))) return rc;
   if ((rc = batcher_sums_join(b, s, reqs.size(), nsum))) return rc;
@@ -4362,7 +4307,7 @@ static int batcher_submit(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs,
 // blocks behind them.
 struct ReadLayout {
   int64_t nfull_slots = 0, ntails = 0, max_nb = 0;
-  size_t table_bytes = 0;  // of the request table (s.hreq -> s.dreq)
+  size_t table_bytes = 0;  // of the request table (s.dreq.h -> s.dreq)
   int npat = 0;            // distinct erasure patterns of the batch
   const uint8_t* rows = nullptr;  // npat == 1: the r x k decode rows of that pattern
   size_t pat_off = 0, bp_off = 0; // npat > 1: SmallPattern[npat] and the uint16_t pattern of every slot, offsets in the table
@@ -4370,7 +4315,7 @@ struct ReadLayout {
 };
 // Every request's reader set — the first k readers of its alive mask — and the decode plan of what it rebuilds: the data shards
 // those readers miss for a GET, the stale drives for a heal (disjoint from the readers: mec_batcher_heal sends the rest to the
-// serial handle).  Fills the request table in s.hreq — a heal's carries out_files[targets[q]] of request z at [z * gp.r + q] behind
+// serial handle).  Fills the request table in s.dreq.h — a heal's carries out_files[targets[q]] of request z at [z * gp.r + q] behind
 // the rows; a batch of several patterns then the pattern table and the per-slot pattern index — each request's placement in the
 // batch, and gp (gp.r = the most targets of any request).
 static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs, BatchGetParams& gp, ReadLayout& lay) {
@@ -4430,9 +4375,8 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
     lay.table_bytes = lay.bp_off + static_cast<size_t>(nslots) * sizeof(uint16_t);
   }
   int rc;
-  if ((rc = s.hreq.ensure(lay.table_bytes))) return rc;
   if ((rc = s.dreq.ensure(lay.table_bytes))) return rc;
-  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
+  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.dreq.h.p);
   for (size_t q = 0; q < nreq; q++) {
     BatchReq* rq = reqs[q];
     BatchGetDesc& d = tab[q];
@@ -4470,7 +4414,7 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
       for (int q = 0; q < tab[z].r; q++) outs[z * rmax + q] = reqs[z]->outs[tab[z].targets[q]];
   }
   if (lay.npat > 1) {
-    uint8_t* base = static_cast<uint8_t*>(s.hreq.p);
+    uint8_t* base = static_cast<uint8_t*>(s.dreq.h.p);
     SmallPattern* sp = reinterpret_cast<SmallPattern*>(base + lay.pat_off);
     for (int pi = 0; pi < lay.npat; pi++) sp[pi] = pats[pi]->sp;
     uint16_t* bp = reinterpret_cast<uint16_t*>(base + lay.bp_off);
@@ -4478,7 +4422,7 @@ static int batch_read_plan(mec_batcher* b, Slot& s, std::vector<BatchReq*>& reqs
       for (int64_t bb = 0; bb < tab[q].nblocks; bb++) bp[get_slot(tab[q], bb)] = static_cast<uint16_t>(req_pat[q]);
   }
   memset(&gp, 0, sizeof(gp));
-  gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.p);
+  gp.reqs = static_cast<const BatchGetDesc*>(s.dreq.d.p);
   gp.nreq = static_cast<int>(nreq); gp.k = k; gp.r = rmax;
   gp.bs = bs; gp.S = S; gp.P = round_up(32 + S, 16); gp.pitch = round_up(S, 16);
   return MEC_OK;
@@ -4496,7 +4440,7 @@ struct WholeFiles {
 static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, const BatchGetDesc* tab, WholeFiles* wf);
 
 // The request table to the device, survivor frames of every block of every request -> the slot's arena, the fused reconstruct of
-// every request's targets over all of them, and the per-frame digest verdicts back to s.hflags.  `tab` is the host copy of the table
+// every request's targets over all of them, and the per-frame digest verdicts back to s.flags.h.  `tab` is the host copy of the table
 // gp.reqs points at; gp holds the geometry and gets the arena and rebuilt rows here.  A batch of several erasure patterns is ONE
 // latency launch with a decode plan per block (batcher_main only merges such a batch when its blocks fit one).  `wf` (a batch with
 // whole-file readers, staged and hashed by batch_whole_stage): their positions are filled from the staged raw shard files by
@@ -4510,14 +4454,13 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
   const int64_t stride = round_up(nslots * P + 512, 256);
   const bool raw = wf && wf->raw;
   if (!wf) mark_phase(b, s, 0);  // a batch with whole-file readers marks the start of its staging (batch_whole_stage)
-  MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.p, tab, lay.table_bytes, cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(cudaMemcpyAsync(s.dreq.d.p, tab, lay.table_bytes, cudaMemcpyHostToDevice, s.st));
   int rc;
   if ((rc = s.aux.ensure(static_cast<size_t>(k * stride)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(nslots * std::max(r, 1) * pitch)))) return rc;
   if (!raw) {
-    if ((rc = s.dig.ensure(static_cast<size_t>(nslots * (k + r) * 32)))) return rc;
+    if ((rc = s.dig.d.ensure(static_cast<size_t>(nslots * (k + r) * 32)))) return rc;
     if ((rc = s.flags.ensure(static_cast<size_t>(nslots * k)))) return rc;
-    if ((rc = s.hflags.ensure(static_cast<size_t>(nslots * k)))) return rc;
   }
   gp.arena = static_cast<uint8_t*>(s.aux.p); gp.arena_stride = stride;
   gp.rebuilt = static_cast<const uint8_t*>(s.out.p);
@@ -4561,10 +4504,10 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     }
   }
   mark_phase(b, s, 1);
-  if (!raw) MEC_CUDA_OK(cudaMemsetAsync(s.flags.p, 0, static_cast<size_t>(nslots * k), s.st));
+  if (!raw) MEC_CUDA_OK(cudaMemsetAsync(s.flags.d.p, 0, static_cast<size_t>(nslots * k), s.st));
   const int32_t* block_len = nullptr;
   const bool mixed = lay.npat > 1;
-  const uint8_t* dtab = static_cast<const uint8_t*>(s.dreq.p);
+  const uint8_t* dtab = static_cast<const uint8_t*>(s.dreq.d.p);
   auto launch = [&](int64_t slot0, int64_t cnt, int64_t shard_len) -> int {
     FusedDesc d;
     d.block_len = block_len;
@@ -4581,8 +4524,8 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     }
     d.out = static_cast<uint8_t*>(s.out.p) + slot0 * r * pitch;
     if (!raw) {
-      d.digests = static_cast<uint8_t*>(s.dig.p) + slot0 * (k + r) * 32;
-      d.corrupt = static_cast<uint8_t*>(s.flags.p) + slot0 * k;
+      d.digests = static_cast<uint8_t*>(s.dig.d.p) + slot0 * (k + r) * 32;
+      d.corrupt = static_cast<uint8_t*>(s.flags.d.p) + slot0 * k;
     }
     return c->eng->launch_fused(d, c->opt, s.st);
   };
@@ -4593,21 +4536,20 @@ static int batch_read_reconstruct(mec_batcher* b, Slot& s, const BatchGetDesc* t
     if ((rc = launch(0, nslots, S))) return rc;
   } else if (lay.ntails > 0 && c->eng->small_ok(c->opt, nslots)) {
     // ONE launch for every block of every caller, the short last ones included (per-block shard lengths in the latency kernel)
-    if ((rc = s.hblk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
     if ((rc = s.blk.ensure(static_cast<size_t>(nslots) * sizeof(int32_t)))) return rc;
-    int32_t* lens = static_cast<int32_t*>(s.hblk.p);
+    int32_t* lens = static_cast<int32_t*>(s.blk.h.p);
     for (int64_t q = 0; q < lay.nfull_slots; q++) lens[q] = static_cast<int32_t>(S);
     for (int q = 0; q < gp.nreq; q++)
       if (tab[q].tail_slot >= 0) lens[tab[q].tail_slot] = static_cast<int32_t>(tab[q].last_len);
-    MEC_CUDA_OK(cudaMemcpyAsync(s.blk.p, lens, static_cast<size_t>(nslots) * sizeof(int32_t), cudaMemcpyHostToDevice, s.st));
-    block_len = static_cast<const int32_t*>(s.blk.p);
+    MEC_CUDA_OK(s.blk.upload(static_cast<size_t>(nslots) * sizeof(int32_t), s.st));
+    block_len = static_cast<const int32_t*>(s.blk.d.p);
     if ((rc = launch(0, nslots, S))) return rc;
   } else {
     if (lay.nfull_slots > 0 && (rc = launch(0, lay.nfull_slots, S))) return rc;  // ONE launch for every caller's full blocks
     for (int q = 0; q < gp.nreq; q++)
       if (tab[q].tail_slot >= 0 && (rc = launch(tab[q].tail_slot, 1, tab[q].last_len))) return rc;
   }
-  if (!raw) MEC_CUDA_OK(cudaMemcpyAsync(s.hflags.p, s.flags.p, static_cast<size_t>(nslots * k), cudaMemcpyDeviceToHost, s.st));
+  if (!raw) MEC_CUDA_OK(s.flags.download(static_cast<size_t>(nslots * k), s.st));
   mark_phase(b, s, 2);
   b->st_patterns += lay.npat;
   if (mixed) b->st_mixed++;
@@ -4628,7 +4570,7 @@ static int batcher_submit_get(mec_batcher* b, Slot& s, std::vector<BatchReq*>& r
   if (rc) return rc;
   const int k = gp.k, r = gp.r;
   const int64_t S = gp.S, P = gp.P, pitch = gp.pitch, nslots = lay.nslots();
-  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.hreq.p);
+  BatchGetDesc* tab = static_cast<BatchGetDesc*>(s.dreq.h.p);
   // writeDataBlocks: 0 = the scatter kernel assembles every object in device memory and ONE copy per request takes it to the caller
   // (fewest driver-side copy descriptors), 1 = the scatter kernel stores straight into the callers' buffers over PCIe, 2 = the copy
   // engine moves every (request, shard, block) piece itself
@@ -4707,7 +4649,7 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
   if (rc) return rc;
   const int r = gp.r;
   const int64_t nslots = lay.nslots();
-  const BatchGetDesc* tab = static_cast<const BatchGetDesc*>(s.hreq.p);
+  const BatchGetDesc* tab = static_cast<const BatchGetDesc*>(s.dreq.h.p);
   const bool whole = reqs.front()->whole_algo != 0;
   WholeFiles wf;
   if (whole) {
@@ -4718,7 +4660,7 @@ static int batcher_submit_heal(mec_batcher* b, Slot& s, std::vector<BatchReq*>& 
   if (r > 0) {
     const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
     batch_heal_scatter_kernel<<<dim3(gx, static_cast<unsigned>(r), static_cast<unsigned>(reqs.size())), 128, 0, s.st>>>(
-        gp, static_cast<const uint8_t*>(s.dig.p), reinterpret_cast<uint8_t* const*>(gp.reqs + gp.nreq));
+        gp, static_cast<const uint8_t*>(s.dig.d.p), reinterpret_cast<uint8_t* const*>(gp.reqs + gp.nreq));
     MEC_CUDA_OK(cudaGetLastError());
     c->eng->count_launch();
   }
@@ -4737,9 +4679,7 @@ static int size_whole_slot(const mec_codec* c, Slot& s, int64_t slots) {
   int rc;
   if ((rc = s.src.ensure(static_cast<size_t>(slots * (c->block_size + 272 * k))))) return rc;
   if ((rc = s.wtab.ensure(tab))) return rc;
-  if ((rc = s.hwtab.ensure(tab))) return rc;
-  if ((rc = s.wdig.ensure(static_cast<size_t>(slots * k * 64)))) return rc;
-  return s.hwdig.ensure(static_cast<size_t>(slots * k * 64));
+  return s.wdig.ensure(static_cast<size_t>(slots * k * 64));
 }
 // the blocks a batcher's slots are sized for (batcher_create)
 static int64_t batcher_slot_blocks(const mec_batcher* b) { return b->max_blocks + std::min<int64_t>(64, b->max_blocks / 8 + 4); }
@@ -4749,7 +4689,7 @@ static int64_t batcher_slot_blocks(const mec_batcher* b) { return b->max_blocks 
 // shard files of every request's whole-file positions (bit t of tab[z].whole_pos: reader tab[z].chosen[t]) -> the file arena in
 // s.src (each 16-byte aligned with 256 readable bytes behind it, as stage_verified_whole lays files out) in ONE batched copy, then
 // ONE whole_hash_kernel launch over a stream table that holds only those files, in request order and ascending position order
-// within a request, and their digests back to s.hwdig, where batcher_finish compares them with every request's expected sums.
+// within a request, and their digests back to s.wdig.h, where batcher_finish compares them with every request's expected sums.
 // Request z's first stream is first[z], stored behind the stream table.  s.src is free: a heal or move batch does not stage object
 // bytes, and a GET batch with whole-file readers scatters straight into its callers' buffers (batcher_submit_get).  Counts
 // "bytes_h2d" as mec_decode_mixed does: the frames of every streaming reader plus one shard file per whole-file reader.
@@ -4762,11 +4702,9 @@ static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq
   size_t nfiles = 0;
   for (size_t z = 0; z < nreq; z++) nfiles += static_cast<size_t>(__builtin_popcount(tab[z].whole_pos));
   const size_t tab_bytes = nfiles * sizeof(WholeStream) + nreq * sizeof(int32_t);
-  if ((rc = s.hwtab.ensure(tab_bytes))) return rc;  // a request larger than the slots' sizing leads its own batch
-  if ((rc = s.wtab.ensure(tab_bytes))) return rc;
+  if ((rc = s.wtab.ensure(tab_bytes))) return rc;  // a request larger than the slots' sizing leads its own batch
   if ((rc = s.wdig.ensure(nfiles * 64))) return rc;
-  if ((rc = s.hwdig.ensure(nfiles * 64))) return rc;
-  WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+  WholeStream* ws = static_cast<WholeStream*>(s.wtab.h.p);
   int32_t* first = reinterpret_cast<int32_t*>(ws + nfiles);
   int64_t arena = 0;
   size_t j = 0;
@@ -4786,7 +4724,7 @@ static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq
   if ((rc = s.src.ensure(static_cast<size_t>(arena)))) return rc;
   uint8_t* files = static_cast<uint8_t*>(s.src.p);
   mark_phase(b, s, 0);
-  MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, tab_bytes, cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(s.wtab.upload(tab_bytes, s.st));
   std::vector<void*> dsts, srcs;
   std::vector<size_t> sizes;
   j = 0;
@@ -4798,11 +4736,11 @@ static int batch_whole_stage(mec_batcher* b, Slot& s, const std::vector<BatchReq
         dsts.push_back(files + w.off); srcs.push_back(const_cast<uint8_t*>(tab[z].files[tab[z].chosen[t]])); sizes.push_back(static_cast<size_t>(w.len));
       }
   if ((rc = copy_batch(dsts, srcs, sizes, s.st))) return rc;
-  const WholeStream* dws = static_cast<const WholeStream*>(s.wtab.p);
-  if ((rc = whole_hash_device(c, reqs.front()->whole_algo, files, 0, 0, static_cast<int64_t>(nfiles), static_cast<uint8_t*>(s.wdig.p), s.st, dws)))
+  const WholeStream* dws = static_cast<const WholeStream*>(s.wtab.d.p);
+  if ((rc = whole_hash_device(c, reqs.front()->whole_algo, files, 0, 0, static_cast<int64_t>(nfiles), static_cast<uint8_t*>(s.wdig.d.p), s.st, dws)))
     return rc;
   c->eng->count_launch();
-  MEC_CUDA_OK(cudaMemcpyAsync(s.hwdig.p, s.wdig.p, nfiles * 64, cudaMemcpyDeviceToHost, s.st));
+  MEC_CUDA_OK(s.wdig.download(nfiles * 64, s.st));
   bool streaming = false;  // a request of the batch reads frames
   for (size_t z = 0; z < nreq; z++) streaming |= tab[z].whole_pos != static_cast<uint32_t>((1ull << k) - 1);
   *wf = WholeFiles{files, dws, reinterpret_cast<const int32_t*>(dws + nfiles), !streaming};
@@ -4836,16 +4774,16 @@ static int batcher_submit_transcode(mec_batcher* b, Slot& s, std::vector<BatchRe
       c->st_h2d += static_cast<int64_t>(c->k) * mec_bitrot_shard_file_size(mec_shard_file_size(c, r->total), c->S(), MEC_HIGHWAYHASH256S);
     e->st_d2h += (nf * eS + (tl ? ceil_frac(tl, ek) : 0)) * en;
   }
-  const BatchReqDesc* dt = static_cast<const BatchReqDesc*>(d.hreq.p);
-  const BatchGetDesc* rt = static_cast<const BatchGetDesc*>(s.hreq.p);
+  const BatchReqDesc* dt = static_cast<const BatchReqDesc*>(d.dreq.h.p);
+  const BatchGetDesc* rt = static_cast<const BatchGetDesc*>(s.dreq.h.p);
   WholeFiles wf;
   if (whole && (rc = batch_whole_stage(b, s, reqs, rt, &wf))) return rc;  // every reader whole-file: wf.raw
   if ((rc = batch_read_reconstruct(b, s, rt, gp, lay, false, whole ? &wf : nullptr))) return rc;
-  MEC_CUDA_OK(cudaMemcpyAsync(d.dreq.p, dt, nreq * sizeof(BatchReqDesc), cudaMemcpyHostToDevice, s.st));
+  MEC_CUDA_OK(d.dreq.upload(nreq * sizeof(BatchReqDesc), s.st));
   BatchCopyParams cp;
-  cp.reqs = static_cast<const BatchReqDesc*>(d.dreq.p);
+  cp.reqs = static_cast<const BatchReqDesc*>(d.dreq.d.p);
   cp.nreq = static_cast<int>(nreq); cp.k = ek; cp.m = e->m; cp.bs = bs; cp.S = eS; cp.pitch = epitch;
-  cp.staged = static_cast<uint8_t*>(d.src.p); cp.parity = static_cast<const uint8_t*>(d.out.p); cp.digests = static_cast<const uint8_t*>(d.dig.p);
+  cp.staged = static_cast<uint8_t*>(d.src.p); cp.parity = static_cast<const uint8_t*>(d.out.p); cp.digests = static_cast<const uint8_t*>(d.dig.d.p);
   const unsigned gx = static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(lay.max_nb, 1), 16));
   batch_transcode_resplit_kernel<<<dim3(gx, static_cast<unsigned>(c->k), static_cast<unsigned>(nreq)), 128, 0, s.st>>>(gp, cp);
   MEC_CUDA_OK(cudaGetLastError());
@@ -4873,7 +4811,7 @@ static VerifyLimits verify_limits(const mec_batcher* b) {
 // s.src + j * P) and every whole-file part (from round_up(nframes * P + 512, 256) on, each 16-byte aligned with 256 readable bytes
 // behind it, as batch_whole_stage lays files out) in ONE batched copy; ONE hash-only launch over every frame with the per-frame
 // length table (verify_frames); ONE whole_hash_kernel launch whose algorithm groups hold every whole-file part (verify_whole_firsts'
-// order); the frame verdicts and file digests back to s.hflags and s.hwdig, where batcher_finish folds them into each caller's
+// order); the frame verdicts and file digests back to s.flags.h and s.wdig.h, where batcher_finish folds them into each caller's
 // results.  Nothing is redone: a corrupt part is a result.
 static int batcher_submit_verify(mec_batcher* b, Slot& s, const std::vector<BatchReq*>& reqs, int64_t* nblocks) {
   mec_codec* c = b->codec;
@@ -4888,13 +4826,13 @@ static int batcher_submit_verify(mec_batcher* b, Slot& s, const std::vector<Batc
   int64_t end = woff;
   for (const BatchReq* r : reqs) end += r->vbytes - r->vframes * P;  // the whole-file parts (verify_staged)
   if ((rc = s.src.ensure(static_cast<size_t>(end)))) return rc;
-  if ((rc = s.hreq.ensure(static_cast<size_t>(nframes) * sizeof(int32_t) + 16))) return rc;
-  if ((rc = s.hwtab.ensure(static_cast<size_t>(nwhole) * sizeof(WholeStream) + 16)) || (rc = s.wtab.ensure(static_cast<size_t>(nwhole) * sizeof(WholeStream) + 16)))
+  if ((rc = s.dreq.h.ensure(static_cast<size_t>(nframes) * sizeof(int32_t) + 16))) return rc;
+  if ((rc = s.wtab.ensure(static_cast<size_t>(nwhole) * sizeof(WholeStream) + 16)))
     return rc;
-  if ((rc = s.wdig.ensure(static_cast<size_t>(nwhole) * 64 + 64)) || (rc = s.hwdig.ensure(static_cast<size_t>(nwhole) * 64 + 64))) return rc;
+  if ((rc = s.wdig.ensure(static_cast<size_t>(nwhole) * 64 + 64))) return rc;
   uint8_t* arena = static_cast<uint8_t*>(s.src.p);
-  int32_t* lens = static_cast<int32_t*>(s.hreq.p);
-  WholeStream* ws = static_cast<WholeStream*>(s.hwtab.p);
+  int32_t* lens = static_cast<int32_t*>(s.dreq.h.p);
+  WholeStream* ws = static_cast<WholeStream*>(s.wtab.h.p);
   CopyList list;
   int64_t f = 0, wpos = woff;
   for (const BatchReq* r : reqs)
@@ -4919,16 +4857,16 @@ static int batcher_submit_verify(mec_batcher* b, Slot& s, const std::vector<Batc
     }
   mark_phase(b, s, 0);
   if (nwhole > 0)
-    MEC_CUDA_OK(cudaMemcpyAsync(s.wtab.p, ws, static_cast<size_t>(nwhole) * sizeof(WholeStream), cudaMemcpyHostToDevice, s.st));
+    MEC_CUDA_OK(s.wtab.upload(static_cast<size_t>(nwhole) * sizeof(WholeStream), s.st));
   if ((rc = list.flush(s.st))) return rc;
   mark_phase(b, s, 1);
   if (nframes > 0 && (rc = verify_frames(c, s, arena, nframes, nframes, lens, c->eng->small_ok(c->opt, nframes)))) return rc;
   if (nwhole > 0) {
-    if ((rc = whole_hash_groups(c, kWholeGroups, kWholeAlgos, counts, arena, 0, 0, static_cast<uint8_t*>(s.wdig.p), s.st,
-                                static_cast<const WholeStream*>(s.wtab.p))))
+    if ((rc = whole_hash_groups(c, kWholeGroups, kWholeAlgos, counts, arena, 0, 0, static_cast<uint8_t*>(s.wdig.d.p), s.st,
+                                static_cast<const WholeStream*>(s.wtab.d.p))))
       return rc;
     c->eng->count_launch();
-    MEC_CUDA_OK(cudaMemcpyAsync(s.hwdig.p, s.wdig.p, static_cast<size_t>(nwhole) * 64, cudaMemcpyDeviceToHost, s.st));
+    MEC_CUDA_OK(s.wdig.download(static_cast<size_t>(nwhole) * 64, s.st));
   }
   mark_phase(b, s, 2);
   mark_phase(b, s, 3);
@@ -5103,24 +5041,18 @@ static int size_put_slot(const mec_codec* c, Slot& s, int64_t blocks) {
   int rc;
   if ((rc = s.src.ensure(static_cast<size_t>(blocks * c->block_size)))) return rc;
   if ((rc = s.out.ensure(static_cast<size_t>(blocks * std::max(c->m, 1) * round_up(c->S(), 16))))) return rc;
-  return s.dig.ensure(static_cast<size_t>(blocks * c->n * 32));
-}
-
-static void batcher_destroy_streams(mec_batcher* b) {
-  for (int i = 0; i < kSlots; i++) {
-    if (b->ev_staged[i]) cudaEventDestroy(b->ev_staged[i]);
-    if (b->ev_summed[i]) cudaEventDestroy(b->ev_summed[i]);
-    if (b->sum_st[i]) cudaStreamDestroy(b->sum_st[i]);
-  }
+  return s.dig.d.ensure(static_cast<size_t>(blocks * c->n * 32));
 }
 
 // mec_batcher_new_ex, and with `dst` (a codec of the destination geometry without an engine yet, owned from here on, freed on
 // failure) mec_batcher_new_transcode: the destination's engine and slots are set up before the worker starts
 static int batcher_create(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
                           mec_codec* dst, mec_batcher** out) {
-  mec_codec* c = nullptr;
-  int rc = mec_codec_new(k, m, block_size, MEC_HIGHWAYHASH256S, device, &c);
-  if (rc) { mec_codec_free(dst); return rc; }
+  std::unique_ptr<mec_batcher> b(new mec_batcher);
+  b->dst = dst;
+  int rc = mec_codec_new(k, m, block_size, MEC_HIGHWAYHASH256S, device, &b->codec);
+  if (rc) return rc;
+  mec_codec* c = b->codec;
   {
     std::lock_guard<std::mutex> lk(c->mu);
     rc = ensure_engine(c);
@@ -5130,10 +5062,7 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     rc = ensure_engine(dst);
   }
   if (rc == MEC_OK && (c->S() >= (1ll << 31) || (dst && dst->S() >= (1ll << 31)))) rc = MEC_ERR_UNSUPPORTED;
-  if (rc) { mec_codec_free(c); mec_codec_free(dst); return rc; }
-  mec_batcher* b = new mec_batcher;
-  b->codec = c;
-  b->dst = dst;
+  if (rc) return rc;
   b->sw = batcher_switches();
   b->mix = (flags & MEC_BATCHER_MIX_PATTERNS) && c->eng->small_ok(c->opt, 1);  // per-block decode plans exist in the latency kernel only
   if (max_batch_blocks > 0) b->max_blocks = max_batch_blocks;
@@ -5147,38 +5076,31 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
-    const int64_t P = round_up(32 + c->S(), 16), slots = batcher_slot_blocks(b);
+    const int64_t P = round_up(32 + c->S(), 16), slots = batcher_slot_blocks(b.get());
     for (Slot& s : c->slots) {
       if (rc == MEC_OK) rc = size_put_slot(c, s, slots);
-      if (rc == MEC_OK) rc = s.hdig.ensure(static_cast<size_t>(slots * c->n * 32));
+      if (rc == MEC_OK) rc = s.dig.h.ensure(static_cast<size_t>(slots * c->n * 32));
       if (rc == MEC_OK) rc = s.aux.ensure(static_cast<size_t>(k * round_up(slots * P + 512, 256)));
       if (rc == MEC_OK) rc = s.flags.ensure(static_cast<size_t>(slots * k));
-      if (rc == MEC_OK) rc = s.hflags.ensure(static_cast<size_t>(slots * k));
       // request tables: PUT rows, or GET rows, or GET rows plus one out-file pointer per rebuilt shard (heal); reads of several
       // erasure patterns add a pattern (at most one per request) and a pattern index per block
       const size_t row = std::max(sizeof(BatchReqDesc), sizeof(BatchGetDesc) + kMaxR * sizeof(uint8_t*) +
                                                             (b->mix ? sizeof(SmallPattern) + sizeof(uint16_t) : 0));
       if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * row + 16);
-      if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * row + 16);
       // object checksums (batcher_crc_enqueue): a batch of at most `slots` requests and slots x block_size bytes has at most
       // slots x block_size / kCrcRegion whole regions plus two partial ones (full-block segment, short block) per request
       const int64_t nwork = ceil_frac(slots * block_size, kCrcRegion) + 2 * slots;
       const size_t tab = static_cast<size_t>(slots) * sizeof(CrcReq) + static_cast<size_t>(nwork) * sizeof(CrcWork);
       if (rc == MEC_OK) rc = s.crc_tab.ensure(tab);
-      if (rc == MEC_OK) rc = s.hcrc_tab.ensure(tab);
       if (rc == MEC_OK) rc = s.crc_part.ensure(static_cast<size_t>(nwork) * kCrcTypes * sizeof(uint64_t));
       if (rc == MEC_OK) rc = s.crc_out.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
-      if (rc == MEC_OK) rc = s.hcrc.ensure(static_cast<size_t>(slots) * kCrcTypes * sizeof(uint64_t));
       // object hashes (batcher_sums_table): at most `slots` requests, each with up to kSumAlgos items and one record
       if (rc == MEC_OK) rc = s.sum_tab.ensure(static_cast<size_t>(slots) * kSumAlgos * sizeof(SumWork));
-      if (rc == MEC_OK) rc = s.hsum_tab.ensure(static_cast<size_t>(slots) * kSumAlgos * sizeof(SumWork));
       if (rc == MEC_OK) rc = s.sum_out.ensure(static_cast<size_t>(slots) * kSumRecord);
-      if (rc == MEC_OK) rc = s.hsum.ensure(static_cast<size_t>(slots) * kSumRecord);
     }
     for (int i = 0; i < kSlots && rc == MEC_OK; i++)
-      if (cudaStreamCreateWithFlags(&b->sum_st[i], cudaStreamNonBlocking) != cudaSuccess ||
-          cudaEventCreateWithFlags(&b->ev_staged[i], cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&b->ev_summed[i], cudaEventDisableTiming) != cudaSuccess) {
+      if (b->sum_st[i].create(cudaStreamNonBlocking) != cudaSuccess || b->ev_staged[i].create(cudaEventDisableTiming) != cudaSuccess ||
+          b->ev_summed[i].create(cudaEventDisableTiming) != cudaSuccess) {
         set_last_error(std::string("object-hash stream: ") + cudaGetErrorString(cudaGetLastError()));
         rc = MEC_ERR_CUDA;
       }
@@ -5196,36 +5118,33 @@ static int batcher_create(int k, int m, int64_t block_size, int device, int64_t 
       for (Slot& s : dst->slots) {
         if (rc == MEC_OK) rc = size_put_slot(dst, s, dslots);
         if (rc == MEC_OK) rc = s.dreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
-        if (rc == MEC_OK) rc = s.hreq.ensure(static_cast<size_t>(slots) * sizeof(BatchReqDesc) + 16);
         if (rc == MEC_OK) rc = s.blk.ensure(static_cast<size_t>(dslots) * sizeof(SmallBlock));
-        if (rc == MEC_OK) rc = s.hblk.ensure(static_cast<size_t>(dslots) * sizeof(SmallBlock));
       }
     }
     cudaSetDevice(cur);
   }
-  if (rc) { batcher_destroy_streams(b); mec_codec_free(c); mec_codec_free(dst); delete b; return rc; }
+  if (rc) return rc;
   if (b->sw.trace) {
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
     for (int i = 0; i < kSlots; i++)
       for (int j = 0; j < 4; j++)
-        if (cudaEventCreate(&b->ev_ph[i][j]) != cudaSuccess) { cudaGetLastError(); b->sw.trace = false; }
+        if (b->ev_ph[i][j].create(cudaEventDefault) != cudaSuccess) { cudaGetLastError(); b->sw.trace = false; }
     cudaSetDevice(cur);
   }
   if (b->sw.gather_pct > 0) {
     int cur = 0;
     cudaGetDevice(&cur);
     cudaSetDevice(device);
-    bool ok = cudaStreamCreateWithFlags(&b->aux, cudaStreamNonBlocking) == cudaSuccess;
+    bool ok = b->aux.create(cudaStreamNonBlocking) == cudaSuccess;
     for (int i = 0; ok && i < kSlots; i++)
-      ok = cudaEventCreateWithFlags(&b->ev_table[i], cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&b->ev_gather[i], cudaEventDisableTiming) == cudaSuccess;
+      ok = b->ev_table[i].create(cudaEventDisableTiming) == cudaSuccess && b->ev_gather[i].create(cudaEventDisableTiming) == cudaSuccess;
     cudaSetDevice(cur);
     if (!ok) { cudaGetLastError(); b->sw.gather_pct = 0; }
   }
-  b->worker = std::thread(batcher_main, b);
-  *out = b;
+  b->worker = std::thread(batcher_main, b.get());
+  *out = b.release();
   return MEC_OK;
 }
 extern "C" int mec_batcher_new_ex(int k, int m, int64_t block_size, int device, int64_t max_batch_blocks, int max_wait_us, int flags,
@@ -5268,19 +5187,6 @@ extern "C" void mec_batcher_free(mec_batcher* b) {
   }
   b->cv_work.notify_all();
   if (b->worker.joinable()) b->worker.join();
-  for (int i = 0; i < kSlots; i++) {
-    if (b->ev_table[i]) cudaEventDestroy(b->ev_table[i]);
-    if (b->ev_gather[i]) cudaEventDestroy(b->ev_gather[i]);
-    for (int j = 0; j < 4; j++)
-      if (b->ev_ph[i][j]) cudaEventDestroy(b->ev_ph[i][j]);
-  }
-  if (b->aux) cudaStreamDestroy(b->aux);
-  batcher_destroy_streams(b);
-  mec_codec_free(b->serial);
-  mec_codec_free(b->serial_dst);
-  for (mec_codec* h : b->serial_whole) mec_codec_free(h);
-  mec_codec_free(b->dst);
-  mec_codec_free(b->codec);
   delete b;
 }
 

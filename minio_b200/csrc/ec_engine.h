@@ -139,12 +139,83 @@ void jit_shutdown();
 // NVRTC-compile (not load) the kernel specialised for `coef`; cubin bytes, 0 on a compile error, -1 without libnvrtc
 int64_t jit_compile_check(int k, int r, const uint8_t* coef, int align, int eb_t, bool rows3d, bool hash_out);
 
-// grow-only device / pinned buffers
+// Grow-only device / page-locked host buffers, freed by their owner.  ensure(n) keeps the buffer when it already holds n bytes and
+// otherwise frees it and allocates n plus slack (device: n/8 + 256, which batch_copy.cuh's tail loads rely on; pinned: n/4 + 4096).
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { release(); }
   int ensure(size_t n);
+
+ private:
   void release();
+};
+
+struct PinBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  PinBuf() = default;
+  PinBuf(const PinBuf&) = delete;
+  PinBuf& operator=(const PinBuf&) = delete;
+  ~PinBuf() { release(); }
+  int ensure(size_t n) {
+    if (n <= cap) return MEC_OK;
+    release();
+    const size_t want = n + (n >> 2) + 4096;
+    MEC_CUDA_OK(cudaHostAlloc(&p, want, cudaHostAllocPortable));
+    cap = want;
+    return MEC_OK;
+  }
+
+ private:
+  void release() {
+    if (p) cudaFreeHost(p);
+    p = nullptr;
+    cap = 0;
+  }
+};
+
+// A device table and its page-locked twin: filled on the host and uploaded, or written by a kernel and downloaded for the host to
+// read.  Sites that need one side only size that side.
+struct Mirror {
+  DevBuf d;
+  PinBuf h;
+  int ensure(size_t n) {
+    const int rc = d.ensure(n);
+    return rc ? rc : h.ensure(n);
+  }
+  cudaError_t upload(size_t n, cudaStream_t st) const { return cudaMemcpyAsync(d.p, h.p, n, cudaMemcpyHostToDevice, st); }
+  cudaError_t download(size_t n, cudaStream_t st) const { return cudaMemcpyAsync(h.p, d.p, n, cudaMemcpyDeviceToHost, st); }
+};
+
+// A CUDA stream / event that stays null until create() and is destroyed by its owner.  create() on one that exists is a no-op.
+class Stream {
+ public:
+  Stream() = default;
+  Stream(const Stream&) = delete;
+  Stream& operator=(const Stream&) = delete;
+  ~Stream() { if (h_) cudaStreamDestroy(h_); }
+  cudaError_t create(unsigned flags) { return h_ ? cudaSuccess : cudaStreamCreateWithFlags(&h_, flags); }
+  operator cudaStream_t() const { return h_; }
+
+ private:
+  cudaStream_t h_ = nullptr;
+};
+
+class Event {
+ public:
+  Event() = default;
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  ~Event() { if (h_) cudaEventDestroy(h_); }
+  cudaError_t create(unsigned flags) { return h_ ? cudaSuccess : cudaEventCreateWithFlags(&h_, flags); }
+  operator cudaEvent_t() const { return h_; }
+
+ private:
+  cudaEvent_t h_ = nullptr;
 };
 
 }  // namespace mec
